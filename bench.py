@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- stereo frames/sec of the circularMatching() hot path on B200 (+ the CPU reference arm).
+"""bench.py -- stereo frames/sec of the circularMatching() hot path on H100 (+ the CPU reference arm).
 
   python bench.py --gpus N --steps K --warmup W            this library (one process per GPU)
   python bench.py --impl reference --gpus N --steps K ...  the reference's OpenCV CPU path on the host cores
@@ -52,6 +52,8 @@ def parse():
     ap.add_argument("--width", type=int, default=W_IMG)
     ap.add_argument("--height", type=int, default=H_IMG)
     ap.add_argument("--calib", default="kitti", choices=["kitti", "zed"], help="intrinsics of the synthetic rig")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed paths returned in their last step to DIR/<name>.npy (rank 0)")
     return ap.parse_args()
 
 
@@ -62,7 +64,32 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
+
+
+RECORD_INTS = ("n_features", "n_detected", "n_tracked", "n_valid", "n_inliers", "ransac_iters", "pnp_status")
+
+
+def dump_outputs(d, res, res_e2e, outputs):
+    """--dump-outputs: the result records of the last resident step and of the last end-to-end step, and the point lists
+    of every unit of that end-to-end step, in float64 (integers are exact) or float32 (the library's float points).  The
+    units' point lists are concatenated; e2e_valid_offsets / e2e_inlier_offsets say where each unit's rows start."""
+    os.makedirs(d, exist_ok=True)
+
+    def save(name, a):
+        np.save(os.path.join(d, name + ".npy"), a)
+
+    for prefix, rs in (("resident", res), ("e2e", res_e2e)):
+        for k in RECORD_INTS:
+            save(f"{prefix}_{k}", np.array([r[k] for r in rs], np.float64))
+        for k in ("rvec", "tvec", "R"):
+            save(f"{prefix}_{k}", np.stack([np.asarray(r[k], np.float64) for r in rs]))
+    for k in ("l0", "r0", "l1", "r1", "X"):
+        save("e2e_" + k, np.concatenate([np.asarray(o[k], np.float32) for o in outputs]))
+    for k in ("kept_idx", "inliers"):
+        save("e2e_" + k, np.concatenate([np.asarray(o[k], np.float64) for o in outputs]))
+    save("e2e_valid_offsets", np.cumsum([0] + [len(o["kept_idx"]) for o in outputs]).astype(np.float64))
+    save("e2e_inlier_offsets", np.cumsum([0] + [len(o["inliers"]) for o in outputs]).astype(np.float64))
 
 
 class ClockSampler:
@@ -620,16 +647,6 @@ def bind_to_gpu_numa_node(torch, index):
         return {"node": None, "why": str(e)[:100]}
 
 
-def lk_profile_constants():
-    """ncu-derived constants of the LK kernel (committed under profiles/, refreshed per round): DRAM traffic per launch,
-    issue-slot utilisation and warp instructions per feature-ring."""
-    tp = os.path.join(ROOT, "profiles", "lk_traffic.json")
-    try:
-        return json.load(open(tp))
-    except Exception:
-        return {}
-
-
 # ------------------------------------------------------------------------------------------------
 def main():
     global W_IMG, H_IMG
@@ -713,6 +730,8 @@ def main():
     ms_e2e, wall_e2e, res_e2e = pt.measure_e2e(args.steps, args.warmup, True, BLOCKS)
     clocks = sampler.stop() if sampler else None
     ms_sum, _w, res_sum = pt.measure_e2e(args.steps, args.warmup, False, 1)       # records only (round-1 definition of e2e)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res, res_e2e, pt.last_outputs)
 
     # ---- parity on hardware: one unit of THIS rank against cv2 through the reference glue (outside the timed region) ----
     t_or = time.perf_counter()
@@ -746,7 +765,6 @@ def main():
         value = frames / (t_dev_ms * 1e-3)
         e2e_value = frames / (t_e2e_ms * 1e-3)
         peak, peak_src = peaks()
-        prof = lk_profile_constants()
 
         def roofline_of(lk_avg, nfeat):
             alg = LK_BYTES_PER_FEATURE * nfeat
@@ -816,16 +834,12 @@ def main():
                     "single_pair": single_pair, "sequence": seq},
             "gpu_launches": int(launches),
             "roofline": {"bound": "hbm", "kernel": "k_lk_ring", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": prof.get("dram_bytes_per_launch"), "peak_source": peak_src,
+                         "frac": achieved / peak, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": alg_bytes, "features_per_launch": feats_per_launch,
                          "avg_launch_ms": lk_avg_ms, "lk_share_of_step": lk_ms / t_single_ms if t_single_ms else None,
                          "single_stream_ms_per_step": t_single_ms / args.steps,
-                         "issue_frac": prof.get("issue_active_frac"),
-                         "warp_inst_per_feature_ring": prof.get("warp_inst_per_feature_ring"),
-                         "profile_source": prof.get("source"),
                          "sweep": sweep,
-                         "note": "algorithmic bytes per SURVEY.md 8(d); the kernel is issue bound (pyramids are L2 resident), see DESIGN.md; "
-                                 "issue_frac / warp_inst_per_feature_ring come from the committed ncu capture named in profile_source"},
+                         "note": "algorithmic bytes per SURVEY.md 8(d); the kernel is issue bound (pyramids are L2 resident), see DESIGN.md"},
             "cpu_baseline": cpu,
             "clocks": clocks,
             "parity": {"vs_oracle": parity_ok, "units_checked": world, "mismatches_rank0": bad, "gathered_records_ok_rank0": gather_ok,

@@ -1,6 +1,6 @@
 // compat/feature.h -- drop-in for the reference's feature.h: every function below has the same name,
 // parameter types and in-place vector semantics as its counterpart in reference src/feature.h:27-79,
-// but is implemented over the B200 C-ABI (include/vo_b200.h) in libvo_facade.so.  A translation unit of
+// but is implemented over the H100 C-ABI (include/vo_b200.h) in libvo_facade.so.  A translation unit of
 // the reference that includes "feature.h" keeps compiling when this directory shadows src/.
 // (Points / Status are plain aliases: the mangled signatures are the reference's.)
 #ifndef FEATURE_H

@@ -1,5 +1,5 @@
 /*
- * vo_b200.h -- C-ABI of the B200-native visual-odometry front-end (libvo_b200.so).
+ * vo_b200.h -- C-ABI of the H100-native visual-odometry front-end (libvo_b200.so).
  *
  * This is the drop-in boundary for the per-frame hot path of ZhenghaoFei/visual_odom:
  * every entry point replaces one OpenCV-backed function of the reference's libfeature /
@@ -14,7 +14,7 @@
  *   - every call is synchronous at return unless it says "async" (then it is ordered on the
  *     context's stream; see vo_set_stream / vo_sync).
  *   - return value: VO_OK (0) or a negative VO_E_* code; vo_last_error() gives the text.
- *   - there is NO CPU fallback: if no sm_100-class GPU is usable, vo_create fails.
+ *   - there is NO CPU fallback: if no compute capability 9.0 GPU (H100) is usable, vo_create fails.
  *   - a context is not thread-safe; distinct contexts are independent (one per host thread/GPU).
  */
 #ifndef VO_B200_H

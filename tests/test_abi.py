@@ -64,7 +64,8 @@ def test_sass_has_tma_and_no_legacy_tensor_ops(built):
     from visual_odom_b200 import capi
     sass = subprocess.run(["cuobjdump", "-sass", capi.LIB_PATH], capture_output=True, text=True).stdout
     assert "UTMALDG" in sass
-    assert "sm_100a" in subprocess.run(["cuobjdump", "-lelf", capi.LIB_PATH], capture_output=True, text=True).stdout
+    elfs = subprocess.run(["cuobjdump", "-lelf", capi.LIB_PATH], capture_output=True, text=True).stdout.splitlines()
+    assert elfs and all(ln.endswith(".sm_90a.cubin") for ln in elfs), elfs
 
 
 def test_result_record_numpy_view_matches_the_ctypes_struct():

@@ -1,5 +1,5 @@
 #!/bin/bash
-# demo (needs a B200): writes 8 synthetic KITTI-shaped stereo pairs as PNGs + a calibration file, runs tools/run_sequence.py on them, scores against itself
+# demo (needs an H100): writes 8 synthetic KITTI-shaped stereo pairs as PNGs + a calibration file, runs tools/run_sequence.py on them, scores against itself
 set -e
 D=$(mktemp -d)
 python - "$D" <<'PY'

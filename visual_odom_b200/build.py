@@ -1,6 +1,6 @@
 """Build the in-tree native artefacts.
 
-  visual_odom_b200/csrc/*.cu   -> visual_odom_b200/libvo_b200.so   (nvcc, sm_100a only)
+  visual_odom_b200/csrc/*.cu   -> visual_odom_b200/libvo_b200.so   (nvcc, sm_90a only)
   oracle/*.c                   -> oracle/_build/liboracle.so       (gcc; test infrastructure)
 
 Both are plain compiler invocations (no cmake, no JIT cache) so the built .so files travel to the
@@ -21,13 +21,17 @@ ORACLE_DIR = os.path.join(REPO, "oracle")
 ORACLE_LIB = os.path.join(ORACLE_DIR, "_build", "liboracle.so")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",   # B200 only; no PTX for other archs
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]    # H100 only; no PTX for other archs
+NVCC_FLAGS = GENCODE + [
     "-lineinfo", "-O3", "-std=c++17",
     "-fmad=false",            # IEEE mul/add kept separate: parity with the CPU reference needs it
     "-Xcompiler", "-fPIC,-fvisibility=hidden",
     "-cudart", "static",
 ]
+# Per-file NVVM optimisation level.  At -O3, NVVM's code for compute_90 turns the EPnP back end of k_pnp_hypotheses into
+# NaN on an H100 (CUDA 12.9; the same arithmetic compiled for the host, or by NVVM at a lower level, gives the exact pose),
+# so every RANSAC hypothesis failed.  ptxas still optimises these files at -O3.
+NVVM_OPT = {"pnp.cu": ["-Xcicc", "-O1"]}
 
 
 def _newer(src_list, target):
@@ -41,12 +45,14 @@ def build_native(verbose=False, force=False):
     srcs = sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cu"))
     hdrs = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".h", ".cuh"))]
     hdrs.append(os.path.join(REPO, "include", "vo_b200.h"))
+    hdrs.append(os.path.abspath(__file__))          # the flags above
     os.makedirs(OBJ, exist_ok=True)
     jobs = []
     for s in srcs:
         o = os.path.join(OBJ, os.path.basename(s)[:-3] + ".o")
         if force or _newer([s] + hdrs, o):
-            cmd = [NVCC] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-c", s, "-o", o]
+            cmd = [NVCC] + NVCC_FLAGS + NVVM_OPT.get(os.path.basename(s), []) + (["-Xptxas", "-v"] if verbose else []) + \
+                ["-c", s, "-o", o]
             jobs.append(cmd)
 
     def run(cmd):
@@ -61,7 +67,7 @@ def build_native(verbose=False, force=False):
                 raise RuntimeError("nvcc failed: " + " ".join(cmd))
     objs = [os.path.join(OBJ, os.path.basename(s)[:-3] + ".o") for s in srcs]
     if force or jobs or _newer(objs, LIB):
-        cmd = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static",
+        cmd = [NVCC, "-shared"] + GENCODE + ["-cudart", "static",
                "-o", LIB] + objs + ["-lz", "-lpthread"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

@@ -2,7 +2,7 @@
 
 This is plumbing only: it loads the in-tree shared library and exposes each C-ABI entry point
 with numpy buffers.  There is no Python/CPU implementation behind it -- if the library is
-missing or no B200-class GPU is present, the calls fail loudly.
+missing or no H100 (compute capability 9.0) is present, the calls fail loudly.
 """
 import ctypes as C
 import os

@@ -1,4 +1,4 @@
-// common.cuh -- shared declarations for the vo_b200 CUDA library (sm_100a only).
+// common.cuh -- shared declarations for the vo_b200 CUDA library (sm_90a only).
 //
 // Device data layout (see DESIGN.md "Data layout in HBM"):
 //   Every pyramid level l of every image lives in ONE allocation per level:

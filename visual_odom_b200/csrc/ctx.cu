@@ -54,8 +54,8 @@ extern "C" int vo_create(int device, const vo_params* params, vo_ctx** out)
     VO_CUDA_CHECK(cudaSetDevice(device));
     cudaDeviceProp prop;
     VO_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) {
-        vo_set_error(ctx, "device %d is sm_%d%d; this library ships sm_100a code only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {      // sm_90a code runs on compute capability 9.0 and nothing else
+        vo_set_error(ctx, "device %d is sm_%d%d; this library ships sm_90a code only", device, prop.major, prop.minor);
         return VO_E_UNSUPPORTED;
     }
     ctx->sm_count = prop.multiProcessorCount;
