@@ -28,10 +28,6 @@ NVCC_FLAGS = GENCODE + [
     "-Xcompiler", "-fPIC,-fvisibility=hidden",
     "-cudart", "static",
 ]
-# Per-file NVVM optimisation level.  At -O3, NVVM's code for compute_90 turns the EPnP back end of k_pnp_hypotheses into
-# NaN on an H100 (CUDA 12.9; the same arithmetic compiled for the host, or by NVVM at a lower level, gives the exact pose),
-# so every RANSAC hypothesis failed.  ptxas still optimises these files at -O3.
-NVVM_OPT = {"pnp.cu": ["-Xcicc", "-O1"]}
 
 
 def _newer(src_list, target):
@@ -51,7 +47,7 @@ def build_native(verbose=False, force=False):
     for s in srcs:
         o = os.path.join(OBJ, os.path.basename(s)[:-3] + ".o")
         if force or _newer([s] + hdrs, o):
-            cmd = [NVCC] + NVCC_FLAGS + NVVM_OPT.get(os.path.basename(s), []) + (["-Xptxas", "-v"] if verbose else []) + \
+            cmd = [NVCC] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + \
                 ["-c", s, "-o", o]
             jobs.append(cmd)
 

@@ -363,7 +363,9 @@ __device__ void rodrigues_jac(const double* r, double* J /* 3 x 9 */)
 }
 
 #define FIN_T 256
-__global__ void __launch_bounds__(FIN_T) k_pnp_finalize(const PnpArgs a)
+// one CTA per unit: minBlocks = 1 lets ptxas use up to 255 registers (with FIN_T alone it stopped at 128 and spilled the
+// LM accumulators)
+__global__ void __launch_bounds__(FIN_T, 1) k_pnp_finalize(const PnpArgs a)
 {
     const int unit = blockIdx.x;
     const PnpState& st = a.state[unit];

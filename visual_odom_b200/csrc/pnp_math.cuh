@@ -16,11 +16,9 @@
 #if defined(__CUDACC__)
 #define VO_HD __host__ __device__ __forceinline__
 #define VO_HDN __host__ __device__
-#define VO_HDNI __host__ __device__ __noinline__      // one copy in the kernel: the hypothesis kernel is I-cache bound
 #else
 #define VO_HD inline
 #define VO_HDN
-#define VO_HDNI
 #endif
 
 namespace vomath {
@@ -64,101 +62,127 @@ VO_HD double cv_hypot(double a, double b)
 // (first n1 rows normalised), W singular values (descending), Vt N x N.
 // WANT_V = false skips the accumulation of V (it never feeds back into At / W, so U^T and W are
 // bit-identical either way); Vt may then be nullptr.
+// The body is written once (JSVD_BODY) and instantiated with or without full unrolling of every loop over a compile-time
+// extent.  Fully unrolled (the 4x4 of triangulate_dlt, one per thread), every index is a constant and At / W / Vt live in
+// registers; the row swap of the sort is a compare per row rather than an index.  Larger systems keep plain loops:
+// unrolled, the 12x12 and 6x6 instances made k_pnp_hypotheses spill several times more.  (A counted `#pragma unroll 4`
+// does not help: it is applied after the arrays have been assigned to memory.)  Both forms do the same operations in the
+// same order.
+#define JSVD_BODY(JSVD_UNROLL)                                                                                              \
+    const double eps = kDblEps * 10;                                                                                        \
+    JSVD_UNROLL for (int i = 0; i < N; i++) {                                                                               \
+        double sd = 0;                                                                                                      \
+        JSVD_UNROLL for (int k = 0; k < M; k++) { double t = At[i * M + k]; sd += t * t; }                                  \
+        W[i] = sd;                                                                                                          \
+        if (WANT_V) {                                                                                                       \
+            JSVD_UNROLL for (int k = 0; k < N; k++) Vt[i * N + k] = 0;                                                      \
+            Vt[i * N + i] = 1;                                                                                              \
+        }                                                                                                                   \
+    }                                                                                                                       \
+    const int max_iter = M > 30 ? M : 30;                                                                                   \
+    for (int iter = 0; iter < max_iter; iter++) {                                                                           \
+        bool changed = false;                                                                                               \
+        JSVD_UNROLL for (int i = 0; i < N - 1; i++)                                                                         \
+            JSVD_UNROLL for (int j = 0; j < N; j++) {      /* j = i + 1 .. N - 1 */                                         \
+                if (j <= i) continue;                                                                                       \
+                double* Ai = At + i * M; double* Aj = At + j * M;                                                           \
+                double a = W[i], p = 0, b = W[j];                                                                           \
+                JSVD_UNROLL for (int k = 0; k < M; k++) p += Ai[k] * Aj[k];                                                 \
+                if (fabs(p) <= eps * sqrt(a * b)) continue;                                                                 \
+                p *= 2;                                                                                                     \
+                double beta = a - b, gamma = cv_hypot(p, beta), c, s;                                                       \
+                if (beta < 0) {                                                                                             \
+                    double delta = (gamma - beta) * 0.5;                                                                    \
+                    s = sqrt(delta / gamma);                                                                                \
+                    c = p / (gamma * s * 2);                                                                                \
+                } else {                                                                                                    \
+                    c = sqrt((gamma + beta) / (gamma * 2));                                                                 \
+                    s = p / (gamma * c * 2);                                                                                \
+                }                                                                                                           \
+                a = b = 0;                                                                                                  \
+                JSVD_UNROLL for (int k = 0; k < M; k++) {                                                                   \
+                    double t0 = c * Ai[k] + s * Aj[k];                                                                      \
+                    double t1 = -s * Ai[k] + c * Aj[k];                                                                     \
+                    Ai[k] = t0; Aj[k] = t1;                                                                                 \
+                    a += t0 * t0; b += t1 * t1;                                                                             \
+                }                                                                                                           \
+                W[i] = a; W[j] = b;                                                                                         \
+                changed = true;                                                                                             \
+                if (WANT_V) {                                                                                               \
+                    double* Vi = Vt + i * N; double* Vj = Vt + j * N;                                                       \
+                    JSVD_UNROLL for (int k = 0; k < N; k++) {                                                               \
+                        double t0 = c * Vi[k] + s * Vj[k];                                                                  \
+                        double t1 = -s * Vi[k] + c * Vj[k];                                                                 \
+                        Vi[k] = t0; Vj[k] = t1;                                                                             \
+                    }                                                                                                       \
+                }                                                                                                           \
+            }                                                                                                               \
+        if (!changed) break;                                                                                                \
+    }                                                                                                                       \
+    JSVD_UNROLL for (int i = 0; i < N; i++) {                                                                               \
+        double sd = 0;                                                                                                      \
+        JSVD_UNROLL for (int k = 0; k < M; k++) { double t = At[i * M + k]; sd += t * t; }                                  \
+        W[i] = sqrt(sd);                                                                                                    \
+    }                                                                                                                       \
+    /* selection sort (first maximum wins); the swap partner is found by comparison, never used as an index */              \
+    JSVD_UNROLL for (int i = 0; i < N - 1; i++) {                                                                           \
+        int j = i;                                                                                                          \
+        double wj = W[i];                                                                                                   \
+        JSVD_UNROLL for (int k = 0; k < N; k++)                                                                             \
+            if (k > i && wj < W[k]) { wj = W[k]; j = k; }                                                                   \
+        JSVD_UNROLL for (int q = 0; q < N; q++) {                                                                           \
+            if (q <= i || q != j) continue;                                                                                 \
+            double t = W[i]; W[i] = W[q]; W[q] = t;                                                                         \
+            JSVD_UNROLL for (int k = 0; k < M; k++) { t = At[i * M + k]; At[i * M + k] = At[q * M + k]; At[q * M + k] = t; } \
+            if (WANT_V) JSVD_UNROLL for (int k = 0; k < N; k++) { t = Vt[i * N + k]; Vt[i * N + k] = Vt[q * N + k]; Vt[q * N + k] = t; } \
+        }                                                                                                                   \
+    }                                                                                                                       \
+    Rng rng(0x12345678);                                                                                                    \
+    JSVD_UNROLL for (int i = 0; i < n1; i++) {                                                                              \
+        double sd = i < N ? W[i] : 0;                                                                                       \
+        for (int ii = 0; ii < 100 && sd <= kDblMin; ii++) {                                                                 \
+            /* exactly-zero singular value: random +-1/M vector, Gram-Schmidt against previous rows */                      \
+            const double val0 = 1. / M;                                                                                     \
+            JSVD_UNROLL for (int k = 0; k < M; k++) At[i * M + k] = (rng.next() & 256) != 0 ? val0 : -val0;                 \
+            for (int it = 0; it < 2; it++)                                                                                  \
+                JSVD_UNROLL for (int j = 0; j < N; j++) {                                                                   \
+                    if (j >= i) continue;                                                                                   \
+                    sd = 0;                                                                                                 \
+                    JSVD_UNROLL for (int k = 0; k < M; k++) sd += At[i * M + k] * At[j * M + k];                            \
+                    double asum = 0;                                                                                        \
+                    JSVD_UNROLL for (int k = 0; k < M; k++) {                                                               \
+                        double t = At[i * M + k] - sd * At[j * M + k];                                                      \
+                        At[i * M + k] = t;                                                                                  \
+                        asum += fabs(t);                                                                                    \
+                    }                                                                                                       \
+                    asum = asum > eps * 100 ? 1 / asum : 0;                                                                 \
+                    JSVD_UNROLL for (int k = 0; k < M; k++) At[i * M + k] *= asum;                                          \
+                }                                                                                                           \
+            sd = 0;                                                                                                         \
+            JSVD_UNROLL for (int k = 0; k < M; k++) { double t = At[i * M + k]; sd += t * t; }                              \
+            sd = sqrt(sd);                                                                                                  \
+        }                                                                                                                   \
+        const double s = sd > kDblMin ? 1 / sd : 0.;                                                                        \
+        JSVD_UNROLL for (int k = 0; k < M; k++) At[i * M + k] *= s;                                                         \
+    }                                                                                                                       \
+
+#if defined(__CUDA_ARCH__)
+#define JSVD_FULL_UNROLL _Pragma("unroll")
+#else
+#define JSVD_FULL_UNROLL
+#endif
+
 template <int M, int N, bool WANT_V = true>
 VO_HDN void jacobi_svd_t(double* At, double* W, double* Vt, int n1)
 {
-    const double eps = kDblEps * 10;
-    for (int i = 0; i < N; i++) {
-        double sd = 0;
-        for (int k = 0; k < M; k++) { double t = At[i * M + k]; sd += t * t; }
-        W[i] = sd;
-        if (WANT_V) {
-            for (int k = 0; k < N; k++) Vt[i * N + k] = 0;
-            Vt[i * N + i] = 1;
-        }
-    }
-    const int max_iter = M > 30 ? M : 30;
-    for (int iter = 0; iter < max_iter; iter++) {
-        bool changed = false;
-        for (int i = 0; i < N - 1; i++)
-            for (int j = i + 1; j < N; j++) {
-                double* Ai = At + i * M; double* Aj = At + j * M;
-                double a = W[i], p = 0, b = W[j];
-                for (int k = 0; k < M; k++) p += Ai[k] * Aj[k];
-                if (fabs(p) <= eps * sqrt(a * b)) continue;
-                p *= 2;
-                double beta = a - b, gamma = cv_hypot(p, beta), c, s;
-                if (beta < 0) {
-                    double delta = (gamma - beta) * 0.5;
-                    s = sqrt(delta / gamma);
-                    c = p / (gamma * s * 2);
-                } else {
-                    c = sqrt((gamma + beta) / (gamma * 2));
-                    s = p / (gamma * c * 2);
-                }
-                a = b = 0;
-                for (int k = 0; k < M; k++) {
-                    double t0 = c * Ai[k] + s * Aj[k];
-                    double t1 = -s * Ai[k] + c * Aj[k];
-                    Ai[k] = t0; Aj[k] = t1;
-                    a += t0 * t0; b += t1 * t1;
-                }
-                W[i] = a; W[j] = b;
-                changed = true;
-                if (WANT_V) {
-                    double* Vi = Vt + i * N; double* Vj = Vt + j * N;
-                    for (int k = 0; k < N; k++) {
-                        double t0 = c * Vi[k] + s * Vj[k];
-                        double t1 = -s * Vi[k] + c * Vj[k];
-                        Vi[k] = t0; Vj[k] = t1;
-                    }
-                }
-            }
-        if (!changed) break;
-    }
-    for (int i = 0; i < N; i++) {
-        double sd = 0;
-        for (int k = 0; k < M; k++) { double t = At[i * M + k]; sd += t * t; }
-        W[i] = sqrt(sd);
-    }
-    for (int i = 0; i < N - 1; i++) {
-        int j = i;
-        for (int k = i + 1; k < N; k++)
-            if (W[j] < W[k]) j = k;
-        if (i != j) {
-            double t = W[i]; W[i] = W[j]; W[j] = t;
-            for (int k = 0; k < M; k++) { t = At[i * M + k]; At[i * M + k] = At[j * M + k]; At[j * M + k] = t; }
-            if (WANT_V) for (int k = 0; k < N; k++) { t = Vt[i * N + k]; Vt[i * N + k] = Vt[j * N + k]; Vt[j * N + k] = t; }
-        }
-    }
-    Rng rng(0x12345678);
-    for (int i = 0; i < n1; i++) {
-        double sd = i < N ? W[i] : 0;
-        for (int ii = 0; ii < 100 && sd <= kDblMin; ii++) {
-            // exactly-zero singular value: random +-1/M vector, Gram-Schmidt against previous rows
-            const double val0 = 1. / M;
-            for (int k = 0; k < M; k++) At[i * M + k] = (rng.next() & 256) != 0 ? val0 : -val0;
-            for (int it = 0; it < 2; it++)
-                for (int j = 0; j < i; j++) {
-                    sd = 0;
-                    for (int k = 0; k < M; k++) sd += At[i * M + k] * At[j * M + k];
-                    double asum = 0;
-                    for (int k = 0; k < M; k++) {
-                        double t = At[i * M + k] - sd * At[j * M + k];
-                        At[i * M + k] = t;
-                        asum += fabs(t);
-                    }
-                    asum = asum > eps * 100 ? 1 / asum : 0;
-                    for (int k = 0; k < M; k++) At[i * M + k] *= asum;
-                }
-            sd = 0;
-            for (int k = 0; k < M; k++) { double t = At[i * M + k]; sd += t * t; }
-            sd = sqrt(sd);
-        }
-        const double s = sd > kDblMin ? 1 / sd : 0.;
-        for (int k = 0; k < M; k++) At[i * M + k] *= s;
+    if constexpr (M == 4 && N == 4) {
+        JSVD_BODY(JSVD_FULL_UNROLL)
+    } else {
+        JSVD_BODY()
     }
 }
+#undef JSVD_FULL_UNROLL
+#undef JSVD_BODY
 
 // cv::solve(A (M x N row-major), b, x, DECOMP_SVD), one right-hand side
 template <int M, int N>
@@ -524,7 +548,11 @@ VO_HDN inline void epnp5_front(const float* Xw_f, const float* uv_f, double fu, 
 // One of EPnP's three beta initialisations (approx = 1: betas from [B11 B12 B13 B14], 2: [B11 B12 B22], 3: [B11 B12 B22 B13
 // B23]) -> Gauss-Newton -> R, t and the mean reprojection error of the 5 points.  The three are independent, so the
 // hypothesis kernel runs them on three lanes in lockstep (run-time system width) and picks like the reference does.
-VO_HDNI inline void epnp5_back_one(const Epnp5State& st, const double* v0, const double* v1, const double* v2, const double* v3,
+// Always inlined.  Compiled as a separate (__noinline__) device function by NVVM at -O3 (CUDA 12.9, compute_90a), the beta
+// least-squares solve below (solve_svd_rt) returned NaN on an H100 although L and rho going into it were exact, and ptxas at
+// -O0 gave the same NaN.  No undefined behaviour was found in this source and the failing PTX instruction has not been
+// isolated, so the cause is unconfirmed: do not make this function out-of-line again without rerunning the GPU PnP tests.
+VO_HD void epnp5_back_one(const Epnp5State& st, const double* v0, const double* v1, const double* v2, const double* v3,
                                   int approx, double* R, double* t, double* err_out)
 {
 
