@@ -202,7 +202,8 @@ VO_API int vo_batch_wait(vo_ctx* ctx, int first_unit, int n_units, vo_unit_resul
  * trackingFrame2Frame() hand back (reference src/visualOdometry.h:27-42): the four point lists, the tracked-feature
  * indices, points3D and the inlier list of every unit, packed on the device and copied with ONE device-to-host copy per
  * submission into pinned staging.  vo_batch_outputs reads a waited unit from that staging (layout as vo_batch_fetch;
- * any pointer may be NULL); *d2h_bytes_per_unit = bytes that crossed PCIe for the unit's packed block. */
+ * any pointer may be NULL) until its slot is resubmitted, whatever feature counts other slot ranges are submitted with;
+ * *d2h_bytes_per_unit = bytes that cross PCIe per unit (a block sized for the largest feature count of the resident slots). */
 VO_API int vo_batch_outputs(vo_ctx* ctx, int unit, vo_point2f* pts4, int32_t* kept_idx, vo_point3f* X, int32_t* inliers,
                             size_t* d2h_bytes_per_unit);
 VO_API int vo_batch_fetch(vo_ctx* ctx, int unit, vo_point2f* pts_in, vo_point2f* pts4, int32_t* kept_idx,

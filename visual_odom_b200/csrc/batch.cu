@@ -7,6 +7,7 @@
 // the benchmark's stride selection), src/main.cpp:170-171 and src/visualOdometry.cpp:132-193.
 #include "ctx.h"
 #include <string.h>
+#include <algorithm>
 
 __global__ void k_pack_counts(vo_unit_result_dev* res, const int* n_pts, const int* n_det, const int* n3, const int* n5,
                               int n_units, int detect)
@@ -43,25 +44,65 @@ __global__ void k_pack_outputs(uint8_t* __restrict__ out, size_t stride, int per
     for (int i = threadIdx.x; i < ni; i += blockDim.x) oi[i] = inliers[ub + i];
 }
 
-// device + pinned blocks of the packed outputs, sized for the configured batch and the resident feature counts
-static int ensure_outputs(vo_ctx* ctx)
+// the four parts of one unit's packed block with `per` point slots (layout of k_pack_outputs)
+struct PackedUnit { float2* o4; int* ok; float* oX; int* oi; };
+static PackedUnit packed_unit(uint8_t* base, int per)
 {
-    int per = ctx->batch_max_pts > 0 ? ctx->batch_max_pts : ctx->cap;
-    per = (per + 63) / 64 * 64;
+    PackedUnit p;
+    p.o4 = (float2*)base;
+    p.ok = (int*)(p.o4 + 4 * (size_t)per);
+    p.oX = (float*)(p.ok + per);
+    p.oi = (int*)(p.oX + 3 * (size_t)per);
+    return p;
+}
+
+// largest feature bound of the slots [u0, u0 + n): the LK launch of that range has no unit with more live features
+static int range_bound(const vo_ctx* ctx, int u0, int n)
+{
+    int b = 0;
+    for (int u = u0; u < u0 + n && u < (int)ctx->slot_pts.size(); u++) b = ctx->slot_pts[u] > b ? ctx->slot_pts[u] : b;
+    return b;
+}
+
+// Device + pinned blocks of the packed outputs before a submission of slots [u0, u0 + n) whose units carry at most
+// `bound` features.  `per` is the largest bound over the resident slots, so it never drops below what a submission that
+// is still in flight, or waited for but not yet read, has packed.  On a resize those submissions are completed first
+// (they stay pending for vo_batch_wait) and every unit's lists are moved into the new layout.
+static int ensure_outputs(vo_ctx* ctx, int u0, int n, int bound)
+{
+    int per = bound;
+    for (int u = 0; u < (int)ctx->slot_pts.size(); u++)
+        if ((u < u0 || u >= u0 + n) && ctx->slot_pts[u] > per) per = ctx->slot_pts[u];
+    per = ((per > 1 ? per : 1) + 63) / 64 * 64;
     if (per > ctx->cap) per = ctx->cap;
+    if (ctx->d_out && ctx->h_out && ctx->out_per == per && ctx->out_units >= ctx->units) return VO_OK;
     const size_t stride = ((size_t)per * VO_OUT_BYTES_PER_SLOT + 255) / 256 * 256;
-    if (ctx->d_out && ctx->out_per == per && ctx->h_out && ctx->out_units >= ctx->units) return VO_OK;
-    int rc = vo_drain_pending(ctx);
-    if (rc) return rc;
-    if (!ctx->d_out || ctx->out_per != per) {
-        void* q = nullptr;                      // freed with the batch state (ctx->allocs)
-        VO_CUDA_CHECK(cudaMalloc(&q, stride * ctx->units + 256));
-        ctx->allocs.push_back(q);
-        ctx->d_out = (uint8_t*)q;
-        vo_drop_graphs(ctx);                    // graphs hold the old pointer / stride
+    for (auto& p : ctx->pending)                // their copies land in the old blocks
+        if (p.active) VO_CUDA_CHECK(cudaEventSynchronize(p.done));
+    void* q = nullptr;                          // both new blocks first: a failed allocation leaves the old ones in use
+    VO_CUDA_CHECK(cudaMalloc(&q, stride * ctx->units + 256));
+    uint8_t* h = nullptr;
+    const cudaError_t e = cudaMallocHost(&h, stride * ctx->units + 256);
+    if (e != cudaSuccess) { cudaFree(q); VO_CUDA_CHECK(e); }
+    if (ctx->h_out) {
+        const int nu = ctx->out_units < ctx->units ? ctx->out_units : ctx->units;
+        const int m = ctx->out_per < per ? ctx->out_per : per;
+        for (int u = 0; u < nu; u++) {
+            const PackedUnit a = packed_unit(ctx->h_out + (size_t)u * ctx->out_stride, ctx->out_per), b = packed_unit(h + (size_t)u * stride, per);
+            for (int k = 0; k < 4; k++) memcpy(b.o4 + (size_t)k * per, a.o4 + (size_t)k * ctx->out_per, (size_t)m * sizeof(float2));
+            memcpy(b.ok, a.ok, (size_t)m * sizeof(int));
+            memcpy(b.oX, a.oX, (size_t)m * 3 * sizeof(float));
+            memcpy(b.oi, a.oi, (size_t)m * sizeof(int));
+        }
+        cudaFreeHost(ctx->h_out);
     }
-    if (ctx->h_out) { cudaFreeHost(ctx->h_out); ctx->h_out = nullptr; }
-    VO_CUDA_CHECK(cudaMallocHost(&ctx->h_out, stride * ctx->units + 256));
+    ctx->h_out = h;
+    if (ctx->d_out) {                           // only a staging area for the D2H copies: nothing in it is kept
+        ctx->allocs.erase(std::find(ctx->allocs.begin(), ctx->allocs.end(), (void*)ctx->d_out));
+        cudaFree(ctx->d_out);
+    }
+    ctx->allocs.push_back(q);                   // freed with the batch state
+    ctx->d_out = (uint8_t*)q;
     ctx->out_units = ctx->units; ctx->out_per = per; ctx->out_stride = stride;
     return VO_OK;
 }
@@ -77,6 +118,7 @@ extern "C" int vo_batch_configure(vo_ctx* ctx, int w, int h, int n_units, const 
     vo_set_calibration(ctx, P_l, P_r);
     ctx->batch_units = n_units;
     ctx->batch_uploaded = 0;
+    ctx->slot_pts.assign(n_units, 0);
     return VO_OK;
 }
 
@@ -100,6 +142,7 @@ static int upload_range(vo_ctx* ctx, const vo_unit* units, int u0, int n, size_t
             VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_pts_in + (size_t)u * cap, U.pts, (size_t)U.n_pts * sizeof(float2),
                                           cudaMemcpyHostToDevice, st));
         h_cnt[u] = U.n_pts;
+        ctx->slot_pts[u] = U.n_pts;
         for (int k = 0; k < 3; k++) h_tprev[3 * u + k] = U.t_prev[k];
     }
     VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_tprev + 3 * (size_t)u0, h_tprev + 3 * (size_t)u0, (size_t)n * 3 * sizeof(double),
@@ -109,7 +152,7 @@ static int upload_range(vo_ctx* ctx, const vo_unit* units, int u0, int n, size_t
     return VO_OK;
 }
 
-static int validate_units(vo_ctx* ctx, const vo_unit* units, int n_units, size_t pitch, bool* detect_out, int* max_pts_out)
+static int validate_units(vo_ctx* ctx, const vo_unit* units, int n_units, size_t pitch, bool* detect_out, int* max_pts_out = nullptr)
 {
     if (!ctx || !units) return VO_E_INVALID;
     if (n_units <= 0 || n_units > ctx->batch_units) { vo_set_error(ctx, "n_units=%d outside the configured batch (%d)", n_units, ctx->batch_units); return VO_E_INVALID; }
@@ -123,7 +166,8 @@ static int validate_units(vo_ctx* ctx, const vo_unit* units, int n_units, size_t
         if (U.n_pts < 0 || U.n_pts > ctx->cap) { vo_set_error(ctx, "unit %d: n_pts=%d outside [0,%d]", u, U.n_pts, ctx->cap); return VO_E_CAPACITY; }
         if (U.n_pts > max_pts) max_pts = U.n_pts;
     }
-    *detect_out = detect; *max_pts_out = max_pts;
+    *detect_out = detect;
+    if (max_pts_out) *max_pts_out = max_pts;
     // pinned staging: t_prev, counts, result records
     const size_t bytes = (size_t)ctx->batch_units * (3 * sizeof(double) + sizeof(int) + sizeof(vo_unit_result_dev)) + 256;
     return vo_ensure_pinned(ctx, bytes);
@@ -138,8 +182,8 @@ static vo_unit_result_dev* pinned_results(vo_ctx* ctx)
 
 extern "C" int vo_batch_upload(vo_ctx* ctx, const vo_unit* units, int n_units, size_t pitch)
 {
-    bool detect; int max_pts;
-    int rc = validate_units(ctx, units, n_units, pitch, &detect, &max_pts);
+    bool detect;
+    int rc = validate_units(ctx, units, n_units, pitch, &detect);
     if (rc) return rc;
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
     if ((rc = vo_claim_buffers(ctx, "vo_batch_upload", true))) return rc;
@@ -148,7 +192,6 @@ extern "C" int vo_batch_upload(vo_ctx* ctx, const vo_unit* units, int n_units, s
     if ((rc = upload_range(ctx, units, 0, n_units, pitch, ctx->stream, detect))) return rc;
     ctx->batch_uploaded = n_units;
     ctx->batch_detect = detect;
-    ctx->batch_max_pts = max_pts;
     return VO_OK;
 }
 
@@ -216,7 +259,7 @@ static int run_range_launch(vo_ctx* ctx, const View& v)
         VO_CUDA_CHECK(cudaStreamWaitEvent(lk.s, ev[1], 0));
     }
     const int ip[4] = {0, 1, 3, 2}, in[4] = {1, 3, 2, 0};      // ring L0->R0->R1->L1->L0 (planes L0,R0,L1,R1)
-    ctx->lk_per_unit = ctx->batch_max_pts;                      // no unit of the resident batch has more live features
+    ctx->lk_per_unit = range_bound(ctx, v.u0, v.n);             // no unit of the range has more live features
     rc = vo_run_lk_ring(ctx, lk, 4, ip, in, false);
     ctx->lk_per_unit = 0;
     if (rc) return rc;
@@ -251,8 +294,9 @@ static int run_range(vo_ctx* ctx, const View& v)
     bool on_side = false;
     for (int k = 0; k < VO_LANES; k++) on_side = on_side || (ctx->side_stream[k] && v.s == ctx->side_stream[k]);
     if (!ctx->use_graphs || ((ctx->use_priorities || ctx->part_on) && on_side && !ctx->batch_graphs)) return run_range_launch(ctx, v);
+    const int max_pts = range_bound(ctx, v.u0, v.n);
     for (auto& g : ctx->graphs)
-        if (g.u0 == v.u0 && g.n == v.n && g.detect == ctx->batch_detect && g.tma == ctx->lk_use_tma && g.s == v.s && g.max_pts == ctx->batch_max_pts) {
+        if (g.u0 == v.u0 && g.n == v.n && g.detect == ctx->batch_detect && g.tma == ctx->lk_use_tma && g.s == v.s && g.max_pts == max_pts) {
             VO_CUDA_CHECK(cudaGraphLaunch(g.exec, v.s));
             ctx->launches += g.launches;
             return VO_OK;
@@ -268,7 +312,7 @@ static int run_range(vo_ctx* ctx, const View& v)
     if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
     VO_CUDA_CHECK(e);
     vo_ctx::RangeGraph g;
-    g.u0 = v.u0; g.n = v.n; g.detect = ctx->batch_detect; g.tma = ctx->lk_use_tma; g.s = v.s; g.max_pts = ctx->batch_max_pts;      // the LK launch geometry depends on max_pts
+    g.u0 = v.u0; g.n = v.n; g.detect = ctx->batch_detect; g.tma = ctx->lk_use_tma; g.s = v.s; g.max_pts = max_pts;      // the LK launch geometry depends on max_pts
     g.launches = ctx->launches - before;
     VO_CUDA_CHECK(cudaGraphInstantiate(&g.exec, graph, 0));
     cudaGraphDestroy(graph);
@@ -319,8 +363,8 @@ extern "C" int vo_batch_download(vo_ctx* ctx, vo_unit_result* results, int n_uni
 // under the kernels of the first (the images arrive over PCIe; compute is ~6x longer than the copy).
 extern "C" int vo_frame_batch(vo_ctx* ctx, const vo_unit* units, int n_units, size_t pitch, vo_unit_result* results)
 {
-    bool detect; int max_pts;
-    int rc = validate_units(ctx, units, n_units, pitch, &detect, &max_pts);
+    bool detect;
+    int rc = validate_units(ctx, units, n_units, pitch, &detect);
     if (rc) return rc;
     if (!results) return VO_E_INVALID;
     if (!ctx->have_P) { vo_set_error(ctx, "vo_frame_batch: projection matrices not set"); return VO_E_INVALID; }
@@ -328,7 +372,7 @@ extern "C" int vo_frame_batch(vo_ctx* ctx, const vo_unit* units, int n_units, si
     if ((rc = vo_claim_buffers(ctx, "vo_frame_batch", true))) return rc;
     if ((rc = vo_drain_pending(ctx))) return rc;
     VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-    ctx->batch_uploaded = n_units; ctx->batch_detect = detect; ctx->batch_max_pts = max_pts;
+    ctx->batch_uploaded = n_units; ctx->batch_detect = detect;
     vo_unit_result_dev* h_res = pinned_results(ctx);
     const int nchunks = (n_units >= 2 && ctx->batch_streams >= 2) ? 2 : 1;
     if (nchunks == 1) {
@@ -375,7 +419,7 @@ extern "C" int vo_batch_submit(vo_ctx* ctx, const vo_unit* units, int first_unit
             vo_set_error(ctx, "vo_batch_submit: slots [%d, %d) overlap a submission that has not been waited for", first_unit, first_unit + n_units);
             return VO_E_INVALID;
         }
-    bool detect = ctx->batch_detect; int max_pts = ctx->batch_max_pts;
+    bool detect = ctx->batch_detect; int max_pts = 0;
     int rc;
     if (units) {
         if ((rc = validate_units(ctx, units, n_units, pitch, &detect, &max_pts))) return rc;
@@ -386,6 +430,7 @@ extern "C" int vo_batch_submit(vo_ctx* ctx, const vo_unit* units, int first_unit
         }
         const size_t bytes = (size_t)ctx->batch_units * (3 * sizeof(double) + sizeof(int) + sizeof(vo_unit_result_dev)) + 256;
         if ((rc = vo_ensure_pinned(ctx, bytes))) return rc;
+        max_pts = range_bound(ctx, first_unit, n_units);
     }
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
     if ((rc = ensure_side_streams(ctx))) return rc;
@@ -397,8 +442,7 @@ extern "C" int vo_batch_submit(vo_ctx* ctx, const vo_unit* units, int first_unit
         ctx->part_pre_with_lk = true;
         if (vo_partition_enable(ctx, 8) != VO_OK) ctx->err[0] = 0;      // no green contexts on this driver: run unpartitioned
     }
-    if (max_pts > ctx->batch_max_pts || units) ctx->batch_max_pts = max_pts;
-    if (ctx->batch_outputs && (rc = ensure_outputs(ctx))) return rc;
+    if (ctx->batch_outputs && (rc = ensure_outputs(ctx, first_unit, n_units, max_pts))) return rc;
     vo_ctx::Pending* slot = nullptr;
     for (auto& p : ctx->pending) if (!p.active) { slot = &p; break; }
     if (!slot) {
@@ -412,7 +456,6 @@ extern "C" int vo_batch_submit(vo_ctx* ctx, const vo_unit* units, int first_unit
     VO_CUDA_CHECK(cudaStreamWaitEvent(st, ctx->fork_ev, 0));
     if ((rc = vo_dist_order_after_gathers(ctx, st))) return rc;
     ctx->batch_detect = detect;
-    if (max_pts > ctx->batch_max_pts || units) ctx->batch_max_pts = max_pts;
     if (units) {
         if ((rc = upload_range(ctx, units, first_unit, n_units, pitch, st, detect, 0))) return rc;
         if (ctx->batch_uploaded < first_unit + n_units) ctx->batch_uploaded = first_unit + n_units;
@@ -464,15 +507,11 @@ extern "C" int vo_batch_outputs(vo_ctx* ctx, int unit, vo_point2f* pts4, int32_t
     const vo_unit_result_dev& r = pinned_results(ctx)[unit];
     const int per = ctx->out_per;
     const int nv = r.n_valid < per ? r.n_valid : per, ni = r.n_inliers < per ? r.n_inliers : per;
-    const uint8_t* base = ctx->h_out + (size_t)unit * ctx->out_stride;
-    const float2* o4 = (const float2*)base;
-    const int* ok = (const int*)(o4 + 4 * (size_t)per);
-    const float* oX = (const float*)(ok + per);
-    const int* oi = (const int*)(oX + 3 * (size_t)per);
-    if (pts4) for (int k = 0; k < 4; k++) memcpy(pts4 + (size_t)k * nv, o4 + (size_t)k * per, (size_t)nv * sizeof(float2));
-    if (kept_idx) memcpy(kept_idx, ok, (size_t)nv * sizeof(int));
-    if (X) memcpy(X, oX, (size_t)nv * 3 * sizeof(float));
-    if (inliers) memcpy(inliers, oi, (size_t)ni * sizeof(int));
+    const PackedUnit o = packed_unit(ctx->h_out + (size_t)unit * ctx->out_stride, per);
+    if (pts4) for (int k = 0; k < 4; k++) memcpy(pts4 + (size_t)k * nv, o.o4 + (size_t)k * per, (size_t)nv * sizeof(float2));
+    if (kept_idx) memcpy(kept_idx, o.ok, (size_t)nv * sizeof(int));
+    if (X) memcpy(X, o.oX, (size_t)nv * 3 * sizeof(float));
+    if (inliers) memcpy(inliers, o.oi, (size_t)ni * sizeof(int));
     if (d2h_bytes_per_unit) *d2h_bytes_per_unit = ctx->out_stride;
     return VO_OK;
 }

@@ -68,7 +68,7 @@ extern "C" int vo_create(int device, const vo_params* params, vo_ctx** out)
     {   // VO_LK_STAGING=ldg switches the LK window staging from TMA to plain loads (debug / A-B runs)
         const char* st = getenv("VO_LK_STAGING");
         ctx->lk_use_tma = !(st && strcmp(st, "ldg") == 0);
-        const char* sp = getenv("VO_LK_SPAN");      // force the LK work-item size (tests run the whole suite at 1)
+        const char* sp = getenv("VO_LK_SPAN");      // force the LK work-item size (tests/test_gpu_lk_variants.py sets it per context with "lk_span")
         if (sp) ctx->lk_span = atoi(sp);
         const char* pt = getenv("VO_SM_PARTITION");  // 0: never partition the SMs (profilers cannot attach to green-context launches)
         if (pt && atoi(pt) == 0) ctx->part_auto = false;

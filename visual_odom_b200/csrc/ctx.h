@@ -148,7 +148,7 @@ struct vo_ctx {
     bool use_graphs = true;         // replay the per-range kernel sequence as a CUDA graph (no LK event timing then)
     struct RangeGraph { int u0, n; bool detect, tma; cudaStream_t s; int max_pts; cudaGraphExec_t exec; long long launches; };   // s: the stream it was captured on (its LK work queue is that stream's)
     std::vector<RangeGraph> graphs; // invalidated when the device state is re-allocated
-    int batch_max_pts = 0;          // largest per-unit feature count of the resident batch
+    std::vector<int> slot_pts;      // [batch_units] feature bound of each slot: n_pts of the unit last uploaded into it
     cudaStream_t hi_stream[VO_LANES] = {};     // high-priority helpers of the side streams (see run_range_launch)
     cudaEvent_t hi_ev[VO_LANES][4] = {};
     bool use_priorities = true;
@@ -163,7 +163,7 @@ struct vo_ctx {
     uint8_t* d_out = nullptr;       // [units][out_stride]  (part of the batch state)
     uint8_t* h_out = nullptr;       // pinned, [out_units][out_stride]
     size_t out_stride = 0;
-    int out_per = 0, out_units = 0; // point slots per unit in a packed block; units the pinned block holds
+    int out_per = 0, out_units = 0; // point slots per unit in a packed block (>= every resident slot's bound); units the pinned block holds
     unsigned submit_count = 0;
 };
 
