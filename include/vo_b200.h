@@ -50,8 +50,11 @@ typedef struct vo_point3f { float x, y, z; } vo_point3f;
 
 /* All literals the reference hard-codes, as run-time parameters (SURVEY.md section 5, "Config"). */
 typedef struct vo_params {
-    int fast_threshold;      /* 20      reference src/feature.cpp:43                          */
-    int fast_nonmax;         /* 1       reference src/feature.cpp:44                          */
+    int fast_threshold;      /* 20      reference src/feature.cpp:43; vo_create refuses values
+                                        outside [0, 255] (VO_E_INVALID)                           */
+    int fast_nonmax;         /* 1       reference src/feature.cpp:44; 0: every FAST corner is kept
+                                        with response 0 (as cv::FAST).  Fixed at vo_create: the
+                                        corner capacity of a frame depends on it                  */
     int lk_win;              /* 21      reference src/feature.cpp:127 (only 21 is built)      */
     int lk_max_level;        /* 3       reference src/feature.cpp:136 (0-based: 4 images)     */
     int lk_max_iters;        /* 30      reference src/feature.cpp:128                         */

@@ -1,18 +1,20 @@
 /*
  * oracle/fast_ref.c -- TEST INFRASTRUCTURE ONLY (never linked into the product).
  *
- * Plain-C CPU restatement of cv::FAST(image, keypoints, threshold, nonmaxSuppression=true)
- * (FastFeatureDetector::TYPE_9_16), the call made by the reference's
- * featureDetectionFast() (reference src/feature.cpp:39-47).  The arithmetic lives in
- * OpenCV (un-vendored; pinned to 4.13.0 as installed: modules/features2d/src/fast.cpp,
+ * Plain-C CPU restatement of cv::FAST(image, keypoints, threshold, nonmaxSuppression)
+ * (FastFeatureDetector::TYPE_9_16); the reference's featureDetectionFast() calls it with
+ * threshold 20 and non-max suppression (reference src/feature.cpp:39-47).  The arithmetic
+ * lives in OpenCV (un-vendored; pinned to 4.13.0 as installed: modules/features2d/src/fast.cpp,
  * fast_score.cpp); the published algorithm is restated here and pinned against cv2 by
- * tests/test_oracle_fast.py (coordinates, raster order and response all identical).
+ * tests/test_oracle_fast.py (coordinates, raster order and response all identical, at
+ * thresholds 0..255 with and without non-max suppression).
  *
  * A pixel p (3-pixel border excluded) is a corner iff >= 9 contiguous pixels of the
  * 16-pixel Bresenham ring are all > p+t or all < p-t.  Its score is the largest t'
  * for which it is still a corner (cornerScore<16>); with non-max suppression a corner
  * is kept iff its score is strictly greater than the scores of its 8 neighbours
- * (non-corners score 0).  Output is in raster order.
+ * (non-corners score 0) and its response is the score; without it every corner is
+ * kept with response 0.  Output is in raster order.
  */
 #include <stdint.h>
 #include <stdlib.h>
@@ -75,34 +77,45 @@ static int is_corner(const uint8_t *p, int step, int t)
     return 0;
 }
 
-/* score map: 0 for non-corners, cornerScore for corners (always >= threshold) */
-void fast_score_map(const uint8_t *img, int w, int h, int step, int threshold, uint8_t *score /* w*h */)
+/* corner map: 1 for corners; score map: cornerScore for corners, 0 for non-corners.  A corner
+ * scores at least the threshold, so at threshold 0 a corner can score 0: whether a pixel is a
+ * corner is read from the corner map, never from the score.                                    */
+void fast_score_map(const uint8_t *img, int w, int h, int step, int threshold,
+                    uint8_t *score /* w*h */, uint8_t *corner /* w*h */)
 {
     memset(score, 0, (size_t)w * h);
+    memset(corner, 0, (size_t)w * h);
     for (int y = 3; y < h - 3; y++)
         for (int x = 3; x < w - 3; x++) {
             const uint8_t *p = img + y * step + x;
-            if (is_corner(p, step, threshold))
+            if (is_corner(p, step, threshold)) {
+                corner[y * w + x] = 1;
                 score[y * w + x] = (uint8_t)corner_score(p, step, threshold);
+            }
         }
 }
 
-/* returns number of keypoints; xy (2 floats each) and response are optional outputs */
+/* returns number of keypoints; xy (2 floats each) and response are optional outputs.  Without
+ * non-max suppression cv::FAST computes no score: every key point then has response 0.          */
 int fast_detect(const uint8_t *img, int w, int h, int step, int threshold, int nms,
                 float *xy, float *response, int cap)
 {
     uint8_t *score = (uint8_t *)malloc((size_t)w * h);
-    fast_score_map(img, w, h, step, threshold, score);
+    uint8_t *corner = (uint8_t *)malloc((size_t)w * h);
+    fast_score_map(img, w, h, step, threshold, score, corner);
     int n = 0;
     for (int y = 3; y < h - 3; y++)
         for (int x = 3; x < w - 3; x++) {
+            if (!corner[y * w + x]) continue;
             int s = score[y * w + x];
-            if (!s) continue;
             if (nms) {
+                /* a score-0 corner (threshold 0) is never strictly greater than all 8 neighbours */
                 const uint8_t *q = score + y * w + x;
                 if (!(s > q[-1] && s > q[1] && s > q[-w - 1] && s > q[-w] && s > q[-w + 1] &&
                       s > q[w - 1] && s > q[w] && s > q[w + 1]))
                     continue;
+            } else {
+                s = 0;
             }
             if (n < cap) {
                 if (xy) { xy[2 * n] = (float)x; xy[2 * n + 1] = (float)y; }
@@ -111,5 +124,6 @@ int fast_detect(const uint8_t *img, int w, int h, int step, int threshold, int n
             n++;
         }
     free(score);
+    free(corner);
     return n;
 }

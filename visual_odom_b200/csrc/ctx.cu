@@ -37,6 +37,11 @@ extern "C" int vo_create(int device, const vo_params* params, vo_ctx** out)
     if (params) ctx->p = *params; else vo_default_params(&ctx->p);
     ctx->device = device;
     *out = ctx;      // returned even on failure so the caller can read vo_last_error()
+    if (ctx->p.fast_threshold < 0 || ctx->p.fast_threshold > 255) {
+        // a pixel difference lies in [-255, 255]: other thresholds have no meaning (cv::FAST gives arbitrary lists for them)
+        vo_set_error(ctx, "fast_threshold=%d outside [0,255]", ctx->p.fast_threshold);
+        return VO_E_INVALID;
+    }
     if (ctx->p.lk_win != VO_WIN) {
         vo_set_error(ctx, "lk_win=%d unsupported: the LK kernel is built for the reference's 21x21 window", ctx->p.lk_win);
         return VO_E_UNSUPPORTED;
@@ -427,8 +432,14 @@ int vo_ensure_state(vo_ctx* ctx, int w, int h, int units, int /*imgs_per_unit*/)
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_valid4, 4 * uc));
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_idx5, uc));
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_n5, (size_t)units));
-    // FAST
-    ctx->corner_cap = (w * h) / 8 > 65536 ? (w * h) / 8 : 65536;
+    // FAST: room for every corner the frame can hold.  Corners lie in the (w-6) x (h-6) interior; under strict 3x3
+    // non-max suppression two survivors are never 8-neighbours, so each 2x2 block holds at most one.
+    {
+        const long iw = w > 6 ? w - 6 : 0, ih = h > 6 ? h - 6 : 0;
+        const long bound = ctx->p.fast_nonmax ? ((iw + 1) / 2) * ((ih + 1) / 2) : iw * ih;
+        if (bound > (1L << 30)) { vo_set_error(ctx, "%dx%d: too many possible FAST corners", w, h); return VO_E_CAPACITY; }
+        ctx->corner_cap = bound > 0 ? (int)bound : 1;
+    }
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_score, (size_t)units * w * h));
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_rowbuf, (size_t)units * h * w));
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_rowcount, (size_t)units * h));

@@ -8,18 +8,20 @@
 //   k_fast_score   one thread per pixel: 16-pixel Bresenham ring, corner iff >= 9 contiguous ring
 //                  pixels are all > p+t or all < p-t; score = max(t, max_arc min(p-r), max_arc
 //                  min(r-p)) - 1 (cornerScore<16>), 0 for non-corners / the 3-pixel border.
+//                  Without non-max suppression every corner is marked 1 instead (a score can be 0).
 //   k_fast_nms_row one CTA per image row: the three score rows are staged in shared memory, a corner
 //                  survives iff its score is strictly greater than its 8 neighbours; survivors are
 //                  compacted in x order into a per-row list (ballot + running offset).
 //   k_fast_scan    one CTA per unit: exclusive scan of the per-row counts -> raster offsets, total.
-//   k_fast_gather  per row: copies the row list to its raster position as (x, y) floats.
+//   k_fast_gather  per row: copies the row list to its raster position as (x, y) floats; response =
+//                  score with non-max suppression, 0 without (as cv::FAST).
 //   k_select_stride  idx_i = i*(M-1)/(N-1): the benchmark's feature selection (SURVEY.md 8d).
 // All HBM-bound byte work (1 B/px read, 1 B/px score write+read, 8 B/corner out).
 #include "common.cuh"
 #include "fast.h"
 
 __global__ void __launch_bounds__(256) k_fast_score(const uint8_t* const* __restrict__ img_tab, int img_stride_idx,
-                                                    int w, int h, int pitch, int threshold,
+                                                    int w, int h, int pitch, int threshold, int nonmax,
                                                     uint8_t* __restrict__ score, size_t score_plane)
 {
     // the 16-pixel Bresenham ring, compile-time: the unrolled loop below folds the offsets into immediates
@@ -68,6 +70,9 @@ __global__ void __launch_bounds__(256) k_fast_score(const uint8_t* const* __rest
                 B = fminf(B, fmaxf(b8, d[(k + 8) & 15]));
             }
             result = max(threshold, (int)fmaxf(A, -B)) - 1;
+            // Without non-max suppression the map only marks the corners (cv::FAST reports response 0): a corner's
+            // score is 0 at threshold 0 when its best arc is one level beyond the centre, so the score cannot be the mark.
+            if (!nonmax) result = 1;
         }
     }
     sc[(size_t)y * w + x] = (uint8_t)result;
@@ -192,7 +197,7 @@ __global__ void __launch_bounds__(1024) k_fast_scan(const int* __restrict__ rowc
 __global__ void __launch_bounds__(128) k_fast_gather(const uint16_t* __restrict__ rowbuf, int rowcap,
                                                      const int* __restrict__ rowcount, const int* __restrict__ rowoff,
                                                      int h, const uint8_t* __restrict__ score, size_t score_plane, int w,
-                                                     float2* __restrict__ out, float* __restrict__ resp, int cap)
+                                                     int nonmax, float2* __restrict__ out, float* __restrict__ resp, int cap)
 {
     const int y = blockIdx.x, unit = blockIdx.y;
     const int n = rowcount[unit * h + y], off = rowoff[unit * h + y];
@@ -202,7 +207,8 @@ __global__ void __launch_bounds__(128) k_fast_gather(const uint16_t* __restrict_
         if (o < cap) {
             const int x = src[i];
             out[(size_t)unit * cap + o] = make_float2((float)x, (float)y);
-            if (resp) resp[(size_t)unit * cap + o] = (float)score[(size_t)unit * score_plane + (size_t)y * w + x];
+            if (resp)        // without non-max suppression the map holds a mark, not a score: response 0, as cv::FAST
+                resp[(size_t)unit * cap + o] = nonmax ? (float)score[(size_t)unit * score_plane + (size_t)y * w + x] : 0.f;
         }
     }
 }
@@ -228,12 +234,13 @@ __global__ void k_select_stride(const float2* __restrict__ corners, int corner_c
 int vo_launch_fast(const FastArgs& a, cudaStream_t stream)
 {
     dim3 g1((a.w + 31) / 32, (a.h + 7) / 8, a.n_units);
-    k_fast_score<<<g1, 256, 0, stream>>>(a.img_tab, a.img_stride_idx, a.w, a.h, a.pitch, a.threshold, a.score, a.score_plane);
+    k_fast_score<<<g1, 256, 0, stream>>>(a.img_tab, a.img_stride_idx, a.w, a.h, a.pitch, a.threshold, a.nonmax, a.score,
+                                          a.score_plane);
     dim3 g2(a.h, a.n_units);
     k_fast_nms_row<<<g2, NMS_T, 0, stream>>>(a.score, a.score_plane, a.w, a.h, a.nonmax, a.rowbuf, a.rowcap, a.rowcount);
     k_fast_scan<<<a.n_units, 1024, 0, stream>>>(a.rowcount, a.h, a.rowoff, a.n_det);
     k_fast_gather<<<g2, 128, 0, stream>>>(a.rowbuf, a.rowcap, a.rowcount, a.rowoff, a.h, a.score, a.score_plane, a.w,
-                                           a.corners, a.resp, a.corner_cap);
+                                           a.nonmax, a.corners, a.resp, a.corner_cap);
     return 4;
 }
 
