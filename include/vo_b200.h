@@ -172,7 +172,8 @@ typedef struct vo_unit_result {
     int n_valid;         /* survivors of checkValidMatch/removeInvalidPoints (A5/A6)   */
     int n_inliers;       /* RANSAC inliers                                             */
     int ransac_iters;    /* iterations the adaptive loop ran                           */
-    int pnp_status;      /* VO_OK, VO_PNP_NO_MODEL or VO_E_TOO_FEW_POINTS (n < 4); n == 4 runs OpenCV's P3P case */
+    int pnp_status;      /* VO_OK, VO_PNP_NO_MODEL or VO_E_TOO_FEW_POINTS (n < 4); n == 4 runs OpenCV's P3P case, n == 5 one
+                            unrefined EPnP on all five (no RANSAC, ransac_iters 0, VO_OK even for a non-finite pose) */
     double rvec[3], tvec[3], R[9];
 } vo_unit_result;
 

@@ -31,6 +31,11 @@ DBL_MIN = 2.2250738585072014e-308
 DBL_EPS = 2.220446049250313e-16
 FLT_EPS = 1.1920928955078125e-07
 
+# EPnP's scalars are Python floats, whose division by zero raises where C++ yields inf / nan.  A degenerate sample (five
+# identical points) is re-run with numpy float64 scalars: the same IEEE double operations, but non-finite results
+# propagate as they do in OpenCV.
+_fl = float
+
 # ----------------------------------------------------------------------------- RNG
 RNG_COEFF = 4164903690
 MASK32 = 0xFFFFFFFF
@@ -100,7 +105,7 @@ def jacobi_svd_t(At, m, n, n1):
     """JacobiSVDImpl_<double>(At, W, Vt, m, n, n1, DBL_MIN, DBL_EPSILON*10).
     At: n rows of length m (= A^T).  Returns (W[n], At_out = U^T rows, Vt)."""
     eps = DBL_EPS * 10
-    At = [[float(v) for v in r] for r in At]
+    At = [[_fl(v) for v in r] for r in At]
     W = [0.0] * n
     Vt = [[1.0 if i == k else 0.0 for k in range(n)] for i in range(n)]
     for i in range(n):
@@ -243,7 +248,7 @@ def solve_svd(A, b):
     A = np.asarray(A, np.float64)
     m, n = A.shape
     W, Ut, Vt = jacobi_svd_t(A.T.tolist(), m, n, n)
-    return np.array(_svbksb(m, n, W, Ut, Vt, [float(v) for v in b]))
+    return np.array(_svbksb(m, n, W, Ut, Vt, [_fl(v) for v in b]))
 
 
 def invert_svd(A):
@@ -316,8 +321,11 @@ def rodrigues_jac(rvec):
 
 
 def rodrigues_inv(R):
-    """cv::Rodrigues matrix -> vector (f64)."""
+    """cv::Rodrigues matrix -> vector (f64).  An entry outside [-100, 100) or non-finite gives the zero vector
+    (OpenCV's checkRange guard)."""
     R = np.asarray(R, np.float64)
+    if not np.all((R >= -100) & (R < 100)):
+        return np.zeros(3)
     _, U, Vt = svd(R)
     Rm = np.zeros((3, 3))
     for i in range(3):
@@ -416,8 +424,8 @@ def _dot3(a, b):
 def _qr_solve_6x4(A, b):
     """epnp::qr_solve (Householder, including its off-by-one column-scale scan)."""
     nr, nc = 6, 4
-    A = [float(v) for v in np.asarray(A, np.float64).ravel()]
-    b = [float(v) for v in b]
+    A = [_fl(v) for v in np.asarray(A, np.float64).ravel()]
+    b = [_fl(v) for v in b]
     A1 = [0.0] * nr
     A2 = [0.0] * nr
     for k in range(nc):
@@ -479,14 +487,28 @@ def _qr_solve_6x4(A, b):
 
 def epnp(X, x, K):
     """cv::solvePnP(..., SOLVEPNP_EPNP) with zero distortion: returns (rvec, tvec) float64."""
+    global _fl
+    try:
+        return _epnp(X, x, K)
+    except ZeroDivisionError:
+        _fl = np.float64
+        try:
+            with np.errstate(all="ignore"):
+                rv, tv = _epnp(X, x, K)
+            return np.asarray(rv, np.float64), np.asarray(tv, np.float64)
+        finally:
+            _fl = float
+
+
+def _epnp(X, x, K):
     X = np.asarray(X, np.float32).reshape(-1, 3).astype(np.float64)
     K = np.asarray(K, np.float64)
     n = len(X)
     fu, fv, uc, vc = float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2])
     xn = undistort_normalize_f32(x, K).astype(np.float64)
     us = np.stack([xn[:, 0] * fu + uc, xn[:, 1] * fv + vc], 1)
-    X = [[float(v) for v in row] for row in X]
-    us = [[float(v) for v in row] for row in us]
+    X = [[_fl(v) for v in row] for row in X]
+    us = [[_fl(v) for v in row] for row in us]
     # choose_control_points
     cws = [[0.0] * 3 for _ in range(4)]
     for i in range(n):
@@ -520,7 +542,7 @@ def epnp(X, x, K):
             M[2 * i + 1, 3 * j + 2] = al[i][j] * (vc - us[i][1])
     _, U, _ = svd(mul_transposed(M))
     ut = U.T
-    v = [[float(t) for t in ut[11 - i]] for i in range(4)]
+    v = [[_fl(t) for t in ut[11 - i]] for i in range(4)]
     pairs = [(0, 1), (0, 2), (0, 3), (1, 2), (1, 3), (2, 3)]
     dv = [[[v[i][3 * a + c] - v[i][3 * b + c] for c in range(3)] for (a, b) in pairs] for i in range(4)]
     L = []
@@ -831,7 +853,8 @@ def p3p_four_points(X, x, K):
 # ----------------------------------------------------------------------------- solvePnPRansac
 def solve_pnp_ransac(X, x, K, rvec0, tvec0, iterations=500, reproj=0.5, confidence=0.999, trace=None,
                      model_fn=None):
-    """cv::solvePnPRansac(..., useExtrinsicGuess=true, SOLVEPNP_ITERATIVE); n == 4 is the P3P case above.
+    """cv::solvePnPRansac(..., useExtrinsicGuess=true, SOLVEPNP_ITERATIVE); n == 4 is the P3P case above, n == 5 a
+    single unrefined EPnP.
     model_fn(Xs, xs, K) -> (rvec, tvec) defaults to the EPnP restatement."""
     X = np.asarray(X, np.float32).reshape(-1, 3)
     x = np.asarray(x, np.float32).reshape(-1, 2)
@@ -845,6 +868,11 @@ def solve_pnp_ransac(X, x, K, rvec0, tvec0, iterations=500, reproj=0.5, confiden
                         inliers=np.zeros(0, np.int32), iters=0)
         return dict(ok=True, rvec=m[0], tvec=m[1], inliers=np.arange(4, dtype=np.int32), iters=0, model=m)
     assert n >= 5, "cv::solvePnPRansac needs at least four points"
+    if n == 5:
+        # n == model_points: no RANSAC, one EPnP solvePnP on all five, no refinement, all five inliers -- also when the
+        # pose is not finite (five identical points: rvec 0, tvec nan)
+        m = model_fn(X, x, K64)
+        return dict(ok=True, rvec=m[0], tvec=m[1], inliers=np.arange(5, dtype=np.int32), iters=0, model=m)
     rng = CvRNG(MASK64)
     thr = np.float32(np.float64(reproj) * np.float64(reproj))
     niters = iterations
@@ -853,10 +881,7 @@ def solve_pnp_ransac(X, x, K, rvec0, tvec0, iterations=500, reproj=0.5, confiden
     best_model = None
     it = 0
     while it < niters:
-        if n > 5:
-            idx = ransac_subset(rng, n, 5)
-        else:
-            idx = list(range(n))
+        idx = ransac_subset(rng, n, 5)
         rv, tv = model_fn(X[idx], x[idx], K64)
         err = reproj_err_f32(X, x, rv, tv, K64)
         mask = err <= thr

@@ -257,6 +257,11 @@ extern "C" int vo_mono_rotation(vo_ctx* ctx, const vo_point2f* pts_t0, const vo_
     for (int k = 0; k < 9; k++) R_out[k] = r.R[k];
     if (n_inliers) *n_inliers = r.n_inliers;
     if (ransac_iters) *ransac_iters = r.iters;
+    if (!r.ok && n == 5) {
+        vo_set_error(ctx, "vo_mono_rotation: with exactly 5 points cv::findEssentialMat runs no RANSAC and returns all %d five-point "
+                          "candidates stacked (%dx3); cv::recoverPose asserts E is 3x3, the reference aborts here", r.n_cand, 3 * r.n_cand);
+        return VO_E_TOO_FEW_POINTS;
+    }
     if (!r.ok) { vo_set_error(ctx, "vo_mono_rotation: RANSAC found no essential matrix with more than 4 inliers (cv::recoverPose would fail on the empty E)"); return VO_E_TOO_FEW_POINTS; }
     return VO_OK;
 }

@@ -8,6 +8,7 @@
 // Structure (same shape as the PnP RANSAC of pnp.cu: waves of iterations, a unit that reached its adaptive bound skips
 // the rest; every kernel reads the bound from device memory, so there is no host round trip):
 //   k_ess_init          normalise the points ((p - pp) / focal in fp64), reset the RANSAC state
+//   k_ess_five          n == 5 only, instead of the RANSAC waves: one five-point solve on all points (no RANSAC in OpenCV)
 //   k_ess_subsets       1 thread: cv::RNG(2^64-1) stream -> 5 distinct indices per iteration (ptsetreg.cpp getSubset)
 //   k_ess_hypotheses    1 thread / iteration: Nister five-point solver (ess_math.cuh) -> up to 10 E per sample
 //   k_ess_count         1 CTA / (iteration, candidate): Sampson error of all N points, err <= (float)thr^2, count
@@ -34,7 +35,7 @@ __global__ void k_ess_init(const EssArgs a)
         s.max_good = 0;
         s.best_it = -1; s.best_cand = -1;
         s.iters_run = 0;
-        s.done = a.n < 5 ? 1 : 0;
+        s.done = a.n <= 5 ? 1 : 0;      // n == 5: no RANSAC (k_ess_five)
         for (int k = 0; k < 4; k++) s.good4[k] = 0;
     }
     if (i >= a.n) return;
@@ -52,20 +53,16 @@ __global__ void k_ess_subsets(const EssArgs a, int it0, int it1)
     Rng rng(s.rng_state);
     const int last = it1 < s.niters ? it1 : s.niters;
     for (int it = it0; it < last; it++) {
-        int idx[5];
-        if (n > 5) {
-            for (int i = 0; i < 5; i++) {
-                int v;
-                bool dup;
-                do {
-                    v = (int)(rng.next() % (unsigned)n);
-                    dup = false;
-                    for (int j = 0; j < i; j++) dup |= (idx[j] == v);
-                } while (dup);
-                idx[i] = v;
-            }
-        } else {
-            for (int i = 0; i < 5; i++) idx[i] = i;
+        int idx[5];                     // n > 5 here
+        for (int i = 0; i < 5; i++) {
+            int v;
+            bool dup;
+            do {
+                v = (int)(rng.next() % (unsigned)n);
+                dup = false;
+                for (int j = 0; j < i; j++) dup |= (idx[j] == v);
+            } while (dup);
+            idx[i] = v;
         }
         for (int i = 0; i < 5; i++) a.subsets[it * 5 + i] = idx[i];
     }
@@ -130,6 +127,22 @@ __global__ void k_ess_replay(const EssArgs a, int it0, int it1)
     if (it >= s.niters || it1 >= a.max_iters) s.done = 1;
 }
 
+// Exactly five correspondences (= model points): OpenCV runs no RANSAC.  findEssentialMat returns every candidate of one
+// five-point solve, stacked (3k x 3), with an all-ones mask; recoverPose only accepts a 3 x 3 E.  So a single candidate is
+// the model, with all five points inliers; any other count leaves no model (the host reports the reference's abort).
+__global__ void k_ess_five(const EssArgs a)
+{
+    if (blockIdx.x || threadIdx.x) return;
+    EssState& s = *a.state;
+    double q0[10], q1[10];
+    for (int i = 0; i < 5; i++) {
+        q0[2 * i] = a.q0[i].x; q0[2 * i + 1] = a.q0[i].y; q1[2 * i] = a.q1[i].x; q1[2 * i + 1] = a.q1[i].y;
+    }
+    const int nm = five_point(q0, q1, a.models);
+    a.nmodels[0] = nm;
+    if (nm == 1) { s.best_it = 0; s.best_cand = 0; s.max_good = 5; }
+}
+
 __global__ void k_ess_mask(const EssArgs a)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -138,7 +151,7 @@ __global__ void k_ess_mask(const EssArgs a)
     if (s.best_it < 0) { a.mask[i] = 0; return; }
     const double* E = a.models + (size_t)s.best_it * 90 + s.best_cand * 9;
     const double2 u = a.q0[i], v = a.q1[i];
-    a.mask[i] = sampson_err(E, u.x, u.y, v.x, v.y) <= a.thr2 ? 1 : 0;
+    a.mask[i] = (a.n == 5 || sampson_err(E, u.x, u.y, v.x, v.y) <= a.thr2) ? 1 : 0;
 }
 
 __global__ void k_ess_decompose(const EssArgs a)
@@ -179,6 +192,7 @@ __global__ void k_ess_pick(const EssArgs a)
     const EssState& s = *a.state;
     EssResult& r = *a.result;
     r.n_inliers = s.max_good; r.iters = s.iters_run; r.ok = s.best_it >= 0 ? 1 : 0;
+    r.n_cand = a.n == 5 ? a.nmodels[0] : 0;
     if (s.best_it < 0) {
         for (int k = 0; k < 9; k++) { r.R[k] = (k % 4 == 0) ? 1.0 : 0.0; r.E[k] = 0.0; }
         r.t[0] = r.t[1] = r.t[2] = 0.0; r.n_good = 0;
@@ -201,8 +215,9 @@ int vo_launch_essential(const EssArgs& a, cudaStream_t s)
     int launches = 0;
     const int nb = (a.n + 127) / 128 > 0 ? (a.n + 127) / 128 : 1;
     k_ess_init<<<nb, 128, 0, s>>>(a); launches++;
+    if (a.n == 5) { k_ess_five<<<1, 32, 0, s>>>(a); launches++; }
     const int waves[4] = {0, 32, 128, a.max_iters};
-    for (int w = 0; w < 3; w++) {
+    for (int w = 0; w < 3 && a.n > 5; w++) {
         const int it0 = waves[w], it1 = waves[w + 1] < a.max_iters ? waves[w + 1] : a.max_iters;
         if (it1 <= it0) break;
         k_ess_subsets<<<1, 32, 0, s>>>(a, it0, it1);

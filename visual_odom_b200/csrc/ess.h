@@ -15,6 +15,7 @@ struct EssState {
 struct EssResult {
     double R[9], t[3], E[9];
     int n_inliers, n_good, iters, ok;
+    int n_cand;       // n == 5 only: five-point candidates of the one solve (OpenCV returns them all, stacked)
 };
 
 struct EssArgs {

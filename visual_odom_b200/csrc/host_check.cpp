@@ -50,15 +50,23 @@ __attribute__((visibility("default"))) int vo_hostcheck_mono_rotation(const floa
     Rng rng(0xffffffffffffffffULL);
     int niters = max_iters, max_good = 0, it = 0;
     bool have = false;
+    if (n == 5) {
+        // no RANSAC: every candidate of one solve comes back stacked, recoverPose accepts only a single (3 x 3) one
+        double Es[90];
+        const int nm = five_point(q0.data(), q1.data(), Es);
+        if (iters_out) *iters_out = 0;
+        if (nm != 1) return 0;
+        for (int k = 0; k < 9; k++) E_best[k] = Es[k];
+        max_good = 5; have = true;
+        niters = 0;
+    }
     for (; it < niters; it++) {
         int idx[5];
-        if (n > 5) {
-            for (int i = 0; i < 5; i++) {
-                int v; bool dup;
-                do { v = (int)(rng.next() % (unsigned)n); dup = false; for (int j = 0; j < i; j++) dup |= idx[j] == v; } while (dup);
-                idx[i] = v;
-            }
-        } else for (int i = 0; i < 5; i++) idx[i] = i;
+        for (int i = 0; i < 5; i++) {
+            int v; bool dup;
+            do { v = (int)(rng.next() % (unsigned)n); dup = false; for (int j = 0; j < i; j++) dup |= idx[j] == v; } while (dup);
+            idx[i] = v;
+        }
         double a[10], b[10], Es[90];
         for (int i = 0; i < 5; i++) { a[2 * i] = q0[2 * idx[i]]; a[2 * i + 1] = q0[2 * idx[i] + 1]; b[2 * i] = q1[2 * idx[i]]; b[2 * i + 1] = q1[2 * idx[i] + 1]; }
         const int nm = five_point(a, b, Es);
@@ -74,7 +82,7 @@ __attribute__((visibility("default"))) int vo_hostcheck_mono_rotation(const floa
     }
     if (iters_out) *iters_out = it;
     if (!have) return 0;
-    for (int i = 0; i < n; i++) mask[i] = sampson_err(E_best, q0[2 * i], q0[2 * i + 1], q1[2 * i], q1[2 * i + 1]) <= t;
+    for (int i = 0; i < n; i++) mask[i] = n == 5 || sampson_err(E_best, q0[2 * i], q0[2 * i + 1], q1[2 * i], q1[2 * i + 1]) <= t;
     double R1[9], R2[9], tt[3], tn[3];
     decompose_essential(E_best, R1, R2, tt);
     for (int k = 0; k < 3; k++) tn[k] = -tt[k];

@@ -15,7 +15,8 @@
 //     k_pnp_hypotheses   1 thread/iteration: 5-point EPnP in fp64 (pnp_math.cuh) -> [R|t]
 //     k_pnp_count        1 CTA/iteration: project all N points (fp64 -> f32), err^2 <= 0.25f, count
 //     k_pnp_replay       1 thread/unit: `if count > max(best,4)`: new best, niters = RANSACUpdateNumIters
-//   k_pnp_finalize       1 CTA/unit: inlier mask of the best model -> ordered index list; LM
+//   k_pnp_init           per unit: RNG / bound reset; n == 5 (no RANSAC in OpenCV): the single unrefined EPnP
+//   k_pnp_finalize       1 CTA/unit (n == 4: OpenCV's P3P case, no RANSAC): inlier mask of the best model -> ordered index list; LM
 //                        (CvLevMarq logic, lambda 1e-3, <=20 iterations, eps FLT_EPSILON) over the
 //                        inliers from (rvec=0, t_prev); Rodrigues.
 #include "common.cuh"
@@ -40,6 +41,30 @@ __global__ void k_triangulate(const TriArgs a)
 }
 
 // ---------------------------------------------------------------------------------------------
+// Exactly five correspondences (= model points): OpenCV runs no RANSAC, one EPnP solvePnP on all five, no refinement,
+// all five inliers.  It reports success whatever EPnP returns: five identical points give rvec = 0 and a nan tvec, and
+// so does this.  Kept out of line and out of k_pnp_finalize, whose LM would spill around the 12x12 SVD.
+__device__ __noinline__ void pnp_five_points(const PnpArgs& a, int unit)
+{
+    const float3* X = a.X + (size_t)unit * a.cap;
+    const float2* x = a.x + (size_t)unit * a.cap;
+    float Xw[15], uv[10];
+    for (int i = 0; i < 5; i++) {
+        Xw[3 * i] = X[i].x; Xw[3 * i + 1] = X[i].y; Xw[3 * i + 2] = X[i].z;
+        uv[2 * i] = x[i].x; uv[2 * i + 1] = x[i].y;
+    }
+    double rv[3], t[3], R[9];
+    epnp5(Xw, uv, a.fu, a.fv, a.uc, a.vc, rv, t, R);      // R = Rodrigues(rvec), the caller's conversion
+    vo_unit_result_dev& res = a.results[unit];
+    int* inl = a.inliers + (size_t)unit * a.cap;
+    res.ransac_iters = 0;
+    res.n_inliers = 5;
+    res.pnp_status = VO_PNP_OK;
+    for (int i = 0; i < 5; i++) inl[i] = i;
+    for (int k = 0; k < 3; k++) { res.rvec[k] = rv[k]; res.tvec[k] = t[k]; }
+    for (int k = 0; k < 9; k++) res.R[k] = R[k];
+}
+
 __global__ void k_pnp_init(const PnpArgs a)
 {
     const int unit = blockIdx.x * blockDim.x + threadIdx.x;
@@ -51,7 +76,9 @@ __global__ void k_pnp_init(const PnpArgs a)
     s.best_it = -1;
     s.iters_run = 0;
     const int n = a.n_pts[unit];
-    s.done = (n < 5) ? 1 : 0;           // n < 4: the reference aborts; n == 4: no RANSAC, k_pnp_finalize runs the P3P solve
+    // n < 4: the reference aborts; n == 4: no RANSAC, k_pnp_finalize runs the P3P solve; n == 5: no RANSAC, the EPnP solve
+    s.done = (n <= 5) ? 1 : 0;
+    if (n == 5) pnp_five_points(a, unit);
 }
 
 __global__ void k_pnp_subsets(const PnpArgs a, int it0, int it1)
@@ -65,20 +92,16 @@ __global__ void k_pnp_subsets(const PnpArgs a, int it0, int it1)
     Rng rng(s.rng_state);
     const int last = it1 < s.niters ? it1 : s.niters;
     for (int it = it0; it < last; it++) {
-        int idx[5];
-        if (n > 5) {
-            for (int i = 0; i < 5; i++) {
-                int v;
-                bool dup;
-                do {
-                    v = (int)(rng.next() % (unsigned)n);
-                    dup = false;
-                    for (int j = 0; j < i; j++) dup |= (idx[j] == v);
-                } while (dup);
-                idx[i] = v;
-            }
-        } else {
-            for (int i = 0; i < 5; i++) idx[i] = i;
+        int idx[5];                     // n > 5 here: smaller units are done before the first wave
+        for (int i = 0; i < 5; i++) {
+            int v;
+            bool dup;
+            do {
+                v = (int)(rng.next() % (unsigned)n);
+                dup = false;
+                for (int j = 0; j < i; j++) dup |= (idx[j] == v);
+            } while (dup);
+            idx[i] = v;
         }
         for (int i = 0; i < 5; i++) out[it * 5 + i] = idx[i];
     }
@@ -413,7 +436,8 @@ __global__ void __launch_bounds__(FIN_T, 1) k_pnp_finalize(const PnpArgs a)
         }
         return;
     }
-    if (st.best_it < 0 || n < 5) {
+    if (n == 5) return;             // k_pnp_init wrote the record (pnp_five_points)
+    if (st.best_it < 0 || n < 4) {
         // solvePnPRansac returns false: rvec / tvec stay what the caller passed in
         if (threadIdx.x == 0) {
             res.n_inliers = 0;

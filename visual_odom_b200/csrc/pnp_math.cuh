@@ -376,9 +376,12 @@ VO_HDN inline void rodrigues_fwd(const double* r, double* R)
     for (int k = 0; k < 9; k++) R[k] = c * ((k % 4 == 0) ? 1. : 0.) + c1 * rrt[k] + s * r_x[k];
 }
 
-// cv::Rodrigues: matrix -> rotation vector
+// cv::Rodrigues: matrix -> rotation vector.  A matrix with an entry outside [-100, 100) or non-finite gives the zero
+// vector (OpenCV's checkRange guard: a degenerate EPnP pose, e.g. five identical points, comes back as rvec = 0)
 VO_HDN inline void rodrigues_inv(const double* Rin, double* r)
 {
+    for (int k = 0; k < 9; k++)
+        if (!(Rin[k] >= -100. && Rin[k] < 100.)) { r[0] = r[1] = r[2] = 0.; return; }
     double w[3], U[9], Vt[9], R[9];
     svd3(Rin, w, U, Vt);
     for (int i = 0; i < 3; i++)
