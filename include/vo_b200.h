@@ -87,7 +87,9 @@ VO_API int vo_lk_kernel_time(vo_ctx* ctx, double* ms_total, long long* n, int re
  * sequences are replayed as CUDA graphs where that does not defeat the priority split) | 0 (plain launches; needed
  * for vo_lk_kernel_time), "priorities" = 1 (default: with several unit ranges in flight the short / latency-bound
  * kernels run on high-priority helper streams and only the LK ring at normal priority; such ranges are launched
- * plainly because captured graph nodes lose the stream priority) | 0, "batch_graphs" = 1 forces graphs for them. */
+ * plainly because captured graph nodes lose the stream priority) | 0, "batch_graphs" = 1 forces graphs for them,
+ * "mono_rotation" = 0 (default) | 1: sequences begun from then on run trackingFrame2Frame(mono_rotation = true), see
+ * vo_seq_wait_mono (a sequence keeps the value it was begun with). */
 VO_API int vo_set_option(vo_ctx* ctx, const char* key, double value);
 
 /* ---- A1: cv::FAST(image, kps, threshold, nonmax) + KeyPoint::convert ------------------------
@@ -234,8 +236,9 @@ VO_API int vo_dist_gather_wait(vo_ctx* ctx, vo_unit_result* all, int cap_records
  * stereo pair, `translation`) lives on the device.  vo_seq_begin uploads the first pair; each vo_seq_push
  * uploads only the NEW pair, builds only its two pyramids and runs matchingFeatures() (FAST refill,
  * bucketing rows/10 x 1, circular matching, 1-px round-trip check) -> triangulation ->
- * trackingFrame2Frame(mono_rotation=false), carrying features / ages / translation to the next frame
- * exactly as the reference does (including the ages-vs-points length skew, SURVEY.md Appendix A item 8).
+ * trackingFrame2Frame(mono_rotation=false, or true with the option "mono_rotation", see vo_seq_wait_mono), carrying
+ * features / ages / translation to the next frame exactly as the reference does (including the ages-vs-points length
+ * skew, SURVEY.md Appendix A item 8).
  *   out      counts + pose of this frame pair
  *   pts4     optional: 4 arrays of pts_cap points (L0, R0, L1, R1 after the circular check); the first
  *            out->n_valid entries of each are meaningful, the rest of the arrays is scratch
@@ -259,6 +262,32 @@ VO_API int vo_seq_push_ex(vo_ctx* ctx, const uint8_t* left1, const uint8_t* righ
  * must stay valid until the call returns for pageable memory, until its vo_seq_wait for pinned memory. */
 VO_API int vo_seq_submit(vo_ctx* ctx, const uint8_t* left1, const uint8_t* right1, size_t pitch, int channels);
 VO_API int vo_seq_wait(vo_ctx* ctx, vo_unit_result* out, vo_point2f* pts4, int pts_cap);
+/* trackingFrame2Frame(..., mono_rotation = true), the reference's header default (src/visualOdometry.h:42), in the sequence
+ * mode: set vo_set_option(ctx, "mono_rotation", 1) before vo_seq_begin[_ex].  Each frame then also runs
+ *     E = cv::findEssentialMat(pointsLeft_t0, pointsLeft_t1, focal, pp, cv::RANSAC, 0.999, 1.0, mask);
+ *     cv::recoverPose(E, pointsLeft_t0, pointsLeft_t1, rotation, translation_mono, focal, pp, mask);
+ * (reference src/visualOdometry.cpp:146-157; focal / pp = the float entries of P_l), and the PnP supplies only
+ * `translation` (:186-189).  The record's R is recoverPose's rotation; rvec, tvec, n_inliers, ransac_iters and pnp_status
+ * stay the PnP's (the same bits as without the option), and the carried translation is the PnP's.  frame_pose integrates
+ * (R, tvec) under the main loop's gates.  Where the reference would abort in the branch (fewer than 5 points, no E with
+ * more than 4 inliers, exactly 5 points with other than one five-point candidate) the frame is reported with
+ * mono.status = VO_E_TOO_FEW_POINTS and R = I, is not integrated, and the sequence goes on -- as a frame whose PnP had
+ * fewer than 4 points.  vo_seq_push / vo_seq_wait work on such a sequence too (R = the mono rotation); vo_seq_wait_mono
+ * is vo_seq_wait plus the branch's details of the same frame:
+ *   mono      the recoverPose result
+ *   ess_mask  optional, mask_cap bytes: the essential inlier mask, aligned with the frame's point lists (first
+ *             out->n_valid entries meaningful)
+ * VO_E_INVALID when the sequence was begun without "mono_rotation". */
+typedef struct vo_mono_result {
+    int status;        /* VO_OK, or VO_E_TOO_FEW_POINTS where cv::findEssentialMat / cv::recoverPose would throw */
+    int n_inliers;     /* essential-matrix RANSAC inliers (the mask's count) */
+    int ransac_iters;
+    int n_good;        /* recoverPose's return value: inliers in front of both cameras for the chosen pose */
+    double R[9];       /* recoverPose rotation (row-major) */
+    double t[3];       /* translation_mono (unused by the reference, returned for completeness) */
+} vo_mono_result;
+VO_API int vo_seq_wait_mono(vo_ctx* ctx, vo_unit_result* out, vo_mono_result* mono, uint8_t* ess_mask, int mask_cap,
+                            vo_point2f* pts4, int pts_cap);
 /* currentVOFeatures (points / ages may differ in length) and the carried translation (waits for frames in flight) */
 VO_API int vo_seq_state(vo_ctx* ctx, vo_point2f* points, int32_t* ages, int cap, int* n_points, int* n_ages, double t_out[3]);
 

@@ -6,7 +6,9 @@
 <dataset>/image_0/%06d.png and image_1/%06d.png are decoded ahead by the library's reader into pinned buffers, frames
 are pushed through vo_seq_submit / vo_seq_wait (two in flight), frame_pose is integrated with the reference's Euler and
 scale gates, the trajectory is written in the KITTI text format and, with --gt, scored with the KITTI segment metric.
-`--check` only validates the inputs (no GPU needed)."""
+`--mono-rotation` runs trackingFrame2Frame as its header default does (mono_rotation = true: the rotation from
+findEssentialMat + recoverPose, the translation from the PnP; frames where that branch would abort are reported and not
+integrated).  `--check` only validates the inputs (no GPU needed)."""
 import argparse
 import os
 import re
@@ -45,6 +47,8 @@ def main():
     ap.add_argument("--poses", help="write the trajectory here (KITTI format)")
     ap.add_argument("--gt", help="ground-truth poses to score against")
     ap.add_argument("--threads", type=int, default=8); ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--mono-rotation", action="store_true",
+                    help="rotation from findEssentialMat + recoverPose (trackingFrame2Frame's header default)")
     ap.add_argument("--check", action="store_true")
     a = ap.parse_args()
     from visual_odom_b200 import capi, synth
@@ -57,9 +61,13 @@ def main():
         raise SystemExit(f"{a.dataset}: need at least two stereo pairs (image_0/%06d.png, image_1/%06d.png from {a.first})")
     w, h, ctype, depth = capi.png_info(open(os.path.join(a.dataset, "image_0", "%06d.png" % a.first), "rb").read())
     print(f"{n} stereo pairs of {w}x{h} (PNG colour type {ctype}, {depth} bit); P_left =\n{P_l}\nP_right =\n{P_r}")
+    print("rotation: " + ("findEssentialMat + recoverPose (mono_rotation = true)" if a.mono_rotation else
+                          "Rodrigues of the PnP rvec (mono_rotation = false)"))
     if a.check:
         return
     ctx = capi.Context(a.device, max_features=4096, max_units=2)
+    ctx.set_option("mono_rotation", 1 if a.mono_rotation else 0)
+    aborted = 0
     rd = capi.SequenceReader(a.dataset, a.first, n, threads=a.threads, depth=a.threads + 3)
     lp, rp, rw, rh, pitch, ch, fid = rd.next_ptr()
     ctx.seq_begin_ptr(rw, rh, lp, rp, pitch, P_l, P_r, ch)
@@ -71,13 +79,17 @@ def main():
         if k + 1 < n:
             lp, rp, rw, rh, pitch, ch, fid = rd.next_ptr()
             ctx.seq_submit_ptr(lp, rp, pitch, ch)
-        res = ctx.seq_wait(want_points=False)
+        res = ctx.seq_wait(want_points=False, mono=a.mono_rotation)
+        if a.mono_rotation and res["mono"]["status"] != capi.VO_OK:
+            aborted += 1
         poses.append(ctx.seq_pose())
         if k % 100 == 0 or k == n - 1:
             dt = time.perf_counter() - t0
             print(f"frame {a.first + k}: {res['n_valid']} matches, {res['n_inliers']} inliers, "
                   f"position {poses[-1][:3, 3].round(2)}, {k / dt:.0f} frames/s")
     rd.close(); ctx.close()
+    if a.mono_rotation:
+        print(f"{aborted} frames where findEssentialMat / recoverPose would abort (reported, not integrated)")
     if a.poses:
         os.makedirs(os.path.dirname(os.path.abspath(a.poses)), exist_ok=True)
         capi.poses_save(a.poses, poses)

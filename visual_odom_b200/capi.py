@@ -46,6 +46,13 @@ class VoUnitResult(C.Structure):
     ]
 
 
+class VoMonoResult(C.Structure):
+    _fields_ = [
+        ("status", C.c_int), ("n_inliers", C.c_int), ("ransac_iters", C.c_int), ("n_good", C.c_int),
+        ("R", C.c_double * 9), ("t", C.c_double * 3),
+    ]
+
+
 # the same record as a numpy structured dtype (C layout, 152 bytes): arrays of records can be handed out without building
 # one Python dict per record (a gathered table of a multi-GPU step has world x units of them)
 RESULT_DTYPE = np.dtype([("n_features", "<i4"), ("n_detected", "<i4"), ("n_tracked", "<i4"), ("n_valid", "<i4"), ("n_inliers", "<i4"),
@@ -87,6 +94,8 @@ SIGNATURES = {
     "vo_seq_push": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(VoUnitResult), C.c_void_p, C.c_int]),
     "vo_seq_submit": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
     "vo_seq_wait": (C.c_int, [C.c_void_p, C.POINTER(VoUnitResult), C.c_void_p, C.c_int]),
+    "vo_seq_wait_mono": (C.c_int, [C.c_void_p, C.POINTER(VoUnitResult), C.POINTER(VoMonoResult), C.c_void_p, C.c_int,
+                                   C.c_void_p, C.c_int]),
     "vo_seq_state": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p]),
     "vo_seq_begin_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
     "vo_seq_push_ex": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.POINTER(VoUnitResult), C.c_void_p, C.c_int]),
@@ -435,8 +444,12 @@ class Context:
         P_l = np.ascontiguousarray(P_l, np.float32).reshape(12); P_r = np.ascontiguousarray(P_r, np.float32).reshape(12)
         self._check(self.lib.vo_seq_begin(self.h, l.shape[1], l.shape[0], _p(P_l), _p(P_r), _p(l), _p(r), l.strides[0]))
 
-    def seq_push(self, left1, right1, pts_cap=4096, want_points=True):
+    def seq_push(self, left1, right1, pts_cap=4096, want_points=True, mono=False):
+        """mono=True (a sequence begun with the option "mono_rotation"): submit + seq_wait(mono=True)."""
         l = self._img(left1); r = self._img(right1)
+        if mono:
+            self._check(self.lib.vo_seq_submit(self.h, _p(l), _p(r), l.strides[0], 1))
+            return self.seq_wait(pts_cap, want_points, mono=True)
         res = VoUnitResult()
         if not want_points:
             self._check(self.lib.vo_seq_push(self.h, _p(l), _p(r), l.strides[0], C.byref(res), None, 0))
@@ -493,8 +506,24 @@ class Context:
     def seq_submit_ptr(self, left_ptr, right_ptr, pitch, channels=1):
         self._check(self.lib.vo_seq_submit(self.h, left_ptr, right_ptr, pitch, channels))
 
-    def seq_wait(self, pts_cap=4096, want_points=True):
+    def seq_wait(self, pts_cap=4096, want_points=True, mono=False):
+        """mono=True: also "mono" (dict: status, n_inliers, ransac_iters, n_good, R 3x3, t) and "ess_mask" (bool, aligned
+        with the point lists) of the same frame (vo_seq_wait_mono)."""
         res = VoUnitResult()
+        if mono:
+            m = VoMonoResult()
+            mask = np.zeros(pts_cap, np.uint8)
+            pts4 = np.zeros((4, pts_cap, 2), np.float32) if want_points else None
+            self._check(self.lib.vo_seq_wait_mono(self.h, C.byref(res), C.byref(m), _p(mask), pts_cap, _p(pts4),
+                                                  pts_cap if want_points else 0))
+            d = self._result_dict(res)
+            n = min(d["n_valid"], pts_cap)
+            if want_points:
+                d.update(l0=pts4[0, :n].copy(), r0=pts4[1, :n].copy(), l1=pts4[2, :n].copy(), r1=pts4[3, :n].copy())
+            d["mono"] = dict(status=m.status, n_inliers=m.n_inliers, ransac_iters=m.ransac_iters, n_good=m.n_good,
+                             R=np.array(m.R[:]).reshape(3, 3), t=np.array(m.t[:]))
+            d["ess_mask"] = mask[:n].astype(bool)
+            return d
         if not want_points:
             self._check(self.lib.vo_seq_wait(self.h, C.byref(res), None, 0))
             return self._result_dict(res)

@@ -107,6 +107,9 @@ extern "C" void vo_destroy(vo_ctx* ctx)
     if (ctx->d_bgr) cudaFree(ctx->d_bgr);
     if (ctx->d_lk_queue) cudaFree(ctx->d_lk_queue);
     if (ctx->d_ess) cudaFree(ctx->d_ess);
+    if (ctx->d_seq_ess) cudaFree(ctx->d_seq_ess);
+    for (int k = 0; k < 2; k++) if (ctx->seq_mono_ev[k]) cudaEventDestroy(ctx->seq_mono_ev[k]);
+    if (ctx->seq_mono_stream) cudaStreamDestroy(ctx->seq_mono_stream);
     if (ctx->h_out) cudaFreeHost(ctx->h_out);
     if (ctx->own_stream) cudaStreamDestroy(ctx->own_stream);
     delete ctx;
@@ -146,6 +149,7 @@ extern "C" int vo_set_option(vo_ctx* ctx, const char* key, double value)
     if (strcmp(key, "graphs") == 0) { ctx->use_graphs = value >= 1; return VO_OK; }
     if (strcmp(key, "batch_graphs") == 0) { ctx->batch_graphs = value >= 1; return VO_OK; }
     if (strcmp(key, "priorities") == 0) { ctx->use_priorities = value >= 1; vo_drop_graphs(ctx); return VO_OK; }
+    if (strcmp(key, "mono_rotation") == 0) { ctx->mono_opt = value >= 1; vo_drop_graphs(ctx); return VO_OK; }
     vo_set_error(ctx, "unknown option %s", key);
     return VO_E_INVALID;
 }

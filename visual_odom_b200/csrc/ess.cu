@@ -6,9 +6,11 @@
 // (src/visualOdometry.h:42), so a drop-in must honour it.
 //
 // Structure (same shape as the PnP RANSAC of pnp.cu: waves of iterations, a unit that reached its adaptive bound skips
-// the rest; every kernel reads the bound from device memory, so there is no host round trip):
+// the rest; every kernel reads the point count and the bound from device memory, so there is no host round trip and the
+// launch sequence is the same for every count -- the sequence mode captures it in the frame's graph):
 //   k_ess_init          normalise the points ((p - pp) / focal in fp64), reset the RANSAC state
-//   k_ess_five          n == 5 only, instead of the RANSAC waves: one five-point solve on all points (no RANSAC in OpenCV)
+//   k_ess_five          n == 5 only, instead of the RANSAC waves: one five-point solve on all points (no RANSAC in OpenCV);
+//                       n < 5 runs neither (no model: the reference aborts)
 //   k_ess_subsets       1 thread: cv::RNG(2^64-1) stream -> 5 distinct indices per iteration (ptsetreg.cpp getSubset)
 //   k_ess_hypotheses    1 thread / iteration: Nister five-point solver (ess_math.cuh) -> up to 10 E per sample
 //   k_ess_count         1 CTA / (iteration, candidate): Sampson error of all N points, err <= (float)thr^2, count
@@ -25,9 +27,17 @@
 
 using namespace vomath;
 
+// the point count of this run; n_max sizes every per-point buffer, so a count beyond it is clamped rather than overrun
+static __device__ __forceinline__ int ess_n(const EssArgs& a)
+{
+    const int n = *a.n;
+    return n < 0 ? 0 : (n < a.n_max ? n : a.n_max);
+}
+
 __global__ void k_ess_init(const EssArgs a)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int n = ess_n(a);
     if (i == 0) {
         EssState& s = *a.state;
         s.rng_state = 0xffffffffffffffffULL;
@@ -35,10 +45,10 @@ __global__ void k_ess_init(const EssArgs a)
         s.max_good = 0;
         s.best_it = -1; s.best_cand = -1;
         s.iters_run = 0;
-        s.done = a.n <= 5 ? 1 : 0;      // n == 5: no RANSAC (k_ess_five)
+        s.done = n <= 5 ? 1 : 0;        // n == 5: no RANSAC (k_ess_five); n < 5: no model
         for (int k = 0; k < 4; k++) s.good4[k] = 0;
     }
-    if (i >= a.n) return;
+    if (i >= n) return;
     const float2 p0 = a.pts0[i], p1 = a.pts1[i];
     a.q0[i] = make_double2(((double)p0.x - a.ppx) / a.focal, ((double)p0.y - a.ppy) / a.focal);
     a.q1[i] = make_double2(((double)p1.x - a.ppx) / a.focal, ((double)p1.y - a.ppy) / a.focal);
@@ -49,7 +59,7 @@ __global__ void k_ess_subsets(const EssArgs a, int it0, int it1)
     if (blockIdx.x || threadIdx.x) return;
     EssState& s = *a.state;
     if (s.done) return;
-    const int n = a.n;
+    const int n = ess_n(a);
     Rng rng(s.rng_state);
     const int last = it1 < s.niters ? it1 : s.niters;
     for (int it = it0; it < last; it++) {
@@ -94,8 +104,9 @@ __global__ void __launch_bounds__(128) k_ess_count(const EssArgs a, int it0, int
     if (threadIdx.x < 9) E[threadIdx.x] = a.models[(size_t)it * 90 + cand * 9 + threadIdx.x];
     if (threadIdx.x == 0) total = 0;
     __syncthreads();
+    const int n = ess_n(a);
     int c = 0;
-    for (int i = threadIdx.x; i < a.n; i += blockDim.x) {
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
         const double2 u = a.q0[i], v = a.q1[i];
         c += sampson_err(E, u.x, u.y, v.x, v.y) <= a.thr2;
     }
@@ -110,7 +121,7 @@ __global__ void k_ess_replay(const EssArgs a, int it0, int it1)
     if (blockIdx.x || threadIdx.x) return;
     EssState& s = *a.state;
     if (s.done) return;
-    const int n = a.n;
+    const int n = ess_n(a);
     int it = it0;
     for (; it < it1 && it < s.niters; it++) {
         const int nm = a.nmodels[it];
@@ -129,10 +140,10 @@ __global__ void k_ess_replay(const EssArgs a, int it0, int it1)
 
 // Exactly five correspondences (= model points): OpenCV runs no RANSAC.  findEssentialMat returns every candidate of one
 // five-point solve, stacked (3k x 3), with an all-ones mask; recoverPose only accepts a 3 x 3 E.  So a single candidate is
-// the model, with all five points inliers; any other count leaves no model (the host reports the reference's abort).
+// the model, with all five points inliers; any other count leaves no model (k_ess_pick reports the reference's abort).
 __global__ void k_ess_five(const EssArgs a)
 {
-    if (blockIdx.x || threadIdx.x) return;
+    if (blockIdx.x || threadIdx.x || ess_n(a) != 5) return;
     EssState& s = *a.state;
     double q0[10], q1[10];
     for (int i = 0; i < 5; i++) {
@@ -147,11 +158,12 @@ __global__ void k_ess_mask(const EssArgs a)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const EssState& s = *a.state;
-    if (i >= a.n) return;
+    const int n = ess_n(a);
+    if (i >= n) return;
     if (s.best_it < 0) { a.mask[i] = 0; return; }
     const double* E = a.models + (size_t)s.best_it * 90 + s.best_cand * 9;
     const double2 u = a.q0[i], v = a.q1[i];
-    a.mask[i] = (a.n == 5 || sampson_err(E, u.x, u.y, v.x, v.y) <= a.thr2) ? 1 : 0;
+    a.mask[i] = (n == 5 || sampson_err(E, u.x, u.y, v.x, v.y) <= a.thr2) ? 1 : 0;
 }
 
 __global__ void k_ess_decompose(const EssArgs a)
@@ -170,7 +182,7 @@ __global__ void __launch_bounds__(128) k_ess_cheirality(const EssArgs a)
     EssState& s = *a.state;
     if (s.best_it < 0) return;
     int ok[4] = {0, 0, 0, 0};
-    if (i < a.n && a.mask[i]) {
+    if (i < ess_n(a) && a.mask[i]) {
         const double2 u = a.q0[i], v = a.q1[i];
         const double* t = a.pose + 18;
         const double tn[3] = {-t[0], -t[1], -t[2]};
@@ -191,8 +203,10 @@ __global__ void k_ess_pick(const EssArgs a)
     if (blockIdx.x || threadIdx.x) return;
     const EssState& s = *a.state;
     EssResult& r = *a.result;
+    const int n = ess_n(a);
     r.n_inliers = s.max_good; r.iters = s.iters_run; r.ok = s.best_it >= 0 ? 1 : 0;
-    r.n_cand = a.n == 5 ? a.nmodels[0] : 0;
+    r.n_cand = n == 5 ? a.nmodels[0] : 0;
+    r.status = s.best_it >= 0 ? ESS_OK : n < 5 ? ESS_TOO_FEW : n == 5 ? ESS_FIVE_CANDIDATES : ESS_NO_MODEL;
     if (s.best_it < 0) {
         for (int k = 0; k < 9; k++) { r.R[k] = (k % 4 == 0) ? 1.0 : 0.0; r.E[k] = 0.0; }
         r.t[0] = r.t[1] = r.t[2] = 0.0; r.n_good = 0;
@@ -210,14 +224,42 @@ __global__ void k_ess_pick(const EssArgs a)
     r.n_good = g[k];
 }
 
+static size_t ess_up(size_t x) { return (x + 255) / 256 * 256; }
+
+// one scratch block: normalised points | state | subsets | models | nmodels | counts | mask | pose | result
+size_t vo_ess_scratch_bytes(int n_max, int max_iters)
+{
+    const size_t n = n_max > 0 ? (size_t)n_max : 1, it = (size_t)max_iters;
+    return 2 * ess_up(n * sizeof(double2)) + ess_up(sizeof(EssState)) + ess_up(it * 5 * sizeof(int)) +
+           ess_up(it * 90 * sizeof(double)) + ess_up(it * sizeof(int)) + ess_up(it * 10 * sizeof(int)) + ess_up(n) +
+           ess_up(30 * sizeof(double)) + ess_up(sizeof(EssResult));
+}
+
+void vo_ess_bind(EssArgs& a, void* scratch, int n_max, int max_iters)
+{
+    const size_t n = n_max > 0 ? (size_t)n_max : 1, it = (size_t)max_iters;
+    uint8_t* b = (uint8_t*)scratch;
+    auto take = [&](size_t bytes) { uint8_t* p = b; b += ess_up(bytes); return p; };
+    a.n_max = n_max; a.max_iters = max_iters;
+    a.q0 = (double2*)take(n * sizeof(double2)); a.q1 = (double2*)take(n * sizeof(double2));
+    a.state = (EssState*)take(sizeof(EssState));
+    a.subsets = (int*)take(it * 5 * sizeof(int));
+    a.models = (double*)take(it * 90 * sizeof(double));
+    a.nmodels = (int*)take(it * sizeof(int));
+    a.counts = (int*)take(it * 10 * sizeof(int));
+    a.mask = take(n);
+    a.pose = (double*)take(30 * sizeof(double));
+    a.result = (EssResult*)take(sizeof(EssResult));
+}
+
 int vo_launch_essential(const EssArgs& a, cudaStream_t s)
 {
     int launches = 0;
-    const int nb = (a.n + 127) / 128 > 0 ? (a.n + 127) / 128 : 1;
+    const int nb = (a.n_max + 127) / 128 > 0 ? (a.n_max + 127) / 128 : 1;
     k_ess_init<<<nb, 128, 0, s>>>(a); launches++;
-    if (a.n == 5) { k_ess_five<<<1, 32, 0, s>>>(a); launches++; }
+    k_ess_five<<<1, 32, 0, s>>>(a); launches++;
     const int waves[4] = {0, 32, 128, a.max_iters};
-    for (int w = 0; w < 3 && a.n > 5; w++) {
+    for (int w = 0; w < 3; w++) {
         const int it0 = waves[w], it1 = waves[w + 1] < a.max_iters ? waves[w + 1] : a.max_iters;
         if (it1 <= it0) break;
         k_ess_subsets<<<1, 32, 0, s>>>(a, it0, it1);

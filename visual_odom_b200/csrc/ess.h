@@ -12,30 +12,58 @@ struct EssState {
     int good4[4];     // recoverPose: points in front of both cameras for (R1,t) (R2,t) (R1,-t) (R2,-t)
 };
 
+// where the reference aborts (cv::findEssentialMat / cv::recoverPose throw); R = I, t = 0 then
+enum EssStatus {
+    ESS_OK = 0,
+    ESS_TOO_FEW = 1,          // n < 5
+    ESS_NO_MODEL = 2,         // no E with more than 4 inliers
+    ESS_FIVE_CANDIDATES = 3,  // n == 5 and the one five-point solve gave other than exactly one E
+};
+
 struct EssResult {
     double R[9], t[3], E[9];
     int n_inliers, n_good, iters, ok;
     int n_cand;       // n == 5 only: five-point candidates of the one solve (OpenCV returns them all, stacked)
+    int status;       // EssStatus
 };
 
 struct EssArgs {
-    int n;                    // correspondences
+    const int* n;             // correspondences (device: the sequence mode's count is only known on the device)
+    int n_max;                // host-known bound of *n: sizes the per-point grids and buffers
     int max_iters;            // 1000 (cv::findEssentialMat's default maxIters)
     const float2* pts0;       // pointsLeft_t0
     const float2* pts1;       // pointsLeft_t1
     double focal, ppx, ppy;   // `double focal = projMatrl.at<float>(0, 0)`, principle_point (visualOdometry.cpp:144-145)
     double prob;              // 0.999
     float thr2;               // (float)((threshold / focal)^2)
-    double2* q0;              // [n] normalised points
+    double2* q0;              // [n_max] normalised points
     double2* q1;
     EssState* state;
     int* subsets;             // [max_iters][5]
     double* models;           // [max_iters][10][9]
     int* nmodels;             // [max_iters]
     int* counts;              // [max_iters][10]
-    uint8_t* mask;            // [n] inliers of the best E
+    uint8_t* mask;            // [n_max] inliers of the best E
     double* pose;             // [30] R1 | R2 | t | E of the best model
     EssResult* result;
 };
 
+#define VO_ESS_ITERS 1000      // cv::findEssentialMat's default maxIters
+
+// the reference's camera values and thresholds: `double focal = projMatrl.at<float>(0, 0)`, pp (visualOdometry.cpp:144-147),
+// prob 0.999 and threshold 1.0 of the findEssentialMat call (:154)
+static inline void vo_ess_set_camera(EssArgs& a, double focal, double ppx, double ppy)
+{
+    a.focal = focal; a.ppx = ppx; a.ppy = ppy;
+    a.prob = 0.999;                                // literal double in the reference's call
+    const double thr = 1.0 / focal;                // threshold /= (fx + fy) / 2
+    a.thr2 = (float)(thr * thr);
+}
+
+// bytes of one scratch block for up to n_max points (everything EssArgs points to except pts0 / pts1 / n), and the args
+// laid out over it
+size_t vo_ess_scratch_bytes(int n_max, int max_iters);
+void vo_ess_bind(EssArgs& a, void* scratch, int n_max, int max_iters);
+// A fixed launch sequence whatever *n turns out to be (graph-capturable, no host sync): n < 5 ends without a model,
+// n == 5 takes k_ess_five, n > 5 the RANSAC waves, which skip themselves once the adaptive bound is reached.
 int vo_launch_essential(const EssArgs& a, cudaStream_t s);

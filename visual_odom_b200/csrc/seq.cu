@@ -111,6 +111,14 @@ __global__ void k_seq_finish(vo_unit_result_dev* res, double* tprev_next, const 
     }
 }
 
+// trackingFrame2Frame(mono_rotation = true) (src/visualOdometry.cpp:146-157,186-189): `rotation` comes from recoverPose,
+// the PnP supplies only `translation`.  Runs after k_seq_finish, so the translation carry is the PnP's as without the branch.
+__global__ void k_seq_mono(vo_unit_result_dev* res, const EssResult* __restrict__ ess)
+{
+    const int k = threadIdx.x;
+    if (k < 9) res->R[k] = ess->status == ESS_OK ? ess->R[k] : (k % 4 == 0 ? 1.0 : 0.0);
+}
+
 int vo_launch_seq_append(const SeqArgs& a, cudaStream_t s)
 {
     k_seq_append<<<1, 1024, 0, s>>>(a.corners, a.n_det, a.corner_cap, a.feat_pts, a.feat_ages, a.cnt, a.feat_cap, a.refill_below, a.err);
@@ -130,5 +138,10 @@ int vo_launch_seq_carry(const SeqArgs& a, cudaStream_t s)
 int vo_launch_seq_finish(const SeqArgs& a, cudaStream_t s)
 {
     k_seq_finish<<<1, 32, 0, s>>>(a.res, a.tprev, a.out_n, a.n_det, a.n3, a.n5, a.err, a.err_out);
+    return 1;
+}
+int vo_launch_seq_mono(vo_unit_result_dev* res, const EssResult* ess, cudaStream_t s)
+{
+    k_seq_mono<<<1, 32, 0, s>>>(res, ess);
     return 1;
 }

@@ -2,6 +2,7 @@
 #pragma once
 #include "common.cuh"
 #include "pnp.h"
+#include "ess.h"
 
 struct SeqArgs {
     // append
@@ -20,3 +21,6 @@ int vo_launch_seq_append(const SeqArgs& a, cudaStream_t s);
 int vo_launch_seq_bucket(const SeqArgs& a, cudaStream_t s);
 int vo_launch_seq_carry(const SeqArgs& a, cudaStream_t s);
 int vo_launch_seq_finish(const SeqArgs& a, cudaStream_t s);
+// mono_rotation = true: the record's R becomes recoverPose's rotation (I where the branch aborted); everything else in
+// the record stays the PnP's
+int vo_launch_seq_mono(vo_unit_result_dev* res, const EssResult* ess, cudaStream_t s);
