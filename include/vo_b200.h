@@ -161,7 +161,7 @@ VO_API int vo_mono_rotation(vo_ctx* ctx, const vo_point2f* pts_t0, const vo_poin
  *   FAST on l0 (when pts == NULL) -> even-stride selection of select_n corners
  *   -> pyramids -> LK ring -> status/negative/circular filters -> triangulation -> PnP/RANSAC. */
 typedef struct vo_unit {
-    const uint8_t *l0, *r0, *l1, *r1;   /* HOST images (w x h, pitch) unless VO_UNIT_DEVICE_IMAGES   */
+    const uint8_t *l0, *r0, *l1, *r1;   /* HOST images (w x h, pitch); see vo_batch_submit_device    */
     const vo_point2f* pts;              /* HOST features of l0, or NULL = detect on the GPU         */
     int n_pts;                          /* features in pts; with pts==NULL: number to select        */
     double t_prev[3];                   /* extrinsic guess for the pose solve                       */
@@ -214,6 +214,49 @@ VO_API int vo_batch_outputs(vo_ctx* ctx, int unit, vo_point2f* pts4, int32_t* ke
                             size_t* d2h_bytes_per_unit);
 VO_API int vo_batch_fetch(vo_ctx* ctx, int unit, vo_point2f* pts_in, vo_point2f* pts4, int32_t* kept_idx,
                           vo_point3f* X, int32_t* inliers);
+
+/* ---- images already in device memory (sequence and batched modes) ----------------------------------------------------
+ * One caller-owned image in device memory of the context's GPU (cudaMalloc'ed or managed; host and pinned-host memory
+ * are refused).  Pixel (x, y), channel c is read at data + y * row_pitch + x * pixel_stride + c * channel_stride, at
+ * any alignment:
+ *   gray (H, W)            pixel_stride 1, row_pitch >= W
+ *   interleaved (H, W, 3)  pixel_stride 3, channel_stride 1      (cv::Mat CV_8UC3, torch HWC)
+ *   planar (3, H, W)       pixel_stride 1, channel_stride = plane size (torch CHW, e.g. torchvision's CUDA decoders)
+ * Colour is converted exactly as cv::cvtColor(BGR2GRAY / RGB2GRAY): (b*3735 + g*19235 + r*9798 + 2^14) >> 15.
+ * Refused (VO_E_INVALID): a pointer that is not device memory of the context's GPU, pixel_stride < 1,
+ * row_pitch < w * pixel_stride, channel_stride < 1 for colour, an unknown format. */
+#define VO_FMT_GRAY 0
+#define VO_FMT_BGR  1
+#define VO_FMT_RGB  2
+typedef struct vo_dimage {
+    const uint8_t* data;    /* device pointer to pixel (0,0), first channel                                   */
+    size_t row_pitch;       /* bytes between rows                                                               */
+    int    pixel_stride;    /* bytes between horizontally adjacent pixels (1: gray / planar, 3: interleaved)    */
+    size_t channel_stride;  /* bytes between a pixel's channels (1: interleaved HWC, plane size: planar CHW);    */
+                            /* ignored for VO_FMT_GRAY                                                          */
+    int    format;          /* VO_FMT_*                                                                         */
+} vo_dimage;
+/* vo_unit with device images in place of the four host pointers and the pitch; pts stays a HOST list (or NULL). */
+typedef struct vo_dunit {
+    vo_dimage l0, r0, l1, r1;
+    const vo_point2f* pts;
+    int n_pts;
+    double t_prev[3];
+} vo_dunit;
+/* Stream contract of the *_device calls (the rule a PyTorch operation follows; no stream argument, see vo_set_stream):
+ *   - the images are read after all work enqueued on the context's stream before the call;
+ *   - work enqueued on that stream after the call returns is ordered after the library's last read of the images, so the
+ *     caller may overwrite or free them stream-ordered without waiting for results.
+ * Every other rule of the host-memory form applies unchanged (frames in flight, slot overlap, mixing of entry points).
+ *   vo_seq_begin_device / vo_seq_submit_device   vo_seq_begin / vo_seq_submit; results through vo_seq_wait[_mono]
+ *                                                (a push is submit + wait).  The conversion runs on the sequence's copy
+ *                                                stream, straight into the image ring, under the previous frame.
+ *   vo_batch_submit_device                       vo_batch_submit; results through vo_batch_wait / vo_batch_outputs /
+ *                                                vo_batch_fetch.  units == NULL re-runs what is resident, as there. */
+VO_API int vo_seq_begin_device(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], const vo_dimage* left0,
+                               const vo_dimage* right0);
+VO_API int vo_seq_submit_device(vo_ctx* ctx, const vo_dimage* left1, const vo_dimage* right1);
+VO_API int vo_batch_submit_device(vo_ctx* ctx, const vo_dunit* units, int first_unit, int n_units);
 
 /* ---- multi-GPU: gather of the result records over NCCL (SURVEY.md 8e; one process per GPU, units sharded) -----------
  * The path has no data-path collective; the only exchange is the gather of the fixed-size records.  NCCL is resolved with

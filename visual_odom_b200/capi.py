@@ -38,6 +38,50 @@ class VoUnit(C.Structure):
     ]
 
 
+VO_FMT_GRAY, VO_FMT_BGR, VO_FMT_RGB = 0, 1, 2
+
+
+class VoDImage(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("row_pitch", C.c_size_t), ("pixel_stride", C.c_int), ("channel_stride", C.c_size_t),
+                ("format", C.c_int)]
+
+
+class VoDUnit(C.Structure):
+    _fields_ = [("l0", VoDImage), ("r0", VoDImage), ("l1", VoDImage), ("r1", VoDImage),
+                ("pts", C.c_void_p), ("n_pts", C.c_int), ("t_prev", C.c_double * 3)]
+
+
+def image_descriptor(shape, strides, data_ptr, order=None):
+    """The vo_dimage of a uint8 image laid out (H, W), (H, W, 3) or (3, H, W) with the given byte strides (as torch's
+    t.shape, t.stride() and t.data_ptr() of a uint8 tensor give them).  Returns (VoDImage, w, h).  Colour images need
+    order="bgr" or "rgb"; there is no default.  Raises ValueError for any other layout, for non-positive strides and for
+    rows that overlap (a transposed image)."""
+    shape, strides = tuple(int(v) for v in shape), tuple(int(v) for v in strides)
+    if len(shape) == 2:
+        (h, w), (rs, ps), cs, fmt = shape, strides, 0, VO_FMT_GRAY
+    elif len(shape) == 3:
+        hwc, chw = shape[2] == 3, shape[0] == 3
+        if hwc == chw:
+            raise ValueError(f"image of shape {shape}: expected (H, W, 3) or (3, H, W)")
+        (h, w), (rs, ps), cs = (shape[:2], strides[:2], strides[2]) if hwc else (shape[1:], strides[1:], strides[0])
+        if order not in ("bgr", "rgb"):
+            raise ValueError(f'colour image: order must be "bgr" or "rgb" (got {order!r})')
+        fmt = VO_FMT_BGR if order == "bgr" else VO_FMT_RGB
+        if cs <= 0:
+            raise ValueError(f"image strides {strides}: strides must be positive")
+    else:
+        raise ValueError(f"image of shape {shape}: expected (H, W), (H, W, 3) or (3, H, W)")
+    if h <= 0 or w <= 0:
+        raise ValueError(f"empty image of shape {shape}")
+    if rs <= 0 or ps <= 0:
+        raise ValueError(f"image strides {strides}: strides must be positive")
+    if rs < w * ps:
+        raise ValueError(f"image strides {strides}: rows of {w} pixels overlap (row pitch {rs} < {w} x {ps})")
+    d = VoDImage()
+    d.data, d.row_pitch, d.pixel_stride, d.channel_stride, d.format = data_ptr, rs, ps, cs, fmt
+    return d, w, h
+
+
 class VoUnitResult(C.Structure):
     _fields_ = [
         ("n_features", C.c_int), ("n_detected", C.c_int), ("n_tracked", C.c_int), ("n_valid", C.c_int),
@@ -125,6 +169,9 @@ SIGNATURES = {
     "vo_dist_gather_post": (C.c_int, [C.c_void_p, C.c_int, C.c_int]),
     "vo_dist_gather_wait": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]),
     "vo_batch_outputs": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_size_t)]),
+    "vo_seq_begin_device": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(VoDImage), C.POINTER(VoDImage)]),
+    "vo_seq_submit_device": (C.c_int, [C.c_void_p, C.POINTER(VoDImage), C.POINTER(VoDImage)]),
+    "vo_batch_submit_device": (C.c_int, [C.c_void_p, C.POINTER(VoDUnit), C.c_int, C.c_int]),
 }
 
 _lib = None
@@ -171,6 +218,9 @@ class Context:
                 raise TypeError(f"unknown vo_params field {k}")
             setattr(p, k, v)
         self.params = p
+        self.device = device
+        self._stream = None           # the stream the context was last pointed at by the *_device calls
+        self._bridge = None
         h = C.c_void_p()
         rc = self.lib.vo_create(device, C.byref(p), C.byref(h))
         self.h = h
@@ -200,6 +250,7 @@ class Context:
     # ---- plumbing --------------------------------------------------------------------------------
     def set_stream(self, cuda_stream_ptr):
         self._check(self.lib.vo_set_stream(self.h, C.c_void_p(cuda_stream_ptr)))
+        self._stream = cuda_stream_ptr
 
     def sync(self):
         self._check(self.lib.vo_sync(self.h))
@@ -505,6 +556,88 @@ class Context:
 
     def seq_submit_ptr(self, left_ptr, right_ptr, pitch, channels=1):
         self._check(self.lib.vo_seq_submit(self.h, left_ptr, right_ptr, pitch, channels))
+
+    # ---- images already on the GPU (CUDA uint8 torch tensors (H, W), (H, W, 3) or (3, H, W)) ----------------------------
+    # The calls run on torch.cuda.current_stream(): the images are read after the work already queued there, and work queued
+    # there after the call is ordered after the library's last read of them, so a tensor may be overwritten or freed
+    # stream-ordered at once (as after any PyTorch operation).  vo_set_stream synchronises the previous stream, so it is
+    # called only when the current stream changes.  The legacy default stream cannot be captured into the library's CUDA
+    # graphs: on it the context runs on a private stream that waits for the default stream before the call and is waited
+    # for after it.
+    def _device_image(self, t, order):
+        import torch
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise TypeError("device images must be CUDA torch tensors (host images go through the host entry points)")
+        if t.dtype != torch.uint8:
+            raise TypeError(f"device images must be uint8, not {t.dtype}")
+        if t.device.index != self.device:
+            raise ValueError(f"image on {t.device}, the context on cuda:{self.device}")
+        return image_descriptor(t.shape, t.stride(), t.data_ptr(), order)
+
+    def _enter_stream(self):
+        import torch
+        cur = torch.cuda.current_stream(self.device)
+        run = cur
+        if cur.cuda_stream == 0:
+            if self._bridge is None:
+                self._bridge = torch.cuda.Stream(self.device)
+            self._bridge.wait_stream(cur)
+            run = self._bridge
+        if run.cuda_stream != self._stream:
+            self.set_stream(run.cuda_stream)
+        return cur, run
+
+    def _device_call(self, fn, *args):
+        cur, run = self._enter_stream()
+        try:
+            self._check(fn(self.h, *args))
+        finally:
+            if run is not cur:
+                cur.wait_stream(run)
+
+    def seq_begin_device(self, left0, right0, P_l, P_r, order=None):
+        (l, w, h), (r, wr, hr) = self._device_image(left0, order), self._device_image(right0, order)
+        if (wr, hr) != (w, h):
+            raise ValueError("left and right images differ in size")
+        P_l = np.ascontiguousarray(P_l, np.float32).reshape(12); P_r = np.ascontiguousarray(P_r, np.float32).reshape(12)
+        self._device_call(self.lib.vo_seq_begin_device, w, h, _p(P_l), _p(P_r), C.byref(l), C.byref(r))
+
+    def seq_submit_device(self, left1, right1, order=None):
+        """Asynchronous push of device images; results through seq_wait.  The tensors may be reused stream-ordered at once."""
+        l, _, _ = self._device_image(left1, order)
+        r, _, _ = self._device_image(right1, order)
+        self._device_call(self.lib.vo_seq_submit_device, C.byref(l), C.byref(r))
+
+    def seq_push_device(self, left1, right1, order=None, pts_cap=4096, want_points=True, mono=False):
+        self.seq_submit_device(left1, right1, order)
+        return self.seq_wait(pts_cap, want_points, mono=mono)
+
+    def batch_submit_device(self, units, first_unit, order=None, n_units=None):
+        """vo_batch_submit_device: units as for make_units, with CUDA tensors for l0, r0, l1, r1 (a colour unit may carry
+        its own "order"); units=None re-runs what is resident (n_units required).  Results through batch_wait."""
+        if units is None:
+            self._device_call(self.lib.vo_batch_submit_device, None, first_unit, n_units)
+            return
+        arr = (VoDUnit * len(units))()
+        keep = []
+        for i, u in enumerate(units):
+            for k in ("l0", "r0", "l1", "r1"):
+                d, w, h = self._device_image(u[k], u.get("order", order))
+                if (w, h) != tuple(self._batch_geom[:2]):
+                    raise ValueError(f"unit {i} {k}: {w} x {h}, the batch is configured for {self._batch_geom[0]} x {self._batch_geom[1]}")
+                setattr(arr[i], k, d)
+            if u.get("pts") is not None:
+                pts = np.ascontiguousarray(u["pts"], np.float32).reshape(-1, 2)
+                keep.append(pts)
+                arr[i].pts = pts.ctypes.data
+                arr[i].n_pts = len(pts)
+            else:
+                arr[i].pts = None
+                arr[i].n_pts = int(u["n_select"])
+            t = u.get("t_prev", (0.0, 0.0, 0.0))
+            for k in range(3):
+                arr[i].t_prev[k] = float(t[k])
+        self._device_call(self.lib.vo_batch_submit_device, arr, first_unit, len(units))
 
     def seq_wait(self, pts_cap=4096, want_points=True, mono=False):
         """mono=True: also "mono" (dict: status, n_inliers, ransac_iters, n_good, R 3x3, t) and "ess_mask" (bool, aligned

@@ -122,22 +122,32 @@ extern "C" int vo_batch_configure(vo_ctx* ctx, int w, int h, int n_units, const 
     return VO_OK;
 }
 
-// H2D of units [u0, u0+n) on stream `st`; scalars go through the pinned staging block (disjoint per unit)
-static int upload_range(vo_ctx* ctx, const vo_unit* units, int u0, int n, size_t pitch, cudaStream_t st, bool detect, int src0 = -1)
+// Pinned staging of the batched path, disjoint per unit: t_prev [batch_units][3] | counts [batch_units] | result records
+// [batch_units] (64-byte aligned) | descriptors of caller device images [batch_units][4]
+static size_t batch_pinned_bytes(const vo_ctx* ctx)
 {
-    if (src0 < 0) src0 = u0;           // units[src0 + i] fills resident slot u0 + i
-    const int w = ctx->w, h = ctx->h, cap = ctx->cap;
+    return (size_t)ctx->batch_units * (3 * sizeof(double) + sizeof(int) + sizeof(vo_unit_result_dev) + 4 * sizeof(vo_dimage)) + 256;
+}
+
+static vo_unit_result_dev* pinned_results(vo_ctx* ctx)
+{
+    char* p = (char*)ctx->h_pinned + (size_t)ctx->batch_units * (3 * sizeof(double) + sizeof(int));
+    p = (char*)(((uintptr_t)p + 63) & ~(uintptr_t)63);
+    return (vo_unit_result_dev*)p;
+}
+
+static vo_dimage* pinned_ingest_tab(vo_ctx* ctx) { return (vo_dimage*)(pinned_results(ctx) + ctx->batch_units); }
+
+// features and scalars of units [u0, u0+n) on stream `st`, through the pinned staging block; units[src0 + i] fills slot u0 + i
+template <typename Unit>
+static int stage_inputs(vo_ctx* ctx, const Unit* units, int u0, int n, cudaStream_t st, bool detect, int src0)
+{
+    const int cap = ctx->cap;
     const int total = ctx->batch_units;
     double* h_tprev = (double*)ctx->h_pinned;
     int* h_cnt = (int*)(h_tprev + 3 * (size_t)total);
     for (int u = u0; u < u0 + n; u++) {
-        const vo_unit& U = units[u - u0 + src0];
-        const uint8_t* imgs[4] = {U.l0, U.r0, U.l1, U.r1};
-        for (int k = 0; k < 4; k++) {
-            uint8_t* dst = ctx->d_raw + ((size_t)u * 4 + k) * w * h;
-            if (pitch == (size_t)w) VO_CUDA_CHECK(cudaMemcpyAsync(dst, imgs[k], (size_t)w * h, cudaMemcpyHostToDevice, st));
-            else VO_CUDA_CHECK(cudaMemcpy2DAsync(dst, w, imgs[k], pitch, w, h, cudaMemcpyHostToDevice, st));
-        }
+        const Unit& U = units[u - u0 + src0];
         if (!detect && U.n_pts > 0)
             VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_pts_in + (size_t)u * cap, U.pts, (size_t)U.n_pts * sizeof(float2),
                                           cudaMemcpyHostToDevice, st));
@@ -152,32 +162,61 @@ static int upload_range(vo_ctx* ctx, const vo_unit* units, int u0, int n, size_t
     return VO_OK;
 }
 
-static int validate_units(vo_ctx* ctx, const vo_unit* units, int n_units, size_t pitch, bool* detect_out, int* max_pts_out = nullptr)
+// H2D of units [u0, u0+n) on stream `st`: the host images, then features and scalars
+static int upload_range(vo_ctx* ctx, const vo_unit* units, int u0, int n, size_t pitch, cudaStream_t st, bool detect, int src0 = -1)
+{
+    if (src0 < 0) src0 = u0;           // units[src0 + i] fills resident slot u0 + i
+    const int w = ctx->w, h = ctx->h;
+    for (int u = u0; u < u0 + n; u++) {
+        const vo_unit& U = units[u - u0 + src0];
+        const uint8_t* imgs[4] = {U.l0, U.r0, U.l1, U.r1};
+        for (int k = 0; k < 4; k++) {
+            uint8_t* dst = ctx->d_raw + ((size_t)u * 4 + k) * w * h;
+            if (pitch == (size_t)w) VO_CUDA_CHECK(cudaMemcpyAsync(dst, imgs[k], (size_t)w * h, cudaMemcpyHostToDevice, st));
+            else VO_CUDA_CHECK(cudaMemcpy2DAsync(dst, w, imgs[k], pitch, w, h, cudaMemcpyHostToDevice, st));
+        }
+    }
+    return stage_inputs(ctx, units, u0, n, st, detect, src0);
+}
+
+static int check_images(vo_ctx* ctx, const vo_unit& U, int u, size_t pitch)
+{
+    if (pitch < (size_t)ctx->w) { vo_set_error(ctx, "pitch %zu < width %d", pitch, ctx->w); return VO_E_INVALID; }
+    if (!U.l0 || !U.r0 || !U.l1 || !U.r1) { vo_set_error(ctx, "unit %d: null image", u); return VO_E_INVALID; }
+    return VO_OK;
+}
+
+static int check_images(vo_ctx* ctx, const vo_dunit& U, int u, size_t)
+{
+    char who[64];
+    snprintf(who, sizeof(who), "vo_batch_submit_device: unit %d", u);
+    const vo_dimage* imgs[4] = {&U.l0, &U.r0, &U.l1, &U.r1};
+    static const char* names[4] = {"l0", "r0", "l1", "r1"};
+    for (int k = 0; k < 4; k++) {
+        const int rc = vo_check_dimage(ctx, who, names[k], imgs[k], ctx->w);
+        if (rc) return rc;
+    }
+    return VO_OK;
+}
+
+template <typename Unit>
+static int validate_units(vo_ctx* ctx, const Unit* units, int n_units, size_t pitch, bool* detect_out, int* max_pts_out = nullptr)
 {
     if (!ctx || !units) return VO_E_INVALID;
     if (n_units <= 0 || n_units > ctx->batch_units) { vo_set_error(ctx, "n_units=%d outside the configured batch (%d)", n_units, ctx->batch_units); return VO_E_INVALID; }
-    if (pitch < (size_t)ctx->w) { vo_set_error(ctx, "pitch %zu < width %d", pitch, ctx->w); return VO_E_INVALID; }
     const bool detect = (units[0].pts == nullptr);
     int max_pts = 0;
     for (int u = 0; u < n_units; u++) {
-        const vo_unit& U = units[u];
-        if (!U.l0 || !U.r0 || !U.l1 || !U.r1) { vo_set_error(ctx, "unit %d: null image", u); return VO_E_INVALID; }
+        const Unit& U = units[u];
+        int rc = check_images(ctx, U, u, pitch);
+        if (rc) return rc;
         if ((U.pts == nullptr) != detect) { vo_set_error(ctx, "units must all carry features or all request detection"); return VO_E_INVALID; }
         if (U.n_pts < 0 || U.n_pts > ctx->cap) { vo_set_error(ctx, "unit %d: n_pts=%d outside [0,%d]", u, U.n_pts, ctx->cap); return VO_E_CAPACITY; }
         if (U.n_pts > max_pts) max_pts = U.n_pts;
     }
     *detect_out = detect;
     if (max_pts_out) *max_pts_out = max_pts;
-    // pinned staging: t_prev, counts, result records
-    const size_t bytes = (size_t)ctx->batch_units * (3 * sizeof(double) + sizeof(int) + sizeof(vo_unit_result_dev)) + 256;
-    return vo_ensure_pinned(ctx, bytes);
-}
-
-static vo_unit_result_dev* pinned_results(vo_ctx* ctx)
-{
-    char* p = (char*)ctx->h_pinned + (size_t)ctx->batch_units * (3 * sizeof(double) + sizeof(int));
-    p = (char*)(((uintptr_t)p + 63) & ~(uintptr_t)63);
-    return (vo_unit_result_dev*)p;
+    return vo_ensure_pinned(ctx, batch_pinned_bytes(ctx));
 }
 
 extern "C" int vo_batch_upload(vo_ctx* ctx, const vo_unit* units, int n_units, size_t pitch)
@@ -405,18 +444,41 @@ extern "C" int vo_frame_batch(vo_ctx* ctx, const vo_unit* units, int n_units, si
 // Submissions on disjoint slot ranges overlap on the GPU: the H2D copy, FAST / pyramids and above all the
 // latency-bound PnP tail (a few warps for ~0.4 ms) of one run under the issue-bound LK ring of the other, which a
 // synchronous vo_frame_batch per batch cannot do for its last unit range.
-extern "C" int vo_batch_submit(vo_ctx* ctx, const vo_unit* units, int first_unit, int n_units, size_t pitch)
+//
+// Host units: H2D copies of the images on the lane stream.  Device units (vo_batch_submit_device): one k_bgr_to_gray
+// launch for the range on the lane stream, which follows fork_ev and so the caller's work on ctx->stream (producer
+// ordering); ctx->stream then waits for that launch only, which releases the caller's images without waiting for the range.
+static int upload_units(vo_ctx* ctx, const vo_unit* units, int u0, int n, size_t pitch, cudaStream_t st, int, bool detect)
+{
+    return upload_range(ctx, units, u0, n, pitch, st, detect, 0);
+}
+
+static int upload_units(vo_ctx* ctx, const vo_dunit* units, int u0, int n, size_t, cudaStream_t st, int lane, bool detect)
+{
+    vo_dimage* tab = pinned_ingest_tab(ctx) + 4 * (size_t)u0;
+    for (int i = 0; i < n; i++) {
+        tab[4 * i] = units[i].l0; tab[4 * i + 1] = units[i].r0; tab[4 * i + 2] = units[i].l1; tab[4 * i + 3] = units[i].r1;
+    }
+    int rc = vo_ingest_device(ctx, tab, 4 * n, 4 * u0, st);
+    if (rc) return rc;
+    VO_CUDA_CHECK(cudaEventRecord(ctx->join_ev[lane], st));
+    VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->join_ev[lane], 0));
+    return stage_inputs(ctx, units, u0, n, st, detect, 0);
+}
+
+template <typename Unit>
+static int batch_submit(vo_ctx* ctx, const char* who, const Unit* units, int first_unit, int n_units, size_t pitch)
 {
     if (!ctx) return VO_E_INVALID;
     if (first_unit < 0 || n_units <= 0 || first_unit + n_units > ctx->batch_units) {
-        vo_set_error(ctx, "vo_batch_submit: slots [%d, %d) outside the configured batch (%d)", first_unit, first_unit + n_units, ctx->batch_units);
+        vo_set_error(ctx, "%s: slots [%d, %d) outside the configured batch (%d)", who, first_unit, first_unit + n_units, ctx->batch_units);
         return VO_E_INVALID;
     }
-    if (!ctx->have_P) { vo_set_error(ctx, "vo_batch_submit: projection matrices not set"); return VO_E_INVALID; }
-    { int rcc = vo_claim_buffers(ctx, "vo_batch_submit", true); if (rcc) return rcc; }
+    if (!ctx->have_P) { vo_set_error(ctx, "%s: projection matrices not set", who); return VO_E_INVALID; }
+    { int rcc = vo_claim_buffers(ctx, who, true); if (rcc) return rcc; }
     for (auto& p : ctx->pending)
         if (p.active && first_unit < p.u0 + p.n && p.u0 < first_unit + n_units) {
-            vo_set_error(ctx, "vo_batch_submit: slots [%d, %d) overlap a submission that has not been waited for", first_unit, first_unit + n_units);
+            vo_set_error(ctx, "%s: slots [%d, %d) overlap a submission that has not been waited for", who, first_unit, first_unit + n_units);
             return VO_E_INVALID;
         }
     bool detect = ctx->batch_detect; int max_pts = 0;
@@ -425,11 +487,10 @@ extern "C" int vo_batch_submit(vo_ctx* ctx, const vo_unit* units, int first_unit
         if ((rc = validate_units(ctx, units, n_units, pitch, &detect, &max_pts))) return rc;
     } else {
         if (ctx->batch_uploaded < first_unit + n_units) {
-            vo_set_error(ctx, "vo_batch_submit: units == NULL but slots [%d, %d) were never uploaded", first_unit, first_unit + n_units);
+            vo_set_error(ctx, "%s: units == NULL but slots [%d, %d) were never uploaded", who, first_unit, first_unit + n_units);
             return VO_E_INVALID;
         }
-        const size_t bytes = (size_t)ctx->batch_units * (3 * sizeof(double) + sizeof(int) + sizeof(vo_unit_result_dev)) + 256;
-        if ((rc = vo_ensure_pinned(ctx, bytes))) return rc;
+        if ((rc = vo_ensure_pinned(ctx, batch_pinned_bytes(ctx)))) return rc;
         max_pts = range_bound(ctx, first_unit, n_units);
     }
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
@@ -457,7 +518,7 @@ extern "C" int vo_batch_submit(vo_ctx* ctx, const vo_unit* units, int first_unit
     if ((rc = vo_dist_order_after_gathers(ctx, st))) return rc;
     ctx->batch_detect = detect;
     if (units) {
-        if ((rc = upload_range(ctx, units, first_unit, n_units, pitch, st, detect, 0))) return rc;
+        if ((rc = upload_units(ctx, units, first_unit, n_units, pitch, st, c, detect))) return rc;
         if (ctx->batch_uploaded < first_unit + n_units) ctx->batch_uploaded = first_unit + n_units;
     }
     if ((rc = run_range(ctx, View{first_unit, n_units, st}))) return rc;
@@ -476,6 +537,16 @@ extern "C" int vo_batch_submit(vo_ctx* ctx, const vo_unit* units, int first_unit
     VO_CUDA_CHECK(cudaEventRecord(slot->done, st));
     slot->u0 = first_unit; slot->n = n_units; slot->active = true;
     return VO_OK;
+}
+
+extern "C" int vo_batch_submit(vo_ctx* ctx, const vo_unit* units, int first_unit, int n_units, size_t pitch)
+{
+    return batch_submit(ctx, "vo_batch_submit", units, first_unit, n_units, pitch);
+}
+
+extern "C" int vo_batch_submit_device(vo_ctx* ctx, const vo_dunit* units, int first_unit, int n_units)
+{
+    return batch_submit(ctx, "vo_batch_submit_device", units, first_unit, n_units, 0);
 }
 
 extern "C" int vo_batch_wait(vo_ctx* ctx, int first_unit, int n_units, vo_unit_result* results)

@@ -414,6 +414,7 @@ int vo_ensure_state(vo_ctx* ctx, int w, int h, int units, int /*imgs_per_unit*/)
     pg.n_img = n_img;
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_raw, (size_t)n_img * w * h));
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_raw_tab, (size_t)n_img));
+    VO_CUDA_CHECK(dalloc(ctx, &ctx->d_ingest_tab, (size_t)n_img));
     {
         std::vector<const uint8_t*> tab(n_img);
         for (int i = 0; i < n_img; i++) tab[i] = ctx->d_raw + (size_t)i * w * h;

@@ -35,7 +35,8 @@ struct vo_ctx {
 
     // ---- device buffers ---------------------------------------------------------------------
     uint8_t* d_raw = nullptr;           // [units*4][h*w] raw images
-    const uint8_t** d_raw_tab = nullptr;// [units*4] pointers into d_raw (or caller device images)
+    const uint8_t** d_raw_tab = nullptr;// [units*4] pointers into d_raw
+    vo_dimage* d_ingest_tab = nullptr;  // [units*4] descriptors of caller device images, per raw plane (staged per submission)
     float2* d_pts_in = nullptr;         // [units][cap]
     int* d_npts = nullptr;              // [units]
     float2* d_pts_out = nullptr;        // [4][units][cap]
@@ -192,8 +193,16 @@ void vo_dist_shutdown(vo_ctx* ctx);
 int vo_claim_buffers(vo_ctx* ctx, const char* who, bool allow_pending_batches = false);
 int vo_ensure_pinned(vo_ctx* ctx, size_t bytes);
 int vo_ensure_bgr(vo_ctx* ctx, size_t bytes);
-int vo_launch_bgr_to_gray(const uint8_t* d_bgr, size_t pitch, size_t img_stride_in, uint8_t* d_gray, size_t img_stride_out,
+// k_bgr_to_gray: images tab[0 .. n_img) (device table), or with d_tab == nullptr `packed` advanced by packed_stride per image,
+// into gray planes img_stride_out apart
+int vo_launch_bgr_to_gray(const vo_dimage* d_tab, const vo_dimage& packed, size_t packed_stride, uint8_t* d_gray, size_t img_stride_out,
                           int w, int h, int n_img, cudaStream_t s);
+vo_dimage vo_packed_bgr(const uint8_t* d_bgr, int w);      // the descriptor of w-pixel packed BGR rows
+// VO_E_INVALID + message unless `im` can be read as an image `w` pixels wide in device memory of the context's GPU
+int vo_check_dimage(vo_ctx* ctx, const char* who, const char* name, const vo_dimage* im, int w);
+// caller device images h_tab[0 .. n) (pinned staging, untouched until the copy has run on st) -> raw planes
+// [plane0, plane0 + n): one descriptor copy into d_ingest_tab + plane0 and one k_bgr_to_gray launch on st
+int vo_ingest_device(vo_ctx* ctx, const vo_dimage* h_tab, int n, int plane0, cudaStream_t st);
 // a contiguous range of resident work units processed on one stream
 // plane0 >= 0 overrides the image-plane base (default u0 * imgs_per_unit): the sequence mode ping-pongs its per-frame
 // buffers between units 0 and 1 while both use the same four image planes

@@ -10,7 +10,9 @@
 //   * a prefetching sequence reader: worker threads decode frames ahead of the consumer straight into a ring of
 //     PINNED buffers, so vo_seq_push's H2D copy is a single async DMA and never waits for the file system;
 //   * for colour sources the BGR bytes go to the device as they are and k_bgr_to_gray converts them there (inside the
-//     frame's CUDA graph); gray sources (KITTI) need no conversion at all (the formula is the identity on b=g=r).
+//     frame's CUDA graph); gray sources (KITTI) need no conversion at all (the formula is the identity on b=g=r);
+//   * images already in device memory (vo_dimage: gray, interleaved or planar BGR / RGB, any pitch and alignment) are
+//     read by the same kernel straight into the raw gray planes (vo_seq_*_device, vo_batch_submit_device).
 #include "ctx.h"
 #include <zlib.h>
 #include <atomic>
@@ -341,22 +343,34 @@ extern "C" void vo_reader_close(vo_reader* rd)
 }
 
 // ------------------------------------------------------------------------------------------------ device gray convert
-// BGR interleaved (pitch bytes per row) -> gray plane (w bytes per row), 4 pixels per thread, 32-bit stores.
-// 3 B read + 1 B written per pixel: pure HBM streaming.
-__global__ void k_bgr_to_gray(const uint8_t* __restrict__ bgr, size_t pitch, size_t img_stride_in, uint8_t* __restrict__ gray,
+// Source image -> raw gray plane (w bytes per row), 4 pixels per thread, 32-bit stores where the destination allows.
+// Image z of the launch is tab[z] (caller device images: descriptors staged per submission), or, with tab == nullptr,
+// `packed` advanced by z * packed_stride (the packed BGR staging of host colour input, whose graph-captured launch
+// cannot take a per-frame table).  Sources may have any alignment, pitch and strides: every pixel is read with byte
+// loads.  Colour: cv::cvtColor(BGR2GRAY / RGB2GRAY)'s fixed point; gray: the identity (which the formula is on b=g=r).
+__global__ void k_bgr_to_gray(const vo_dimage* __restrict__ tab, vo_dimage packed, size_t packed_stride, uint8_t* __restrict__ gray,
                               size_t img_stride_out, int w, int h)
 {
     const int img = blockIdx.z, y = blockIdx.y;
     const int x0 = 4 * (blockIdx.x * blockDim.x + threadIdx.x);
     if (x0 >= w) return;
-    const uint8_t* s = bgr + (size_t)img * img_stride_in + (size_t)y * pitch + 3 * (size_t)x0;
+    vo_dimage src = packed;
+    if (tab) src = tab[img];
+    else src.data += (size_t)img * packed_stride;
+    const uint8_t* s = src.data + (size_t)y * src.row_pitch + (size_t)x0 * src.pixel_stride;
+    const size_t cs = src.channel_stride;
     uint8_t* d = gray + (size_t)img * img_stride_out + (size_t)y * w + x0;
     uint8_t o[4];
 #pragma unroll
     for (int i = 0; i < 4; i++) {
         if (x0 + i < w) {
-            const int b = s[3 * i], g = s[3 * i + 1], r = s[3 * i + 2];
-            o[i] = (uint8_t)((b * 3735 + g * 19235 + r * 9798 + (1 << 14)) >> 15);
+            const uint8_t* p = s + (size_t)i * src.pixel_stride;
+            if (src.format == VO_FMT_GRAY) o[i] = p[0];
+            else {
+                const int c0 = p[0], g = p[cs], c2 = p[2 * cs];
+                const int b = src.format == VO_FMT_RGB ? c2 : c0, r = src.format == VO_FMT_RGB ? c0 : c2;
+                o[i] = (uint8_t)((b * 3735 + g * 19235 + r * 9798 + (1 << 14)) >> 15);
+            }
         } else o[i] = 0;
     }
     if (x0 + 3 < w && ((size_t)(d - gray) & 3) == 0 && (((size_t)gray) & 3) == 0)
@@ -365,12 +379,56 @@ __global__ void k_bgr_to_gray(const uint8_t* __restrict__ bgr, size_t pitch, siz
         for (int i = 0; i < 4 && x0 + i < w; i++) d[i] = o[i];
 }
 
-int vo_launch_bgr_to_gray(const uint8_t* d_bgr, size_t pitch, size_t img_stride_in, uint8_t* d_gray, size_t img_stride_out,
+int vo_launch_bgr_to_gray(const vo_dimage* d_tab, const vo_dimage& packed, size_t packed_stride, uint8_t* d_gray, size_t img_stride_out,
                           int w, int h, int n_img, cudaStream_t s)
 {
     dim3 grid(((w + 3) / 4 + 127) / 128, h, n_img);
-    k_bgr_to_gray<<<grid, 128, 0, s>>>(d_bgr, pitch, img_stride_in, d_gray, img_stride_out, w, h);
+    k_bgr_to_gray<<<grid, 128, 0, s>>>(d_tab, packed, packed_stride, d_gray, img_stride_out, w, h);
     return 1;
+}
+
+vo_dimage vo_packed_bgr(const uint8_t* d_bgr, int w)
+{
+    vo_dimage a;
+    a.data = d_bgr; a.row_pitch = (size_t)3 * w; a.pixel_stride = 3; a.channel_stride = 1; a.format = VO_FMT_BGR;
+    return a;
+}
+
+int vo_check_dimage(vo_ctx* ctx, const char* who, const char* name, const vo_dimage* im, int w)
+{
+    if (!im || !im->data) { vo_set_error(ctx, "%s: %s: null image", who, name); return VO_E_INVALID; }
+    if (im->format != VO_FMT_GRAY && im->format != VO_FMT_BGR && im->format != VO_FMT_RGB) {
+        vo_set_error(ctx, "%s: %s: unknown format %d (VO_FMT_GRAY, VO_FMT_BGR or VO_FMT_RGB)", who, name, im->format);
+        return VO_E_INVALID;
+    }
+    if (im->pixel_stride < 1) { vo_set_error(ctx, "%s: %s: pixel_stride %d < 1", who, name, im->pixel_stride); return VO_E_INVALID; }
+    if (im->row_pitch < (size_t)w * im->pixel_stride) {
+        vo_set_error(ctx, "%s: %s: row_pitch %zu < %d pixels x pixel_stride %d", who, name, im->row_pitch, w, im->pixel_stride);
+        return VO_E_INVALID;
+    }
+    if (im->format != VO_FMT_GRAY && im->channel_stride < 1) { vo_set_error(ctx, "%s: %s: channel_stride 0 for a colour image", who, name); return VO_E_INVALID; }
+    VO_CUDA_CHECK(cudaSetDevice(ctx->device));
+    cudaPointerAttributes a;
+    const cudaError_t e = cudaPointerGetAttributes(&a, im->data);
+    if (e != cudaSuccess) { cudaGetLastError(); vo_set_error(ctx, "%s: %s: not a CUDA pointer (%s)", who, name, cudaGetErrorString(e)); return VO_E_INVALID; }
+    if (a.type == cudaMemoryTypeManaged) return VO_OK;
+    if (a.type != cudaMemoryTypeDevice) {
+        vo_set_error(ctx, "%s: %s is %s memory; the *_device entry points take device memory", who, name,
+                     a.type == cudaMemoryTypeHost ? "pinned host" : "host");
+        return VO_E_INVALID;
+    }
+    if (a.device != ctx->device) { vo_set_error(ctx, "%s: %s is on device %d, the context on device %d", who, name, a.device, ctx->device); return VO_E_INVALID; }
+    return VO_OK;
+}
+
+int vo_ingest_device(vo_ctx* ctx, const vo_dimage* h_tab, int n, int plane0, cudaStream_t st)
+{
+    const size_t plane = (size_t)ctx->w * ctx->h;
+    VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_ingest_tab + plane0, h_tab, (size_t)n * sizeof(vo_dimage), cudaMemcpyHostToDevice, st));
+    ctx->launches += vo_launch_bgr_to_gray(ctx->d_ingest_tab + plane0, vo_dimage{}, 0, ctx->d_raw + (size_t)plane0 * plane, plane,
+                                           ctx->w, ctx->h, n, st);
+    VO_CUDA_CHECK(cudaGetLastError());
+    return VO_OK;
 }
 
 int vo_ensure_bgr(vo_ctx* ctx, size_t bytes)
@@ -396,7 +454,7 @@ extern "C" int vo_bgr_to_gray(vo_ctx* ctx, const uint8_t* bgr, size_t pitch, int
     uint8_t* d_in = ctx->d_bgr;
     uint8_t* d_out = ctx->d_bgr + in_bytes;
     VO_CUDA_CHECK(cudaMemcpy2DAsync(d_in, (size_t)3 * w, bgr, pitch, (size_t)3 * w, h, cudaMemcpyHostToDevice, ctx->stream));
-    ctx->launches += vo_launch_bgr_to_gray(d_in, (size_t)3 * w, 0, d_out, 0, w, h, 1, ctx->stream);
+    ctx->launches += vo_launch_bgr_to_gray(nullptr, vo_packed_bgr(d_in, w), 0, d_out, 0, w, h, 1, ctx->stream);
     VO_CUDA_CHECK(cudaGetLastError());
     VO_CUDA_CHECK(cudaMemcpy2DAsync(gray, gray_pitch, d_out, w, w, h, cudaMemcpyDeviceToHost, ctx->stream));
     VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));

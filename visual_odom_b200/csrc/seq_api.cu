@@ -46,7 +46,7 @@ static int upload_pair(vo_ctx* ctx, int slot, const uint8_t* left, const uint8_t
 static int convert_pair(vo_ctx* ctx, int slot)
 {
     const int w = ctx->w, h = ctx->h;
-    ctx->launches += vo_launch_bgr_to_gray(ctx->d_bgr, (size_t)3 * w, (size_t)3 * w * h, ctx->d_raw + (size_t)(2 * slot) * w * h,
+    ctx->launches += vo_launch_bgr_to_gray(nullptr, vo_packed_bgr(ctx->d_bgr, w), (size_t)3 * w * h, ctx->d_raw + (size_t)(2 * slot) * w * h,
                                            (size_t)w * h, w, h, 2, ctx->stream);
     VO_CUDA_CHECK(cudaGetLastError());
     return VO_OK;
@@ -202,6 +202,10 @@ static int seq_graph(vo_ctx* ctx, int key, cudaStream_t st, F launch)
 }
 
 struct SeqRecord { vo_unit_result_dev r; int err; int pad_[3]; EssResult ess; /* mono sequences only */ };
+// pinned staging of the sequence mode: SeqRecord[2] (one per buffer unit) | vo_dimage[6] (device-image descriptors, one per
+// raw plane of the three-slot ring; plane 2s + k is restaged only after the frame that last used it has been waited for)
+static const size_t SEQ_PINNED_BYTES = 2 * sizeof(SeqRecord) + 6 * sizeof(vo_dimage) + 256;
+static vo_dimage* seq_pinned_tab(vo_ctx* ctx) { return (vo_dimage*)((SeqRecord*)ctx->h_pinned + 2); }
 
 static int seq_events(vo_ctx* ctx)
 {
@@ -236,13 +240,10 @@ extern "C" int vo_seq_begin(vo_ctx* ctx, int w, int h, const float P_l[12], cons
     return vo_seq_begin_ex(ctx, w, h, P_l, P_r, left0, right0, pitch, 1);
 }
 
-extern "C" int vo_seq_begin_ex(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], const uint8_t* left0,
-                               const uint8_t* right0, size_t pitch, int channels)
+// a new sequence whose first pair `fill_slot0` enqueues into image slot 0 on ctx->stream (arguments already checked)
+template <typename F>
+static int seq_begin(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], F fill_slot0)
 {
-    if (!ctx) return VO_E_INVALID;
-    if (channels != 1 && channels != 3) { vo_set_error(ctx, "vo_seq_begin: channels must be 1 (gray) or 3 (BGR)"); return VO_E_INVALID; }
-    if (!P_l || !P_r || !left0 || !right0 || w <= 0 || h <= 0 || pitch < (size_t)w * channels) { vo_set_error(ctx, "vo_seq_begin: bad argument"); return VO_E_INVALID; }
-    if (h / 10 <= 0) { vo_set_error(ctx, "vo_seq_begin: image too small for the rows/10 bucket size"); return VO_E_UNSUPPORTED; }
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
     int rc;
     if (ctx->seq_active && (rc = seq_drain(ctx))) return rc;
@@ -252,7 +253,7 @@ extern "C" int vo_seq_begin_ex(vo_ctx* ctx, int w, int h, const float P_l[12], c
     // the option holds for the whole sequence; the frame graphs are captured with or without the branch
     if (ctx->seq_mono != ctx->mono_opt) { vo_drop_graphs(ctx); ctx->seq_mono = ctx->mono_opt; }
     if (ctx->seq_mono && (rc = seq_mono_scratch(ctx))) return rc;
-    if ((rc = vo_ensure_pinned(ctx, 2 * sizeof(SeqRecord) + 256))) return rc;
+    if ((rc = vo_ensure_pinned(ctx, SEQ_PINNED_BYTES))) return rc;
     vo_set_calibration(ctx, P_l, P_r);
     ctx->imgs_per_unit = 4;
     ctx->seq_slot = 0;
@@ -262,8 +263,7 @@ extern "C" int vo_seq_begin_ex(vo_ctx* ctx, int w, int h, const float P_l[12], c
     VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_feat_cnt, 0, 2 * sizeof(int), ctx->stream));
     VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_seq_err, 0, 4 * sizeof(int), ctx->stream));
     VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_tprev, 0, 6 * sizeof(double), ctx->stream));      // translation = zeros (main.cpp:82)
-    if ((rc = upload_pair(ctx, 0, left0, right0, pitch, channels, ctx->stream))) return rc;
-    if (channels == 3 && (rc = convert_pair(ctx, 0))) return rc;
+    if ((rc = fill_slot0())) return rc;
     if ((rc = vo_run_pyramid(ctx, 0, 2, ctx->stream))) return rc;
     // both event pairs start out signalled, so the first two frames do not wait for a predecessor
     for (int k = 0; k < 2; k++) {
@@ -274,6 +274,37 @@ extern "C" int vo_seq_begin_ex(vo_ctx* ctx, int w, int h, const float P_l[12], c
     ctx->seq_active = true;
     return VO_OK;
 }
+
+extern "C" int vo_seq_begin_ex(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], const uint8_t* left0,
+                               const uint8_t* right0, size_t pitch, int channels)
+{
+    if (!ctx) return VO_E_INVALID;
+    if (channels != 1 && channels != 3) { vo_set_error(ctx, "vo_seq_begin: channels must be 1 (gray) or 3 (BGR)"); return VO_E_INVALID; }
+    if (!P_l || !P_r || !left0 || !right0 || w <= 0 || h <= 0 || pitch < (size_t)w * channels) { vo_set_error(ctx, "vo_seq_begin: bad argument"); return VO_E_INVALID; }
+    if (h / 10 <= 0) { vo_set_error(ctx, "vo_seq_begin: image too small for the rows/10 bucket size"); return VO_E_UNSUPPORTED; }
+    return seq_begin(ctx, w, h, P_l, P_r, [&] {
+        int rc = upload_pair(ctx, 0, left0, right0, pitch, channels, ctx->stream);
+        return rc ? rc : channels == 3 ? convert_pair(ctx, 0) : VO_OK;
+    });
+}
+
+extern "C" int vo_seq_begin_device(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], const vo_dimage* left0,
+                                   const vo_dimage* right0)
+{
+    if (!ctx) return VO_E_INVALID;
+    if (!P_l || !P_r || w <= 0 || h <= 0) { vo_set_error(ctx, "vo_seq_begin_device: bad argument"); return VO_E_INVALID; }
+    int rc;
+    if ((rc = vo_check_dimage(ctx, "vo_seq_begin_device", "left0", left0, w)) || (rc = vo_check_dimage(ctx, "vo_seq_begin_device", "right0", right0, w))) return rc;
+    if (h / 10 <= 0) { vo_set_error(ctx, "vo_seq_begin_device: image too small for the rows/10 bucket size"); return VO_E_UNSUPPORTED; }
+    // on the caller's stream, after the work already enqueued there; vo_seq_begin ends with a synchronise (the release)
+    return seq_begin(ctx, w, h, P_l, P_r, [&] {
+        vo_dimage* tab = seq_pinned_tab(ctx);
+        tab[0] = *left0; tab[1] = *right0;
+        return vo_ingest_device(ctx, tab, 2, 0, ctx->stream);
+    });
+}
+
+static int seq_enqueue(vo_ctx* ctx, int unit, int s0, int s1, bool bgr);
 
 extern "C" int vo_seq_submit(vo_ctx* ctx, const uint8_t* left1, const uint8_t* right1, size_t pitch, int channels)
 {
@@ -304,6 +335,14 @@ extern "C" int vo_seq_submit(vo_ctx* ctx, const uint8_t* left1, const uint8_t* r
         VO_CUDA_CHECK(cudaEventRecord(ctx->join_ev[1], sc));
         VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->join_ev[1], 0));
     }
+    return seq_enqueue(ctx, unit, s0, s1, bgr);
+}
+
+// The rest of vo_seq_submit[_device] once the new pair is (being) written into image slot s1: the front stage (gray frames
+// replay the gray graph whatever their source), the back stage, the record copies
+static int seq_enqueue(vo_ctx* ctx, int unit, int s0, int s1, bool bgr)
+{
+    int rc;
     if ((rc = seq_graph(ctx, -1 - (s0 + 3 * unit + 6 * (bgr ? 1 : 0)), ctx->stream, [&] { return seq_front(ctx, s0, s1, unit, bgr); }))) return rc;
     VO_CUDA_CHECK(cudaEventRecord(ctx->seq_front_ev[unit], ctx->stream));
     // back stage: after this frame's front stage; after the previous frame's back stage by stream order
@@ -316,10 +355,42 @@ extern "C" int vo_seq_submit(vo_ctx* ctx, const uint8_t* left1, const uint8_t* r
     if (ctx->seq_mono) VO_CUDA_CHECK(cudaMemcpyAsync(&rec->ess, seq_ess_result(ctx, unit), sizeof(rec->ess), cudaMemcpyDeviceToHost, sb));
     VO_CUDA_CHECK(cudaEventRecord(ctx->seq_back_ev[unit], sb));
     ctx->seq_slot = s1;                 // imageLeft_t0 = imageLeft_t1 (main.cpp:157-158)
-    ctx->seq_channels[unit] = channels;
+    ctx->seq_channels[unit] = bgr ? 3 : 1;
     ctx->seq_submitted++;
     ctx->seq_inflight++;
     return VO_OK;
+}
+
+extern "C" int vo_seq_submit_device(vo_ctx* ctx, const vo_dimage* left1, const vo_dimage* right1)
+{
+    if (!ctx) return VO_E_INVALID;
+    if (!ctx->seq_active) { vo_set_error(ctx, "vo_seq_submit_device: call vo_seq_begin first"); return VO_E_INVALID; }
+    int rc;
+    if ((rc = vo_check_dimage(ctx, "vo_seq_submit_device", "left1", left1, ctx->w)) ||
+        (rc = vo_check_dimage(ctx, "vo_seq_submit_device", "right1", right1, ctx->w))) return rc;
+    if (ctx->seq_inflight >= 2) { vo_set_error(ctx, "vo_seq_submit_device: two frames are in flight already; call vo_seq_wait"); return VO_E_INVALID; }
+    VO_CUDA_CHECK(cudaSetDevice(ctx->device));
+    const int unit = (int)(ctx->seq_submitted & 1);
+    const int s0 = ctx->seq_slot, s1 = (s0 + 1) % 3;
+    // Producer ordering: the conversion reads the images after the caller's work enqueued so far.  The event is recorded
+    // BEFORE the front stream waits for frame k-2's back stage below, so that the conversion does not queue behind that
+    // pose solve.
+    VO_CUDA_CHECK(cudaEventRecord(ctx->fork_ev, ctx->stream));
+    VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->seq_back_ev[unit], 0));
+    // As the host gray upload: on the copy stream, into slot s1 once the frame that last read it has finished its front
+    // stage, so the conversion runs under the frame in flight; it is launched outside the frame graph (its source pointers
+    // change every frame), and the frame replays the gray front graph.
+    cudaStream_t sc = ctx->side_stream[1];
+    VO_CUDA_CHECK(cudaStreamWaitEvent(sc, ctx->seq_front_ev[unit], 0));
+    VO_CUDA_CHECK(cudaStreamWaitEvent(sc, ctx->fork_ev, 0));
+    vo_dimage* tab = seq_pinned_tab(ctx) + 2 * s1;
+    tab[0] = *left1; tab[1] = *right1;
+    if ((rc = vo_ingest_device(ctx, tab, 2, 2 * s1, sc))) return rc;
+    // The join is also the release: the caller's later work on ctx->stream is ordered after the conversion, the last read
+    // of the images.
+    VO_CUDA_CHECK(cudaEventRecord(ctx->join_ev[1], sc));
+    VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->join_ev[1], 0));
+    return seq_enqueue(ctx, unit, s0, s1, false);
 }
 
 static int seq_wait(vo_ctx* ctx, vo_unit_result* out, vo_mono_result* mono, uint8_t* ess_mask, int mask_cap, vo_point2f* pts4,
