@@ -334,6 +334,38 @@ VO_API int vo_seq_wait_mono(vo_ctx* ctx, vo_unit_result* out, vo_mono_result* mo
 /* currentVOFeatures (points / ages may differ in length) and the carried translation (waits for frames in flight) */
 VO_API int vo_seq_state(vo_ctx* ctx, vo_point2f* points, int32_t* ages, int cap, int* n_points, int* n_ages, double t_out[3]);
 
+/* ---- several independent sequences through the streaming sequence mode ----------------------------------------------
+ * n_seq sequences of one image size and one calibration advance in lockstep, one frame each per submission, through the
+ * stages of the sequence mode above; every stage is ONE kernel launch for all of them, so a submission costs the launches
+ * of one vo_seq_submit whatever n_seq is.  Each sequence's records, point lists, carried state and frame_pose are those of
+ * running it alone through vo_seq_begin / vo_seq_push (the same kernels on its own units), bit for bit.
+ *   vo_mseq_begin   starts n_seq sequences from their first pairs left0[q] / right0[q] (channels 1 = gray, 3 = BGR, as
+ *                   vo_seq_begin_ex; one pitch for all images)
+ *   vo_mseq_submit  asynchronous: advances every live sequence by one frame.  left1[q] == right1[q] == NULL retires
+ *                   sequence q for the rest of the run (sequences of unequal length): its state and frame_pose freeze and
+ *                   its units do no tracking or pose work from then on.  At most two submissions may be in flight, as with
+ *                   vo_seq_submit (the front stage of submission k+1 runs under the pose solve of submission k).
+ *   vo_mseq_wait    waits for the oldest submission: out[q] as vo_seq_wait's record, status[q] = VO_OK, VO_E_CAPACITY
+ *                   (that sequence's glue capacity bits, see vo_last_error) or VO_MSEQ_RETIRED (out[q] zeroed), and
+ *                   frame_pose of each live sequence integrated under the main loop's gates.  pts4 is optional:
+ *                   n_seq x 4 x pts_cap points, the four lists of sequence q from pts4 + 4 * pts_cap * q.  Returns
+ *                   VO_E_CAPACITY when a status is, else VO_OK; every record is filled either way.
+ *   vo_mseq_pose / vo_mseq_state   vo_seq_pose / vo_seq_state of sequence q
+ * Refused with VO_E_INVALID: n_seq < 1, a third submission in flight, a wait with nothing in flight, a pair with one NULL
+ * image, a pair for a retired sequence.  VO_E_UNSUPPORTED: the option "mono_rotation" is on.  VO_E_CAPACITY: n_seq above
+ * VO_MSEQ_MAX.  Device-memory inputs (vo_dimage) are not accepted in this mode.
+ * Starting either sequence mode ends the other one if it is idle and is refused while it has frames in flight; the
+ * vo_seq_* frame calls are refused while vo_mseq_* sequences run and the other way round.  Every other entry point that
+ * reuses the shared buffers is refused while submissions are in flight, as for vo_seq_submit. */
+#define VO_MSEQ_MAX 64
+#define VO_MSEQ_RETIRED 2        /* vo_mseq_wait status: the sequence was retired by this or an earlier submission */
+VO_API int vo_mseq_begin(vo_ctx* ctx, int n_seq, int w, int h, const float P_l[12], const float P_r[12], const uint8_t* const* left0,
+                         const uint8_t* const* right0, size_t pitch, int channels);
+VO_API int vo_mseq_submit(vo_ctx* ctx, const uint8_t* const* left1, const uint8_t* const* right1, size_t pitch, int channels);
+VO_API int vo_mseq_wait(vo_ctx* ctx, vo_unit_result* out, int* status, vo_point2f* pts4, int pts_cap);
+VO_API int vo_mseq_pose(vo_ctx* ctx, int q, double frame_pose[16]);
+VO_API int vo_mseq_state(vo_ctx* ctx, int q, vo_point2f* points, int32_t* ages, int cap, int* n_points, int* n_ages, double t_out[3]);
+
 /* ---- image ingest (SURVEY.md 8f, row N3) ---------------------------------------------------------------
  * What loadImageLeft / loadImageRight do (reference src/utils.cpp:172-190): read <dir>/image_0/%06d.png and
  * <dir>/image_1/%06d.png with cv::imread(IMREAD_COLOR) and cvtColor(BGR2GRAY).  The decoder is host code

@@ -1,0 +1,144 @@
+#!/usr/bin/env python
+"""Scaling of the multi-sequence streaming mode (vo_mseq_*) with the number of sequences, measured on the GPU.
+
+    python tools/mseq_timing.py [--frames 40] [--rounds 5] [--counts 1,2,4,8,16,32] [--json out.json]
+
+Synthetic 1241x376 drives (synth.stereo_unit; eight seeds, each with its own motion) of `--frames` frames each;
+sequence q replays drive q % 8, forwards for even q // 8 and backwards for odd, so up to 16 sequences are distinct and
+larger counts repeat them (the work per sequence is the same either way).  One context runs, alternated round by round:
+  - "seq": the single-sequence mode, vo_seq_submit / vo_seq_wait with two frames in flight
+  - n_seq = each count: vo_mseq_submit / vo_mseq_wait with two submissions in flight
+and reports per mode the median over the rounds of the aggregate frames/s (sequence-frames per second of wall time), the
+per-step latency (wall time per submission in the pipelined loop) and the kernel launches per submission
+(vo_kernel_launches).  The card's name, power limit and max SM clock, read in the same run, are printed with the numbers;
+they are part of them."""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+from concurrent.futures import ProcessPoolExecutor
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import numpy as np
+
+W, H, DRIVES = 1241, 376, 8
+
+
+def card():
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        return out or "unknown"
+    except Exception:
+        return "unknown (nvidia-smi unavailable)"
+
+
+def motion(d):
+    rng = np.random.default_rng(100 + d)
+    return rng.uniform(-0.004, 0.004, 3) * np.array([1.0, 1.0, 0.25]), np.array([0.0, 0.0, -0.2]) + rng.uniform(-0.02, 0.02, 3)
+
+
+def render(job):
+    from visual_odom_b200 import synth
+    d, k = job
+    r, t = motion(d)
+    u = synth.stereo_unit(W, H, 50 + d, rvec=r * k, tvec=t * k)
+    return (u["l0"], u["r0"]) if k == 0 else (u["l1"], u["r1"])
+
+
+def drives(n_frames):
+    """[drive][frame] = (left, right), rendered in parallel (one synth call per frame)."""
+    jobs = [(d, k) for d in range(DRIVES) for k in range(n_frames)]
+    with ProcessPoolExecutor(max_workers=min(32, os.cpu_count() or 1)) as ex:
+        pairs = list(ex.map(render, jobs, chunksize=4))
+    return [pairs[d * n_frames:(d + 1) * n_frames] for d in range(DRIVES)]
+
+
+def sequence(dr, q):
+    fr = dr[q % DRIVES]
+    return fr if (q // DRIVES) % 2 == 0 else fr[::-1]
+
+
+def run_seq(ctx, P_l, P_r, fr):
+    ctx.seq_begin(fr[0][0], fr[0][1], P_l, P_r)
+    l0 = ctx.kernel_launches()
+    t0 = time.perf_counter()
+    ctx.seq_submit(*fr[1])
+    for k in range(1, len(fr)):
+        if k + 1 < len(fr):
+            ctx.seq_submit(*fr[k + 1])
+        ctx.seq_wait(want_points=False)
+    dt = time.perf_counter() - t0
+    steps = len(fr) - 1
+    return steps / dt, dt / steps, (ctx.kernel_launches() - l0) / steps
+
+
+def run_mseq(ctx, P_l, P_r, seqs):
+    n, nf = len(seqs), len(seqs[0])
+    ctx.mseq_begin([s[0][0] for s in seqs], [s[0][1] for s in seqs], P_l, P_r)
+    frame = [([s[k][0] for s in seqs], [s[k][1] for s in seqs]) for k in range(nf)]
+    l0 = ctx.kernel_launches()
+    t0 = time.perf_counter()
+    ctx.mseq_submit(*frame[1])
+    for k in range(1, nf):
+        if k + 1 < nf:
+            ctx.mseq_submit(*frame[k + 1])
+        ctx.mseq_wait(want_points=False)
+    dt = time.perf_counter() - t0
+    steps = nf - 1
+    return n * steps / dt, dt / steps, (ctx.kernel_launches() - l0) / steps
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("--frames", type=int, default=40)
+    ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--counts", default="1,2,4,8,16,32")
+    ap.add_argument("--json", help="also write the result here")
+    a = ap.parse_args()
+    counts = [int(c) for c in a.counts.split(",")]
+    from visual_odom_b200 import capi, synth
+    P_l, P_r = synth.proj_matrices()
+    t0 = time.perf_counter()
+    dr = drives(a.frames + 1)
+    print(f"rendered {DRIVES} drives x {a.frames + 1} frames in {time.perf_counter() - t0:.0f} s", flush=True)
+    ctx = capi.Context(0, max_features=4096)
+    modes = ["seq"] + counts
+    seqs = {n: [sequence(dr, q) for q in range(n)] for n in counts}
+    res = {m: dict(fps=[], lat=[], launches=[]) for m in modes}
+
+    def run(m, fr_cut=None):
+        if m == "seq":
+            fr = dr[0] if fr_cut is None else dr[0][:fr_cut]
+            return run_seq(ctx, P_l, P_r, fr)
+        s = seqs[m] if fr_cut is None else [x[:fr_cut] for x in seqs[m]]
+        return run_mseq(ctx, P_l, P_r, s)
+
+    for _ in range(a.rounds):
+        for m in modes:
+            run(m, 4)                     # warm-up: (re-)captures the mode's graphs, untimed
+            fps, lat, launches = run(m)
+            res[m]["fps"].append(fps); res[m]["lat"].append(lat); res[m]["launches"].append(launches)
+    ctx.close()
+    out = dict(card=card(), image=f"{W}x{H}", frames=a.frames, rounds=a.rounds, in_flight=2, modes={})
+    print(f"card (name, power limit, max SM clock): {out['card']}")
+    for m in modes:
+        r = res[m]
+        o = dict(aggregate_fps=float(np.median(r["fps"])), aggregate_fps_min=float(np.min(r["fps"])),
+                 aggregate_fps_max=float(np.max(r["fps"])), step_latency_ms=1e3 * float(np.median(r["lat"])),
+                 launches_per_submission=float(np.median(r["launches"])))
+        out["modes"][str(m)] = o
+        name = "vo_seq (1 sequence)" if m == "seq" else f"vo_mseq n_seq = {m:2d}"
+        print(f"{name:22s}: {o['aggregate_fps']:8.0f} frames/s [{o['aggregate_fps_min']:.0f}, {o['aggregate_fps_max']:.0f}], "
+              f"step {o['step_latency_ms']:.3f} ms, {o['launches_per_submission']:.1f} launches / submission")
+    print(json.dumps(out))
+    if a.json:
+        os.makedirs(os.path.dirname(os.path.abspath(a.json)), exist_ok=True)
+        with open(a.json, "w") as f:
+            json.dump(out, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()

@@ -1,0 +1,117 @@
+#!/usr/bin/env python
+"""Several KITTI sequences that share one calibration through ONE context (the multi-sequence mode, vo_mseq_*):
+
+    python tools/run_sequences.py /data/kitti/sequences/00/ /data/kitti/sequences/02/ calibration/kitti00.yaml \\
+        --poses out/ [--gt /data/kitti/poses/]
+
+Every <dataset>/image_0/%06d.png and image_1/%06d.png is decoded ahead by its own library reader into pinned buffers; one
+submission advances every sequence by one frame (two submissions in flight), and a sequence is retired at its last
+frame, so sequences of unequal length share the run.  frame_pose of each is integrated with the reference's Euler and
+scale gates (src/main.cpp:196-208), written to OUTDIR/<name>.txt in the KITTI text format (<name> = the dataset
+directory's name) and, with --gt, scored against GTDIR/<name>.txt with the KITTI segment metric.  All sequences must
+have the image size of the first.  `--check` only validates the inputs (no GPU needed)."""
+import argparse
+import os
+import sys
+import time
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import numpy as np
+
+from run_sequence import count_frames, read_calibration
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("datasets", nargs="+", metavar="DIR")
+    ap.add_argument("calibration")
+    ap.add_argument("--poses", required=True, metavar="OUTDIR", help="write OUTDIR/<name>.txt per sequence (KITTI format)")
+    ap.add_argument("--gt", metavar="GTDIR", help="score each sequence against GTDIR/<name>.txt")
+    ap.add_argument("--threads", type=int, default=4, help="decoder threads per sequence")
+    ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--check", action="store_true")
+    a = ap.parse_args()
+    from visual_odom_b200 import capi, synth
+    cal = read_calibration(a.calibration)
+    P_l, P_r = synth.proj_matrices(cal)
+    if len(a.datasets) > capi.VO_MSEQ_MAX:
+        raise SystemExit(f"{len(a.datasets)} sequences: one context runs at most {capi.VO_MSEQ_MAX}")
+    names = [os.path.basename(os.path.normpath(d)) for d in a.datasets]
+    if len(set(names)) != len(names):
+        raise SystemExit(f"two datasets share a directory name ({names}): their pose files would collide")
+    seqs = []
+    for d, name in zip(a.datasets, names):
+        n = count_frames(d, 0)
+        if n < 2:
+            raise SystemExit(f"{d}: need at least two stereo pairs (image_0/%06d.png, image_1/%06d.png from 0)")
+        w, h, ctype, depth = capi.png_info(open(os.path.join(d, "image_0", "%06d.png" % 0), "rb").read())
+        if seqs and (w, h) != (seqs[0]["w"], seqs[0]["h"]):
+            raise SystemExit(f"{d}: {w}x{h} images, {a.datasets[0]} has {seqs[0]['w']}x{seqs[0]['h']}: "
+                             "one context runs one image size (group the sequences by size)")
+        gt = os.path.join(a.gt, name + ".txt") if a.gt else None
+        if gt and not os.path.exists(gt):
+            raise SystemExit(f"{gt}: no ground truth for sequence {name}")
+        seqs.append(dict(dir=d, name=name, n=n, w=w, h=h, gray=ctype == 0, gt=gt))
+        print(f"{name}: {n} stereo pairs of {w}x{h} (PNG colour type {ctype}, {depth} bit)")
+    print(f"P_left =\n{P_l}\nP_right =\n{P_r}")
+    if a.check:
+        return
+    # one pitch and one channel count per submission: colour files are read as BGR (converted on the device) unless the
+    # sequences mix gray and colour files, then all are converted to gray while decoding
+    force = 0 if len({s["gray"] for s in seqs}) == 1 else 1
+    ctx = capi.Context(a.device, max_features=4096)
+    rds = [capi.SequenceReader(s["dir"], 0, s["n"], threads=a.threads, depth=a.threads + 3, force_channels=force) for s in seqs]
+
+    def pairs(k):
+        """pointers of frame k of every sequence (None past a sequence's last frame), pitch, channels"""
+        lp, rp, fmt = [], [], set()
+        for s, rd in zip(seqs, rds):
+            if k >= s["n"]:
+                lp.append(None); rp.append(None)
+                continue
+            l, r, _, _, pitch, ch, _ = rd.next_ptr()
+            lp.append(l); rp.append(r); fmt.add((pitch, ch))
+        if len(fmt) > 1:
+            raise SystemExit(f"frame {k}: the readers deliver different layouts {sorted(fmt)}")
+        pitch, ch = fmt.pop() if fmt else (seqs[0]["w"], 1)
+        return lp, rp, pitch, ch
+
+    lp, rp, pitch, ch = pairs(0)
+    ctx.mseq_begin_ptr(seqs[0]["w"], seqs[0]["h"], lp, rp, pitch, P_l, P_r, ch)
+    poses = [[np.eye(4)] for _ in seqs]
+    steps = max(s["n"] for s in seqs)
+    t0 = time.perf_counter()
+    done = 0
+    ctx.mseq_submit_ptr(*pairs(1))
+    for k in range(1, steps):
+        if k + 1 < steps:
+            ctx.mseq_submit_ptr(*pairs(k + 1))
+        recs = ctx.mseq_wait(want_points=False)
+        for q, r in enumerate(recs):
+            if r["status"] == capi.VO_MSEQ_RETIRED:
+                continue
+            if r["status"] != capi.VO_OK:
+                print(f"{seqs[q]['name']} frame {k}: status {r['status']} ({ctx.lib.vo_last_error(ctx.h).decode()})")
+            poses[q].append(ctx.mseq_pose(q))
+            done += 1
+        if k % 100 == 0 or k == steps - 1:
+            print(f"step {k}: {done} sequence-frames, {done / (time.perf_counter() - t0):.0f} frames/s")
+    for rd in rds:
+        rd.close()
+    ctx.close()
+    os.makedirs(a.poses, exist_ok=True)
+    for s, p in zip(seqs, poses):
+        path = os.path.join(a.poses, s["name"] + ".txt")
+        capi.poses_save(path, p)
+        line = f"{s['name']}: {len(p)} poses -> {path}"
+        if s["gt"]:
+            gt = capi.poses_load(s["gt"])[:len(p)]
+            seg, t_err, r_err = capi.eval_segments(gt, p[:len(gt)])
+            line += (", ground-truth path shorter than the 100 m minimum segment" if len(seg) == 0 else
+                     f", KITTI metric over {len(seg)} segments: t_err {100 * t_err:.2f} %, r_err {r_err * 180 / np.pi * 100:.4f} deg / 100 m")
+        print(line)
+
+
+if __name__ == "__main__":
+    main()

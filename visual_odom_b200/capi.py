@@ -19,6 +19,8 @@ VO_E_TOO_FEW_POINTS = -3
 VO_E_UNSUPPORTED = -4
 VO_DIST_DEPTH = 8          # gathers that may be outstanding (include/vo_b200.h)
 VO_E_CAPACITY = -5
+VO_MSEQ_MAX = 64           # sequences one vo_mseq_begin may start (include/vo_b200.h)
+VO_MSEQ_RETIRED = 2        # vo_mseq_wait status of a retired sequence
 
 
 class VoParams(C.Structure):
@@ -172,6 +174,13 @@ SIGNATURES = {
     "vo_seq_begin_device": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(VoDImage), C.POINTER(VoDImage)]),
     "vo_seq_submit_device": (C.c_int, [C.c_void_p, C.POINTER(VoDImage), C.POINTER(VoDImage)]),
     "vo_batch_submit_device": (C.c_int, [C.c_void_p, C.POINTER(VoDUnit), C.c_int, C.c_int]),
+    "vo_mseq_begin": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                C.c_int]),
+    "vo_mseq_submit": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
+    "vo_mseq_wait": (C.c_int, [C.c_void_p, C.POINTER(VoUnitResult), C.c_void_p, C.c_void_p, C.c_int]),
+    "vo_mseq_pose": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
+    "vo_mseq_state": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                C.c_void_p]),
 }
 
 _lib = None
@@ -678,6 +687,99 @@ class Context:
         pose = np.zeros((4, 4))
         self._check(self.lib.vo_seq_pose(self.h, _p(pose)))
         return pose
+
+    # ---- several sequences in lockstep (vo_mseq_*) --------------------------------------------------------------------
+    @staticmethod
+    def _pairs(lefts, rights, allow_none):
+        """(left pointer table, right pointer table, pitch, channels, keep-alive) of one image per sequence: gray H x W or
+        BGR H x W x 3, all of one shape and pitch; a None pair (allow_none) is passed as two NULL pointers."""
+        if len(lefts) != len(rights):
+            raise ValueError(f"{len(lefts)} left and {len(rights)} right images")
+        n = len(lefts)
+        lp, rp = (C.c_void_p * n)(), (C.c_void_p * n)()
+        keep, geom = [], None
+        for q, (l, r) in enumerate(zip(lefts, rights)):
+            if l is None and r is None and allow_none:
+                continue
+            if l is None or r is None:
+                raise ValueError(f"sequence {q}: a pair needs both images (None, None retires a sequence)")
+            l = np.asarray(l); r = np.asarray(r)
+            if l.dtype != np.uint8 or l.ndim not in (2, 3) or (l.ndim == 3 and l.shape[2] != 3):
+                raise ValueError(f"sequence {q}: images must be uint8 H x W (gray) or H x W x 3 (BGR)")
+            l = np.ascontiguousarray(l); r = np.ascontiguousarray(r)
+            if geom is None:
+                geom = l.shape
+            if l.shape != geom or r.shape != geom:
+                raise ValueError(f"sequence {q}: image shape {l.shape} / {r.shape}, expected {geom}")
+            keep += [l, r]
+            lp[q], rp[q] = l.ctypes.data, r.ctypes.data
+        if geom is None:
+            return lp, rp, 0, 1, keep, None
+        ch = 1 if len(geom) == 2 else 3
+        return lp, rp, geom[1] * ch, ch, keep, geom
+
+    def mseq_begin(self, lefts, rights, P_l, P_r):
+        """Start len(lefts) sequences (one calibration, one image size) from their first stereo pairs."""
+        lp, rp, pitch, ch, keep, geom = self._pairs(lefts, rights, False)
+        P_l = np.ascontiguousarray(P_l, np.float32).reshape(12); P_r = np.ascontiguousarray(P_r, np.float32).reshape(12)
+        h, w = (geom or (0, 0))[:2]
+        self._check(self.lib.vo_mseq_begin(self.h, len(lefts), w, h, _p(P_l), _p(P_r), lp, rp, pitch, ch))
+        self._mseq_n, self._mseq_pitch = len(lefts), pitch
+        self._mseq_keep = [None, None]
+
+    def mseq_begin_ptr(self, w, h, left_ptrs, right_ptrs, pitch, P_l, P_r, channels=1):
+        """Raw host pointers, one pair per sequence (e.g. the pinned buffers of one SequenceReader each)."""
+        n = len(left_ptrs)
+        lp, rp = (C.c_void_p * n)(*left_ptrs), (C.c_void_p * n)(*right_ptrs)
+        Pl = np.ascontiguousarray(P_l, np.float32); Pr = np.ascontiguousarray(P_r, np.float32)
+        self._check(self.lib.vo_mseq_begin(self.h, n, w, h, _p(Pl), _p(Pr), lp, rp, pitch, channels))
+        self._mseq_n, self._mseq_pitch = n, pitch
+        self._mseq_keep = [None, None]
+
+    def mseq_submit_ptr(self, left_ptrs, right_ptrs, pitch, channels=1):
+        """Raw host pointers; None in both lists retires that sequence.  The memory must stay valid until the wait."""
+        n = len(left_ptrs)
+        lp, rp = (C.c_void_p * n)(*left_ptrs), (C.c_void_p * n)(*right_ptrs)
+        self._check(self.lib.vo_mseq_submit(self.h, lp, rp, pitch, channels))
+
+    def mseq_submit(self, lefts, rights):
+        """Asynchronous: one frame of every sequence; a (None, None) pair retires that sequence.  At most two submissions
+        in flight.  The arrays are kept alive by the context until their submission has been waited for."""
+        lp, rp, pitch, ch, keep, _ = self._pairs(lefts, rights, True)
+        if len(lefts) != getattr(self, "_mseq_n", len(lefts)):
+            raise ValueError(f"{len(lefts)} pairs for {self._mseq_n} sequences")
+        # with every sequence retired no image is read: the pitch of the first pairs passes the width check
+        self._check(self.lib.vo_mseq_submit(self.h, lp, rp, pitch or self._mseq_pitch, ch))
+        self._mseq_keep = [self._mseq_keep[1], keep]
+
+    def mseq_wait(self, pts_cap=4096, want_points=True):
+        """The oldest submission: one dict per sequence with seq_wait's keys plus "status" (VO_OK, VO_E_CAPACITY or
+        VO_MSEQ_RETIRED)."""
+        n = self._mseq_n
+        res = (VoUnitResult * n)()
+        st = np.zeros(n, np.int32)
+        pts4 = np.zeros((n, 4, pts_cap, 2), np.float32) if want_points else None
+        self._check(self.lib.vo_mseq_wait(self.h, res, _p(st), _p(pts4), pts_cap if want_points else 0), ok=(VO_OK, VO_E_CAPACITY))
+        out = []
+        for q in range(n):
+            d = self._result_dict(res[q])
+            d["status"] = int(st[q])
+            if want_points:
+                m = min(d["n_valid"], pts_cap) if d["status"] != VO_MSEQ_RETIRED else 0
+                d.update(l0=pts4[q, 0, :m].copy(), r0=pts4[q, 1, :m].copy(), l1=pts4[q, 2, :m].copy(), r1=pts4[q, 3, :m].copy())
+            out.append(d)
+        return out
+
+    def mseq_pose(self, q):
+        pose = np.zeros((4, 4))
+        self._check(self.lib.vo_mseq_pose(self.h, int(q), _p(pose)))
+        return pose
+
+    def mseq_state(self, q, cap=1 << 17):
+        pts = np.zeros((cap, 2), np.float32); ages = np.zeros(cap, np.int32); t = np.zeros(3)
+        npts = C.c_int(); nages = C.c_int()
+        self._check(self.lib.vo_mseq_state(self.h, int(q), _p(pts), _p(ages), cap, C.byref(npts), C.byref(nages), _p(t)))
+        return pts[:npts.value].copy(), ages[:nages.value].copy(), t
 
 
 # ---- host-only pose bookkeeping (SURVEY.md 8f row N2; no GPU needed) ------------------------------------------------

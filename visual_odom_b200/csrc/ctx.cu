@@ -321,6 +321,9 @@ void vo_free_state(vo_ctx* ctx)
     vo_drop_graphs(ctx);
     for (void* p : ctx->allocs) cudaFree(p);
     ctx->allocs.clear();
+    if (ctx->d_seq_state) cudaFree(ctx->d_seq_state);
+    ctx->d_seq_state = nullptr; ctx->seq_n_cap = 0;
+    ctx->d_feat_pts = nullptr; ctx->d_feat_ages = nullptr; ctx->d_feat_cnt = ctx->d_bucket = ctx->d_seq_err = ctx->d_seq_live = nullptr;
     ctx->d_out = nullptr; ctx->out_stride = 0; ctx->out_per = 0;
     ctx->w = ctx->h = ctx->units = 0;
 }
@@ -463,13 +466,8 @@ int vo_ensure_state(vo_ctx* ctx, int w, int h, int units, int /*imgs_per_unit*/)
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_counts, (size_t)units * its));
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_inliers, uc));
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_results, (size_t)units));
-    // sequence mode state
+    // sequence mode state: sized per sequence at vo_seq_begin / vo_mseq_begin (seq_api.cu)
     ctx->feat_cap = ctx->corner_cap + cap;
-    VO_CUDA_CHECK(dalloc(ctx, &ctx->d_feat_pts, (size_t)ctx->feat_cap));
-    VO_CUDA_CHECK(dalloc(ctx, &ctx->d_feat_ages, (size_t)ctx->feat_cap));
-    VO_CUDA_CHECK(dalloc(ctx, &ctx->d_feat_cnt, (size_t)2));
-    VO_CUDA_CHECK(dalloc(ctx, &ctx->d_bucket, (size_t)ctx->bucket_cap));
-    VO_CUDA_CHECK(dalloc(ctx, &ctx->d_seq_err, (size_t)4));     // [0] sticky bits, [1 + unit] per-frame copy
     ctx->seq_active = false;
     VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_results, 0, (size_t)units * sizeof(vo_unit_result_dev), ctx->stream));
     VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_tprev, 0, (size_t)units * 3 * sizeof(double), ctx->stream));

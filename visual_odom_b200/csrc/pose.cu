@@ -95,6 +95,7 @@ extern "C" int vo_pose_step(double frame_pose[16], const double R[9], const doub
 extern "C" int vo_seq_pose(vo_ctx* ctx, double frame_pose[16])
 {
     if (!ctx || !ctx->seq_active || !frame_pose) return VO_E_INVALID;
-    memcpy(frame_pose, ctx->seq_pose, sizeof(ctx->seq_pose));
+    if (ctx->seq_multi) { vo_set_error(ctx, "vo_seq_pose: the sequences were begun with vo_mseq_begin; use vo_mseq_pose"); return VO_E_INVALID; }
+    memcpy(frame_pose, ctx->seq_pose.data(), 16 * sizeof(double));
     return VO_OK;
 }

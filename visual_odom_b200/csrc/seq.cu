@@ -11,16 +11,23 @@
 //        refused, a full one-slot cell is overwritten: the LAST admitted feature in input order wins
 //   the ages / points length skew after the circular check (src/visualOdometry.cpp:122-127): point i is
 //        paired with ages[i] even though the ages vector is longer and shifted.
+//
+// Each kernel serves n_seq independent sequences in one launch (blockIdx.y = sequence, strides in SeqArgs); the
+// single-sequence mode launches them with n_seq = 1.
 #include "common.cuh"
 #include "seq.h"
 
 __global__ void __launch_bounds__(1024) k_seq_append(const float2* __restrict__ corners, const int* __restrict__ n_det,
                                                      int corner_cap, float2* feat_pts, int* feat_ages, int* cnt, int feat_cap,
-                                                     int refill_below, int* err)
+                                                     int refill_below, int* err, const int* __restrict__ live)
 {
+    const int q = blockIdx.y;
+    corners += (size_t)q * corner_cap; n_det += q; feat_pts += (size_t)q * feat_cap; feat_ages += (size_t)q * feat_cap;
+    cnt += 2 * q; err += q;
     // the error bits are per frame: this is the first glue kernel of a frame's front stage, it clears the frame's word
     if (threadIdx.x == 0) *err = 0;
     __syncthreads();
+    if (!live[q]) return;                              // retired: the state stays as it is
     const int n_pts = cnt[0], n_ages = cnt[1];
     if (n_pts >= refill_below) return;                 // `if (currentVOFeatures.size() < 2000)`
     int m = *n_det;
@@ -35,10 +42,15 @@ __global__ void __launch_bounds__(1024) k_seq_append(const float2* __restrict__ 
 }
 
 __global__ void __launch_bounds__(1024) k_seq_bucket(const float2* __restrict__ feat_pts, const int* __restrict__ feat_ages,
-                                                     const int* __restrict__ cnt, int rows, int cols, int bucket_size,
+                                                     int feat_cap, const int* __restrict__ cnt, int rows, int cols, int bucket_size,
                                                      int* bucket /* [nb] scratch */, int nb_cap,
-                                                     float2* out_pts, int* out_ages, int* out_n, int out_cap, int* err)
+                                                     float2* out_pts, int* out_ages, int* out_n, int out_cap, int* err,
+                                                     const int* __restrict__ live)
 {
+    const int q = blockIdx.y;
+    feat_pts += (size_t)q * feat_cap; feat_ages += (size_t)q * feat_cap; cnt += 2 * q; bucket += (size_t)q * nb_cap;
+    out_pts += (size_t)q * out_cap; out_ages += (size_t)q * out_cap; out_n += q; err += q;
+    if (!live[q]) { if (threadIdx.x == 0) *out_n = 0; return; }        // retired: no features, so no work downstream
     const int nh = rows / bucket_size, nw = cols / bucket_size;
     const int nb = (nh + 1) * (nw + 1);
     if (nb > nb_cap) { if (threadIdx.x == 0) { atomicOr(err, 4); *out_n = 0; } return; }
@@ -89,8 +101,13 @@ __global__ void __launch_bounds__(1024) k_seq_bucket(const float2* __restrict__ 
 // (src/visualOdometry.cpp:122-127).  Runs before the pose solve, so the next frame's front half can start under it.
 __global__ void __launch_bounds__(256) k_seq_carry(const float2* __restrict__ valid_l1, const int* __restrict__ n5,
                                                    const int* __restrict__ ages_out, const int* __restrict__ n3,
-                                                   float2* feat_pts, int* feat_ages, int* cnt)
+                                                   int cap, float2* feat_pts, int* feat_ages, int feat_cap, int* cnt,
+                                                   const int* __restrict__ live)
 {
+    const int q = blockIdx.y;
+    if (!live[q]) return;
+    valid_l1 += (size_t)q * cap; n5 += q; ages_out += (size_t)q * cap; n3 += q;
+    feat_pts += (size_t)q * feat_cap; feat_ages += (size_t)q * feat_cap; cnt += 2 * q;
     const int np = *n5, na = *n3;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < max(np, na); i += gridDim.x * blockDim.x) {
         if (i < np) feat_pts[i] = valid_l1[i];
@@ -100,10 +117,16 @@ __global__ void __launch_bounds__(256) k_seq_carry(const float2* __restrict__ va
 }
 
 // after the pose solve: `translation` carries the solved tvec to the next frame's solve; counts into the result record
-__global__ void k_seq_finish(vo_unit_result_dev* res, double* tprev_next, const int* __restrict__ n_feat,
-                             const int* __restrict__ n_det, const int* __restrict__ n3, const int* __restrict__ n5,
-                             const int* __restrict__ err, int* err_out)
+__global__ void k_seq_finish(vo_unit_result_dev* res, double* tprev_next, const double* __restrict__ tprev_cur,
+                             const int* __restrict__ n_feat, const int* __restrict__ n_det, const int* __restrict__ n3,
+                             const int* __restrict__ n5, const int* __restrict__ err, int* err_out, const int* __restrict__ live)
 {
+    const int q = blockIdx.y;
+    res += q; tprev_next += 3 * q; tprev_cur += 3 * q; n_feat += q; n_det += q; n3 += q; n5 += q; err += q; err_out += q;
+    if (!live[q]) {                                    // retired: the translation stays frozen in both buffer slots
+        if (threadIdx.x < 3) tprev_next[threadIdx.x] = tprev_cur[threadIdx.x];
+        return;
+    }
     if (threadIdx.x == 0) {
         for (int k = 0; k < 3; k++) tprev_next[k] = res->tvec[k];
         res->n_features = *n_feat; res->n_detected = *n_det; res->n_tracked = *n3; res->n_valid = *n5;
@@ -119,25 +142,27 @@ __global__ void k_seq_mono(vo_unit_result_dev* res, const EssResult* __restrict_
     if (k < 9) res->R[k] = ess->status == ESS_OK ? ess->R[k] : (k % 4 == 0 ? 1.0 : 0.0);
 }
 
-int vo_launch_seq_append(const SeqArgs& a, cudaStream_t s)
+int vo_launch_seq_append(const SeqArgs& a, int n_seq, cudaStream_t s)
 {
-    k_seq_append<<<1, 1024, 0, s>>>(a.corners, a.n_det, a.corner_cap, a.feat_pts, a.feat_ages, a.cnt, a.feat_cap, a.refill_below, a.err);
+    k_seq_append<<<dim3(1, n_seq), 1024, 0, s>>>(a.corners, a.n_det, a.corner_cap, a.feat_pts, a.feat_ages, a.cnt, a.feat_cap,
+                                                 a.refill_below, a.err, a.live);
     return 1;
 }
-int vo_launch_seq_bucket(const SeqArgs& a, cudaStream_t s)
+int vo_launch_seq_bucket(const SeqArgs& a, int n_seq, cudaStream_t s)
 {
-    k_seq_bucket<<<1, 1024, 0, s>>>(a.feat_pts, a.feat_ages, a.cnt, a.rows, a.cols, a.bucket_size, a.bucket, a.bucket_cap,
-                                    a.out_pts, a.out_ages, a.out_n, a.out_cap, a.err);
+    k_seq_bucket<<<dim3(1, n_seq), 1024, 0, s>>>(a.feat_pts, a.feat_ages, a.feat_cap, a.cnt, a.rows, a.cols, a.bucket_size,
+                                                 a.bucket, a.bucket_cap, a.out_pts, a.out_ages, a.out_n, a.out_cap, a.err, a.live);
     return 1;
 }
-int vo_launch_seq_carry(const SeqArgs& a, cudaStream_t s)
+int vo_launch_seq_carry(const SeqArgs& a, int n_seq, cudaStream_t s)
 {
-    k_seq_carry<<<8, 256, 0, s>>>(a.valid_l1, a.n5, a.ages_out, a.n3, a.feat_pts, a.feat_ages, a.cnt);
+    k_seq_carry<<<dim3(8, n_seq), 256, 0, s>>>(a.valid_l1, a.n5, a.ages_out, a.n3, a.out_cap, a.feat_pts, a.feat_ages, a.feat_cap,
+                                               a.cnt, a.live);
     return 1;
 }
-int vo_launch_seq_finish(const SeqArgs& a, cudaStream_t s)
+int vo_launch_seq_finish(const SeqArgs& a, int n_seq, cudaStream_t s)
 {
-    k_seq_finish<<<1, 32, 0, s>>>(a.res, a.tprev, a.out_n, a.n_det, a.n3, a.n5, a.err, a.err_out);
+    k_seq_finish<<<dim3(1, n_seq), 32, 0, s>>>(a.res, a.tprev, a.tprev_cur, a.out_n, a.n_det, a.n3, a.n5, a.err, a.err_out, a.live);
     return 1;
 }
 int vo_launch_seq_mono(vo_unit_result_dev* res, const EssResult* ess, cudaStream_t s)

@@ -4,6 +4,9 @@
 #include "pnp.h"
 #include "ess.h"
 
+// The pointers are those of sequence 0; one launch covers n_seq sequences (blockIdx.y = q) and finds sequence q's part of
+// each array `stride` elements further on: corner_cap (corners), feat_cap (feat_pts, feat_ages), 2 (cnt), bucket_cap
+// (bucket), out_cap (out_pts, out_ages, valid_l1, ages_out), 3 (tprev, tprev_cur), 1 (everything else).
 struct SeqArgs {
     // append
     const float2* corners; const int* n_det; int corner_cap;
@@ -13,14 +16,16 @@ struct SeqArgs {
     float2* out_pts; int* out_ages; int* out_n; int out_cap;
     // update
     const float2* valid_l1; const int* n5; const int* ages_out; const int* n3;
-    vo_unit_result_dev* res; double* tprev /* the NEXT frame's t_prev slot */;
+    vo_unit_result_dev* res; double* tprev /* the NEXT frame's t_prev slot */; const double* tprev_cur /* this frame's */;
     int* err; int* err_out /* per-frame copy of the sticky error bits, read back with the record */;
+    // 0 once the sequence is retired: its block writes no features (out_n = 0) and leaves its state and translation alone
+    const int* live;
 };
 
-int vo_launch_seq_append(const SeqArgs& a, cudaStream_t s);
-int vo_launch_seq_bucket(const SeqArgs& a, cudaStream_t s);
-int vo_launch_seq_carry(const SeqArgs& a, cudaStream_t s);
-int vo_launch_seq_finish(const SeqArgs& a, cudaStream_t s);
+int vo_launch_seq_append(const SeqArgs& a, int n_seq, cudaStream_t s);
+int vo_launch_seq_bucket(const SeqArgs& a, int n_seq, cudaStream_t s);
+int vo_launch_seq_carry(const SeqArgs& a, int n_seq, cudaStream_t s);
+int vo_launch_seq_finish(const SeqArgs& a, int n_seq, cudaStream_t s);
 // mono_rotation = true: the record's R becomes recoverPose's rotation (I where the branch aborted); everything else in
 // the record stays the PnP's
 int vo_launch_seq_mono(vo_unit_result_dev* res, const EssResult* ess, cudaStream_t s);
