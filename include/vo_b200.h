@@ -83,13 +83,18 @@ VO_API long long vo_kernel_launches(const vo_ctx* ctx);
  * measured with CUDA events on the launching stream; n = launches counted. */
 VO_API int vo_lk_kernel_time(vo_ctx* ctx, double* ms_total, long long* n, int reset);
 /* Run-time knobs (measurement / debugging): "batch_streams" = 1|2 (unit ranges the batched path runs
- * concurrently, default 2), "lk_staging" = 0 (TMA, default) | 1 (plain loads), "graphs" = 1 (default: kernel
- * sequences are replayed as CUDA graphs where that does not defeat the priority split) | 0 (plain launches; needed
- * for vo_lk_kernel_time), "priorities" = 1 (default: with several unit ranges in flight the short / latency-bound
- * kernels run on high-priority helper streams and only the LK ring at normal priority; such ranges are launched
- * plainly because captured graph nodes lose the stream priority) | 0, "batch_graphs" = 1 forces graphs for them,
- * "mono_rotation" = 0 (default) | 1: sequences begun from then on run trackingFrame2Frame(mono_rotation = true), see
- * vo_seq_wait_mono (a sequence keeps the value it was begun with). */
+ * concurrently, default 2), "lk_staging" = 0 (TMA, default) | 1 (plain loads), "lk_span" = phases (level-solves)
+ * per LK work item (0 = automatic, default), "graphs" = 1 (default: kernel sequences on the context's stream, and
+ * the two stages of a sequence frame, are replayed as CUDA graphs; unit ranges on the side streams of
+ * vo_frame_batch, vo_batch_run and vo_batch_submit are always launched plainly, because their kernels fork to the
+ * SM partition or to high-priority helper streams) | 0 (plain launches; needed for vo_lk_kernel_time),
+ * "sm_partition" = k > 0: the kernels after the LK ring (filters, triangulation, PnP) of side-stream ranges run on
+ * k SMs of their own while FAST, the pyramids and the LK ring share the others | 0: no partition, those kernels run
+ * on high-priority helper streams (k < 0 is refused with VO_E_INVALID; without the option the first
+ * vo_batch_submit sets aside 8 SMs when the driver supports green contexts), "batch_outputs" = 1: vo_batch_submit
+ * also copies the point lists back (vo_batch_outputs), "mono_rotation" = 0 (default) | 1: sequences begun from then
+ * on run trackingFrame2Frame(mono_rotation = true), see vo_seq_wait_mono (a sequence keeps the value it was begun
+ * with). */
 VO_API int vo_set_option(vo_ctx* ctx, const char* key, double value);
 
 /* ---- A1: cv::FAST(image, kps, threshold, nonmax) + KeyPoint::convert ------------------------

@@ -93,11 +93,8 @@ def test_frame_batch(pool, streams):
 SUBMIT_CONFIGS = {
     "partition-auto": {},
     "partition+8": {"sm_partition": 8},
-    "partition-8": {"sm_partition": -8},
-    "partition-off": {"sm_partition": 0},
-    "partition-off-priorities-0": {"sm_partition": 0, "priorities": 0},
+    "partition-off": {"sm_partition": 0},      # the high-priority helper streams
     "graphs-0": {"graphs": 0},
-    "batch_graphs-1": {"batch_graphs": 1},
 }
 
 
@@ -122,10 +119,14 @@ def test_two_submissions_in_flight(pool, name):
 
 def test_three_submissions_in_flight_and_resident_rerun(pool):
     """The benchmark's e2e loop: three ranges in flight, then a re-run of what is resident (units = NULL) submitted
-    while the other two are still in flight."""
+    while the other two are still in flight.  A negative SM count for the partition is refused and changes nothing."""
+    from visual_odom_b200.capi import VO_E_INVALID, VoError
     big = pool["big"]
     c = _context(batch_outputs=1)
     try:
+        with pytest.raises(VoError) as e:
+            c.set_option("sm_partition", -8)
+        assert e.value.code == VO_E_INVALID
         c.batch_configure(W, H, 3 * B, big[0]["units"][0]["P_l"], big[0]["units"][0]["P_r"])
         keep = [_submit(c, big[(j + 1) % 3], j * B) for j in range(3)]
         _check(c, 0, c.batch_wait(0, B), big[1], per=2048)

@@ -2,14 +2,11 @@
 (oracle/lk_ref.c, pinned to cv2 in test_oracle_lk.py).
 
 The default launch is what test_gpu_lk.py sees.  Here every configuration gets a fresh context and runs the same inputs:
-- k_lk_ring<true, 8 | 10 | 12> (lk_ctas_per_sm): at 10 and 12 CTAs per SM the packed I patch and the residuals are
-  parked in shared memory instead of registers;
-- k_lk_ring<false, 8> (lk_staging = 1): plain loads instead of TMA boxes;
+- k_lk_ring<true> (TMA boxes) and k_lk_ring<false> (lk_staging = 1: plain loads);
 - work items of 1, 2, 3, 5, 7 phases (lk_span): the running estimate and the progress counter are handed from item to
-  item, items straddle call boundaries, and an item may end mid-call;
-- retiring warps (lk_quota): the grid is larger than the resident set.
-The automatic span and the quota only apply to a launch with more features than resident warps; the tests check that
-their inputs are that large on the GPU they run on.  Consecutive configurations alternate between two input sets, so a
+  item, items straddle call boundaries, and an item may end mid-call.
+The automatic span only applies to a launch with more features than resident warps; the tests check that their inputs
+are that large on the GPU they run on.  Consecutive configurations alternate between two input sets, so a
 launch that skipped work cannot pass on what the previous context left in recycled device memory.
 """
 import numpy as np
@@ -23,7 +20,7 @@ W, H = 1241, 376
 N_FAST = 6000
 SPANS = (0, 1, 2, 3, 5, 7, 16)         # 0 = automatic
 LK_WARPS_PER_CTA = 2                   # visual_odom_b200/csrc/lk_ring.h
-DEFAULT_CPS = 8                        # LK_CTAS_PER_SM: also the plain-load instantiation
+LK_CTAS_PER_SM = 8
 
 
 def _border_points(w, h):
@@ -97,9 +94,8 @@ def _run(case, opts, need_big):
     try:
         for k, v in opts.items():
             c.set_option(k, v)
-        cps = DEFAULT_CPS if opts.get("lk_staging") else opts.get("lk_ctas_per_sm", DEFAULT_CPS)
-        resident_warps = torch.cuda.get_device_properties(0).multi_processor_count * cps * LK_WARPS_PER_CTA
-        if need_big:            # the automatic span / the quota only apply above the resident warps
+        resident_warps = torch.cuda.get_device_properties(0).multi_processor_count * LK_CTAS_PER_SM * LK_WARPS_PER_CTA
+        if need_big:            # the automatic span only applies above the resident warps
             assert len(case["pts"]) > resident_warps, (len(case["pts"]), resident_warps)
         ro, rs, re = case["single_ref"]
         go, gs, ge = c.lk_track(case["imgs"][0], case["imgs"][2], case["pts"])
@@ -114,13 +110,11 @@ def _run(case, opts, need_big):
         c.close()
 
 
-CONFIGS = ([dict(lk_ctas_per_sm=cps, lk_span=s) for cps in (8, 10, 12) for s in SPANS]
-           + [dict(lk_staging=1, lk_span=s) for s in SPANS]
-           + [dict(lk_ctas_per_sm=cps, lk_quota=q, lk_span=s) for cps in (8, 12) for q in (1, 7) for s in (0, 1, 3)])
+CONFIGS = [dict(lk_span=s) for s in SPANS] + [dict(lk_staging=1, lk_span=s) for s in SPANS]
 
 
 @pytest.mark.parametrize("i", range(len(CONFIGS)),
                          ids=["-".join(f"{k}={v}" for k, v in cfg.items()) for cfg in CONFIGS])
 def test_lk_variant_bit_exact(cases, i):
     cfg = CONFIGS[i]
-    _run(cases[i % 2], cfg, need_big=cfg["lk_span"] == 0 or cfg.get("lk_quota", 0) > 0)
+    _run(cases[i % 2], cfg, need_big=cfg["lk_span"] == 0)

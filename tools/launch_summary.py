@@ -9,7 +9,7 @@
 Run each workload in a process of its own.  The table also lists torch's own kernels (the bench loop's cache flush).  The
 last line compares the launches of the library's kernels (names `k_*`) the profiler saw with those the library counted:
 CUPTI may not report kernels launched into the SM partition's green contexts, and if the counts differ the table is
-partial -- rerun with VO_SM_PARTITION=0 (the context then never partitions the SMs) and say so beside it.
+partial -- rerun with VO_OPT_SM_PARTITION=0 (the context then never partitions the SMs) and say so beside it.
 `--trace FILE` keeps the Chrome trace; otherwise it goes to a temporary directory.
 """
 import argparse
@@ -118,7 +118,7 @@ def main():
         path = args.trace or os.path.join(tmp, "trace.json")
         prof.export_chrome_trace(path)
         agg = kernel_table(path)
-    print(f"{torch.cuda.get_device_name(0)}, workload {args.workload}, VO_SM_PARTITION={os.environ.get('VO_SM_PARTITION', 'default')}, "
+    print(f"{torch.cuda.get_device_name(0)}, workload {args.workload}, "
           f"VO_OPT_SM_PARTITION={os.environ.get('VO_OPT_SM_PARTITION', 'default')}")
     print_table(agg, launches)
 

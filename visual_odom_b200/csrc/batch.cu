@@ -114,7 +114,7 @@ extern "C" int vo_batch_configure(vo_ctx* ctx, int w, int h, int n_units, const 
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
     int rc = vo_claim_buffers(ctx, "vo_batch_configure");
     if (rc) return rc;
-    if ((rc = vo_ensure_state(ctx, w, h, n_units, 4))) return rc;
+    if ((rc = vo_ensure_state(ctx, w, h, n_units))) return rc;
     vo_set_calibration(ctx, P_l, P_r);
     ctx->batch_units = n_units;
     ctx->batch_uploaded = 0;
@@ -234,130 +234,81 @@ extern "C" int vo_batch_upload(vo_ctx* ctx, const vo_unit* units, int n_units, s
     return VO_OK;
 }
 
-static int ensure_side_streams(vo_ctx* ctx)
-{
-    if (ctx->fork_ev) return VO_OK;
-    VO_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->fork_ev, cudaEventDisableTiming));
-    for (int c = 0; c < VO_LANES; c++) {
-        VO_CUDA_CHECK(cudaStreamCreateWithFlags(&ctx->side_stream[c], cudaStreamNonBlocking));
-        VO_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->join_ev[c], cudaEventDisableTiming));
-    }
-    return VO_OK;
-}
-
 // high-priority helper streams: the short and the latency-bound kernels of a range (FAST, pyramids, filters,
-// triangulation, PnP) are issued there, the LK ring at normal priority.  With two ranges in flight the helpers' few
-// CTAs are then never queued behind the thousands of pending CTAs of the OTHER range's LK launch, so consecutive LK
-// launches follow each other directly and the ramp-down of one (a feature-ring lasts ~0.3 ms) fills with the next.
-static int ensure_hi_streams(vo_ctx* ctx)
+// triangulation, PnP) are issued there, the LK ring at normal priority on the lane's side stream.  With two ranges in
+// flight the helpers' few CTAs are then never queued behind the thousands of pending CTAs of the OTHER range's LK launch,
+// so consecutive LK launches follow each other directly and the ramp-down of one (a feature-ring lasts ~0.3 ms) fills
+// with the next.  The lanes' schedule when the SM partition is off (vo_partition_enable fills them in otherwise).
+static int ensure_helpers(vo_ctx* ctx)
 {
-    if (ctx->hi_stream[0]) return VO_OK;
+    if (ctx->lane[0].pre) return VO_OK;
     int lo = 0, hi = 0;
     VO_CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&lo, &hi));      // hi is the numerically smallest value
-    for (int c = 0; c < VO_LANES; c++) {
-        VO_CUDA_CHECK(cudaStreamCreateWithPriority(&ctx->hi_stream[c], cudaStreamNonBlocking, hi));
-        for (int k = 0; k < 4; k++) VO_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->hi_ev[c][k], cudaEventDisableTiming));
+    for (auto& L : ctx->lane) {
+        VO_CUDA_CHECK(cudaStreamCreateWithPriority(&L.pre, cudaStreamNonBlocking, hi));
+        L.post = L.pre;
+        L.lk = L.side;
     }
     return VO_OK;
 }
 
-// the whole path for the resident units of `v`, asynchronous on v.s.  When v.s is one of the side streams and
-// priorities are enabled, everything but the LK ring is forked to that side stream's high-priority helper.
+// the whole path for the resident units of `v`, asynchronous on v.s.  A range on a lane's side stream runs the lane's
+// schedule (ctx.h, vo_ctx::Lane); any other range runs on v.s alone.
 static int run_range_launch(vo_ctx* ctx, const View& v)
 {
-    ctx->imgs_per_unit = 4;
     int rc;
-    int c = -1;
-    for (int k = 0; k < VO_LANES; k++) if (ctx->side_stream[k] && v.s == ctx->side_stream[k]) c = k;
-    // With the SM partition on, a side-stream range runs its LK ring on the LK partition's stream and everything else on the
-    // helper partition's stream; otherwise (priorities) everything but the LK ring goes to the side stream's high-priority helper.
-    const bool part = ctx->part_on && c >= 0;
-    const bool prio = !part && ctx->use_priorities && c >= 0;
-    View h = v, lk = v;                          // the views the helper kernels / the LK ring run on
+    View pre = v, lk = v, post = v;              // FAST + pyramids / the LK ring / the kernels after the ring
     cudaEvent_t* ev = nullptr;
-    if (part) {
-        h.s = ctx->part_hp_stream[c]; lk.s = ctx->part_lk_stream[c]; ev = ctx->part_ev[c];
-    } else if (prio) {
-        if ((rc = ensure_hi_streams(ctx))) return rc;
-        h.s = ctx->hi_stream[c]; ev = ctx->hi_ev[c];
-    }
-    View pre = h;                                // FAST + pyramids
-    if (part && ctx->part_pre_with_lk) pre.s = lk.s;
-    if (ev) {
-        VO_CUDA_CHECK(cudaEventRecord(ev[0], v.s));
-        VO_CUDA_CHECK(cudaStreamWaitEvent(pre.s, ev[0], 0));
-        if (pre.s != h.s) VO_CUDA_CHECK(cudaStreamWaitEvent(h.s, ev[0], 0));
-    }
+    for (auto& L : ctx->lane)
+        if (L.side && v.s == L.side) {
+            if ((rc = ensure_helpers(ctx))) return rc;
+            pre.s = L.pre; lk.s = L.lk; post.s = L.post; ev = L.ev;
+        }
+    // work on `to` after the work enqueued so far on `from`
+    auto hand_over = [&](int k, cudaStream_t from, cudaStream_t to) -> int {
+        if (from == to) return VO_OK;
+        VO_CUDA_CHECK(cudaEventRecord(ev[k], from));
+        VO_CUDA_CHECK(cudaStreamWaitEvent(to, ev[k], 0));
+        return VO_OK;
+    };
+    if ((rc = hand_over(0, v.s, pre.s))) return rc;
     if (ctx->batch_detect) {
         if ((rc = vo_run_fast(ctx, pre, 0, false))) return rc;
         if ((rc = vo_run_select(ctx, pre))) return rc;
     }
-    if ((rc = vo_run_pyramid(ctx, v.u0 * ctx->imgs_per_unit, v.n * ctx->imgs_per_unit, pre.s))) return rc;
-    if (ev && pre.s != lk.s) {
-        VO_CUDA_CHECK(cudaEventRecord(ev[1], pre.s));
-        VO_CUDA_CHECK(cudaStreamWaitEvent(lk.s, ev[1], 0));
-    }
+    if ((rc = vo_run_pyramid(ctx, v.u0 * v.imgs, v.n * v.imgs, pre.s))) return rc;
+    if ((rc = hand_over(1, pre.s, lk.s))) return rc;
     const int ip[4] = {0, 1, 3, 2}, in[4] = {1, 3, 2, 0};      // ring L0->R0->R1->L1->L0 (planes L0,R0,L1,R1)
-    ctx->lk_per_unit = range_bound(ctx, v.u0, v.n);             // no unit of the range has more live features
-    rc = vo_run_lk_ring(ctx, lk, 4, ip, in, false);
-    ctx->lk_per_unit = 0;
-    if (rc) return rc;
-    if (ev) {
-        VO_CUDA_CHECK(cudaEventRecord(ev[2], lk.s));
-        VO_CUDA_CHECK(cudaStreamWaitEvent(h.s, ev[2], 0));
-    }
-    if ((rc = vo_run_filter(ctx, h, false))) return rc;
+    if ((rc = vo_run_lk_ring(ctx, lk, 4, ip, in, false))) return rc;
+    if ((rc = hand_over(2, lk.s, post.s))) return rc;
+    if ((rc = vo_run_filter(ctx, post, false))) return rc;
     const size_t cs = (size_t)ctx->units * ctx->cap;
-    if ((rc = vo_run_triangulate(ctx, h, ctx->d_valid4, ctx->d_valid4 + cs, ctx->d_n5))) return rc;
+    if ((rc = vo_run_triangulate(ctx, post, ctx->d_valid4, ctx->d_valid4 + cs, ctx->d_n5))) return rc;
     float K9[9] = {ctx->P_l[0], ctx->P_l[1], ctx->P_l[2], ctx->P_l[4], ctx->P_l[5], ctx->P_l[6], ctx->P_l[8], ctx->P_l[9], ctx->P_l[10]};
-    if ((rc = vo_run_pnp(ctx, h, ctx->d_valid4 + 2 * cs, ctx->d_n5, K9))) return rc;
-    k_pack_counts<<<(v.n + 63) / 64, 64, 0, h.s>>>(ctx->d_results + v.u0, ctx->d_npts + v.u0, ctx->d_ndet + v.u0, ctx->d_n3 + v.u0,
-                                                  ctx->d_n5 + v.u0, v.n, ctx->batch_detect ? 1 : 0);
+    if ((rc = vo_run_pnp(ctx, post, ctx->d_valid4 + 2 * cs, ctx->d_n5, K9))) return rc;
+    k_pack_counts<<<(v.n + 63) / 64, 64, 0, post.s>>>(ctx->d_results + v.u0, ctx->d_npts + v.u0, ctx->d_ndet + v.u0, ctx->d_n3 + v.u0,
+                                                     ctx->d_n5 + v.u0, v.n, ctx->batch_detect ? 1 : 0);
     ctx->launches += 1;
     VO_CUDA_CHECK(cudaGetLastError());
-    if (ev) {                                    // join: later work on v.s (result copy, the next submission) sees everything
-        VO_CUDA_CHECK(cudaEventRecord(ev[3], h.s));
-        VO_CUDA_CHECK(cudaStreamWaitEvent(v.s, ev[3], 0));
-    }
-    return VO_OK;
+    return hand_over(3, post.s, v.s);            // join: later work on v.s (result copy, the next submission) sees everything
 }
 
-// Replays (or first captures) the kernel sequence of one unit range as a CUDA graph on v.s.  All kernel
-// arguments are device pointers / sizes fixed by (range, detect, staging), so the graph is reusable until
-// the device state is re-allocated.  The LK event timing is not part of graphs.
-static int run_range(vo_ctx* ctx, const View& v)
+// The kernel sequence of the units [u0, u0 + n) on `s`.  On ctx->stream it is replayed (or first captured) as a CUDA
+// graph: all kernel arguments are device pointers / sizes fixed by (range, feature bound, detect, staging), so the graph
+// is reusable until the device state is re-allocated.  A range on a side stream is launched plainly: its kernels fork to
+// the lane's partition or high-priority streams, which kernel nodes of a captured graph do not keep, and that split is
+// worth more (+7 % on the pipelined step) than the graph's launch savings (+2 %).
+static int run_range(vo_ctx* ctx, int u0, int n, cudaStream_t s)
 {
-    // Kernel nodes of a captured graph do not keep the capture streams' priorities (measured: no effect), and the
-    // priority split is worth more (+7 % on the pipelined step) than the graph's launch savings (+2 %): ranges that run
-    // on a side stream with priorities enabled are launched plainly unless "batch_graphs" forces graphs.
+    View v{u0, n, s};
+    v.max_pts = range_bound(ctx, u0, n);         // the LK launch geometry depends on it
     bool on_side = false;
-    for (int k = 0; k < VO_LANES; k++) on_side = on_side || (ctx->side_stream[k] && v.s == ctx->side_stream[k]);
-    if (!ctx->use_graphs || ((ctx->use_priorities || ctx->part_on) && on_side && !ctx->batch_graphs)) return run_range_launch(ctx, v);
-    const int max_pts = range_bound(ctx, v.u0, v.n);
-    for (auto& g : ctx->graphs)
-        if (g.u0 == v.u0 && g.n == v.n && g.detect == ctx->batch_detect && g.tma == ctx->lk_use_tma && g.s == v.s && g.max_pts == max_pts) {
-            VO_CUDA_CHECK(cudaGraphLaunch(g.exec, v.s));
-            ctx->launches += g.launches;
-            return VO_OK;
-        }
-    const bool timing = ctx->lk_timing;
-    const long long before = ctx->launches;
-    ctx->lk_timing = false;
-    cudaGraph_t graph = nullptr;
-    VO_CUDA_CHECK(cudaStreamBeginCapture(v.s, cudaStreamCaptureModeThreadLocal));
-    int rc = run_range_launch(ctx, v);
-    cudaError_t e = cudaStreamEndCapture(v.s, &graph);
-    ctx->lk_timing = timing;
-    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-    VO_CUDA_CHECK(e);
-    vo_ctx::RangeGraph g;
-    g.u0 = v.u0; g.n = v.n; g.detect = ctx->batch_detect; g.tma = ctx->lk_use_tma; g.s = v.s; g.max_pts = max_pts;      // the LK launch geometry depends on max_pts
-    g.launches = ctx->launches - before;
-    VO_CUDA_CHECK(cudaGraphInstantiate(&g.exec, graph, 0));
-    cudaGraphDestroy(graph);
-    ctx->graphs.push_back(g);
-    VO_CUDA_CHECK(cudaGraphLaunch(g.exec, v.s));
-    return VO_OK;
+    for (const auto& L : ctx->lane) on_side = on_side || (L.side && s == L.side);
+    if (on_side) return run_range_launch(ctx, v);
+    GraphKey key{};
+    key.kind = GraphKey::BATCH_RANGE; key.s = s; key.tma = ctx->lk_use_tma;
+    key.u0 = u0; key.n = n; key.max_pts = v.max_pts; key.detect = ctx->batch_detect;
+    return vo_run_graph(ctx, key, [&] { return run_range_launch(ctx, v); });
 }
 
 extern "C" int vo_batch_run(vo_ctx* ctx)
@@ -368,20 +319,20 @@ extern "C" int vo_batch_run(vo_ctx* ctx)
     if (!ctx->have_P) { vo_set_error(ctx, "vo_batch_run: projection matrices not set"); return VO_E_INVALID; }
     { int rcc = vo_claim_buffers(ctx, "vo_batch_run"); if (rcc) return rcc; }
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
-    if (units < 2 || ctx->batch_streams < 2) return run_range(ctx, View{0, units, ctx->stream});
+    if (units < 2 || ctx->batch_streams < 2) return run_range(ctx, 0, units, ctx->stream);
     // two unit ranges on two side streams: the latency-bound PnP kernels of one range run under the
     // LK ring of the other (fork from / join into the context's stream, so callers see one stream)
-    int rc = ensure_side_streams(ctx);
+    int rc = vo_ensure_lanes(ctx);
     if (rc) return rc;
     VO_CUDA_CHECK(cudaEventRecord(ctx->fork_ev, ctx->stream));
     const int half = (units + 1) / 2;
     for (int c = 0; c < 2; c++) {
         const int u0 = c ? half : 0, n = c ? units - half : half;
-        cudaStream_t st = ctx->side_stream[c];
+        cudaStream_t st = ctx->lane[c].side;
         VO_CUDA_CHECK(cudaStreamWaitEvent(st, ctx->fork_ev, 0));
-        if ((rc = run_range(ctx, View{u0, n, st}))) return rc;
-        VO_CUDA_CHECK(cudaEventRecord(ctx->join_ev[c], st));
-        VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->join_ev[c], 0));
+        if ((rc = run_range(ctx, u0, n, st))) return rc;
+        VO_CUDA_CHECK(cudaEventRecord(ctx->lane[c].join, st));
+        VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->lane[c].join, 0));
     }
     return VO_OK;
 }
@@ -416,21 +367,21 @@ extern "C" int vo_frame_batch(vo_ctx* ctx, const vo_unit* units, int n_units, si
     const int nchunks = (n_units >= 2 && ctx->batch_streams >= 2) ? 2 : 1;
     if (nchunks == 1) {
         if ((rc = upload_range(ctx, units, 0, n_units, pitch, ctx->stream, detect))) return rc;
-        if ((rc = run_range(ctx, View{0, n_units, ctx->stream}))) return rc;
+        if ((rc = run_range(ctx, 0, n_units, ctx->stream))) return rc;
         VO_CUDA_CHECK(cudaMemcpyAsync(h_res, ctx->d_results, (size_t)n_units * sizeof(vo_unit_result_dev), cudaMemcpyDeviceToHost, ctx->stream));
     } else {
-        if ((rc = ensure_side_streams(ctx))) return rc;
+        if ((rc = vo_ensure_lanes(ctx))) return rc;
         VO_CUDA_CHECK(cudaEventRecord(ctx->fork_ev, ctx->stream));
         const int half = (n_units + 1) / 2;
         for (int c = 0; c < 2; c++) {
             const int u0 = c ? half : 0, n = c ? n_units - half : half;
-            cudaStream_t st = ctx->side_stream[c];
+            cudaStream_t st = ctx->lane[c].side;
             VO_CUDA_CHECK(cudaStreamWaitEvent(st, ctx->fork_ev, 0));
             if ((rc = upload_range(ctx, units, u0, n, pitch, st, detect))) return rc;
-            if ((rc = run_range(ctx, View{u0, n, st}))) return rc;
+            if ((rc = run_range(ctx, u0, n, st))) return rc;
             VO_CUDA_CHECK(cudaMemcpyAsync(h_res + u0, ctx->d_results + u0, (size_t)n * sizeof(vo_unit_result_dev), cudaMemcpyDeviceToHost, st));
-            VO_CUDA_CHECK(cudaEventRecord(ctx->join_ev[c], st));
-            VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->join_ev[c], 0));
+            VO_CUDA_CHECK(cudaEventRecord(ctx->lane[c].join, st));
+            VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->lane[c].join, 0));
         }
     }
     VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
@@ -461,8 +412,8 @@ static int upload_units(vo_ctx* ctx, const vo_dunit* units, int u0, int n, size_
     }
     int rc = vo_ingest_device(ctx, tab, 4 * n, 4 * u0, st);
     if (rc) return rc;
-    VO_CUDA_CHECK(cudaEventRecord(ctx->join_ev[lane], st));
-    VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->join_ev[lane], 0));
+    VO_CUDA_CHECK(cudaEventRecord(ctx->lane[lane].join, st));
+    VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->lane[lane].join, 0));
     return stage_inputs(ctx, units, u0, n, st, detect, 0);
 }
 
@@ -494,13 +445,12 @@ static int batch_submit(vo_ctx* ctx, const char* who, const Unit* units, int fir
         max_pts = range_bound(ctx, first_unit, n_units);
     }
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
-    if ((rc = ensure_side_streams(ctx))) return rc;
+    if ((rc = vo_ensure_lanes(ctx))) return rc;
     if (ctx->part_auto) {
         // Pipelined submissions: the persistent LK ring of one range would keep the latency-bound kernels after the other
         // range's ring (filters, triangulation, PnP) off the SMs until it ends.  8 SMs are set aside for them (green
         // contexts); FAST / pyramids stay with the ring.  Measured: value 4239 -> 4603, e2e 3854 -> 4540 frames/s.
         ctx->part_auto = false;
-        ctx->part_pre_with_lk = true;
         if (vo_partition_enable(ctx, 8) != VO_OK) ctx->err[0] = 0;      // no green contexts on this driver: run unpartitioned
     }
     if (ctx->batch_outputs && (rc = ensure_outputs(ctx, first_unit, n_units, max_pts))) return rc;
@@ -512,7 +462,7 @@ static int batch_submit(vo_ctx* ctx, const char* who, const Unit* units, int fir
         VO_CUDA_CHECK(cudaEventCreateWithFlags(&slot->done, cudaEventDisableTiming));
     }
     const int c = (int)((ctx->submit_count++) % VO_LANES);     // up to VO_LANES submissions in flight, each on its own lane
-    cudaStream_t st = ctx->side_stream[c];
+    cudaStream_t st = ctx->lane[c].side;
     VO_CUDA_CHECK(cudaEventRecord(ctx->fork_ev, ctx->stream));
     VO_CUDA_CHECK(cudaStreamWaitEvent(st, ctx->fork_ev, 0));
     if ((rc = vo_dist_order_after_gathers(ctx, st))) return rc;
@@ -521,7 +471,7 @@ static int batch_submit(vo_ctx* ctx, const char* who, const Unit* units, int fir
         if ((rc = upload_units(ctx, units, first_unit, n_units, pitch, st, c, detect))) return rc;
         if (ctx->batch_uploaded < first_unit + n_units) ctx->batch_uploaded = first_unit + n_units;
     }
-    if ((rc = run_range(ctx, View{first_unit, n_units, st}))) return rc;
+    if ((rc = run_range(ctx, first_unit, n_units, st))) return rc;
     vo_unit_result_dev* h_res = pinned_results(ctx);
     VO_CUDA_CHECK(cudaMemcpyAsync(h_res + first_unit, ctx->d_results + first_unit, (size_t)n_units * sizeof(vo_unit_result_dev), cudaMemcpyDeviceToHost, st));
     if (ctx->batch_outputs) {                    // the point lists of the submission: one packed block, one copy

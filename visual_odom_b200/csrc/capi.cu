@@ -27,19 +27,14 @@ extern "C" int vo_lk_track(vo_ctx* ctx, const uint8_t* prev, const uint8_t* next
     if (n == 0) return VO_OK;          // OpenCV's LK returns early on 0 points
     if (!prev || !next || !prev_pts || !next_pts || !status) { vo_set_error(ctx, "null argument"); return VO_E_INVALID; }
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
-    rc = vo_ensure_state(ctx, w, h, 1, 2);
+    rc = vo_ensure_state(ctx, w, h, 1);
     if (rc) return rc;
-    ctx->imgs_per_unit = 2;
     if ((rc = upload_image(ctx, 0, prev, w, h, pitch))) return rc;
     if ((rc = upload_image(ctx, 1, next, w, h, pitch))) return rc;
     VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_pts_in, prev_pts, (size_t)n * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
     VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_npts, &n, sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
     const int ip[1] = {0}, in[1] = {1};
-    ctx->lk_per_unit = n;
-    rc = vo_run_lk(ctx, View{0, 1, ctx->stream}, 1, ip, in, err != nullptr);
-    ctx->lk_per_unit = 0;
-    ctx->imgs_per_unit = 4;
-    if (rc) return rc;
+    if ((rc = vo_run_lk(ctx, View{0, 1, ctx->stream, -1, 2, n}, 1, ip, in, err != nullptr))) return rc;
     VO_CUDA_CHECK(cudaMemcpyAsync(next_pts, ctx->d_pts_out, (size_t)n * sizeof(float2), cudaMemcpyDeviceToHost, ctx->stream));
     VO_CUDA_CHECK(cudaMemcpyAsync(status, ctx->d_status, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
     if (err) VO_CUDA_CHECK(cudaMemcpyAsync(err, ctx->d_err, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
@@ -60,9 +55,8 @@ extern "C" int vo_circular_match(vo_ctx* ctx, const uint8_t* l0, const uint8_t* 
     if (n == 0) return VO_OK;
     if (!l0 || !r0 || !l1 || !r1 || !pts_l0) { vo_set_error(ctx, "null argument"); return VO_E_INVALID; }
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
-    rc = vo_ensure_state(ctx, w, h, 1, 4);
+    rc = vo_ensure_state(ctx, w, h, 1);
     if (rc) return rc;
-    ctx->imgs_per_unit = 4;
     const uint8_t* imgs[4] = {l0, r0, l1, r1};
     for (int i = 0; i < 4; i++)
         if ((rc = upload_image(ctx, i, imgs[i], w, h, pitch))) return rc;
@@ -72,10 +66,7 @@ extern "C" int vo_circular_match(vo_ctx* ctx, const uint8_t* l0, const uint8_t* 
         VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_ages_in, ages_io, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
     // ring order: L0->R0, R0->R1, R1->L1, L1->L0   (planes: L0=0, R0=1, L1=2, R1=3)
     const int ip[4] = {0, 1, 3, 2}, in[4] = {1, 3, 2, 0};
-    ctx->lk_per_unit = n;
-    rc = vo_run_lk(ctx, View{0, 1, ctx->stream}, 4, ip, in, false);
-    ctx->lk_per_unit = 0;
-    if (rc) return rc;
+    if ((rc = vo_run_lk(ctx, View{0, 1, ctx->stream, -1, 4, n}, 4, ip, in, false))) return rc;
     if ((rc = vo_run_filter(ctx, View{0, 1, ctx->stream}, ages_io != nullptr))) return rc;
     int n3 = 0;
     VO_CUDA_CHECK(cudaMemcpyAsync(&n3, ctx->d_n3, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
@@ -104,7 +95,7 @@ extern "C" int vo_circular_match(vo_ctx* ctx, const uint8_t* l0, const uint8_t* 
 static int ensure_any_state(vo_ctx* ctx)
 {
     if (ctx->units > 0) return VO_OK;
-    return vo_ensure_state(ctx, 64, 64, 1, 4);
+    return vo_ensure_state(ctx, 64, 64, 1);
 }
 
 extern "C" int vo_fast_detect(vo_ctx* ctx, const uint8_t* img, int w, int h, size_t pitch, vo_point2f* out,
@@ -115,8 +106,7 @@ extern "C" int vo_fast_detect(vo_ctx* ctx, const uint8_t* img, int w, int h, siz
     if ((rc = vo_claim_buffers(ctx, "vo_fast_detect"))) return rc;
     if (!img || !n_out || (cap > 0 && !out)) { vo_set_error(ctx, "null argument"); return VO_E_INVALID; }
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
-    if ((rc = vo_ensure_state(ctx, w, h, 1, 4))) return rc;
-    ctx->imgs_per_unit = 4;
+    if ((rc = vo_ensure_state(ctx, w, h, 1))) return rc;
     if ((rc = upload_image(ctx, 0, img, w, h, pitch))) return rc;
     if ((rc = vo_run_fast(ctx, View{0, 1, ctx->stream}, 0, response != nullptr))) return rc;
     int n = 0;

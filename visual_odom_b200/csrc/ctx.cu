@@ -75,8 +75,6 @@ extern "C" int vo_create(int device, const vo_params* params, vo_ctx** out)
         ctx->lk_use_tma = !(st && strcmp(st, "ldg") == 0);
         const char* sp = getenv("VO_LK_SPAN");      // force the LK work-item size (tests/test_gpu_lk_variants.py sets it per context with "lk_span")
         if (sp) ctx->lk_span = atoi(sp);
-        const char* pt = getenv("VO_SM_PARTITION");  // 0: never partition the SMs (profilers cannot attach to green-context launches)
-        if (pt && atoi(pt) == 0) ctx->part_auto = false;
     }
     return VO_OK;
 }
@@ -97,11 +95,10 @@ extern "C" void vo_destroy(vo_ctx* ctx)
         if (ctx->seq_back_ev[k]) cudaEventDestroy(ctx->seq_back_ev[k]);
     }
     if (ctx->fork_ev) cudaEventDestroy(ctx->fork_ev);
-    for (int c = 0; c < VO_LANES; c++) {
-        if (ctx->join_ev[c]) cudaEventDestroy(ctx->join_ev[c]);
-        if (ctx->side_stream[c]) cudaStreamDestroy(ctx->side_stream[c]);
-        if (ctx->hi_stream[c]) cudaStreamDestroy(ctx->hi_stream[c]);
-        for (int k = 0; k < 4; k++) if (ctx->hi_ev[c][k]) cudaEventDestroy(ctx->hi_ev[c][k]);
+    for (auto& L : ctx->lane) {
+        if (L.join) cudaEventDestroy(L.join);
+        if (L.side) cudaStreamDestroy(L.side);
+        for (cudaEvent_t e : L.ev) if (e) cudaEventDestroy(e);
     }
     if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
     if (ctx->d_bgr) cudaFree(ctx->d_bgr);
@@ -137,18 +134,14 @@ extern "C" int vo_set_option(vo_ctx* ctx, const char* key, double value)
     if (!ctx || !key) return VO_E_INVALID;
     if (strcmp(key, "batch_streams") == 0) { ctx->batch_streams = value >= 2 ? 2 : 1; return VO_OK; }
     if (strcmp(key, "lk_staging") == 0) { ctx->lk_use_tma = !(value >= 1); return VO_OK; }
-    if (strcmp(key, "lk_ctas_per_sm") == 0) { ctx->lk_ctas_per_sm = (int)value; vo_drop_graphs(ctx); return VO_OK; }
     if (strcmp(key, "batch_outputs") == 0) { ctx->batch_outputs = value >= 1; vo_drop_graphs(ctx); return VO_OK; }
-    if (strcmp(key, "sm_partition") == 0) {          // k > 0: every helper kernel on k SMs; k < 0: only the kernels after the ring on |k| SMs
-        ctx->part_pre_with_lk = value < 0;
+    if (strcmp(key, "sm_partition") == 0) {          // k > 0: the kernels after the LK ring on k SMs of their own; 0: no partition
+        if (value < 0) { vo_set_error(ctx, "sm_partition=%g: the number of SMs must not be negative", value); return VO_E_INVALID; }
         ctx->part_auto = false;
-        return vo_partition_enable(ctx, value < 0 ? (int)-value : (int)value);
+        return vo_partition_enable(ctx, (int)value);
     }
-    if (strcmp(key, "lk_quota") == 0) { ctx->lk_quota = (int)value; vo_drop_graphs(ctx); return VO_OK; }
     if (strcmp(key, "lk_span") == 0) { ctx->lk_span = (int)value; vo_drop_graphs(ctx); return VO_OK; }
     if (strcmp(key, "graphs") == 0) { ctx->use_graphs = value >= 1; return VO_OK; }
-    if (strcmp(key, "batch_graphs") == 0) { ctx->batch_graphs = value >= 1; return VO_OK; }
-    if (strcmp(key, "priorities") == 0) { ctx->use_priorities = value >= 1; vo_drop_graphs(ctx); return VO_OK; }
     if (strcmp(key, "mono_rotation") == 0) { ctx->mono_opt = value >= 1; vo_drop_graphs(ctx); return VO_OK; }
     vo_set_error(ctx, "unknown option %s", key);
     return VO_E_INVALID;
@@ -218,13 +211,13 @@ static bool drv(const char* name, F* fn)
     return true;
 }
 
+// also drops the lanes' priority helpers: a lane without pre / lk / post streams gets them again on first use (batch.cu)
 void vo_partition_destroy(vo_ctx* ctx)
 {
-    for (int c = 0; c < VO_LANES; c++) {
-        if (ctx->part_lk_stream[c]) cudaStreamDestroy(ctx->part_lk_stream[c]);
-        if (ctx->part_hp_stream[c]) cudaStreamDestroy(ctx->part_hp_stream[c]);
-        ctx->part_lk_stream[c] = ctx->part_hp_stream[c] = nullptr;
-        for (int k = 0; k < 4; k++) if (ctx->part_ev[c][k]) { cudaEventDestroy(ctx->part_ev[c][k]); ctx->part_ev[c][k] = nullptr; }
+    for (auto& L : ctx->lane) {
+        if (L.pre) cudaStreamDestroy(L.pre);                            // partition: pre = lk; helpers: pre = post, lk = side
+        if (L.post && L.post != L.pre) cudaStreamDestroy(L.post);
+        L.pre = L.lk = L.post = nullptr;
     }
     PFN_cuGreenCtxDestroy destroy = nullptr;
     if (drv("cuGreenCtxDestroy", &destroy))
@@ -278,8 +271,9 @@ int vo_partition_enable(vo_ctx* ctx, int helper_sms)
             vo_partition_destroy(ctx);
             return VO_E_UNSUPPORTED;
         }
-        ctx->part_hp_stream[c] = (cudaStream_t)a; ctx->part_lk_stream[c] = (cudaStream_t)b;
-        for (int k = 0; k < 4; k++) VO_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->part_ev[c][k], cudaEventDisableTiming));
+        vo_ctx::Lane& L = ctx->lane[c];
+        L.pre = L.lk = (cudaStream_t)b;
+        L.post = (cudaStream_t)a;
     }
     ctx->part_on = true;
     return VO_OK;
@@ -294,7 +288,7 @@ int vo_drain_pending(vo_ctx* ctx)
             p.active = false;
         }
     // frames of the sequence mode still in flight on the pose-solve stream
-    if (ctx->seq_inflight > 0 && ctx->side_stream[0]) VO_CUDA_CHECK(cudaStreamSynchronize(ctx->side_stream[0]));
+    if (ctx->seq_inflight > 0 && ctx->lane[0].side) VO_CUDA_CHECK(cudaStreamSynchronize(ctx->lane[0].side));
     return VO_OK;
 }
 
@@ -303,6 +297,53 @@ void vo_drop_graphs(vo_ctx* ctx)
 {
     for (auto& g : ctx->graphs) cudaGraphExecDestroy(g.exec);
     ctx->graphs.clear();
+}
+
+static bool same_key(const GraphKey& a, const GraphKey& b)
+{
+    return a.kind == b.kind && a.s == b.s && a.tma == b.tma && a.u0 == b.u0 && a.n == b.n && a.max_pts == b.max_pts &&
+           a.detect == b.detect && a.slot == b.slot && a.parity == b.parity && a.bgr == b.bgr;
+}
+
+int vo_run_graph(vo_ctx* ctx, const GraphKey& key, const std::function<int()>& launch)
+{
+    if (!ctx->use_graphs) return launch();
+    for (auto& g : ctx->graphs)
+        if (same_key(g.key, key)) {
+            VO_CUDA_CHECK(cudaGraphLaunch(g.exec, key.s));
+            ctx->launches += g.launches;
+            return VO_OK;
+        }
+    const bool timing = ctx->lk_timing;
+    const long long before = ctx->launches;
+    ctx->lk_timing = false;
+    cudaGraph_t graph = nullptr;
+    VO_CUDA_CHECK(cudaStreamBeginCapture(key.s, cudaStreamCaptureModeThreadLocal));
+    int rc = launch();
+    cudaError_t e = cudaStreamEndCapture(key.s, &graph);
+    ctx->lk_timing = timing;
+    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
+    VO_CUDA_CHECK(e);
+    vo_ctx::CachedGraph g;
+    g.key = key;
+    g.launches = ctx->launches - before;
+    VO_CUDA_CHECK(cudaGraphInstantiate(&g.exec, graph, 0));
+    cudaGraphDestroy(graph);
+    ctx->graphs.push_back(g);
+    VO_CUDA_CHECK(cudaGraphLaunch(g.exec, key.s));
+    return VO_OK;
+}
+
+int vo_ensure_lanes(vo_ctx* ctx)
+{
+    if (ctx->fork_ev) return VO_OK;
+    VO_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->fork_ev, cudaEventDisableTiming));
+    for (auto& L : ctx->lane) {
+        VO_CUDA_CHECK(cudaStreamCreateWithFlags(&L.side, cudaStreamNonBlocking));
+        VO_CUDA_CHECK(cudaEventCreateWithFlags(&L.join, cudaEventDisableTiming));
+        for (cudaEvent_t& e : L.ev) VO_CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    }
+    return VO_OK;
 }
 
 void vo_set_calibration(vo_ctx* ctx, const float P_l[12], const float P_r[12])
@@ -383,7 +424,7 @@ static int encode_maps(vo_ctx* ctx)
     return VO_OK;
 }
 
-int vo_ensure_state(vo_ctx* ctx, int w, int h, int units, int /*imgs_per_unit*/)
+int vo_ensure_state(vo_ctx* ctx, int w, int h, int units)
 {
     if (w <= 0 || h <= 0 || units <= 0) { vo_set_error(ctx, "bad geometry %dx%d units=%d", w, h, units); return VO_E_INVALID; }
     if (ctx->w == w && ctx->h == h && ctx->units >= units) return VO_OK;
@@ -495,7 +536,7 @@ int vo_run_pyramid(vo_ctx* ctx, int plane0, int nplanes, cudaStream_t s)
 
 int vo_run_lk(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, const int* img_next, bool want_err)
 {
-    int rc = vo_run_pyramid(ctx, v.u0 * ctx->imgs_per_unit, v.n * ctx->imgs_per_unit, v.s);
+    int rc = vo_run_pyramid(ctx, v.u0 * v.imgs, v.n * v.imgs, v.s);
     if (rc) return rc;
     return vo_run_lk_ring(ctx, v, ncalls, img_prev, img_next, want_err);
 }
@@ -503,7 +544,6 @@ int vo_run_lk(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, const
 // the ring kernel alone (pyramids of every plane it touches must be up to date)
 int vo_run_lk_ring(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, const int* img_next, bool want_err)
 {
-    const int ipu = ctx->imgs_per_unit;
     const size_t uo = (size_t)v.u0 * ctx->cap;
     const PyrGeom& pg = ctx->pg;
 
@@ -512,8 +552,8 @@ int vo_run_lk_ring(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, 
     a.n_units = v.n;
     a.cap = ctx->cap;
     a.n_pts = ctx->d_npts + v.u0;
-    a.imgs_per_unit = ipu;
-    a.img_plane0 = v.plane0 >= 0 ? v.plane0 : v.u0 * ipu;
+    a.imgs_per_unit = v.imgs;
+    a.img_plane0 = v.plane0 >= 0 ? v.plane0 : v.u0 * v.imgs;
     a.ncalls = ncalls;
     for (int c = 0; c < ncalls; c++) { a.img_prev[c] = img_prev[c]; a.img_next[c] = img_next[c]; }
     a.nlevels = pg.nlevels;
@@ -555,19 +595,14 @@ int vo_run_lk_ring(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, 
             ctx->lk_queue_streams.push_back(v.s);
         }
         a.queue = ctx->d_lk_queue + 2 * qi;
-        a.per_unit = ctx->lk_per_unit > 0 && ctx->lk_per_unit < ctx->cap ? ctx->lk_per_unit : ctx->cap;
+        a.per_unit = v.max_pts > 0 && v.max_pts < ctx->cap ? v.max_pts : ctx->cap;
         a.progress = ctx->d_lk_progress + uo;
-        {   // a launch with fewer features than resident warps gains nothing from splitting its rings
-            int lk_sms = ctx->sm_count;
-            for (int c = 0; c < VO_LANES; c++) if (ctx->part_on && v.s == ctx->part_lk_stream[c]) lk_sms = ctx->part_lk_sms;
-            const long resident_warps = (long)lk_sms * vo_lk_ctas_per_sm(ctx->lk_ctas_per_sm) * LK_WARPS_PER_CTA;
-            const bool big = (long)a.n_units * a.per_unit > resident_warps;
-            a.span = ctx->lk_span > 0 ? ctx->lk_span : (big ? 2 : 0);
-            a.quota = big ? ctx->lk_quota : 0;
-        }
         int lk_sms = ctx->sm_count;
-        for (int c = 0; c < VO_LANES; c++) if (ctx->part_on && v.s == ctx->part_lk_stream[c]) lk_sms = ctx->part_lk_sms;
-        VO_CUDA_CHECK(vo_launch_lk_ring(ctx->maps, a, lk_sms, ctx->lk_ctas_per_sm, v.s));
+        for (const auto& L : ctx->lane) if (ctx->part_on && v.s == L.lk) lk_sms = ctx->part_lk_sms;
+        // a launch with fewer features than resident warps gains nothing from splitting its rings
+        const bool big = (long)a.n_units * a.per_unit > (long)lk_sms * LK_CTAS_PER_SM * LK_WARPS_PER_CTA;
+        a.span = ctx->lk_span > 0 ? ctx->lk_span : (big ? 2 : 0);
+        VO_CUDA_CHECK(vo_launch_lk_ring(ctx->maps, a, lk_sms, v.s));
     }
     ctx->launches += 1;
     if (e1) VO_CUDA_CHECK(cudaEventRecord(e1, v.s));
@@ -605,8 +640,8 @@ int vo_run_fast(vo_ctx* ctx, const View& v, int plane_in_unit, bool want_resp)
     memset(&a, 0, sizeof(a));
     const size_t plane = (size_t)ctx->w * ctx->h;
     a.n_units = v.n;
-    a.img_tab = ctx->d_raw_tab + (size_t)(v.plane0 >= 0 ? v.plane0 : v.u0 * ctx->imgs_per_unit) + plane_in_unit;
-    a.img_stride_idx = ctx->imgs_per_unit;
+    a.img_tab = ctx->d_raw_tab + (size_t)(v.plane0 >= 0 ? v.plane0 : v.u0 * v.imgs) + plane_in_unit;
+    a.img_stride_idx = v.imgs;
     a.w = ctx->w; a.h = ctx->h; a.pitch = ctx->w;
     a.threshold = ctx->p.fast_threshold; a.nonmax = ctx->p.fast_nonmax;
     a.score = ctx->d_score + v.u0 * plane; a.score_plane = plane;

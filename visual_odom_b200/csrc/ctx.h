@@ -9,11 +9,22 @@
 #include "ess.h"
 #include "../../include/vo_b200.h"
 #include <vector>
+#include <functional>
 #include <stdarg.h>
 #define LK_QUEUES 32
 #define VO_DIST_BUCKET 4       // posted steps per collective
 #define VO_DIST_NB 4           // buckets (ring)
 #define VO_LANES 3            // submissions in flight, each with its own side stream / partition streams / events
+
+// what a cached CUDA graph was captured for: its kind, the stream (the LK work queue is that stream's), the LK staging,
+// and the kind's own fields (the others stay zero)
+struct GraphKey {
+    enum Kind { BATCH_RANGE, SEQ_FRONT, SEQ_BACK } kind;
+    cudaStream_t s;
+    bool tma;
+    int u0, n, max_pts; bool detect;        // BATCH_RANGE: the unit range, its feature bound, on-GPU detection
+    int slot, parity; bool bgr;             // SEQ_FRONT / SEQ_BACK: image slot of the previous pairs, buffer parity, colour input
+};
 
 struct vo_ctx {
     int device = 0;
@@ -26,7 +37,6 @@ struct vo_ctx {
     // ---- geometry of the currently allocated batch state -----------------------------------
     int w = 0, h = 0;             // image size
     int units = 0;                // allocated work-unit slots
-    int imgs_per_unit = 4;
     int cap = 0;                  // feature capacity per unit
     PyrGeom pg;                   // device plane pointers per level
     LkMaps maps;                  // TMA descriptors per level
@@ -96,17 +106,13 @@ struct vo_ctx {
     uint8_t* d_bgr = nullptr;           // staging of colour (BGR) inputs, converted by k_bgr_to_gray (ingest.cu)
     size_t bgr_bytes = 0;
     // SM partition (green contexts, ctx.cu vo_partition_enable): the LK ring kernel -- persistent, 100 % of the registers of
-    // every SM it runs on -- gets its own SMs, every other kernel of the batched path (FAST, pyramids, filters, triangulation,
-    // PnP) runs on the rest, so the helper kernels of one unit range execute WHILE the other range's LK ring does
+    // every SM it runs on -- shares its SMs only with the throughput kernels before it (FAST, pyramids); the latency-bound
+    // kernels after the ring (filters, triangulation, PnP) run on the rest, so those of one unit range execute WHILE the
+    // other range's LK ring does
     bool part_on = false;
     bool part_auto = true;              // the first vo_batch_submit turns the partition on (8 SMs for the kernels after the ring)
-    bool part_pre_with_lk = false;      // FAST / pyramids (throughput kernels) stay on the LK partition, only the latency-bound
-                                        // kernels after the ring (filters, triangulation, PnP) go to the small one
     int part_helper_sms = 0, part_lk_sms = 0;
     void* part_gctx[2] = {nullptr, nullptr};            // CUgreenCtx: [0] helpers, [1] LK
-    cudaStream_t part_lk_stream[VO_LANES] = {};     // per side stream
-    cudaStream_t part_hp_stream[VO_LANES] = {};
-    cudaEvent_t part_ev[VO_LANES][4] = {};
     // multi-GPU record gather over NCCL (dist.cu); NCCL is dlopen'ed at vo_dist_init
     void* dist_comm = nullptr;
     int dist_rank = 0, dist_world = 1;
@@ -147,13 +153,9 @@ struct vo_ctx {
     long long lk_n = 0;
     bool lk_timing = true;
     bool lk_use_tma = true;
-    int lk_ctas_per_sm = 0;             // 0 = the default instantiation (LK_CTAS_PER_SM)
-    int lk_quota = 0;                   // work items a warp takes before its CTA retires (0 = persistent): retiring CTAs let the
-                                        // high-priority helper kernels of the other unit range onto the SMs between LK work
     int lk_span = 0;                    // phases per LK work item: 0 = automatic (one level-solve per item when a launch has
                                         // more features than resident warps, else one item per feature-ring)
     int* d_lk_progress = nullptr;       // [units][cap] hand-over counters of the LK work items (zero between launches)
-    int lk_per_unit = 0;                // upper bound of live features per unit known to the host (0 = cap)
     // work queues of the persistent LK warps: one (next, dry) pair per stream that launches the kernel,
     // so launches of different streams never share a pair; a pair resets itself at the end of a launch
     int* d_lk_queue = nullptr;          // [LK_QUEUES][2]
@@ -165,15 +167,22 @@ struct vo_ctx {
     bool batch_detect = false;      // features come from the on-GPU FAST + stride selection
     int batch_streams = 2;          // unit ranges run concurrently by the batched path
     bool use_graphs = true;         // replay the per-range kernel sequence as a CUDA graph (no LK event timing then)
-    struct RangeGraph { int u0, n; bool detect, tma; cudaStream_t s; int max_pts; cudaGraphExec_t exec; long long launches; };   // s: the stream it was captured on (its LK work queue is that stream's)
-    std::vector<RangeGraph> graphs; // invalidated when the device state is re-allocated
+    struct CachedGraph { GraphKey key; cudaGraphExec_t exec; long long launches; };
+    std::vector<CachedGraph> graphs; // invalidated when the device state is re-allocated
     std::vector<int> slot_pts;      // [batch_units] feature bound of each slot: n_pts of the unit last uploaded into it
-    cudaStream_t hi_stream[VO_LANES] = {};     // high-priority helpers of the side streams (see run_range_launch)
-    cudaEvent_t hi_ev[VO_LANES][4] = {};
-    bool use_priorities = true;
-    bool batch_graphs = false;      // force CUDA graphs for side-stream ranges even though they lose the priority split
-    cudaStream_t side_stream[VO_LANES] = {};   // pipelining of vo_frame_batch (H2D of chunk k+1 under compute of chunk k) and of vo_batch_submit
-    cudaEvent_t fork_ev = nullptr, join_ev[VO_LANES] = {};
+    // One lane per submission in flight: vo_frame_batch / vo_batch_run put their unit ranges on lanes 0 and 1 (H2D of one
+    // under the compute of the other), vo_batch_submit cycles through all of them, and the sequence mode solves poses on
+    // lane 0 and uploads on lane 1.  A range on a lane runs FAST + pyramids on `pre`, its LK ring on `lk` and everything
+    // after the ring on `post`, ordered by ev[0..3].  With the SM partition on, pre = lk = the LK partition's stream and
+    // post = the helper partition's (vo_partition_enable); otherwise pre = post = a high-priority helper stream and lk =
+    // side (created on first use), so the helpers' few CTAs never queue behind the other range's LK launch.
+    struct Lane {
+        cudaStream_t side = nullptr;                    // forked from / joined into ctx->stream
+        cudaStream_t pre = nullptr, lk = nullptr, post = nullptr;
+        cudaEvent_t join = nullptr, ev[4] = {};
+    };
+    Lane lane[VO_LANES];
+    cudaEvent_t fork_ev = nullptr;
     struct Pending { int u0 = 0, n = 0; bool active = false; cudaEvent_t done = nullptr; };
     std::vector<Pending> pending;   // vo_batch_submit / vo_batch_wait
     // full outputs of a submission (what matchingFeatures / trackingFrame2Frame hand back): packed per unit on the
@@ -187,9 +196,15 @@ struct vo_ctx {
 };
 
 void vo_set_error(vo_ctx* ctx, const char* fmt, ...);
-int vo_ensure_state(vo_ctx* ctx, int w, int h, int units, int imgs_per_unit);
+int vo_ensure_state(vo_ctx* ctx, int w, int h, int units);
 void vo_free_state(vo_ctx* ctx);
 void vo_drop_graphs(vo_ctx* ctx);
+// replays the graph cached for `key` on key.s, or captures what `launch` enqueues there, caches and replays it (plain
+// `launch` with the option graphs = 0).  LK event timing is off during a capture.
+int vo_run_graph(vo_ctx* ctx, const GraphKey& key, const std::function<int()>& launch);
+// the lanes' side streams and fork / join events (their pre / lk / post streams are filled in by the partition or on
+// first use of the priority helpers)
+int vo_ensure_lanes(vo_ctx* ctx);
 // new projection matrices: cached graphs carry the old calibration in their kernel arguments, so they are dropped
 void vo_set_calibration(vo_ctx* ctx, const float P_l[12], const float P_r[12]);
 int vo_drain_pending(vo_ctx* ctx);
@@ -213,9 +228,11 @@ int vo_check_dimage(vo_ctx* ctx, const char* who, const char* name, const vo_dim
 // [plane0, plane0 + n): one descriptor copy into d_ingest_tab + plane0 and one k_bgr_to_gray launch on st
 int vo_ingest_device(vo_ctx* ctx, const vo_dimage* h_tab, int n, int plane0, cudaStream_t st);
 // a contiguous range of resident work units processed on one stream
-// plane0 >= 0 overrides the image-plane base (default u0 * imgs_per_unit): the sequence mode ping-pongs its per-frame
-// buffers between two buffer parities while both address the same image ring
-struct View { int u0, n; cudaStream_t s; int plane0 = -1; };
+// plane0 >= 0 overrides the image-plane base (default u0 * imgs): the sequence mode ping-pongs its per-frame buffers
+// between two buffer parities while both address the same image ring.  imgs: image planes per unit (4: a stereo pair at
+// t0 and t1; 2: one LK call, or one sequence's pair in the sequence mode).  max_pts: live features per unit at most
+// (0 = cap), which sizes the LK launch.
+struct View { int u0, n; cudaStream_t s; int plane0 = -1; int imgs = 4; int max_pts = 0; };
 // run pyramids + LK (ncalls chained) for the units of `v`; images must already be in d_raw/d_raw_tab
 int vo_run_lk(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, const int* img_next, bool want_err);
 int vo_run_pyramid(vo_ctx* ctx, int plane0, int nplanes, cudaStream_t s);

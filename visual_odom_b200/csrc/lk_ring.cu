@@ -11,7 +11,7 @@
 //
 // Parallelisation: ONE WARP PER FEATURE-RING.  A feature's track never depends on another feature, so a warp
 // runs the whole ring (up to 4 chained calls x all pyramid levels x <= 30 Newton iterations) of one feature
-// and then takes the next feature from a global work queue (persistent warps: 12 CTAs of 2 warps per SM,
+// and then takes the next feature from a global work queue (persistent warps: 8 CTAs of 2 warps per SM,
 // every warp independent -- no CTA-level synchronisation after the start).  Ring durations differ by more
 // than 2x between features (the iteration count is heavy-tailed), so static assignment would idle.
 //
@@ -39,9 +39,10 @@
 // RUNNER lane per (quantity, chain) adds them strictly in order with 128-bit loads.  The A sums
 // always take the faithful path (they pass 2^24 on any corner-like texture).
 //
-// Shared memory is re-used over a level's life so that 24 warps fit per SM: the derivative window is dead
-// once the patch is extracted and then holds A22's chain slots and, during the iterations, the packed
-// residuals a faithful replay needs; the I window then holds the packed I patch.
+// Shared memory is re-used over a level's life: the derivative window is dead once the patch is extracted and then
+// holds A22's chain slots; the packed I patch and the packed residuals stay in registers.  WarpSmem keeps the 8960 B
+// layout that lets 24 warps fit per SM: shrinking it would move every shared-memory address, a change to be measured
+// on its own.
 #include "common.cuh"
 #include "lk_ring.h"
 
@@ -219,8 +220,8 @@ __device__ __forceinline__ float combine_chains(float acc)
 } // namespace
 
 // ---------------------------------------------------------------------------------------------
-template <bool USE_TMA, int CPS>
-__global__ void __launch_bounds__(LK_WARPS_PER_CTA * 32, CPS)
+template <bool USE_TMA>
+__global__ void __launch_bounds__(LK_WARPS_PER_CTA * 32, LK_CTAS_PER_SM)
 k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
 {
     extern __shared__ __align__(128) uint8_t smem_raw[];
@@ -249,8 +250,6 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
     const int run_off = rc < 4 ? rc * SLOT_S : TAIL_OFF;
     const float* const run_slot = (rq < 2 ? sm.chain + rq * QSTRIDE : reinterpret_cast<const float*>(sm.dwin) + A22_OFF) + run_off;
     float* const a22 = reinterpret_cast<float*>(sm.dwin) + A22_OFF;
-    uint4* const ipk_s = reinterpret_cast<uint4*>(sm.iwin);         // [2][32] packed I patch (after extraction)
-    uint4* const dpk_s = reinterpret_cast<uint4*>(sm.dwin);         // [2][32] packed residuals (during iterations)
 
     if (USE_TMA) {
         if (lane == 0) {
@@ -260,9 +259,6 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
         __syncwarp();
     }
     uint32_t phase = 0;
-    // instantiations with 128 registers per thread keep the packed I patch and the packed residuals in registers;
-    // the others park them in the (then dead) window buffers
-    constexpr bool IN_REGS = CPS <= 8;
 
     const float half_win = (VO_WIN - 1) * 0.5f;
     const float FLT_SCALE = 1.f / (1 << 20);
@@ -282,7 +278,7 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
     const int per_group = args.n_units * args.per_unit;
     const int items = ((nphases + span - 1) / span) * per_group;
 
-    for (int taken = 0; args.quota <= 0 || taken < args.quota; taken++) {
+    for (;;) {
         int item = 0;
         if (lane == 0) item = atomicAdd(args.queue, 1);
         item = __shfl_sync(FULL, item, 0);
@@ -403,10 +399,6 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                         const int k = e < 11 ? e : e - 11;
                         if (k < (e < 11 ? nvalid_s : tn)) a22[(e < 11 ? a_pos + k * 4 : t_pos + k * 5)] = a22v[e];
                     }
-                    if (!IN_REGS) {
-                        ipk_s[lane] = make_uint4(Ipk[0], Ipk[1], Ipk[2], Ipk[3]);
-                        ipk_s[32 + lane] = make_uint4(Ipk[4], Ipk[5], Ipk[6], Ipk[7]);
-                    }
                     __syncwarp();
                     float acc = 0.f;
                     if (lane < 15) acc = run_chain<84>(run_slot, rc == 4);
@@ -468,11 +460,6 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                     // light pass and goes straight to the replay (always valid, only slower than the exact path).
                     auto residual_pass = [&](auto with_sums) {
                         constexpr bool WITH_SUMS = decltype(with_sums)::value;
-                        if (!IN_REGS) {
-                            const uint4 i03 = ipk_s[lane], i47 = ipk_s[32 + lane];
-                            Ipk[0] = (int)i03.x; Ipk[1] = (int)i03.y; Ipk[2] = (int)i03.z; Ipk[3] = (int)i03.w;
-                            Ipk[4] = (int)i47.x; Ipk[5] = (int)i47.y; Ipk[6] = (int)i47.z; Ipk[7] = (int)i47.w;
-                        }
 #pragma unroll
                         for (int part = 0; part < 2; part++) {
                             const int c0 = part ? tcol : col, row0 = part ? tr0 : r0, ne = part ? 4 : 11;
@@ -496,10 +483,6 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                                 }
                                 ptop = pbot;
                             }
-                        }
-                        if (!IN_REGS) {
-                            dpk_s[lane] = make_uint4(dpk[0], dpk[1], dpk[2], dpk[3]);
-                            dpk_s[32 + lane] = make_uint4(dpk[4], dpk[5], dpk[6], dpk[7]);
                         }
                     };
                     bool exact = false;
@@ -526,11 +509,6 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                         ib1 = __shfl_sync(FULL, tot, 0); ib2 = __shfl_sync(FULL, tot, 1);
                     } else {
                         // faithful replay: float addends in chain order, runner lanes add them
-                        if (!IN_REGS) {
-                            const uint4 d03 = dpk_s[lane], d47 = dpk_s[32 + lane];
-                            dpk[0] = (int)d03.x; dpk[1] = (int)d03.y; dpk[2] = (int)d03.z; dpk[3] = (int)d03.w;
-                            dpk[4] = (int)d47.x; dpk[5] = (int)d47.y; dpk[6] = (int)d47.z; dpk[7] = (int)d47.w;
-                        }
 #pragma unroll
                         for (int k = 0; k < 11; k++) {
                             const int d = (k & 1) ? (dpk[k >> 1] >> 16) : (int)(short)(dpk[k >> 1] & 0xffff);
@@ -606,11 +584,6 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                         const unsigned wt = (unsigned)w00 | ((unsigned)w01 << 16), wb = (unsigned)w10 | ((unsigned)(w11 & 0xffff) << 16);
                         // errval += |diff| is a plain row-major float sum of small integers
                         // (<= 441 * 8160 < 2^24): exact, so any order gives the same float.
-                        if (!IN_REGS) {
-                            const uint4 i03 = ipk_s[lane], i47 = ipk_s[32 + lane];
-                            Ipk[0] = (int)i03.x; Ipk[1] = (int)i03.y; Ipk[2] = (int)i03.z; Ipk[3] = (int)i03.w;
-                            Ipk[4] = (int)i47.x; Ipk[5] = (int)i47.y; Ipk[6] = (int)i47.z; Ipk[7] = (int)i47.w;
-                        }
                         int s = 0;
 #pragma unroll
                         for (int part = 0; part < 2; part++) {
@@ -668,48 +641,28 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
 // ---------------------------------------------------------------------------------------------
 size_t vo_lk_smem_bytes() { return sizeof(WarpSmem) * LK_WARPS_PER_CTA; }
 
-template <bool T, int CPS>
+template <bool T>
 static cudaError_t prep()
 {
-    return cudaFuncSetAttribute(k_lk_ring<T, CPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)vo_lk_smem_bytes());
+    return cudaFuncSetAttribute(k_lk_ring<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)vo_lk_smem_bytes());
 }
 
 cudaError_t vo_lk_prepare()
 {
-    cudaError_t e;
-    if ((e = prep<false, LK_CTAS_PER_SM>()) != cudaSuccess) return e;
-    if ((e = prep<true, 12>()) != cudaSuccess) return e;
-    if ((e = prep<true, 10>()) != cudaSuccess) return e;
-    if ((e = prep<true, 8>()) != cudaSuccess) return e;
-    return cudaSuccess;
+    cudaError_t e = prep<false>();
+    return e != cudaSuccess ? e : prep<true>();
 }
 
-int vo_lk_ctas_per_sm(int requested)
+cudaError_t vo_launch_lk_ring(const LkMaps& maps, const LkArgs& args, int sm_count, cudaStream_t stream)
 {
-    return (requested == 12 || requested == 10 || requested == 8) ? requested : LK_CTAS_PER_SM;
-}
-
-cudaError_t vo_launch_lk_ring(const LkMaps& maps, const LkArgs& args, int sm_count, int ctas_per_sm, cudaStream_t stream)
-{
-    const int nphases = args.ncalls * args.nlevels;
-    const int span = args.span > 0 && args.span < nphases ? args.span : nphases;
     const long items = (long)args.n_units * args.per_unit;          // features; every feature has (nphases / span) work items
     if (items <= 0) return cudaSuccess;
-    const int cps = args.use_tma ? vo_lk_ctas_per_sm(ctas_per_sm) : LK_CTAS_PER_SM;
-    const long resident = (long)(sm_count > 0 ? sm_count : 148) * cps;
-    long ctas;
-    if (args.quota > 0) {           // every warp takes `quota` items: enough CTAs for all of them (they queue for SM slots)
-        const long work_items = ((nphases + span - 1) / span) * items;
-        ctas = (work_items + (long)args.quota * LK_WARPS_PER_CTA - 1) / ((long)args.quota * LK_WARPS_PER_CTA);
-    } else {
-        ctas = (items + LK_WARPS_PER_CTA - 1) / LK_WARPS_PER_CTA;
-        if (ctas > resident) ctas = resident;
-    }
+    const long resident = (long)(sm_count > 0 ? sm_count : 148) * LK_CTAS_PER_SM;
+    long ctas = (items + LK_WARPS_PER_CTA - 1) / LK_WARPS_PER_CTA;
+    if (ctas > resident) ctas = resident;
     const int thr = LK_WARPS_PER_CTA * 32;
     const size_t sh = vo_lk_smem_bytes();
-    if (!args.use_tma) k_lk_ring<false, LK_CTAS_PER_SM><<<(int)ctas, thr, sh, stream>>>(maps, args);
-    else if (cps == 12) k_lk_ring<true, 12><<<(int)ctas, thr, sh, stream>>>(maps, args);
-    else if (cps == 10) k_lk_ring<true, 10><<<(int)ctas, thr, sh, stream>>>(maps, args);
-    else k_lk_ring<true, 8><<<(int)ctas, thr, sh, stream>>>(maps, args);
+    if (args.use_tma) k_lk_ring<true><<<(int)ctas, thr, sh, stream>>>(maps, args);
+    else k_lk_ring<false><<<(int)ctas, thr, sh, stream>>>(maps, args);
     return cudaGetLastError();
 }

@@ -2,9 +2,7 @@
 #pragma once
 #include "common.cuh"
 
-// The kernel is built for 8 persistent CTAs of 2 warps per SM (128 registers per thread: the whole register file) and, for
-// A/B measurement, for 10 and 12 (96 / 80 registers; 8960 B of shared memory per warp: 12 x (2 x 8960 + 1024 reserved) =
-// 227 328 B of the SM's 233 472 B).
+// The kernel is built for 8 persistent CTAs of 2 warps per SM: 128 registers per thread, the whole register file.
 #define LK_WARPS_PER_CTA 2
 #define LK_CTAS_PER_SM 8
 
@@ -38,7 +36,6 @@ struct LkArgs {
     int* queue;
     int per_unit;           // feature slots per unit that can be live (<= cap)
     int span;               // phases (level-solves) per work item; 0 or >= ncalls*nlevels = one item per feature-ring
-    int quota;              // work items a warp takes before it retires (0 = until the queue is empty)
     int* progress;          // [n_units][cap] phases completed per feature (hand-over between items; all zero between launches)
     // plain-load staging (debug / A-B measurement; VO_LK_STAGING=ldg): plane geometry per level
     int use_tma;
@@ -51,7 +48,5 @@ struct LkArgs {
 size_t vo_lk_smem_bytes();
 cudaError_t vo_lk_prepare();
 // sm_count sizes the persistent grid (CTAs = min(needed, sm_count * LK_CTAS_PER_SM))
-// ctas_per_sm: 0 = LK_CTAS_PER_SM; 10 / 12 select the instantiations built with fewer registers (A/B measurement)
-cudaError_t vo_launch_lk_ring(const LkMaps& maps, const LkArgs& args, int sm_count, int ctas_per_sm, cudaStream_t stream);
-int vo_lk_ctas_per_sm(int requested);     // the instantiation a request maps to
+cudaError_t vo_launch_lk_ring(const LkMaps& maps, const LkArgs& args, int sm_count, cudaStream_t stream);
 int vo_launch_pyramid(const PyrGeom& pg, const uint8_t* const* src_tab_dev, int src_pitch, cudaStream_t stream);

@@ -137,9 +137,9 @@ static const EssResult* seq_ess_result(vo_ctx* ctx, int unit)
 static int seq_front(vo_ctx* ctx, int s0, int s1, int p, bool bgr)
 {
     const int n = ctx->seq_n, unit = p * n;
-    ctx->imgs_per_unit = 2;                                   // sequence q's pair of a slot: planes 2q, 2q + 1 of it
     const int L0 = 2 * n * s0, R0 = L0 + 1, L1 = 2 * n * s1, R1 = L1 + 1;
-    const View v{unit, n, ctx->stream, 0};                    // image planes are addressed from plane 0 whatever the parity
+    // image planes are addressed from plane 0 whatever the parity; sequence q's pair of a slot is planes 2q, 2q + 1 of it
+    const View v{unit, n, ctx->stream, 0, 2, seq_grid(ctx)};
     int rc;
     if (bgr && (rc = convert_pairs(ctx, s1))) return rc;
     // the new pairs' pyramids (the previous pairs' are already resident)
@@ -151,10 +151,7 @@ static int seq_front(vo_ctx* ctx, int s0, int s1, int p, bool bgr)
     ctx->launches += vo_launch_seq_append(a, n, ctx->stream);
     ctx->launches += vo_launch_seq_bucket(a, n, ctx->stream);
     const int ip[4] = {L0, R0, R1, L1}, in[4] = {R0, R1, L1, L0};
-    ctx->lk_per_unit = seq_grid(ctx);
-    rc = vo_run_lk_ring(ctx, v, 4, ip, in, false);
-    ctx->lk_per_unit = 0;
-    if (rc) return rc;
+    if ((rc = vo_run_lk_ring(ctx, v, 4, ip, in, false))) return rc;
     if ((rc = vo_run_filter(ctx, v, true))) return rc;
     if (ctx->seq_mono) {        // findEssentialMat + recoverPose on (L0, L1), beside the carry and the triangulation (n_seq = 1)
         EssArgs e;
@@ -177,7 +174,7 @@ static int seq_front(vo_ctx* ctx, int s0, int s1, int p, bool bgr)
 // back stage on side stream 0: trackingFrame2Frame's PnP + translation carry (+ the mono rotation into the record)
 static int seq_back(vo_ctx* ctx, int p)
 {
-    cudaStream_t st = ctx->side_stream[0];
+    cudaStream_t st = ctx->lane[0].side;
     const int n = ctx->seq_n, unit = p * n;
     const View v{unit, n, st, 0};
     const size_t cs = (size_t)ctx->units * ctx->cap;
@@ -189,37 +186,6 @@ static int seq_back(vo_ctx* ctx, int p)
     ctx->launches += vo_launch_seq_finish(a, n, st);
     if (ctx->seq_mono) ctx->launches += vo_launch_seq_mono(ctx->d_results + unit, seq_ess_result(ctx, unit), st);
     VO_CUDA_CHECK(cudaGetLastError());
-    return VO_OK;
-}
-
-// replay (or first capture) one stage as a CUDA graph on stream `st`
-template <typename F>
-static int seq_graph(vo_ctx* ctx, int key, cudaStream_t st, F launch)
-{
-    if (!ctx->use_graphs) return launch();
-    for (auto& g : ctx->graphs)
-        if (g.u0 == key && g.tma == ctx->lk_use_tma && g.s == st) {
-            VO_CUDA_CHECK(cudaGraphLaunch(g.exec, st));
-            ctx->launches += g.launches;
-            return VO_OK;
-        }
-    const bool timing = ctx->lk_timing;
-    const long long before = ctx->launches;
-    ctx->lk_timing = false;
-    cudaGraph_t graph = nullptr;
-    VO_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    int rc = launch();
-    cudaError_t e = cudaStreamEndCapture(st, &graph);
-    ctx->lk_timing = timing;
-    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-    VO_CUDA_CHECK(e);
-    vo_ctx::RangeGraph g;
-    g.u0 = key; g.n = 1; g.detect = true; g.tma = ctx->lk_use_tma; g.s = st; g.max_pts = 0;
-    g.launches = ctx->launches - before;
-    VO_CUDA_CHECK(cudaGraphInstantiate(&g.exec, graph, 0));
-    cudaGraphDestroy(graph);
-    ctx->graphs.push_back(g);
-    VO_CUDA_CHECK(cudaGraphLaunch(g.exec, st));
     return VO_OK;
 }
 
@@ -259,26 +225,19 @@ static int seq_state_alloc(vo_ctx* ctx, int n)
 
 static int seq_events(vo_ctx* ctx)
 {
-    if (ctx->seq_front_ev[0]) return VO_OK;
-    for (int k = 0; k < 2; k++) {
-        VO_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->seq_front_ev[k], cudaEventDisableTiming));
-        VO_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->seq_back_ev[k], cudaEventDisableTiming));
-    }
-    if (!ctx->side_stream[0]) {
-        VO_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->fork_ev, cudaEventDisableTiming));
-        for (int c = 0; c < VO_LANES; c++) {
-            VO_CUDA_CHECK(cudaStreamCreateWithFlags(&ctx->side_stream[c], cudaStreamNonBlocking));
-            VO_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->join_ev[c], cudaEventDisableTiming));
+    if (!ctx->seq_front_ev[0])
+        for (int k = 0; k < 2; k++) {
+            VO_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->seq_front_ev[k], cudaEventDisableTiming));
+            VO_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->seq_back_ev[k], cudaEventDisableTiming));
         }
-    }
-    return VO_OK;
+    return vo_ensure_lanes(ctx);
 }
 
 // retire every frame in flight without reporting it (state queries / re-begin / destroy)
 static int seq_drain(vo_ctx* ctx)
 {
     if (ctx->seq_inflight > 0) {
-        VO_CUDA_CHECK(cudaStreamSynchronize(ctx->side_stream[0]));
+        VO_CUDA_CHECK(cudaStreamSynchronize(ctx->lane[0].side));
         VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
     }
     return VO_OK;
@@ -307,7 +266,7 @@ static int seq_begin(vo_ctx* ctx, int n, bool multi, int w, int h, const float P
     if (ctx->seq_active && (rc = seq_drain(ctx))) return rc;
     ctx->seq_inflight = 0;
     ctx->seq_active = false;
-    if ((rc = vo_ensure_state(ctx, w, h, 2 * n, 4))) return rc;      // two per-frame buffer units per sequence (frames in flight)
+    if ((rc = vo_ensure_state(ctx, w, h, 2 * n))) return rc;      // two per-frame buffer units per sequence (frames in flight)
     if ((rc = seq_state_alloc(ctx, n))) return rc;
     if ((rc = seq_events(ctx))) return rc;
     // the frame graphs are captured for one sequence count, and with or without the mono branch (which a sequence keeps)
@@ -317,7 +276,6 @@ static int seq_begin(vo_ctx* ctx, int n, bool multi, int w, int h, const float P
     if (ctx->seq_mono && (rc = seq_mono_scratch(ctx))) return rc;
     if ((rc = vo_ensure_pinned(ctx, seq_pinned(ctx, n).bytes))) return rc;
     vo_set_calibration(ctx, P_l, P_r);
-    ctx->imgs_per_unit = 2;
     ctx->seq_slot = 0;
     ctx->seq_frames = 0;
     ctx->seq_submitted = 0;
@@ -411,11 +369,11 @@ static int seq_submit(vo_ctx* ctx, const uint8_t* const* lefts, const uint8_t* c
         // current one (it is re-recorded below).  So this copy runs under the front stage of the frame in flight.
         // (No ordering against the caller's stream is needed: vo_seq_begin synchronises, and every later access to
         // the image slots is made by this file and ordered through these events.)
-        cudaStream_t sc = ctx->side_stream[1];
+        cudaStream_t sc = ctx->lane[1].side;
         VO_CUDA_CHECK(cudaStreamWaitEvent(sc, ctx->seq_front_ev[p], 0));
         if ((rc = upload_pairs(ctx, s1, lefts, rights, pitch, channels, sc))) return rc;
-        VO_CUDA_CHECK(cudaEventRecord(ctx->join_ev[1], sc));
-        VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->join_ev[1], 0));
+        VO_CUDA_CHECK(cudaEventRecord(ctx->lane[1].join, sc));
+        VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->lane[1].join, 0));
     }
     return seq_enqueue(ctx, p, s0, s1, bgr);
 }
@@ -436,12 +394,17 @@ extern "C" int vo_seq_submit(vo_ctx* ctx, const uint8_t* left1, const uint8_t* r
 static int seq_enqueue(vo_ctx* ctx, int p, int s0, int s1, bool bgr)
 {
     int rc;
-    if ((rc = seq_graph(ctx, -1 - (s0 + 3 * p + 6 * (bgr ? 1 : 0)), ctx->stream, [&] { return seq_front(ctx, s0, s1, p, bgr); }))) return rc;
+    GraphKey key{};
+    key.kind = GraphKey::SEQ_FRONT; key.s = ctx->stream; key.tma = ctx->lk_use_tma;
+    key.slot = s0; key.parity = p; key.bgr = bgr;
+    if ((rc = vo_run_graph(ctx, key, [&] { return seq_front(ctx, s0, s1, p, bgr); }))) return rc;
     VO_CUDA_CHECK(cudaEventRecord(ctx->seq_front_ev[p], ctx->stream));
     // back stage: after this frame's front stage; after the previous frame's back stage by stream order
-    cudaStream_t sb = ctx->side_stream[0];
+    cudaStream_t sb = ctx->lane[0].side;
     VO_CUDA_CHECK(cudaStreamWaitEvent(sb, ctx->seq_front_ev[p], 0));
-    if ((rc = seq_graph(ctx, -100 - p, sb, [&] { return seq_back(ctx, p); }))) return rc;
+    key = GraphKey{};
+    key.kind = GraphKey::SEQ_BACK; key.s = sb; key.tma = ctx->lk_use_tma; key.parity = p;
+    if ((rc = vo_run_graph(ctx, key, [&] { return seq_back(ctx, p); }))) return rc;
     const int n = ctx->seq_n, u0 = p * n;
     const SeqPinned pin = seq_pinned(ctx, n);
     VO_CUDA_CHECK(cudaMemcpyAsync(pin.rec + u0, ctx->d_results + u0, n * sizeof(vo_unit_result_dev), cudaMemcpyDeviceToHost, sb));
@@ -474,7 +437,7 @@ extern "C" int vo_seq_submit_device(vo_ctx* ctx, const vo_dimage* left1, const v
     // As the host gray upload: on the copy stream, into slot s1 once the frame that last read it has finished its front
     // stage, so the conversion runs under the frame in flight; it is launched outside the frame graph (its source pointers
     // change every frame), and the frame replays the gray front graph.
-    cudaStream_t sc = ctx->side_stream[1];
+    cudaStream_t sc = ctx->lane[1].side;
     VO_CUDA_CHECK(cudaStreamWaitEvent(sc, ctx->seq_front_ev[unit], 0));
     VO_CUDA_CHECK(cudaStreamWaitEvent(sc, ctx->fork_ev, 0));
     vo_dimage* tab = seq_pinned_tab(ctx) + 2 * s1;
@@ -482,8 +445,8 @@ extern "C" int vo_seq_submit_device(vo_ctx* ctx, const vo_dimage* left1, const v
     if ((rc = vo_ingest_device(ctx, tab, 2, 2 * s1, sc))) return rc;
     // The join is also the release: the caller's later work on ctx->stream is ordered after the conversion, the last read
     // of the images.
-    VO_CUDA_CHECK(cudaEventRecord(ctx->join_ev[1], sc));
-    VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->join_ev[1], 0));
+    VO_CUDA_CHECK(cudaEventRecord(ctx->lane[1].join, sc));
+    VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->lane[1].join, 0));
     return seq_enqueue(ctx, unit, s0, s1, false);
 }
 
@@ -501,7 +464,7 @@ static int seq_wait(vo_ctx* ctx, vo_unit_result* out, int* status, vo_mono_resul
     ctx->seq_inflight--;
     ctx->seq_frames++;
     const size_t cs = (size_t)ctx->units * ctx->cap;
-    cudaStream_t sb = ctx->side_stream[0];
+    cudaStream_t sb = ctx->lane[0].side;
     bool copies = false;
     int rc = VO_OK;
     for (int q = 0; q < n; q++) {
