@@ -1,7 +1,9 @@
 """Streaming sequence mode (vo_seq_*): 20+ synthetic frames with the main-loop state (features, ages,
 translation) resident on the GPU, compared frame by frame with the reference path (cv2 through the
-verbatim glue of oracle/ref_path.py): FAST refill, bucketing (aliasing, age limit, overwrite rule),
-ages/points length skew, circular matching, triangulation, PnP with the carried extrinsic guess."""
+verbatim glue of oracle/ref_path.py): FAST refill, bucketing (aliasing, overwrite rule), the carried
+ages/points length skew, circular matching, triangulation, PnP with the carried extrinsic guess.
+On this dense texture ages never pass 1, so neither the age limit of the buckets nor a stale age paired
+with a fresh corner decides anything here: tests/test_gpu_long_tracks.py covers those on a sparse drive."""
 import numpy as np
 import pytest
 

@@ -97,6 +97,59 @@ def stereo_unit(w=1241, h=376, seed=0, cal=KITTI00, scene="v1", noise=1.0, rvec=
                 K=P_l[:, :3].copy(), rvec=np.asarray(rvec, np.float64), tvec=np.asarray(tvec, np.float64))
 
 
+SEQ_STEP_R = np.array([0.001, -0.004, 0.0005])          # per-frame ego-motion of the synthetic drives
+SEQ_STEP_T = np.array([0.01, -0.003, -0.2])
+
+
+def _rodrigues_np(r):
+    r = np.asarray(r, np.float64)
+    th = float(np.linalg.norm(r))
+    if th == 0.0:
+        return np.eye(3)
+    k = r / th
+    Kx = np.array([[0, -k[2], k[1]], [k[2], 0, -k[0]], [-k[1], k[0], 0]])
+    return np.eye(3) + np.sin(th) * Kx + (1.0 - np.cos(th)) * (Kx @ Kx)
+
+
+def blob_sequence(w=1241, h=376, seed=4, n_points=160, n_frames=24, sharp=lambda k: k < 3 or k >= 18,
+                  cal=KITTI00, step_r=SEQ_STEP_R, step_t=SEQ_STEP_T):
+    """A sparse drive on which features live for many frames: n_points isolated world points (X in U(-25, 25),
+    Y in U(-4, 3), Z in U(10, 45) m), each drawn as a Gaussian blob at its exact projection on a flat background of 100
+    with N(0, 1) noise, rounded to u8.  Frame k is rendered at rotation Rodrigues(k step_r) and translation k step_t.
+    Sharp frames (sharp(k) true: sigma 1.3 px, amplitude +80) fire FAST; soft frames (sigma 3.5 px, amplitude +50: the
+    centre-to-ring contrast stays below FAST's threshold of 20) detect nothing new while LK still tracks the blobs, so
+    through a soft stretch the tracked features age by one per frame.  numpy only, deterministic in the seed.
+    Returns (P_l, P_r, frames) with frames[k] = (left, right)."""
+    P_l, P_r = proj_matrices(cal)
+    K = P_l[:, :3].astype(np.float64)
+    base = float(cal["bf"]) / float(cal["fx"])              # X_r = X_l + (base, 0, 0)
+    rng = np.random.default_rng(seed)
+    X = np.stack([rng.uniform(-25, 25, n_points), rng.uniform(-4, 3, n_points), rng.uniform(10, 45, n_points)], 1)
+    yy, xx = np.mgrid[0:h, 0:w].astype(np.float64)
+    r = 15                                                  # blob support: +-15 px (4.3 sigma of a soft blob)
+
+    def render(R, t, is_sharp, noise_seed):
+        Xc = X @ R.T + t
+        u = Xc[:, 0] / Xc[:, 2] * K[0, 0] + K[0, 2]
+        v = Xc[:, 1] / Xc[:, 2] * K[1, 1] + K[1, 2]
+        s, A = (1.3, 80.0) if is_sharp else (3.5, 50.0)
+        img = np.full((h, w), 100.0)
+        for a, b in zip(u, v):
+            x0, x1, y0, y1 = int(max(0, a - r)), int(min(w, a + r + 1)), int(max(0, b - r)), int(min(h, b + r + 1))
+            if x0 >= x1 or y0 >= y1:
+                continue
+            img[y0:y1, x0:x1] += A * np.exp(-((xx[y0:y1, x0:x1] - a) ** 2 + (yy[y0:y1, x0:x1] - b) ** 2) / (2 * s * s))
+        img += np.random.default_rng(noise_seed).normal(0, 1.0, img.shape)
+        return np.clip(np.rint(img), 0, 255).astype(np.uint8)
+
+    frames = []
+    for k in range(n_frames):
+        R = _rodrigues_np(np.asarray(step_r, np.float64) * k)
+        t = np.asarray(step_t, np.float64) * k
+        frames.append((render(R, t, sharp(k), (seed, k, 0)), render(R, t + np.array([base, 0.0, 0.0]), sharp(k), (seed, k, 1))))
+    return P_l, P_r, frames
+
+
 def select_features(corners, n):
     """Even-stride selection over the raster-ordered FAST list (SURVEY.md 8d "Features")."""
     corners = np.asarray(corners, np.float32).reshape(-1, 2)
