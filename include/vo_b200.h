@@ -93,8 +93,8 @@ VO_API int vo_lk_kernel_time(vo_ctx* ctx, double* ms_total, long long* n, int re
  * on high-priority helper streams (k < 0 is refused with VO_E_INVALID; without the option the first
  * vo_batch_submit sets aside 8 SMs when the driver supports green contexts), "batch_outputs" = 1: vo_batch_submit
  * also copies the point lists back (vo_batch_outputs), "mono_rotation" = 0 (default) | 1: sequences begun from then
- * on run trackingFrame2Frame(mono_rotation = true), see vo_seq_wait_mono (a sequence keeps the value it was begun
- * with). */
+ * on with vo_seq_begin* run trackingFrame2Frame(mono_rotation = true), see vo_seq_wait_mono (a sequence keeps the value
+ * it was begun with; vo_mseq_begin* refuse the option, they take the flag VO_MSEQ_MONO_ROTATION instead). */
 VO_API int vo_set_option(vo_ctx* ctx, const char* key, double value);
 
 /* ---- A1: cv::FAST(image, kps, threshold, nonmax) + KeyPoint::convert ------------------------
@@ -357,17 +357,34 @@ VO_API int vo_seq_state(vo_ctx* ctx, vo_point2f* points, int32_t* ages, int cap,
  *                   VO_E_CAPACITY when a status is, else VO_OK; every record is filled either way.
  *   vo_mseq_pose / vo_mseq_state   vo_seq_pose / vo_seq_state of sequence q
  * Refused with VO_E_INVALID: n_seq < 1, a third submission in flight, a wait with nothing in flight, a pair with one NULL
- * image, a pair for a retired sequence.  VO_E_UNSUPPORTED: the option "mono_rotation" is on.  VO_E_CAPACITY: n_seq above
- * VO_MSEQ_MAX.  Device-memory inputs (vo_dimage) are not accepted in this mode.
+ * image, a pair for a retired sequence, unknown flag bits.  VO_E_UNSUPPORTED: the option "mono_rotation" is on (in this
+ * mode the branch is asked for with the flag below, for every sequence at once).  VO_E_CAPACITY: n_seq above VO_MSEQ_MAX.
+ * Device-memory inputs (vo_dimage) are not accepted in this mode.
+ * trackingFrame2Frame(mono_rotation = true) for every sequence: vo_mseq_begin_ex with the flag VO_MSEQ_MONO_ROTATION
+ * (vo_mseq_begin is vo_mseq_begin_ex with flags = 0).  Each sequence then gets what vo_seq_wait_mono gives a single
+ * sequence begun with the option "mono_rotation" -- the record's R is recoverPose's rotation, rvec / tvec / n_inliers /
+ * ransac_iters / pnp_status and the carried translation stay the PnP's, a frame where the reference would throw is
+ * reported with mono.status = VO_E_TOO_FEW_POINTS and R = I and is not integrated -- bit for bit as running it alone.
+ * The essential-matrix RANSAC of all sequences runs as one launch per stage, so the launches per submission stay those
+ * of one vo_seq_submit with the option.  Device scratch: about 0.8 MB per sequence and frame in flight at 1241x376.
+ *   vo_mseq_wait_mono  vo_mseq_wait plus, per sequence q, mono[q] (zeroed for a retired sequence) and, optionally, the
+ *                      essential inlier mask at ess_mask + mask_cap * q, aligned with sequence q's point lists (the first
+ *                      out[q].n_valid entries meaningful).  VO_E_INVALID on sequences begun without the flag.
+ *                      vo_mseq_wait works on flagged sequences too (R = the mono rotation).
  * Starting either sequence mode ends the other one if it is idle and is refused while it has frames in flight; the
  * vo_seq_* frame calls are refused while vo_mseq_* sequences run and the other way round.  Every other entry point that
  * reuses the shared buffers is refused while submissions are in flight, as for vo_seq_submit. */
 #define VO_MSEQ_MAX 64
 #define VO_MSEQ_RETIRED 2        /* vo_mseq_wait status: the sequence was retired by this or an earlier submission */
+#define VO_MSEQ_MONO_ROTATION 1  /* vo_mseq_begin_ex flag: every sequence runs trackingFrame2Frame(mono_rotation = true) */
 VO_API int vo_mseq_begin(vo_ctx* ctx, int n_seq, int w, int h, const float P_l[12], const float P_r[12], const uint8_t* const* left0,
                          const uint8_t* const* right0, size_t pitch, int channels);
+VO_API int vo_mseq_begin_ex(vo_ctx* ctx, int n_seq, int w, int h, const float P_l[12], const float P_r[12],
+                            const uint8_t* const* left0, const uint8_t* const* right0, size_t pitch, int channels, int flags);
 VO_API int vo_mseq_submit(vo_ctx* ctx, const uint8_t* const* left1, const uint8_t* const* right1, size_t pitch, int channels);
 VO_API int vo_mseq_wait(vo_ctx* ctx, vo_unit_result* out, int* status, vo_point2f* pts4, int pts_cap);
+VO_API int vo_mseq_wait_mono(vo_ctx* ctx, vo_unit_result* out, int* status, vo_mono_result* mono,
+                             uint8_t* ess_mask, int mask_cap, vo_point2f* pts4, int pts_cap);
 VO_API int vo_mseq_pose(vo_ctx* ctx, int q, double frame_pose[16]);
 VO_API int vo_mseq_state(vo_ctx* ctx, int q, vo_point2f* points, int32_t* ages, int cap, int* n_points, int* n_ages, double t_out[3]);
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Scaling of the multi-sequence streaming mode (vo_mseq_*) with the number of sequences, measured on the GPU.
 
-    python tools/mseq_timing.py [--frames 40] [--rounds 5] [--counts 1,2,4,8,16,32] [--json out.json]
+    python tools/mseq_timing.py [--frames 40] [--rounds 5] [--counts 1,2,4,8,16,32] [--mono-rotation] [--json out.json]
 
 Synthetic 1241x376 drives (synth.stereo_unit; eight seeds, each with its own motion) of `--frames` frames each;
 sequence q replays drive q % 8, forwards for even q // 8 and backwards for odd, so up to 16 sequences are distinct and
@@ -10,7 +10,9 @@ larger counts repeat them (the work per sequence is the same either way).  One c
   - n_seq = each count: vo_mseq_submit / vo_mseq_wait with two submissions in flight
 and reports per mode the median over the rounds of the aggregate frames/s (sequence-frames per second of wall time), the
 per-step latency (wall time per submission in the pipelined loop) and the kernel launches per submission
-(vo_kernel_launches).  The card's name, power limit and max SM clock, read in the same run, are printed with the numbers;
+(vo_kernel_launches).  `--mono-rotation` runs every mode twice per round, without and with trackingFrame2Frame's
+mono_rotation branch (the option "mono_rotation" for vo_seq_*, the flag VO_MSEQ_MONO_ROTATION for vo_mseq_*), and
+reports both.  The card's name, power limit and max SM clock, read in the same run, are printed with the numbers;
 they are part of them."""
 import argparse
 import json
@@ -61,23 +63,25 @@ def sequence(dr, q):
     return fr if (q // DRIVES) % 2 == 0 else fr[::-1]
 
 
-def run_seq(ctx, P_l, P_r, fr):
+def run_seq(ctx, P_l, P_r, fr, mono=False):
+    ctx.set_option("mono_rotation", 1 if mono else 0)
     ctx.seq_begin(fr[0][0], fr[0][1], P_l, P_r)
+    ctx.set_option("mono_rotation", 0)             # the sequence keeps the value it was begun with
     l0 = ctx.kernel_launches()
     t0 = time.perf_counter()
     ctx.seq_submit(*fr[1])
     for k in range(1, len(fr)):
         if k + 1 < len(fr):
             ctx.seq_submit(*fr[k + 1])
-        ctx.seq_wait(want_points=False)
+        ctx.seq_wait(want_points=False, mono=mono)
     dt = time.perf_counter() - t0
     steps = len(fr) - 1
     return steps / dt, dt / steps, (ctx.kernel_launches() - l0) / steps
 
 
-def run_mseq(ctx, P_l, P_r, seqs):
+def run_mseq(ctx, P_l, P_r, seqs, mono=False):
     n, nf = len(seqs), len(seqs[0])
-    ctx.mseq_begin([s[0][0] for s in seqs], [s[0][1] for s in seqs], P_l, P_r)
+    ctx.mseq_begin([s[0][0] for s in seqs], [s[0][1] for s in seqs], P_l, P_r, mono_rotation=mono)
     frame = [([s[k][0] for s in seqs], [s[k][1] for s in seqs]) for k in range(nf)]
     l0 = ctx.kernel_launches()
     t0 = time.perf_counter()
@@ -85,7 +89,7 @@ def run_mseq(ctx, P_l, P_r, seqs):
     for k in range(1, nf):
         if k + 1 < nf:
             ctx.mseq_submit(*frame[k + 1])
-        ctx.mseq_wait(want_points=False)
+        ctx.mseq_wait(want_points=False, mono=mono)
     dt = time.perf_counter() - t0
     steps = nf - 1
     return n * steps / dt, dt / steps, (ctx.kernel_launches() - l0) / steps
@@ -96,6 +100,7 @@ def main():
     ap.add_argument("--frames", type=int, default=40)
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--counts", default="1,2,4,8,16,32")
+    ap.add_argument("--mono-rotation", action="store_true", help="also time every mode with the mono_rotation branch")
     ap.add_argument("--json", help="also write the result here")
     a = ap.parse_args()
     counts = [int(c) for c in a.counts.split(",")]
@@ -105,16 +110,18 @@ def main():
     dr = drives(a.frames + 1)
     print(f"rendered {DRIVES} drives x {a.frames + 1} frames in {time.perf_counter() - t0:.0f} s", flush=True)
     ctx = capi.Context(0, max_features=4096)
-    modes = ["seq"] + counts
+    monos = (False, True) if a.mono_rotation else (False,)
+    modes = [(m, mono) for m in ["seq"] + counts for mono in monos]
     seqs = {n: [sequence(dr, q) for q in range(n)] for n in counts}
     res = {m: dict(fps=[], lat=[], launches=[]) for m in modes}
 
-    def run(m, fr_cut=None):
+    def run(mode, fr_cut=None):
+        m, mono = mode
         if m == "seq":
             fr = dr[0] if fr_cut is None else dr[0][:fr_cut]
-            return run_seq(ctx, P_l, P_r, fr)
+            return run_seq(ctx, P_l, P_r, fr, mono)
         s = seqs[m] if fr_cut is None else [x[:fr_cut] for x in seqs[m]]
-        return run_mseq(ctx, P_l, P_r, s)
+        return run_mseq(ctx, P_l, P_r, s, mono)
 
     for _ in range(a.rounds):
         for m in modes:
@@ -124,14 +131,15 @@ def main():
     ctx.close()
     out = dict(card=card(), image=f"{W}x{H}", frames=a.frames, rounds=a.rounds, in_flight=2, modes={})
     print(f"card (name, power limit, max SM clock): {out['card']}")
-    for m in modes:
-        r = res[m]
+    for mode in modes:
+        r = res[mode]
         o = dict(aggregate_fps=float(np.median(r["fps"])), aggregate_fps_min=float(np.min(r["fps"])),
                  aggregate_fps_max=float(np.max(r["fps"])), step_latency_ms=1e3 * float(np.median(r["lat"])),
                  launches_per_submission=float(np.median(r["launches"])))
-        out["modes"][str(m)] = o
-        name = "vo_seq (1 sequence)" if m == "seq" else f"vo_mseq n_seq = {m:2d}"
-        print(f"{name:22s}: {o['aggregate_fps']:8.0f} frames/s [{o['aggregate_fps_min']:.0f}, {o['aggregate_fps_max']:.0f}], "
+        m, mono = mode
+        out["modes"][str(m) + ("+mono" if mono else "")] = o
+        name = ("vo_seq (1 sequence)" if m == "seq" else f"vo_mseq n_seq = {m:2d}") + (", mono" if mono else "")
+        print(f"{name:28s}: {o['aggregate_fps']:8.0f} frames/s [{o['aggregate_fps_min']:.0f}, {o['aggregate_fps_max']:.0f}], "
               f"step {o['step_latency_ms']:.3f} ms, {o['launches_per_submission']:.1f} launches / submission")
     print(json.dumps(out))
     if a.json:

@@ -9,7 +9,9 @@ submission advances every sequence by one frame (two submissions in flight), and
 frame, so sequences of unequal length share the run.  frame_pose of each is integrated with the reference's Euler and
 scale gates (src/main.cpp:196-208), written to OUTDIR/<name>.txt in the KITTI text format (<name> = the dataset
 directory's name) and, with --gt, scored against GTDIR/<name>.txt with the KITTI segment metric.  All sequences must
-have the image size of the first.  `--check` only validates the inputs (no GPU needed)."""
+have the image size of the first.  `--mono-rotation` runs trackingFrame2Frame as its header default does, for every
+sequence (mono_rotation = true: the rotation from findEssentialMat + recoverPose, the translation from the PnP; frames
+where that branch would abort are reported and not integrated).  `--check` only validates the inputs (no GPU needed)."""
 import argparse
 import os
 import sys
@@ -30,6 +32,8 @@ def main():
     ap.add_argument("--gt", metavar="GTDIR", help="score each sequence against GTDIR/<name>.txt")
     ap.add_argument("--threads", type=int, default=4, help="decoder threads per sequence")
     ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--mono-rotation", action="store_true",
+                    help="rotation from findEssentialMat + recoverPose (trackingFrame2Frame's header default)")
     ap.add_argument("--check", action="store_true")
     a = ap.parse_args()
     from visual_odom_b200 import capi, synth
@@ -55,6 +59,8 @@ def main():
         seqs.append(dict(dir=d, name=name, n=n, w=w, h=h, gray=ctype == 0, gt=gt))
         print(f"{name}: {n} stereo pairs of {w}x{h} (PNG colour type {ctype}, {depth} bit)")
     print(f"P_left =\n{P_l}\nP_right =\n{P_r}")
+    print("rotation: " + ("findEssentialMat + recoverPose (mono_rotation = true)" if a.mono_rotation else
+                          "Rodrigues of the PnP rvec (mono_rotation = false)"))
     if a.check:
         return
     # one pitch and one channel count per submission: colour files are read as BGR (converted on the device) unless the
@@ -78,8 +84,9 @@ def main():
         return lp, rp, pitch, ch
 
     lp, rp, pitch, ch = pairs(0)
-    ctx.mseq_begin_ptr(seqs[0]["w"], seqs[0]["h"], lp, rp, pitch, P_l, P_r, ch)
+    ctx.mseq_begin_ptr(seqs[0]["w"], seqs[0]["h"], lp, rp, pitch, P_l, P_r, ch, mono_rotation=a.mono_rotation)
     poses = [[np.eye(4)] for _ in seqs]
+    aborted = [0] * len(seqs)
     steps = max(s["n"] for s in seqs)
     t0 = time.perf_counter()
     done = 0
@@ -87,12 +94,14 @@ def main():
     for k in range(1, steps):
         if k + 1 < steps:
             ctx.mseq_submit_ptr(*pairs(k + 1))
-        recs = ctx.mseq_wait(want_points=False)
+        recs = ctx.mseq_wait(want_points=False, mono=a.mono_rotation)
         for q, r in enumerate(recs):
             if r["status"] == capi.VO_MSEQ_RETIRED:
                 continue
             if r["status"] != capi.VO_OK:
                 print(f"{seqs[q]['name']} frame {k}: status {r['status']} ({ctx.lib.vo_last_error(ctx.h).decode()})")
+            if a.mono_rotation and r["mono"]["status"] != capi.VO_OK:
+                aborted[q] += 1
             poses[q].append(ctx.mseq_pose(q))
             done += 1
         if k % 100 == 0 or k == steps - 1:
@@ -101,10 +110,12 @@ def main():
         rd.close()
     ctx.close()
     os.makedirs(a.poses, exist_ok=True)
-    for s, p in zip(seqs, poses):
+    for s, p, n_abort in zip(seqs, poses, aborted):
         path = os.path.join(a.poses, s["name"] + ".txt")
         capi.poses_save(path, p)
         line = f"{s['name']}: {len(p)} poses -> {path}"
+        if a.mono_rotation:
+            line += f", {n_abort} frames where findEssentialMat / recoverPose would abort (reported, not integrated)"
         if s["gt"]:
             gt = capi.poses_load(s["gt"])[:len(p)]
             seg, t_err, r_err = capi.eval_segments(gt, p[:len(gt)])

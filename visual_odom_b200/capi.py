@@ -21,6 +21,7 @@ VO_DIST_DEPTH = 8          # gathers that may be outstanding (include/vo_b200.h)
 VO_E_CAPACITY = -5
 VO_MSEQ_MAX = 64           # sequences one vo_mseq_begin may start (include/vo_b200.h)
 VO_MSEQ_RETIRED = 2        # vo_mseq_wait status of a retired sequence
+VO_MSEQ_MONO_ROTATION = 1  # vo_mseq_begin_ex flag: every sequence runs trackingFrame2Frame(mono_rotation = true)
 
 
 class VoParams(C.Structure):
@@ -176,8 +177,12 @@ SIGNATURES = {
     "vo_batch_submit_device": (C.c_int, [C.c_void_p, C.POINTER(VoDUnit), C.c_int, C.c_int]),
     "vo_mseq_begin": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                 C.c_int]),
+    "vo_mseq_begin_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_size_t, C.c_int, C.c_int]),
     "vo_mseq_submit": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
     "vo_mseq_wait": (C.c_int, [C.c_void_p, C.POINTER(VoUnitResult), C.c_void_p, C.c_void_p, C.c_int]),
+    "vo_mseq_wait_mono": (C.c_int, [C.c_void_p, C.POINTER(VoUnitResult), C.c_void_p, C.POINTER(VoMonoResult), C.c_void_p,
+                                    C.c_int, C.c_void_p, C.c_int]),
     "vo_mseq_pose": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     "vo_mseq_state": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
                                 C.c_void_p]),
@@ -718,21 +723,24 @@ class Context:
         ch = 1 if len(geom) == 2 else 3
         return lp, rp, geom[1] * ch, ch, keep, geom
 
-    def mseq_begin(self, lefts, rights, P_l, P_r):
-        """Start len(lefts) sequences (one calibration, one image size) from their first stereo pairs."""
+    def mseq_begin(self, lefts, rights, P_l, P_r, mono_rotation=False):
+        """Start len(lefts) sequences (one calibration, one image size) from their first stereo pairs.  mono_rotation=True:
+        every sequence runs trackingFrame2Frame(mono_rotation = true) (flag VO_MSEQ_MONO_ROTATION; see mseq_wait(mono=True))."""
         lp, rp, pitch, ch, keep, geom = self._pairs(lefts, rights, False)
         P_l = np.ascontiguousarray(P_l, np.float32).reshape(12); P_r = np.ascontiguousarray(P_r, np.float32).reshape(12)
         h, w = (geom or (0, 0))[:2]
-        self._check(self.lib.vo_mseq_begin(self.h, len(lefts), w, h, _p(P_l), _p(P_r), lp, rp, pitch, ch))
+        flags = VO_MSEQ_MONO_ROTATION if mono_rotation else 0
+        self._check(self.lib.vo_mseq_begin_ex(self.h, len(lefts), w, h, _p(P_l), _p(P_r), lp, rp, pitch, ch, flags))
         self._mseq_n, self._mseq_pitch = len(lefts), pitch
         self._mseq_keep = [None, None]
 
-    def mseq_begin_ptr(self, w, h, left_ptrs, right_ptrs, pitch, P_l, P_r, channels=1):
+    def mseq_begin_ptr(self, w, h, left_ptrs, right_ptrs, pitch, P_l, P_r, channels=1, mono_rotation=False):
         """Raw host pointers, one pair per sequence (e.g. the pinned buffers of one SequenceReader each)."""
         n = len(left_ptrs)
         lp, rp = (C.c_void_p * n)(*left_ptrs), (C.c_void_p * n)(*right_ptrs)
         Pl = np.ascontiguousarray(P_l, np.float32); Pr = np.ascontiguousarray(P_r, np.float32)
-        self._check(self.lib.vo_mseq_begin(self.h, n, w, h, _p(Pl), _p(Pr), lp, rp, pitch, channels))
+        flags = VO_MSEQ_MONO_ROTATION if mono_rotation else 0
+        self._check(self.lib.vo_mseq_begin_ex(self.h, n, w, h, _p(Pl), _p(Pr), lp, rp, pitch, channels, flags))
         self._mseq_n, self._mseq_pitch = n, pitch
         self._mseq_keep = [None, None]
 
@@ -752,21 +760,33 @@ class Context:
         self._check(self.lib.vo_mseq_submit(self.h, lp, rp, pitch or self._mseq_pitch, ch))
         self._mseq_keep = [self._mseq_keep[1], keep]
 
-    def mseq_wait(self, pts_cap=4096, want_points=True):
+    def mseq_wait(self, pts_cap=4096, want_points=True, mono=False):
         """The oldest submission: one dict per sequence with seq_wait's keys plus "status" (VO_OK, VO_E_CAPACITY or
-        VO_MSEQ_RETIRED)."""
+        VO_MSEQ_RETIRED).  mono=True (sequences begun with mono_rotation=True): also "mono" and "ess_mask" per sequence, as
+        seq_wait(mono=True) gives them (vo_mseq_wait_mono; a retired sequence's "mono" is zeroed, its mask empty)."""
         n = self._mseq_n
         res = (VoUnitResult * n)()
         st = np.zeros(n, np.int32)
         pts4 = np.zeros((n, 4, pts_cap, 2), np.float32) if want_points else None
-        self._check(self.lib.vo_mseq_wait(self.h, res, _p(st), _p(pts4), pts_cap if want_points else 0), ok=(VO_OK, VO_E_CAPACITY))
+        npts = pts_cap if want_points else 0
+        if mono:
+            ms = (VoMonoResult * n)()
+            mask = np.zeros((n, pts_cap), np.uint8)
+            self._check(self.lib.vo_mseq_wait_mono(self.h, res, _p(st), ms, _p(mask), pts_cap, _p(pts4), npts), ok=(VO_OK, VO_E_CAPACITY))
+        else:
+            self._check(self.lib.vo_mseq_wait(self.h, res, _p(st), _p(pts4), npts), ok=(VO_OK, VO_E_CAPACITY))
         out = []
         for q in range(n):
             d = self._result_dict(res[q])
             d["status"] = int(st[q])
+            m = min(d["n_valid"], pts_cap) if d["status"] != VO_MSEQ_RETIRED else 0
             if want_points:
-                m = min(d["n_valid"], pts_cap) if d["status"] != VO_MSEQ_RETIRED else 0
                 d.update(l0=pts4[q, 0, :m].copy(), r0=pts4[q, 1, :m].copy(), l1=pts4[q, 2, :m].copy(), r1=pts4[q, 3, :m].copy())
+            if mono:
+                r = ms[q]
+                d["mono"] = dict(status=r.status, n_inliers=r.n_inliers, ransac_iters=r.ransac_iters, n_good=r.n_good,
+                                 R=np.array(r.R[:]).reshape(3, 3), t=np.array(r.t[:]))
+                d["ess_mask"] = mask[q, :m].astype(bool)
             out.append(d)
         return out
 

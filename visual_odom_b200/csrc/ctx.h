@@ -131,13 +131,15 @@ struct vo_ctx {
     // mono_rotation branch (ess.cu): scratch of the essential-matrix RANSAC, allocated on first use
     void* d_ess = nullptr;
     int ess_cap = 0;
-    // the same branch inside the sequence mode (vo_set_option "mono_rotation"): one scratch block per buffer unit (two frames
-    // in flight), separate from d_ess, allocated at vo_seq_begin; the front graph runs it on seq_mono_stream
-    bool mono_opt = false;              // the option; a sequence takes it at vo_seq_begin
-    bool seq_mono = false;              // the running sequence's value
-    void* d_seq_ess = nullptr;          // [2][seq_ess_bytes]
+    // the same branch inside the sequence mode (vo_set_option "mono_rotation" for vo_seq_begin*, the flag
+    // VO_MSEQ_MONO_ROTATION for vo_mseq_begin_ex): one scratch block per buffer unit (2 * seq_n: two frames in flight),
+    // separate from d_ess, allocated at the begin call; the front graph runs it for every sequence on seq_mono_stream
+    bool mono_opt = false;              // the option; a vo_seq_* sequence takes it at vo_seq_begin
+    bool seq_mono = false;              // the running sequences' value
+    void* d_seq_ess = nullptr;          // [seq_ess_units][seq_ess_bytes], block u = buffer unit u
     size_t seq_ess_bytes = 0;
     int seq_ess_cap = 0;                // points each block holds (the bucket grid, at most cap)
+    int seq_ess_units = 0;              // blocks allocated
     cudaStream_t seq_mono_stream = nullptr;
     cudaEvent_t seq_mono_ev[2] = {nullptr, nullptr};     // fork, join
     std::vector<void*> allocs;          // everything cudaMalloc'ed for the batch state

@@ -11,14 +11,18 @@
 //   k_ess_init          normalise the points ((p - pp) / focal in fp64), reset the RANSAC state
 //   k_ess_five          n == 5 only, instead of the RANSAC waves: one five-point solve on all points (no RANSAC in OpenCV);
 //                       n < 5 runs neither (no model: the reference aborts)
-//   k_ess_subsets       1 thread: cv::RNG(2^64-1) stream -> 5 distinct indices per iteration (ptsetreg.cpp getSubset)
+//   k_ess_subsets       1 thread / problem: cv::RNG(2^64-1) stream -> 5 distinct indices per iteration (ptsetreg.cpp getSubset)
 //   k_ess_hypotheses    1 thread / iteration: Nister five-point solver (ess_math.cuh) -> up to 10 E per sample
 //   k_ess_count         1 CTA / (iteration, candidate): Sampson error of all N points, err <= (float)thr^2, count
-//   k_ess_replay        1 thread: candidates in order, `count > max(best, 4)` -> new best, RANSACUpdateNumIters
+//   k_ess_replay        1 thread / problem: candidates in order, `count > max(best, 4)` -> new best, RANSACUpdateNumIters
 //   k_ess_mask          inlier mask of the best E
-//   k_ess_decompose     decomposeEssentialMat
+//   k_ess_decompose     1 thread / problem: decomposeEssentialMat
 //   k_ess_cheirality    1 thread / point: the four [R|t] hypotheses of recoverPose (fp64 DLT, distance threshold 50)
-//   k_ess_pick          recoverPose's vote -> rotation
+//   k_ess_pick          1 thread / problem: recoverPose's vote -> rotation
+// One launch serves n_prob independent problems (EssArgs strides): the grid kernels take theirs from blockIdx.y
+// (k_ess_count, whose x and y are (iteration, candidate), from blockIdx.z), the per-problem bookkeeping kernels run one
+// thread per problem.  Only the addressing depends on the problem count, so each problem's results are bit for bit those
+// of running it alone, and a problem that reached its adaptive bound skips the later waves while the others go on.
 // Restated in oracle/essential_ref.py; the math of ess_math.cuh is checked on the host against cv2 4.13.0
 // (tests/test_oracle_essential.py) and on the GPU through vo_mono_rotation (tests/test_gpu_stages.py).
 #include "common.cuh"
@@ -34,8 +38,35 @@ static __device__ __forceinline__ int ess_n(const EssArgs& a)
     return n < 0 ? 0 : (n < a.n_max ? n : a.n_max);
 }
 
-__global__ void k_ess_init(const EssArgs a)
+template <typename T> static __device__ __forceinline__ T* ess_at(T* ptr, size_t bytes)
 {
+    return (T*)((const char*)ptr + bytes);
+}
+
+// problem p's arguments: every pointer moved by its stride
+static __device__ __forceinline__ EssArgs ess_prob(const EssArgs& a0, int p)
+{
+    EssArgs a = a0;
+    const size_t so = (size_t)p * a0.scratch_stride;
+    a.n += (size_t)p * a0.n_stride;
+    a.pts0 += (size_t)p * a0.pts_stride; a.pts1 += (size_t)p * a0.pts_stride;
+    a.q0 = ess_at(a0.q0, so); a.q1 = ess_at(a0.q1, so); a.state = ess_at(a0.state, so);
+    a.subsets = ess_at(a0.subsets, so); a.models = ess_at(a0.models, so); a.nmodels = ess_at(a0.nmodels, so);
+    a.counts = ess_at(a0.counts, so); a.mask = ess_at(a0.mask, so); a.pose = ess_at(a0.pose, so);
+    a.result = ess_at(a0.result, (size_t)p * a0.result_stride);
+    return a;
+}
+
+// the problem of a one-thread-per-problem kernel, -1 for a thread beyond the last
+static __device__ __forceinline__ int ess_thread_prob(const EssArgs& a0)
+{
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    return p < a0.n_prob ? p : -1;
+}
+
+__global__ void k_ess_init(const EssArgs a0)
+{
+    const EssArgs a = ess_prob(a0, blockIdx.y);
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int n = ess_n(a);
     if (i == 0) {
@@ -54,9 +85,11 @@ __global__ void k_ess_init(const EssArgs a)
     a.q1[i] = make_double2(((double)p1.x - a.ppx) / a.focal, ((double)p1.y - a.ppy) / a.focal);
 }
 
-__global__ void k_ess_subsets(const EssArgs a, int it0, int it1)
+__global__ void k_ess_subsets(const EssArgs a0, int it0, int it1)
 {
-    if (blockIdx.x || threadIdx.x) return;
+    const int p = ess_thread_prob(a0);
+    if (p < 0) return;
+    const EssArgs a = ess_prob(a0, p);
     EssState& s = *a.state;
     if (s.done) return;
     const int n = ess_n(a);
@@ -79,8 +112,9 @@ __global__ void k_ess_subsets(const EssArgs a, int it0, int it1)
     s.rng_state = rng.state;
 }
 
-__global__ void __launch_bounds__(32) k_ess_hypotheses(const EssArgs a, int it0, int it1)
+__global__ void __launch_bounds__(32) k_ess_hypotheses(const EssArgs a0, int it0, int it1)
 {
+    const EssArgs a = ess_prob(a0, blockIdx.y);
     const int it = it0 + blockIdx.x * blockDim.x + threadIdx.x;
     const EssState& s = *a.state;
     if (s.done || it >= it1 || it >= s.niters) return;
@@ -93,8 +127,9 @@ __global__ void __launch_bounds__(32) k_ess_hypotheses(const EssArgs a, int it0,
     a.nmodels[it] = five_point(q0, q1, a.models + (size_t)it * 90);
 }
 
-__global__ void __launch_bounds__(128) k_ess_count(const EssArgs a, int it0, int it1)
+__global__ void __launch_bounds__(128) k_ess_count(const EssArgs a0, int it0, int it1)
 {
+    const EssArgs a = ess_prob(a0, blockIdx.z);
     const int it = it0 + blockIdx.x, cand = blockIdx.y;
     const EssState& s = *a.state;
     if (s.done || it >= it1 || it >= s.niters) return;
@@ -116,9 +151,11 @@ __global__ void __launch_bounds__(128) k_ess_count(const EssArgs a, int it0, int
     if (threadIdx.x == 0) a.counts[it * 10 + cand] = total;
 }
 
-__global__ void k_ess_replay(const EssArgs a, int it0, int it1)
+__global__ void k_ess_replay(const EssArgs a0, int it0, int it1)
 {
-    if (blockIdx.x || threadIdx.x) return;
+    const int p = ess_thread_prob(a0);
+    if (p < 0) return;
+    const EssArgs a = ess_prob(a0, p);
     EssState& s = *a.state;
     if (s.done) return;
     const int n = ess_n(a);
@@ -141,9 +178,12 @@ __global__ void k_ess_replay(const EssArgs a, int it0, int it1)
 // Exactly five correspondences (= model points): OpenCV runs no RANSAC.  findEssentialMat returns every candidate of one
 // five-point solve, stacked (3k x 3), with an all-ones mask; recoverPose only accepts a 3 x 3 E.  So a single candidate is
 // the model, with all five points inliers; any other count leaves no model (k_ess_pick reports the reference's abort).
-__global__ void k_ess_five(const EssArgs a)
+__global__ void k_ess_five(const EssArgs a0)
 {
-    if (blockIdx.x || threadIdx.x || ess_n(a) != 5) return;
+    const int p = ess_thread_prob(a0);
+    if (p < 0) return;
+    const EssArgs a = ess_prob(a0, p);
+    if (ess_n(a) != 5) return;
     EssState& s = *a.state;
     double q0[10], q1[10];
     for (int i = 0; i < 5; i++) {
@@ -154,8 +194,9 @@ __global__ void k_ess_five(const EssArgs a)
     if (nm == 1) { s.best_it = 0; s.best_cand = 0; s.max_good = 5; }
 }
 
-__global__ void k_ess_mask(const EssArgs a)
+__global__ void k_ess_mask(const EssArgs a0)
 {
+    const EssArgs a = ess_prob(a0, blockIdx.y);
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const EssState& s = *a.state;
     const int n = ess_n(a);
@@ -166,9 +207,11 @@ __global__ void k_ess_mask(const EssArgs a)
     a.mask[i] = (n == 5 || sampson_err(E, u.x, u.y, v.x, v.y) <= a.thr2) ? 1 : 0;
 }
 
-__global__ void k_ess_decompose(const EssArgs a)
+__global__ void k_ess_decompose(const EssArgs a0)
 {
-    if (blockIdx.x || threadIdx.x) return;
+    const int p = ess_thread_prob(a0);
+    if (p < 0) return;
+    const EssArgs a = ess_prob(a0, p);
     const EssState& s = *a.state;
     if (s.best_it < 0) return;
     const double* E = a.models + (size_t)s.best_it * 90 + s.best_cand * 9;
@@ -176,8 +219,9 @@ __global__ void k_ess_decompose(const EssArgs a)
     decompose_essential(E, a.pose, a.pose + 9, a.pose + 18);      // R1 | R2 | t | E
 }
 
-__global__ void __launch_bounds__(128) k_ess_cheirality(const EssArgs a)
+__global__ void __launch_bounds__(128) k_ess_cheirality(const EssArgs a0)
 {
+    const EssArgs a = ess_prob(a0, blockIdx.y);
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     EssState& s = *a.state;
     if (s.best_it < 0) return;
@@ -198,9 +242,11 @@ __global__ void __launch_bounds__(128) k_ess_cheirality(const EssArgs a)
     }
 }
 
-__global__ void k_ess_pick(const EssArgs a)
+__global__ void k_ess_pick(const EssArgs a0)
 {
-    if (blockIdx.x || threadIdx.x) return;
+    const int p = ess_thread_prob(a0);
+    if (p < 0) return;
+    const EssArgs a = ess_prob(a0, p);
     const EssState& s = *a.state;
     EssResult& r = *a.result;
     const int n = ess_n(a);
@@ -241,6 +287,7 @@ void vo_ess_bind(EssArgs& a, void* scratch, int n_max, int max_iters)
     uint8_t* b = (uint8_t*)scratch;
     auto take = [&](size_t bytes) { uint8_t* p = b; b += ess_up(bytes); return p; };
     a.n_max = n_max; a.max_iters = max_iters;
+    a.n_prob = 1; a.scratch_stride = 0; a.pts_stride = 0; a.n_stride = 0; a.result_stride = 0;
     a.q0 = (double2*)take(n * sizeof(double2)); a.q1 = (double2*)take(n * sizeof(double2));
     a.state = (EssState*)take(sizeof(EssState));
     a.subsets = (int*)take(it * 5 * sizeof(int));
@@ -255,22 +302,24 @@ void vo_ess_bind(EssArgs& a, void* scratch, int n_max, int max_iters)
 int vo_launch_essential(const EssArgs& a, cudaStream_t s)
 {
     int launches = 0;
+    const int np = a.n_prob;
     const int nb = (a.n_max + 127) / 128 > 0 ? (a.n_max + 127) / 128 : 1;
-    k_ess_init<<<nb, 128, 0, s>>>(a); launches++;
-    k_ess_five<<<1, 32, 0, s>>>(a); launches++;
+    const int nt = (np + 31) / 32;                       // one thread per problem
+    k_ess_init<<<dim3(nb, np), 128, 0, s>>>(a); launches++;
+    k_ess_five<<<nt, 32, 0, s>>>(a); launches++;
     const int waves[4] = {0, 32, 128, a.max_iters};
     for (int w = 0; w < 3; w++) {
         const int it0 = waves[w], it1 = waves[w + 1] < a.max_iters ? waves[w + 1] : a.max_iters;
         if (it1 <= it0) break;
-        k_ess_subsets<<<1, 32, 0, s>>>(a, it0, it1);
-        k_ess_hypotheses<<<(it1 - it0 + 31) / 32, 32, 0, s>>>(a, it0, it1);
-        k_ess_count<<<dim3(it1 - it0, 10), 128, 0, s>>>(a, it0, it1);
-        k_ess_replay<<<1, 32, 0, s>>>(a, it0, it1);
+        k_ess_subsets<<<nt, 32, 0, s>>>(a, it0, it1);
+        k_ess_hypotheses<<<dim3((it1 - it0 + 31) / 32, np), 32, 0, s>>>(a, it0, it1);
+        k_ess_count<<<dim3(it1 - it0, 10, np), 128, 0, s>>>(a, it0, it1);
+        k_ess_replay<<<nt, 32, 0, s>>>(a, it0, it1);
         launches += 4;
     }
-    k_ess_mask<<<nb, 128, 0, s>>>(a);
-    k_ess_decompose<<<1, 32, 0, s>>>(a);
-    k_ess_cheirality<<<nb, 128, 0, s>>>(a);
-    k_ess_pick<<<1, 32, 0, s>>>(a);
+    k_ess_mask<<<dim3(nb, np), 128, 0, s>>>(a);
+    k_ess_decompose<<<nt, 32, 0, s>>>(a);
+    k_ess_cheirality<<<dim3(nb, np), 128, 0, s>>>(a);
+    k_ess_pick<<<nt, 32, 0, s>>>(a);
     return launches + 4;
 }

@@ -46,6 +46,13 @@ struct EssArgs {
     uint8_t* mask;            // [n_max] inliers of the best E
     double* pose;             // [30] R1 | R2 | t | E of the best model
     EssResult* result;
+    // n_prob independent problems in one launch: the pointers above are problem 0's, problem p finds its own `stride`
+    // further on (vo_ess_bind sets one problem with zero strides)
+    int n_prob;
+    size_t scratch_stride;    // bytes, q0 .. pose (one scratch block per problem)
+    int pts_stride;           // float2 elements, pts0 / pts1
+    int n_stride;             // ints, n
+    size_t result_stride;     // bytes, result
 };
 
 #define VO_ESS_ITERS 1000      // cv::findEssentialMat's default maxIters
@@ -61,9 +68,11 @@ static inline void vo_ess_set_camera(EssArgs& a, double focal, double ppx, doubl
 }
 
 // bytes of one scratch block for up to n_max points (everything EssArgs points to except pts0 / pts1 / n), and the args
-// laid out over it
+// of one problem laid out over it
 size_t vo_ess_scratch_bytes(int n_max, int max_iters);
 void vo_ess_bind(EssArgs& a, void* scratch, int n_max, int max_iters);
-// A fixed launch sequence whatever *n turns out to be (graph-capturable, no host sync): n < 5 ends without a model,
-// n == 5 takes k_ess_five, n > 5 the RANSAC waves, which skip themselves once the adaptive bound is reached.
+// A fixed launch sequence whatever each *n turns out to be and whatever n_prob is (graph-capturable, no host sync): per
+// problem, n < 5 ends without a model, n == 5 takes k_ess_five, n > 5 the RANSAC waves, which skip themselves once that
+// problem's adaptive bound is reached.  Every kernel takes its problem from a grid dimension or, for the per-problem
+// bookkeeping, one thread per problem; a problem's arithmetic is that of running it alone.
 int vo_launch_essential(const EssArgs& a, cudaStream_t s);

@@ -136,8 +136,13 @@ __global__ void k_seq_finish(vo_unit_result_dev* res, double* tprev_next, const 
 
 // trackingFrame2Frame(mono_rotation = true) (src/visualOdometry.cpp:146-157,186-189): `rotation` comes from recoverPose,
 // the PnP supplies only `translation`.  Runs after k_seq_finish, so the translation carry is the PnP's as without the branch.
-__global__ void k_seq_mono(vo_unit_result_dev* res, const EssResult* __restrict__ ess)
+// Sequence q's result is ess_stride bytes after sequence q - 1's.
+__global__ void k_seq_mono(vo_unit_result_dev* res, const EssResult* __restrict__ ess, size_t ess_stride, const int* __restrict__ live)
 {
+    const int q = blockIdx.y;
+    if (!live[q]) return;
+    res += q;
+    ess = (const EssResult*)((const char*)ess + (size_t)q * ess_stride);
     const int k = threadIdx.x;
     if (k < 9) res->R[k] = ess->status == ESS_OK ? ess->R[k] : (k % 4 == 0 ? 1.0 : 0.0);
 }
@@ -165,8 +170,8 @@ int vo_launch_seq_finish(const SeqArgs& a, int n_seq, cudaStream_t s)
     k_seq_finish<<<dim3(1, n_seq), 32, 0, s>>>(a.res, a.tprev, a.tprev_cur, a.out_n, a.n_det, a.n3, a.n5, a.err, a.err_out, a.live);
     return 1;
 }
-int vo_launch_seq_mono(vo_unit_result_dev* res, const EssResult* ess, cudaStream_t s)
+int vo_launch_seq_mono(const SeqArgs& a, const EssResult* ess, size_t ess_stride, int n_seq, cudaStream_t s)
 {
-    k_seq_mono<<<1, 32, 0, s>>>(res, ess);
+    k_seq_mono<<<dim3(1, n_seq), 32, 0, s>>>(a.res, ess, ess_stride, a.live);
     return 1;
 }

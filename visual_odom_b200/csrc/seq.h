@@ -26,6 +26,6 @@ int vo_launch_seq_append(const SeqArgs& a, int n_seq, cudaStream_t s);
 int vo_launch_seq_bucket(const SeqArgs& a, int n_seq, cudaStream_t s);
 int vo_launch_seq_carry(const SeqArgs& a, int n_seq, cudaStream_t s);
 int vo_launch_seq_finish(const SeqArgs& a, int n_seq, cudaStream_t s);
-// mono_rotation = true: the record's R becomes recoverPose's rotation (I where the branch aborted); everything else in
-// the record stays the PnP's
-int vo_launch_seq_mono(vo_unit_result_dev* res, const EssResult* ess, cudaStream_t s);
+// mono_rotation = true: each live sequence's record R becomes recoverPose's rotation (I where the branch aborted);
+// everything else in the record stays the PnP's.  ess: sequence 0's result, sequence q's ess_stride bytes further on.
+int vo_launch_seq_mono(const SeqArgs& a, const EssResult* ess, size_t ess_stride, int n_seq, cudaStream_t s);
