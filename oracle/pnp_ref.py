@@ -385,7 +385,7 @@ def reproj_err_f32(X, x, rvec, tvec, K):
 # ----------------------------------------------------------------------------- triangulation
 def triangulate(P_l, P_r, pts_l, pts_r):
     """cv::triangulatePoints (per-point 4x4 DLT, last row of V^T, stored f32) followed by
-    cv::convertPointsFromHomogeneous (f32: scale = 1/w, x*scale)."""
+    cv::convertPointsFromHomogeneous (f32: scale = 1/w where |w| > FLT_EPSILON, else 1; x*scale)."""
     Pl = np.asarray(P_l, np.float32).astype(np.float64)
     Pr = np.asarray(P_r, np.float32).astype(np.float64)
     a = np.asarray(pts_l, np.float32).reshape(-1, 2)
@@ -401,10 +401,12 @@ def triangulate(P_l, P_r, pts_l, pts_r):
 
 
 def dehomogenize_f32(X4):
+    """cv::convertPointsFromHomogeneous on f32 4-vectors: it divides only where |w| > FLT_EPSILON (strictly, so
+    |w| == FLT_EPSILON and a NaN w keep scale 1).  A zero-disparity point (w ~ 1e-18) stays the unit-norm column."""
     X4 = np.asarray(X4, np.float32)
     w = X4[:, 3]
-    with np.errstate(divide="ignore"):
-        scale = np.where(w != 0, np.float32(1.0) / w, np.float32(1.0)).astype(np.float32)
+    with np.errstate(divide="ignore", over="ignore", invalid="ignore"):
+        scale = np.where(np.abs(w) > np.finfo(np.float32).eps, np.float32(1.0) / w, np.float32(1.0)).astype(np.float32)
     return (X4[:, :3] * scale[:, None]).astype(np.float32)
 
 

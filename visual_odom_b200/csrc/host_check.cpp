@@ -16,6 +16,14 @@ __attribute__((visibility("default"))) void vo_hostcheck_triangulate(const float
     for (int k = 0; k < 12; k++) { Pl[k] = Pl12[k]; Pr[k] = Pr12[k]; }
     for (int i = 0; i < n; i++) vomath::triangulate_dlt(Pl, Pr, a[2 * i], a[2 * i + 1], b[2 * i], b[2 * i + 1], X + 3 * i);
 }
+// the same, with the unit-norm homogeneous column k_triangulate stores for vo_triangulate_homogeneous (n x 4)
+__attribute__((visibility("default"))) void vo_hostcheck_triangulate4(const float* Pl12, const float* Pr12, const float* a, const float* b, int n, float* X, float* X4)
+{
+    double Pl[12], Pr[12];
+    for (int k = 0; k < 12; k++) { Pl[k] = Pl12[k]; Pr[k] = Pr12[k]; }
+    for (int i = 0; i < n; i++)
+        vomath::triangulate_dlt(Pl, Pr, a[2 * i], a[2 * i + 1], b[2 * i], b[2 * i + 1], X + 3 * i, X4 + 4 * i);
+}
 __attribute__((visibility("default"))) void vo_hostcheck_rodrigues(const double* r, double* R, double* r_back)
 {
     vomath::rodrigues_fwd(r, R);

@@ -10,6 +10,7 @@
 // build: compile with -fmad=false (no FMA contraction) -- visual_odom_b200/build.py does.
 // Restated independently in oracle/pnp_ref.py (pinned bit-for-bit against cv2).
 #pragma once
+#include <float.h>
 #include <math.h>
 #include <stdint.h>
 
@@ -716,7 +717,9 @@ VO_HDN inline void epnp5(const float* Xw_f, const float* uv_f, double fu, double
 }
 
 // per-point DLT of cv::triangulatePoints: X4 = last row of V^T of the 4x4 system (stored float),
-// then convertPointsFromHomogeneous in float.
+// then convertPointsFromHomogeneous in float, which divides by w only where |w| > FLT_EPSILON (strictly; a NaN w
+// fails the test) and otherwise keeps scale 1: a zero-disparity point (w ~ 1e-18 from the DLT) comes out as the
+// unit-norm column, not as a point 1e17 away.
 // out4 (optional): the unit-norm homogeneous 4-vector itself, i.e. the column cv::triangulatePoints stores.
 VO_HDN inline void triangulate_dlt(const double* Pl, const double* Pr, float xl, float yl, float xr, float yr,
                                    float* out3, float* out4 = nullptr)
@@ -733,7 +736,7 @@ VO_HDN inline void triangulate_dlt(const double* Pl, const double* Pr, float xl,
     jacobi_svd_t<4, 4>(At, W, Vt, 4);
     const float X0 = (float)Vt[12], X1 = (float)Vt[13], X2 = (float)Vt[14], X3 = (float)Vt[15];
     if (out4) { out4[0] = X0; out4[1] = X1; out4[2] = X2; out4[3] = X3; }
-    const float scale = X3 != 0.f ? 1.f / X3 : 1.f;
+    const float scale = fabsf(X3) > FLT_EPSILON ? 1.f / X3 : 1.f;
     out3[0] = X0 * scale; out3[1] = X1 * scale; out3[2] = X2 * scale;
 }
 

@@ -39,12 +39,20 @@ def _rodrigues(r):
     return R
 
 
-def stereo_unit(w=1241, h=376, seed=0, cal=KITTI00, scene="v1", noise=1.0, rvec=EGO_RVEC, tvec=EGO_T):
-    """Returns dict(l0, r0, l1, r1 : uint8 HxW, P_l, P_r, K, rvec, tvec)."""
+def stereo_unit(w=1241, h=376, seed=0, cal=KITTI00, scene="v1", noise=1.0, rvec=EGO_RVEC, tvec=EGO_T, sky=0.0):
+    """Returns dict(l0, r0, l1, r1 : uint8 HxW, P_l, P_r, K, rvec, tvec).
+
+    sky > 0 (scene "v1" only) overwrites the top `sky` fraction of L0's rows with a textured band at infinity: in each
+    view it is drawn through the rotation-only homography K R K^-1, so the left and right images of one time carry the
+    same pixels there, sensor noise included (zero disparity), and t1 sees the band rotated by `rvec` only.  The default
+    0 leaves every image, and the noise drawn for it, as before."""
     P_l, P_r = proj_matrices(cal)
     K = P_l[:, :3].astype(np.float64)
     rng = np.random.default_rng(1000 + seed)
     margin = 96
+    if sky and scene != "v1":
+        raise ValueError("sky needs scene 'v1'")
+    sky_masks = []
     if scene == "v0":
         T = texture(h, w, seed, margin)
         def crop(dx, dy):
@@ -65,6 +73,7 @@ def stereo_unit(w=1241, h=376, seed=0, cal=KITTI00, scene="v1", noise=1.0, rvec=
         uu, vv = np.meshgrid(np.arange(w, dtype=np.float64), np.arange(h, dtype=np.float64))
         pix = np.stack([uu.ravel(), vv.ravel(), np.ones(w * h)], 0)
         Kinv = np.linalg.inv(K)
+        sky_tex = texture(h, w, 10007 + seed, margin) if sky > 0 else None
         views = []
         for (R, t) in poses:
             img = np.zeros((h, w), np.uint8)
@@ -87,12 +96,25 @@ def stereo_unit(w=1241, h=376, seed=0, cal=KITTI00, scene="v1", noise=1.0, rvec=
                               ((p0[1] / p0[2]).reshape(h, w) + margin).astype(np.float32),
                               cv2.INTER_LINEAR, borderMode=cv2.BORDER_REFLECT_101)
                 img[~filled] = m[~filled]
+            if sky > 0:                                        # the band at infinity: L0 pixel -> view pixel is K R K^-1
+                p0 = np.linalg.inv(K @ R @ Kinv) @ pix
+                x0 = (p0[0] / p0[2]).reshape(h, w)
+                y0 = (p0[1] / p0[2]).reshape(h, w)
+                inside = y0 < sky * h
+                m = cv2.remap(sky_tex, (x0 + margin).astype(np.float32),
+                              (y0 + margin).astype(np.float32), cv2.INTER_LINEAR, borderMode=cv2.BORDER_REFLECT_101)
+                img[inside] = m[inside]
+                sky_masks.append(inside)
             views.append(img)
     out = []
     for v in views:
         if noise > 0:
             v = np.clip(v.astype(np.int32) + np.rint(rng.normal(0, noise, v.shape)).astype(np.int32), 0, 255).astype(np.uint8)
         out.append(np.ascontiguousarray(v))
+    if sky > 0:                                                # right = left in the band, noise included
+        for left, right in ((0, 1), (2, 3)):
+            assert np.array_equal(sky_masks[left], sky_masks[right])
+            out[right][sky_masks[left]] = out[left][sky_masks[left]]
     return dict(l0=out[0], r0=out[1], l1=out[2], r1=out[3], P_l=P_l, P_r=P_r,
                 K=P_l[:, :3].copy(), rvec=np.asarray(rvec, np.float64), tvec=np.asarray(tvec, np.float64))
 
