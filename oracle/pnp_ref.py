@@ -662,8 +662,11 @@ def _epnp(X, x, K):
 
 
 # ----------------------------------------------------------------------------- LM refinement
-def lm_refine(X, x, K, rvec0, tvec0, max_iter=20, eps=FLT_EPS):
-    """cvFindExtrinsicCameraParams2's refinement: CvLevMarq over (rvec, tvec), pixel residuals."""
+def lm_refine(X, x, K, rvec0, tvec0, max_iter=20, eps=FLT_EPS, trace=None):
+    """cvFindExtrinsicCameraParams2's refinement: CvLevMarq over (rvec, tvec), pixel residuals.
+    trace: a dict that receives iters (iterations run), rejected (steps rejected for raising the error, over all
+    iterations) and stop ("cap" when max_iter ended it, "eps" when the relative step fell below eps); it changes nothing
+    else."""
     X = np.asarray(X, np.float32).reshape(-1, 3).astype(np.float64)
     m = np.asarray(x, np.float32).reshape(-1, 2).astype(np.float64)
     K = np.asarray(K, np.float64)
@@ -695,7 +698,7 @@ def lm_refine(X, x, K, rvec0, tvec0, max_iter=20, eps=FLT_EPS):
         return err, J
 
     lam_lg10 = -3
-    iters = 0
+    iters = rejected = 0
     err, J = proj(param, True)
     prev_err_norm = None
     while True:
@@ -717,6 +720,7 @@ def lm_refine(X, x, K, rvec0, tvec0, max_iter=20, eps=FLT_EPS):
             err_norm = math.sqrt(float(err @ err))
             if err_norm > prev_err_norm:
                 lam_lg10 += 1
+                rejected += 1
                 if lam_lg10 <= 16:
                     param = step()
                     continue
@@ -725,6 +729,8 @@ def lm_refine(X, x, K, rvec0, tvec0, max_iter=20, eps=FLT_EPS):
         iters += 1
         rel = np.linalg.norm(param - prev_param) / max(np.linalg.norm(prev_param), DBL_EPS)
         if iters >= max_iter or rel < eps:
+            if trace is not None:
+                trace.update(iters=iters, rejected=rejected, stop="eps" if rel < eps else "cap")
             break
         prev_err_norm = err_norm
         err, J = proj(param, True)

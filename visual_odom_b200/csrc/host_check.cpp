@@ -38,6 +38,11 @@ __attribute__((visibility("default"))) int vo_hostcheck_p3p(const float* X4, con
     vomath::rodrigues_fwd(rvec, R);
     return 1;
 }
+// the LM step solve of k_pnp_finalize: returns 1 if it took the Cholesky path, 0 if OpenCV's SVD solve
+__attribute__((visibility("default"))) int vo_hostcheck_lm_solve6(const double* JtJ, const double* JtErr, double lambda, double* dx)
+{
+    return vomath::lm_solve6(JtJ, JtErr, lambda, dx) ? 1 : 0;
+}
 __attribute__((visibility("default"))) int vo_hostcheck_five_point(const double* q1, const double* q2, double* E_out)
 {
     return vomath::five_point(q1, q2, E_out);

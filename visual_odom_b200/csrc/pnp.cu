@@ -530,33 +530,10 @@ __global__ void __launch_bounds__(FIN_T, 1) k_pnp_finalize(const PnpArgs a)
     auto lm_step = [&]() {      // thread 0: param = prev_param - solve((JtJ with scaled diagonal), JtErr)
         if (threadIdx.x == 0) {
             const double lambda = exp(lambda_lg10 * log(10.));
-            // (J^T J + lambda diag) dx = J^T e.  OpenCV solves this 6x6 SPD system by SVD; the pose gate is
-            // 1e-4 relative (not bit-exactness), so a Cholesky factorisation is used: same solution to
-            // ~1e-15, a few hundred flops instead of a Jacobi SVD on one thread.
-            double A[36], dx[6], y[6];
-            for (int k = 0; k < 36; k++) A[k] = JtJ[k];
-            for (int k = 0; k < 6; k++) A[k * 7] *= 1. + lambda;
-            bool spd = true;
-            for (int j = 0; j < 6 && spd; j++) {
-                double d = A[j * 7];
-                for (int k = 0; k < j; k++) d -= A[j * 6 + k] * A[j * 6 + k];
-                if (!(d > 0)) { spd = false; break; }
-                d = sqrt(d);
-                A[j * 7] = d;
-                for (int i = j + 1; i < 6; i++) {
-                    double v = A[i * 6 + j];
-                    for (int k = 0; k < j; k++) v -= A[i * 6 + k] * A[j * 6 + k];
-                    A[i * 6 + j] = v / d;
-                }
-            }
-            if (spd) {
-                for (int i = 0; i < 6; i++) { double v = JtErr[i]; for (int k = 0; k < i; k++) v -= A[i * 6 + k] * y[k]; y[i] = v / A[i * 7]; }
-                for (int i = 5; i >= 0; i--) { double v = y[i]; for (int k = i + 1; k < 6; k++) v -= A[k * 6 + i] * dx[k]; dx[i] = v / A[i * 7]; }
-            } else {            // rank-deficient normal equations: fall back to the SVD solve OpenCV uses
-                for (int k = 0; k < 36; k++) A[k] = JtJ[k];
-                for (int k = 0; k < 6; k++) A[k * 7] *= 1. + lambda;
-                solve_svd<6, 6>(A, JtErr, dx);
-            }
+            // (J^T J + lambda diag) dx = J^T e: Cholesky while positive definite, OpenCV's SVD solve otherwise
+            // (lm_solve6 in pnp_math.cuh; the refined pose is pinned to cv2 at 1e-8 by tests/test_gpu_pnp_refine.py)
+            double dx[6];
+            lm_solve6(JtJ, JtErr, lambda, dx);
             for (int k = 0; k < 6; k++) param[k] = prev_param[k] - dx[k];
         }
         __syncthreads();

@@ -325,6 +325,42 @@ VO_HDN void solve_svd_rt(const double* A, const double* b, double* x, int N)
     }
 }
 
+// The step of CvLevMarq: (JtJ with its diagonal scaled by 1 + lambda) dx = JtErr, JtJ 6x6 row-major symmetric.
+// OpenCV solves this system with cv::solve(DECOMP_SVD).  A Cholesky factorisation is used instead while the damped
+// matrix is positive definite: a few hundred flops rather than a Jacobi SVD on one thread, and a solution whose backward
+// error is as small (tests/test_oracle_lm_refine.py checks it against OpenCV's SVD solve on the host;
+// tests/test_gpu_pnp_refine.py pins the refined pose to cv2 at 1e-8).  A matrix
+// that is not positive definite in floating point (rank-deficient normal equations) takes OpenCV's own SVD solve, so
+// there the step is OpenCV's bit for bit.  Returns true when the Cholesky path was taken.
+VO_HD bool lm_solve6(const double* JtJ, const double* JtErr, double lambda, double* dx)
+{
+    double A[36], y[6];
+    for (int k = 0; k < 36; k++) A[k] = JtJ[k];
+    for (int k = 0; k < 6; k++) A[k * 7] *= 1. + lambda;
+    bool spd = true;
+    for (int j = 0; j < 6 && spd; j++) {
+        double d = A[j * 7];
+        for (int k = 0; k < j; k++) d -= A[j * 6 + k] * A[j * 6 + k];
+        if (!(d > 0)) { spd = false; break; }
+        d = sqrt(d);
+        A[j * 7] = d;
+        for (int i = j + 1; i < 6; i++) {
+            double v = A[i * 6 + j];
+            for (int k = 0; k < j; k++) v -= A[i * 6 + k] * A[j * 6 + k];
+            A[i * 6 + j] = v / d;
+        }
+    }
+    if (spd) {
+        for (int i = 0; i < 6; i++) { double v = JtErr[i]; for (int k = 0; k < i; k++) v -= A[i * 6 + k] * y[k]; y[i] = v / A[i * 7]; }
+        for (int i = 5; i >= 0; i--) { double v = y[i]; for (int k = i + 1; k < 6; k++) v -= A[k * 6 + i] * dx[k]; dx[i] = v / A[i * 7]; }
+    } else {
+        for (int k = 0; k < 36; k++) A[k] = JtJ[k];
+        for (int k = 0; k < 6; k++) A[k * 7] *= 1. + lambda;
+        solve_svd<6, 6>(A, JtErr, dx);
+    }
+    return spd;
+}
+
 // cv::invert(A 3x3, Ainv, DECOMP_SVD)
 VO_HDN inline void invert3_svd(const double* A, double* Ainv)
 {
