@@ -184,8 +184,16 @@ typedef struct vo_unit_result {
     double rvec[3], tvec[3], R[9];
 } vo_unit_result;
 
-/* Allocate/resize the device-resident batch state for n_units units of w x h images. */
+/* Allocate/resize the device-resident batch state for n_units units of w x h images; every unit gets the calibration
+ * P_l / P_r.  Image size and feature capacity are per context: group rigs with different image sizes by context. */
 VO_API int vo_batch_configure(vo_ctx* ctx, int w, int h, int n_units, const float P_l[12], const float P_r[12]);
+/* Units [first_unit, first_unit + n_units) get their own calibrations: unit first_unit + i runs its triangulation and PnP
+ * with P_l + 12 i / P_r + 12 i (n_units row-major 3 x 4 matrices each), e.g. one context for several stereo rigs of one
+ * image size.  A unit keeps its calibration across submissions until it is set again (vo_batch_configure sets every
+ * unit); each unit's results are those of a context configured with its calibration alone, bit for bit.  Refused
+ * (VO_E_INVALID): a range outside the configured units, NULL matrices, or a call while submissions are in flight
+ * (vo_batch_wait them first); like vo_batch_configure it ends an idle sequence-mode run. */
+VO_API int vo_batch_calibrate(vo_ctx* ctx, int first_unit, int n_units, const float* P_l, const float* P_r);
 /* async: copy the units' images (and features) host->device on the context's stream. */
 VO_API int vo_batch_upload(vo_ctx* ctx, const vo_unit* units, int n_units, size_t pitch);
 /* async: run the whole path for the uploaded units. */
@@ -340,7 +348,8 @@ VO_API int vo_seq_wait_mono(vo_ctx* ctx, vo_unit_result* out, vo_mono_result* mo
 VO_API int vo_seq_state(vo_ctx* ctx, vo_point2f* points, int32_t* ages, int cap, int* n_points, int* n_ages, double t_out[3]);
 
 /* ---- several independent sequences through the streaming sequence mode ----------------------------------------------
- * n_seq sequences of one image size and one calibration advance in lockstep, one frame each per submission, through the
+ * n_seq sequences of one image size, each with its own calibration (vo_mseq_begin_calib) or all with one, advance in
+ * lockstep, one frame each per submission, through the
  * stages of the sequence mode above; every stage is ONE kernel launch for all of them, so a submission costs the launches
  * of one vo_seq_submit whatever n_seq is.  Each sequence's records, point lists, carried state and frame_pose are those of
  * running it alone through vo_seq_begin / vo_seq_push (the same kernels on its own units), bit for bit.
@@ -381,6 +390,13 @@ VO_API int vo_mseq_begin(vo_ctx* ctx, int n_seq, int w, int h, const float P_l[1
                          const uint8_t* const* right0, size_t pitch, int channels);
 VO_API int vo_mseq_begin_ex(vo_ctx* ctx, int n_seq, int w, int h, const float P_l[12], const float P_r[12],
                             const uint8_t* const* left0, const uint8_t* const* right0, size_t pitch, int channels, int flags);
+/* vo_mseq_begin_ex with one calibration per sequence: P_l / P_r hold n_seq row-major 3 x 4 matrices each, and sequence q
+ * runs with P_l + 12 q / P_r + 12 q, as the reference's main() builds them from its own calibration file
+ * (src/main.cpp:67-74).  With VO_MSEQ_MONO_ROTATION each sequence's focal / principal point come from its own P_l.
+ * Each sequence's results are those of running it alone through vo_seq_begin with its matrices, bit for bit, and a
+ * submission costs the same launches as with one calibration.  vo_mseq_begin_ex is this call with its matrices repeated. */
+VO_API int vo_mseq_begin_calib(vo_ctx* ctx, int n_seq, int w, int h, const float* P_l, const float* P_r,
+                               const uint8_t* const* left0, const uint8_t* const* right0, size_t pitch, int channels, int flags);
 VO_API int vo_mseq_submit(vo_ctx* ctx, const uint8_t* const* left1, const uint8_t* const* right1, size_t pitch, int channels);
 VO_API int vo_mseq_wait(vo_ctx* ctx, vo_unit_result* out, int* status, vo_point2f* pts4, int pts_cap);
 VO_API int vo_mseq_wait_mono(vo_ctx* ctx, vo_unit_result* out, int* status, vo_mono_result* mono,

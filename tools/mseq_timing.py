@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Scaling of the multi-sequence streaming mode (vo_mseq_*) with the number of sequences, measured on the GPU.
 
-    python tools/mseq_timing.py [--frames 40] [--rounds 5] [--counts 1,2,4,8,16,32] [--mono-rotation] [--json out.json]
+    python tools/mseq_timing.py [--frames 40] [--rounds 5] [--counts 1,2,4,8,16,32] [--mono-rotation] [--mixed-calibration]
+                                [--json out.json]
 
 Synthetic 1241x376 drives (synth.stereo_unit; eight seeds, each with its own motion) of `--frames` frames each;
 sequence q replays drive q % 8, forwards for even q // 8 and backwards for odd, so up to 16 sequences are distinct and
@@ -12,7 +13,10 @@ and reports per mode the median over the rounds of the aggregate frames/s (seque
 per-step latency (wall time per submission in the pipelined loop) and the kernel launches per submission
 (vo_kernel_launches).  `--mono-rotation` runs every mode twice per round, without and with trackingFrame2Frame's
 mono_rotation branch (the option "mono_rotation" for vo_seq_*, the flag VO_MSEQ_MONO_ROTATION for vo_mseq_*), and
-reports both.  The card's name, power limit and max SM clock, read in the same run, are printed with the numbers;
+reports both.  `--mixed-calibration` also runs every vo_mseq_* count with one calibration per sequence
+(vo_mseq_begin_calib): sequence q is then rendered with, and run with, its own camera (focal length, principal point and
+baseline spread over +-10 %, +-20 px and +-15 %), so that no two sequences share a calibration; the motions are those
+of the one-calibration run.  Both are timed in the same rounds, alternated.  The card's name, power limit and max SM clock, read in the same run, are printed with the numbers;
 they are part of them."""
 import argparse
 import json
@@ -42,20 +46,31 @@ def motion(d):
     return rng.uniform(-0.004, 0.004, 3) * np.array([1.0, 1.0, 0.25]), np.array([0.0, 0.0, -0.2]) + rng.uniform(-0.02, 0.02, 3)
 
 
+def calibration(q, n):
+    """the camera of sequence q of n in the mixed-calibration runs (KITTI 00's, spread over the sequences)"""
+    from visual_odom_b200 import synth
+    f = -1.0 + 2.0 * q / max(n - 1, 1)                # -1 .. 1
+    c = synth.KITTI00
+    return dict(fx=c["fx"] * (1 + 0.1 * f), fy=c["fy"] * (1 + 0.1 * f), cx=c["cx"] + 20 * f, cy=c["cy"] - 20 * f,
+                bf=c["bf"] * (1 - 0.15 * f))
+
+
 def render(job):
     from visual_odom_b200 import synth
-    d, k = job
+    d, k, cal = job
     r, t = motion(d)
-    u = synth.stereo_unit(W, H, 50 + d, rvec=r * k, tvec=t * k)
+    u = synth.stereo_unit(W, H, 50 + d, rvec=r * k, tvec=t * k, **({} if cal is None else dict(cal=cal)))
     return (u["l0"], u["r0"]) if k == 0 else (u["l1"], u["r1"])
 
 
-def drives(n_frames):
-    """[drive][frame] = (left, right), rendered in parallel (one synth call per frame)."""
-    jobs = [(d, k) for d in range(DRIVES) for k in range(n_frames)]
+def drives(n_frames, cals=None):
+    """[drive][frame] = (left, right), rendered in parallel (one synth call per frame).  cals: one calibration per drive
+    (drive i then replays the motion of drive i % DRIVES), else DRIVES drives at KITTI 00's."""
+    ids = [(d, None) for d in range(DRIVES)] if cals is None else [(i % DRIVES, c) for i, c in enumerate(cals)]
+    jobs = [(d, k, c) for d, c in ids for k in range(n_frames)]
     with ProcessPoolExecutor(max_workers=min(32, os.cpu_count() or 1)) as ex:
         pairs = list(ex.map(render, jobs, chunksize=4))
-    return [pairs[d * n_frames:(d + 1) * n_frames] for d in range(DRIVES)]
+    return [pairs[i * n_frames:(i + 1) * n_frames] for i in range(len(ids))]
 
 
 def sequence(dr, q):
@@ -101,6 +116,8 @@ def main():
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--counts", default="1,2,4,8,16,32")
     ap.add_argument("--mono-rotation", action="store_true", help="also time every mode with the mono_rotation branch")
+    ap.add_argument("--mixed-calibration", action="store_true",
+                    help="also time every vo_mseq_* count with a distinct calibration per sequence")
     ap.add_argument("--json", help="also write the result here")
     a = ap.parse_args()
     counts = [int(c) for c in a.counts.split(",")]
@@ -109,19 +126,30 @@ def main():
     t0 = time.perf_counter()
     dr = drives(a.frames + 1)
     print(f"rendered {DRIVES} drives x {a.frames + 1} frames in {time.perf_counter() - t0:.0f} s", flush=True)
-    ctx = capi.Context(0, max_features=4096)
     monos = (False, True) if a.mono_rotation else (False,)
-    modes = [(m, mono) for m in ["seq"] + counts for mono in monos]
+    mixes = (False, True) if a.mixed_calibration else (False,)
+    modes = [(m, mono, mix) for m in ["seq"] + counts for mono in monos for mix in mixes if not (m == "seq" and mix)]
     seqs = {n: [sequence(dr, q) for q in range(n)] for n in counts}
+    mixed = {}
+    if a.mixed_calibration:              # per count n: sequence q rendered with calibration(q, n), played like sequence(dr, q)
+        t0 = time.perf_counter()
+        for n in counts:
+            cals = [calibration(q, n) for q in range(n)]
+            md = drives(a.frames + 1, cals)
+            mixed[n] = ([md[q] if (q // DRIVES) % 2 == 0 else md[q][::-1] for q in range(n)],
+                        np.stack([synth.proj_matrices(c)[0] for c in cals]), np.stack([synth.proj_matrices(c)[1] for c in cals]))
+        print(f"rendered the mixed-calibration sequences in {time.perf_counter() - t0:.0f} s", flush=True)
+    ctx = capi.Context(0, max_features=4096)
     res = {m: dict(fps=[], lat=[], launches=[]) for m in modes}
 
     def run(mode, fr_cut=None):
-        m, mono = mode
+        m, mono, mix = mode
         if m == "seq":
             fr = dr[0] if fr_cut is None else dr[0][:fr_cut]
             return run_seq(ctx, P_l, P_r, fr, mono)
-        s = seqs[m] if fr_cut is None else [x[:fr_cut] for x in seqs[m]]
-        return run_mseq(ctx, P_l, P_r, s, mono)
+        s, Pl, Pr = mixed[m] if mix else (seqs[m], P_l, P_r)
+        s = s if fr_cut is None else [x[:fr_cut] for x in s]
+        return run_mseq(ctx, Pl, Pr, s, mono)
 
     for _ in range(a.rounds):
         for m in modes:
@@ -136,10 +164,11 @@ def main():
         o = dict(aggregate_fps=float(np.median(r["fps"])), aggregate_fps_min=float(np.min(r["fps"])),
                  aggregate_fps_max=float(np.max(r["fps"])), step_latency_ms=1e3 * float(np.median(r["lat"])),
                  launches_per_submission=float(np.median(r["launches"])))
-        m, mono = mode
-        out["modes"][str(m) + ("+mono" if mono else "")] = o
-        name = ("vo_seq (1 sequence)" if m == "seq" else f"vo_mseq n_seq = {m:2d}") + (", mono" if mono else "")
-        print(f"{name:28s}: {o['aggregate_fps']:8.0f} frames/s [{o['aggregate_fps_min']:.0f}, {o['aggregate_fps_max']:.0f}], "
+        m, mono, mix = mode
+        out["modes"][str(m) + ("+mono" if mono else "") + ("+mixed" if mix else "")] = o
+        name = ("vo_seq (1 sequence)" if m == "seq" else f"vo_mseq n_seq = {m:2d}") + (", mono" if mono else "") + \
+            (", mixed cal." if mix else "")
+        print(f"{name:40s}: {o['aggregate_fps']:8.0f} frames/s [{o['aggregate_fps_min']:.0f}, {o['aggregate_fps_max']:.0f}], "
               f"step {o['step_latency_ms']:.3f} ms, {o['launches_per_submission']:.1f} launches / submission")
     print(json.dumps(out))
     if a.json:

@@ -1,17 +1,19 @@
 #!/usr/bin/env python
-"""Several KITTI sequences that share one calibration through ONE context (the multi-sequence mode, vo_mseq_*):
+"""Several KITTI sequences through ONE context (the multi-sequence mode, vo_mseq_*), each with its own calibration:
 
-    python tools/run_sequences.py /data/kitti/sequences/00/ /data/kitti/sequences/02/ calibration/kitti00.yaml \\
-        --poses out/ [--gt /data/kitti/poses/]
+    python tools/run_sequences.py /data/kitti/sequences/00/ /data/kitti/sequences/04/ calibration/kitti00.yaml \\
+        --calibration-for 04=calibration/kitti04.yaml --poses out/ [--gt /data/kitti/poses/]
 
 Every <dataset>/image_0/%06d.png and image_1/%06d.png is decoded ahead by its own library reader into pinned buffers; one
 submission advances every sequence by one frame (two submissions in flight), and a sequence is retired at its last
 frame, so sequences of unequal length share the run.  frame_pose of each is integrated with the reference's Euler and
 scale gates (src/main.cpp:196-208), written to OUTDIR/<name>.txt in the KITTI text format (<name> = the dataset
 directory's name) and, with --gt, scored against GTDIR/<name>.txt with the KITTI segment metric.  All sequences must
-have the image size of the first.  `--mono-rotation` runs trackingFrame2Frame as its header default does, for every
-sequence (mono_rotation = true: the rotation from findEssentialMat + recoverPose, the translation from the PnP; frames
-where that branch would abort are reported and not integrated).  `--check` only validates the inputs (no GPU needed)."""
+have the image size of the first.  The positional calibration applies to every sequence that no
+`--calibration-for NAME=YAML` names (NAME = the dataset directory's name); each sequence runs with the matrices built from
+its own file, as the reference's main() builds them (src/main.cpp:67-74).  `--mono-rotation` runs trackingFrame2Frame
+as its header default does, for every sequence (mono_rotation = true: the rotation from findEssentialMat + recoverPose,
+the translation from the PnP; frames where that branch would abort are reported and not integrated).  `--check` only validates the inputs (no GPU needed)."""
 import argparse
 import os
 import sys
@@ -34,16 +36,29 @@ def main():
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--mono-rotation", action="store_true",
                     help="rotation from findEssentialMat + recoverPose (trackingFrame2Frame's header default)")
+    ap.add_argument("--calibration-for", action="append", default=[], metavar="NAME=YAML",
+                    help="calibration of the dataset named NAME (repeatable; the others use the positional one)")
     ap.add_argument("--check", action="store_true")
     a = ap.parse_args()
     from visual_odom_b200 import capi, synth
-    cal = read_calibration(a.calibration)
-    P_l, P_r = synth.proj_matrices(cal)
+    default_cal = read_calibration(a.calibration)
     if len(a.datasets) > capi.VO_MSEQ_MAX:
         raise SystemExit(f"{len(a.datasets)} sequences: one context runs at most {capi.VO_MSEQ_MAX}")
     names = [os.path.basename(os.path.normpath(d)) for d in a.datasets]
     if len(set(names)) != len(names):
         raise SystemExit(f"two datasets share a directory name ({names}): their pose files would collide")
+    cal_for = {}
+    for spec in a.calibration_for:
+        name, sep, path = spec.partition("=")
+        if not sep or not name or not path:
+            raise SystemExit(f"--calibration-for {spec}: expected NAME=YAML")
+        if name not in names:
+            raise SystemExit(f"--calibration-for {spec}: no dataset is named {name} (names: {', '.join(names)})")
+        if name in cal_for:
+            raise SystemExit(f"--calibration-for: {name} is given twice")
+        if not os.path.isfile(path):
+            raise SystemExit(f"--calibration-for {spec}: {path} does not exist")
+        cal_for[name] = (path, read_calibration(path))
     seqs = []
     for d, name in zip(a.datasets, names):
         n = count_frames(d, 0)
@@ -56,9 +71,11 @@ def main():
         gt = os.path.join(a.gt, name + ".txt") if a.gt else None
         if gt and not os.path.exists(gt):
             raise SystemExit(f"{gt}: no ground truth for sequence {name}")
-        seqs.append(dict(dir=d, name=name, n=n, w=w, h=h, gray=ctype == 0, gt=gt))
-        print(f"{name}: {n} stereo pairs of {w}x{h} (PNG colour type {ctype}, {depth} bit)")
-    print(f"P_left =\n{P_l}\nP_right =\n{P_r}")
+        cal_path, cal = cal_for.get(name, (a.calibration, default_cal))
+        P_l, P_r = synth.proj_matrices(cal)
+        seqs.append(dict(dir=d, name=name, n=n, w=w, h=h, gray=ctype == 0, gt=gt, P_l=P_l, P_r=P_r))
+        print(f"{name}: {n} stereo pairs of {w}x{h} (PNG colour type {ctype}, {depth} bit), calibration {cal_path}")
+        print(f"  P_left =\n{P_l}\n  P_right =\n{P_r}")
     print("rotation: " + ("findEssentialMat + recoverPose (mono_rotation = true)" if a.mono_rotation else
                           "Rodrigues of the PnP rvec (mono_rotation = false)"))
     if a.check:
@@ -84,6 +101,7 @@ def main():
         return lp, rp, pitch, ch
 
     lp, rp, pitch, ch = pairs(0)
+    P_l = np.stack([s["P_l"] for s in seqs]); P_r = np.stack([s["P_r"] for s in seqs])
     ctx.mseq_begin_ptr(seqs[0]["w"], seqs[0]["h"], lp, rp, pitch, P_l, P_r, ch, mono_rotation=a.mono_rotation)
     poses = [[np.eye(4)] for _ in seqs]
     aborted = [0] * len(seqs)

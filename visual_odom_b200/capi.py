@@ -179,6 +179,9 @@ SIGNATURES = {
                                 C.c_int]),
     "vo_mseq_begin_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_size_t, C.c_int, C.c_int]),
+    "vo_mseq_begin_calib": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_size_t, C.c_int, C.c_int]),
+    "vo_batch_calibrate": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "vo_mseq_submit": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
     "vo_mseq_wait": (C.c_int, [C.c_void_p, C.POINTER(VoUnitResult), C.c_void_p, C.c_void_p, C.c_int]),
     "vo_mseq_wait_mono": (C.c_int, [C.c_void_p, C.POINTER(VoUnitResult), C.c_void_p, C.POINTER(VoMonoResult), C.c_void_p,
@@ -380,6 +383,14 @@ class Context:
         P_l = np.ascontiguousarray(P_l, np.float32).reshape(12); P_r = np.ascontiguousarray(P_r, np.float32).reshape(12)
         self._check(self.lib.vo_batch_configure(self.h, w, h, n_units, _p(P_l), _p(P_r)))
         self._batch_geom = (w, h, n_units)
+
+    def batch_calibrate(self, first_unit, P_l, P_r):
+        """Units [first_unit, first_unit + n) get their own calibrations: P_l / P_r of shape (n, 3, 4) (vo_batch_calibrate).
+        Refused while submissions are in flight."""
+        P_l = np.ascontiguousarray(P_l, np.float32); P_r = np.ascontiguousarray(P_r, np.float32)
+        if P_l.ndim != 3 or P_l.shape[1:] != (3, 4) or P_r.shape != P_l.shape:
+            raise ValueError(f"P_l / P_r must be (n, 3, 4), got {P_l.shape} / {P_r.shape}")
+        self._check(self.lib.vo_batch_calibrate(self.h, first_unit, len(P_l), _p(P_l), _p(P_r)))
 
     def make_units(self, units):
         """units: list of dicts(l0,r0,l1,r1 uint8 HxW [, pts (n,2) f32 | n_select int] [, t_prev]).
@@ -723,26 +734,35 @@ class Context:
         ch = 1 if len(geom) == 2 else 3
         return lp, rp, geom[1] * ch, ch, keep, geom
 
-    def mseq_begin(self, lefts, rights, P_l, P_r, mono_rotation=False):
-        """Start len(lefts) sequences (one calibration, one image size) from their first stereo pairs.  mono_rotation=True:
-        every sequence runs trackingFrame2Frame(mono_rotation = true) (flag VO_MSEQ_MONO_ROTATION; see mseq_wait(mono=True))."""
-        lp, rp, pitch, ch, keep, geom = self._pairs(lefts, rights, False)
-        P_l = np.ascontiguousarray(P_l, np.float32).reshape(12); P_r = np.ascontiguousarray(P_r, np.float32).reshape(12)
-        h, w = (geom or (0, 0))[:2]
+    def _mseq_begin(self, n, w, h, lp, rp, pitch, ch, P_l, P_r, mono_rotation):
+        """P_l / P_r (3, 4): one calibration for every sequence (vo_mseq_begin_ex); (n, 3, 4): sequence q runs with
+        P_l[q] / P_r[q] (vo_mseq_begin_calib)."""
+        P_l = np.ascontiguousarray(P_l, np.float32); P_r = np.ascontiguousarray(P_r, np.float32)
         flags = VO_MSEQ_MONO_ROTATION if mono_rotation else 0
-        self._check(self.lib.vo_mseq_begin_ex(self.h, len(lefts), w, h, _p(P_l), _p(P_r), lp, rp, pitch, ch, flags))
-        self._mseq_n, self._mseq_pitch = len(lefts), pitch
-        self._mseq_keep = [None, None]
-
-    def mseq_begin_ptr(self, w, h, left_ptrs, right_ptrs, pitch, P_l, P_r, channels=1, mono_rotation=False):
-        """Raw host pointers, one pair per sequence (e.g. the pinned buffers of one SequenceReader each)."""
-        n = len(left_ptrs)
-        lp, rp = (C.c_void_p * n)(*left_ptrs), (C.c_void_p * n)(*right_ptrs)
-        Pl = np.ascontiguousarray(P_l, np.float32); Pr = np.ascontiguousarray(P_r, np.float32)
-        flags = VO_MSEQ_MONO_ROTATION if mono_rotation else 0
-        self._check(self.lib.vo_mseq_begin_ex(self.h, n, w, h, _p(Pl), _p(Pr), lp, rp, pitch, channels, flags))
+        if P_l.ndim == 3 or P_r.ndim == 3:
+            if P_l.shape != (n, 3, 4) or P_r.shape != (n, 3, 4):
+                raise ValueError(f"per-sequence calibrations must be ({n}, 3, 4), got {P_l.shape} / {P_r.shape}")
+            self._check(self.lib.vo_mseq_begin_calib(self.h, n, w, h, _p(P_l), _p(P_r), lp, rp, pitch, ch, flags))
+        else:
+            P_l = P_l.reshape(12); P_r = P_r.reshape(12)
+            self._check(self.lib.vo_mseq_begin_ex(self.h, n, w, h, _p(P_l), _p(P_r), lp, rp, pitch, ch, flags))
         self._mseq_n, self._mseq_pitch = n, pitch
         self._mseq_keep = [None, None]
+
+    def mseq_begin(self, lefts, rights, P_l, P_r, mono_rotation=False):
+        """Start len(lefts) sequences (one image size) from their first stereo pairs.  P_l / P_r: (3, 4) for one calibration,
+        or (n_seq, 3, 4) for one per sequence.  mono_rotation=True: every sequence runs trackingFrame2Frame(mono_rotation =
+        true) (flag VO_MSEQ_MONO_ROTATION; see mseq_wait(mono=True))."""
+        lp, rp, pitch, ch, keep, geom = self._pairs(lefts, rights, False)
+        h, w = (geom or (0, 0))[:2]
+        self._mseq_begin(len(lefts), w, h, lp, rp, pitch, ch, P_l, P_r, mono_rotation)
+
+    def mseq_begin_ptr(self, w, h, left_ptrs, right_ptrs, pitch, P_l, P_r, channels=1, mono_rotation=False):
+        """Raw host pointers, one pair per sequence (e.g. the pinned buffers of one SequenceReader each); P_l / P_r as for
+        mseq_begin."""
+        n = len(left_ptrs)
+        lp, rp = (C.c_void_p * n)(*left_ptrs), (C.c_void_p * n)(*right_ptrs)
+        self._mseq_begin(n, w, h, lp, rp, pitch, channels, P_l, P_r, mono_rotation)
 
     def mseq_submit_ptr(self, left_ptrs, right_ptrs, pitch, channels=1):
         """Raw host pointers; None in both lists retires that sequence.  The memory must stay valid until the wait."""

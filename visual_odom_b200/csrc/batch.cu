@@ -115,11 +115,27 @@ extern "C" int vo_batch_configure(vo_ctx* ctx, int w, int h, int n_units, const 
     int rc = vo_claim_buffers(ctx, "vo_batch_configure");
     if (rc) return rc;
     if ((rc = vo_ensure_state(ctx, w, h, n_units))) return rc;
-    vo_set_calibration(ctx, P_l, P_r);
+    if ((rc = vo_set_calibration(ctx, 0, ctx->units, P_l, P_r, 1))) return rc;        // every unit, as the resident state holds them
     ctx->batch_units = n_units;
     ctx->batch_uploaded = 0;
     ctx->slot_pts.assign(n_units, 0);
     return VO_OK;
+}
+
+// Refused while submissions are in flight (they read the table); an idle sequence is ended, as by vo_batch_configure,
+// since its units may be among those set.  The write is queued on the context's stream, ahead of every later submission.
+extern "C" int vo_batch_calibrate(vo_ctx* ctx, int first_unit, int n_units, const float* P_l, const float* P_r)
+{
+    if (!ctx) return VO_E_INVALID;
+    if (!P_l || !P_r) { vo_set_error(ctx, "vo_batch_calibrate: null projection matrices"); return VO_E_INVALID; }
+    if (first_unit < 0 || n_units <= 0 || first_unit + n_units > ctx->batch_units) {
+        vo_set_error(ctx, "vo_batch_calibrate: units [%d, %d) outside the configured batch (%d)", first_unit, first_unit + n_units, ctx->batch_units);
+        return VO_E_INVALID;
+    }
+    VO_CUDA_CHECK(cudaSetDevice(ctx->device));
+    int rc = vo_claim_buffers(ctx, "vo_batch_calibrate");
+    if (rc) return rc;
+    return vo_set_calibration(ctx, first_unit, n_units, P_l, P_r, n_units);
 }
 
 // Pinned staging of the batched path, disjoint per unit: t_prev [batch_units][3] | counts [batch_units] | result records
@@ -283,9 +299,8 @@ static int run_range_launch(vo_ctx* ctx, const View& v)
     if ((rc = hand_over(2, lk.s, post.s))) return rc;
     if ((rc = vo_run_filter(ctx, post, false))) return rc;
     const size_t cs = (size_t)ctx->units * ctx->cap;
-    if ((rc = vo_run_triangulate(ctx, post, ctx->d_valid4, ctx->d_valid4 + cs, ctx->d_n5))) return rc;
-    float K9[9] = {ctx->P_l[0], ctx->P_l[1], ctx->P_l[2], ctx->P_l[4], ctx->P_l[5], ctx->P_l[6], ctx->P_l[8], ctx->P_l[9], ctx->P_l[10]};
-    if ((rc = vo_run_pnp(ctx, post, ctx->d_valid4 + 2 * cs, ctx->d_n5, K9))) return rc;
+    if ((rc = vo_run_triangulate(ctx, post, ctx->d_valid4, ctx->d_valid4 + cs, ctx->d_n5, ctx->d_cal))) return rc;
+    if ((rc = vo_run_pnp(ctx, post, ctx->d_valid4 + 2 * cs, ctx->d_n5, ctx->d_cal))) return rc;
     k_pack_counts<<<(v.n + 63) / 64, 64, 0, post.s>>>(ctx->d_results + v.u0, ctx->d_npts + v.u0, ctx->d_ndet + v.u0, ctx->d_n3 + v.u0,
                                                      ctx->d_n5 + v.u0, v.n, ctx->batch_detect ? 1 : 0);
     ctx->launches += 1;
@@ -316,7 +331,6 @@ extern "C" int vo_batch_run(vo_ctx* ctx)
     if (!ctx) return VO_E_INVALID;
     const int units = ctx->batch_uploaded;
     if (units <= 0) { vo_set_error(ctx, "vo_batch_run: nothing uploaded"); return VO_E_INVALID; }
-    if (!ctx->have_P) { vo_set_error(ctx, "vo_batch_run: projection matrices not set"); return VO_E_INVALID; }
     { int rcc = vo_claim_buffers(ctx, "vo_batch_run"); if (rcc) return rcc; }
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
     if (units < 2 || ctx->batch_streams < 2) return run_range(ctx, 0, units, ctx->stream);
@@ -357,7 +371,6 @@ extern "C" int vo_frame_batch(vo_ctx* ctx, const vo_unit* units, int n_units, si
     int rc = validate_units(ctx, units, n_units, pitch, &detect);
     if (rc) return rc;
     if (!results) return VO_E_INVALID;
-    if (!ctx->have_P) { vo_set_error(ctx, "vo_frame_batch: projection matrices not set"); return VO_E_INVALID; }
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
     if ((rc = vo_claim_buffers(ctx, "vo_frame_batch", true))) return rc;
     if ((rc = vo_drain_pending(ctx))) return rc;
@@ -425,7 +438,6 @@ static int batch_submit(vo_ctx* ctx, const char* who, const Unit* units, int fir
         vo_set_error(ctx, "%s: slots [%d, %d) outside the configured batch (%d)", who, first_unit, first_unit + n_units, ctx->batch_units);
         return VO_E_INVALID;
     }
-    if (!ctx->have_P) { vo_set_error(ctx, "%s: projection matrices not set", who); return VO_E_INVALID; }
     { int rcc = vo_claim_buffers(ctx, who, true); if (rcc) return rcc; }
     for (auto& p : ctx->pending)
         if (p.active && first_unit < p.u0 + p.n && p.u0 < first_unit + n_units) {

@@ -136,14 +136,16 @@ static int triangulate_impl(vo_ctx* ctx, const float P_l[12], const float P_r[12
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
     int rc = ensure_any_state(ctx);
     if (rc) return rc;
-    vo_set_calibration(ctx, P_l, P_r);
+    CamCalib c = ctx->cal[0];           // the stage calls' entry: the sequence and batched units keep their cameras
+    for (int k = 0; k < 12; k++) { c.Pl[k] = (double)P_l[k]; c.Pr[k] = (double)P_r[k]; }
+    if ((rc = vo_write_calib(ctx, -1, 1, &c))) return rc;
     const size_t cs = (size_t)ctx->units * ctx->cap;
     VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_valid4, pts_l, (size_t)n * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
     VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_valid4 + cs, pts_r, (size_t)n * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
     VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_n5, &n, sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
     // the homogeneous points use the (then idle) A5 point lists 2..3 of unit 0 as scratch: n float4 = 2 n float2
     float4* d_X4 = X4 ? reinterpret_cast<float4*>(ctx->d_kept5) : nullptr;
-    if ((rc = vo_run_triangulate(ctx, View{0, 1, ctx->stream}, ctx->d_valid4, ctx->d_valid4 + cs, ctx->d_n5, d_X4))) return rc;
+    if ((rc = vo_run_triangulate(ctx, View{0, 1, ctx->stream}, ctx->d_valid4, ctx->d_valid4 + cs, ctx->d_n5, ctx->d_cal_tab, d_X4))) return rc;
     if (X) VO_CUDA_CHECK(cudaMemcpyAsync(X, ctx->d_X, (size_t)n * sizeof(float3), cudaMemcpyDeviceToHost, ctx->stream));
     if (X4) VO_CUDA_CHECK(cudaMemcpyAsync(X4, d_X4, (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, ctx->stream));
     VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
@@ -185,7 +187,10 @@ extern "C" int vo_pnp_ransac(vo_ctx* ctx, const vo_point3f* X, const vo_point2f*
     VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_valid4 + 2 * cs, x, (size_t)n * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
     VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_n5, &n, sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
     VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_tprev, tvec_io, 3 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    if ((rc = vo_run_pnp(ctx, View{0, 1, ctx->stream}, ctx->d_valid4 + 2 * cs, ctx->d_n5, K))) return rc;
+    CamCalib c = ctx->cal[0];           // the stage calls' entry
+    vo_calib_set_pnp(c, K);
+    if ((rc = vo_write_calib(ctx, -1, 1, &c))) return rc;
+    if ((rc = vo_run_pnp(ctx, View{0, 1, ctx->stream}, ctx->d_valid4 + 2 * cs, ctx->d_n5, ctx->d_cal_tab))) return rc;
     vo_unit_result_dev r;
     VO_CUDA_CHECK(cudaMemcpyAsync(&r, ctx->d_results, sizeof(r), cudaMemcpyDeviceToHost, ctx->stream));
     VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
@@ -211,11 +216,11 @@ extern "C" int vo_mono_rotation(vo_ctx* ctx, const vo_point2f* pts_t0, const vo_
     if (!pts_t0 || !pts_t1) { vo_set_error(ctx, "null argument"); return VO_E_INVALID; }
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
     const int iters = VO_ESS_ITERS;
-    // one scratch block: points | count | the kernels' scratch (vo_ess_bind).  Separate from the sequence mode's
-    // per-frame scratch, so this call never touches a sequence's state.
+    // one scratch block: points | count | camera | the kernels' scratch (vo_ess_bind).  Separate from the sequence mode's
+    // per-frame scratch and calibration table, so this call never touches a sequence's state.
     auto up = [](size_t x) { return (x + 255) / 256 * 256; };
-    const size_t o_p0 = 0, o_p1 = o_p0 + up((size_t)n * 8), o_n = o_p1 + up((size_t)n * 8), o_ess = o_n + up(sizeof(int)),
-                 total = o_ess + vo_ess_scratch_bytes(n, iters);
+    const size_t o_p0 = 0, o_p1 = o_p0 + up((size_t)n * 8), o_n = o_p1 + up((size_t)n * 8), o_cal = o_n + up(sizeof(int)),
+                 o_ess = o_cal + up(sizeof(CamCalib)), total = o_ess + vo_ess_scratch_bytes(n, iters);
     if (!ctx->d_ess || ctx->ess_cap < n) {
         VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
         if (ctx->d_ess) { cudaFree(ctx->d_ess); ctx->d_ess = nullptr; }
@@ -225,10 +230,14 @@ extern "C" int vo_mono_rotation(vo_ctx* ctx, const vo_point2f* pts_t0, const vo_
     uint8_t* b = (uint8_t*)ctx->d_ess;
     EssArgs a;
     memset(&a, 0, sizeof(a));
-    vo_ess_set_camera(a, focal, ppx, ppy);
+    CamCalib cal;
+    memset(&cal, 0, sizeof(cal));
+    vo_calib_set_ess(cal, focal, ppx, ppy);
     vo_ess_bind(a, b + o_ess, n, iters);
     a.n = (const int*)(b + o_n);
+    a.cal = (const CamCalib*)(b + o_cal);
     a.pts0 = (const float2*)(b + o_p0); a.pts1 = (const float2*)(b + o_p1);
+    VO_CUDA_CHECK(cudaMemcpyAsync(b + o_cal, &cal, sizeof(cal), cudaMemcpyHostToDevice, ctx->stream));
     VO_CUDA_CHECK(cudaMemcpyAsync(b + o_p0, pts_t0, (size_t)n * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
     VO_CUDA_CHECK(cudaMemcpyAsync(b + o_p1, pts_t1, (size_t)n * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
     VO_CUDA_CHECK(cudaMemcpyAsync(b + o_n, &n, sizeof(int), cudaMemcpyHostToDevice, ctx->stream));

@@ -32,6 +32,44 @@ struct PyrGeom {
     LevelGeom lv[VO_MAX_LEVELS];
 };
 
+// One camera as the triangulation, PnP and five-point kernels read it: one entry per buffer unit in the context's
+// calibration table (ctx.h vo_ctx::d_cal).  Every value is computed on the host with the expressions of the reference's
+// callers (vo_calib_from), so a kernel sees the same bits whichever unit or problem it serves.
+struct CamCalib {
+    double Pl[12], Pr[12];        // k_triangulate: the float projection matrices widened to double
+    double fu, fv, uc, vc;        // PnP: K = P_l(0:3, 0:3) as floats (main.cpp:75 / visualOdometry.cpp:141), widened
+    double focal, ppx, ppy;       // five-point branch: `double focal = projMatrl.at<float>(0, 0)`, principle_point
+                                  // (visualOdometry.cpp:144-145)
+    float thr2;                   // (float)((threshold / focal)^2), threshold 1.0 of the findEssentialMat call (:154)
+    int pad_;
+};
+
+// the five-point branch's camera values (also vo_mono_rotation's, which takes focal / pp directly)
+static inline void vo_calib_set_ess(CamCalib& c, double focal, double ppx, double ppy)
+{
+    c.focal = focal; c.ppx = ppx; c.ppy = ppy;
+    const double thr = 1.0 / focal;                // threshold /= (fx + fy) / 2
+    c.thr2 = (float)(thr * thr);
+}
+
+// the PnP intrinsics of a float K (row-major 3 x 3)
+static inline void vo_calib_set_pnp(CamCalib& c, const float K9[9])
+{
+    c.fu = (double)K9[0]; c.fv = (double)K9[4]; c.uc = (double)K9[2]; c.vc = (double)K9[5];
+}
+
+// every value from one stereo pair of projection matrices (row-major 3 x 4 floats)
+static inline CamCalib vo_calib_from(const float P_l[12], const float P_r[12])
+{
+    CamCalib c;
+    for (int k = 0; k < 12; k++) { c.Pl[k] = (double)P_l[k]; c.Pr[k] = (double)P_r[k]; }
+    const float K9[9] = {P_l[0], P_l[1], P_l[2], P_l[4], P_l[5], P_l[6], P_l[8], P_l[9], P_l[10]};
+    vo_calib_set_pnp(c, K9);
+    vo_calib_set_ess(c, (double)P_l[0], (double)P_l[2], (double)P_l[6]);
+    c.pad_ = 0;
+    return c;
+}
+
 static __host__ __device__ __forceinline__ int vo_reflect101(int p, int len)
 {
     if (len == 1) return 0;

@@ -346,15 +346,22 @@ int vo_ensure_lanes(vo_ctx* ctx)
     return VO_OK;
 }
 
-void vo_set_calibration(vo_ctx* ctx, const float P_l[12], const float P_r[12])
+int vo_write_calib(vo_ctx* ctx, int u0, int n, const CamCalib* c)
 {
-    const bool same = ctx->have_P && memcmp(ctx->P_l, P_l, 12 * sizeof(float)) == 0 && memcmp(ctx->P_r, P_r, 12 * sizeof(float)) == 0;
-    if (same) return;
-    // TriArgs / PnpArgs are passed by value: a captured graph would keep replaying the old matrices
-    vo_drop_graphs(ctx);
-    memcpy(ctx->P_l, P_l, 12 * sizeof(float));
-    memcpy(ctx->P_r, P_r, 12 * sizeof(float));
-    ctx->have_P = true;
+    const size_t e0 = (size_t)(1 + u0);
+    if (memcmp(ctx->cal.data() + e0, c, n * sizeof(CamCalib)) == 0) return VO_OK;
+    memcpy(ctx->cal.data() + e0, c, n * sizeof(CamCalib));
+    for (auto& p : ctx->pending)
+        if (p.active) VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, p.done, 0));
+    VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_cal_tab + e0, ctx->cal.data() + e0, n * sizeof(CamCalib), cudaMemcpyHostToDevice, ctx->stream));
+    return VO_OK;
+}
+
+int vo_set_calibration(vo_ctx* ctx, int u0, int n, const float* P_l, const float* P_r, int n_mat)
+{
+    std::vector<CamCalib> c(n);
+    for (int i = 0; i < n; i++) c[i] = vo_calib_from(P_l + 12 * (i % n_mat), P_r + 12 * (i % n_mat));
+    return vo_write_calib(ctx, u0, n, c.data());
 }
 
 void vo_free_state(vo_ctx* ctx)
@@ -366,6 +373,7 @@ void vo_free_state(vo_ctx* ctx)
     ctx->d_seq_state = nullptr; ctx->seq_n_cap = 0;
     ctx->d_feat_pts = nullptr; ctx->d_feat_ages = nullptr; ctx->d_feat_cnt = ctx->d_bucket = ctx->d_seq_err = ctx->d_seq_live = nullptr;
     ctx->d_out = nullptr; ctx->out_stride = 0; ctx->out_per = 0;
+    ctx->d_cal_tab = ctx->d_cal = nullptr;
     ctx->w = ctx->h = ctx->units = 0;
 }
 
@@ -507,6 +515,11 @@ int vo_ensure_state(vo_ctx* ctx, int w, int h, int units)
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_counts, (size_t)units * its));
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_inliers, uc));
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_results, (size_t)units));
+    // calibration table: the entries set so far carry over (a unit keeps its camera until it is set again)
+    VO_CUDA_CHECK(dalloc(ctx, &ctx->d_cal_tab, 1 + (size_t)units));
+    ctx->d_cal = ctx->d_cal_tab + 1;
+    ctx->cal.resize(1 + (size_t)units, CamCalib{});
+    VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_cal_tab, ctx->cal.data(), (1 + (size_t)units) * sizeof(CamCalib), cudaMemcpyHostToDevice, ctx->stream));
     // sequence mode state: sized per sequence at vo_seq_begin / vo_mseq_begin (seq_api.cu)
     ctx->feat_cap = ctx->corner_cap + cap;
     ctx->seq_active = false;
@@ -665,26 +678,27 @@ int vo_run_select(vo_ctx* ctx, const View& v)
     return VO_OK;
 }
 
-int vo_run_triangulate(vo_ctx* ctx, const View& v, const float2* pts_l, const float2* pts_r, const int* n, float4* X4)
+int vo_run_triangulate(vo_ctx* ctx, const View& v, const float2* pts_l, const float2* pts_r, const int* n, const CamCalib* cal,
+                       float4* X4)
 {
     const size_t uo = (size_t)v.u0 * ctx->cap;
     TriArgs t;
     memset(&t, 0, sizeof(t));
     t.cap = ctx->cap; t.n_pts = n + v.u0; t.pts_l = pts_l + uo; t.pts_r = pts_r + uo; t.X = ctx->d_X + uo; t.X4 = X4;
-    for (int k = 0; k < 12; k++) { t.Pl[k] = (double)ctx->P_l[k]; t.Pr[k] = (double)ctx->P_r[k]; }
+    t.cal = cal + v.u0;
     ctx->launches += vo_launch_triangulate(t, v.n, v.s);
     VO_CUDA_CHECK(cudaGetLastError());
     return VO_OK;
 }
 
-int vo_run_pnp(vo_ctx* ctx, const View& v, const float2* pts2d, const int* n, const float* K9)
+int vo_run_pnp(vo_ctx* ctx, const View& v, const float2* pts2d, const int* n, const CamCalib* cal)
 {
     const size_t uo = (size_t)v.u0 * ctx->cap, its = (size_t)ctx->p.pnp_iterations;
     PnpArgs a;
     memset(&a, 0, sizeof(a));
     a.n_units = v.n; a.cap = ctx->cap; a.iterations = ctx->p.pnp_iterations;
     a.n_pts = n + v.u0; a.X = ctx->d_X + uo; a.x = pts2d + uo;
-    a.fu = (double)K9[0]; a.fv = (double)K9[4]; a.uc = (double)K9[2]; a.vc = (double)K9[5];
+    a.cal = cal + v.u0;
     const double thr = (double)ctx->p.pnp_reproj_error;      // float -> double, squared in double, stored float
     a.thr2 = (float)(thr * thr);
     a.confidence = ctx->p.pnp_confidence;

@@ -40,8 +40,12 @@ struct vo_ctx {
     int cap = 0;                  // feature capacity per unit
     PyrGeom pg;                   // device plane pointers per level
     LkMaps maps;                  // TMA descriptors per level
-    bool have_P = false;
-    float P_l[12], P_r[12];
+    // calibration table (part of the batch state, so its address is fixed for as long as any captured graph lives):
+    // entry 0 is the stage calls' (vo_triangulate, vo_pnp_ransac), entry 1 + u buffer unit u's.  The kernels read their
+    // unit's entry, so captured graphs carry no calibration and a table write needs no graph drop.  cal mirrors it.
+    CamCalib* d_cal_tab = nullptr;      // [1 + units]
+    CamCalib* d_cal = nullptr;          // d_cal_tab + 1: indexed by buffer unit
+    std::vector<CamCalib> cal;          // [1 + units] host copy (kept across re-allocations of the batch state)
 
     // ---- device buffers ---------------------------------------------------------------------
     uint8_t* d_raw = nullptr;           // [units*4][h*w] raw images
@@ -207,8 +211,12 @@ int vo_run_graph(vo_ctx* ctx, const GraphKey& key, const std::function<int()>& l
 // the lanes' side streams and fork / join events (their pre / lk / post streams are filled in by the partition or on
 // first use of the priority helpers)
 int vo_ensure_lanes(vo_ctx* ctx);
-// new projection matrices: cached graphs carry the old calibration in their kernel arguments, so they are dropped
-void vo_set_calibration(vo_ctx* ctx, const float P_l[12], const float P_r[12]);
+// Calibration table entries [1 + u0, 1 + u0 + n) (buffer units u0 ..; u0 = -1 is the stage calls' entry) = c[0 .. n),
+// written on ctx->stream only where they change.  The copy is queued after every batch submission still in flight, so
+// it never lands under one; sequence frames in flight are the caller's to refuse or drain.
+int vo_write_calib(vo_ctx* ctx, int u0, int n, const CamCalib* c);
+// buffer units [u0, u0 + n): unit u0 + i from the matrices P_l + 12 * (i % n_mat), P_r + 12 * (i % n_mat)
+int vo_set_calibration(vo_ctx* ctx, int u0, int n, const float* P_l, const float* P_r, int n_mat);
 int vo_drain_pending(vo_ctx* ctx);
 // Entry points that overwrite the shared image planes / unit-0 buffers call this first: refused (VO_E_INVALID) while
 // sequence frames or batch submissions are in flight; an idle sequence is ended (its planes are about to be reused).
@@ -243,6 +251,8 @@ int vo_run_filter(vo_ctx* ctx, const View& v, bool with_ages);
 // FAST on raw plane `plane_in_unit` of each unit -> d_corners / d_ndet ; stride selection -> d_pts_in / d_npts
 int vo_run_fast(vo_ctx* ctx, const View& v, int plane_in_unit, bool want_resp);
 int vo_run_select(vo_ctx* ctx, const View& v);
-// triangulate pts_l/pts_r ([units][cap], counts n) -> d_X ; PnP on (d_X, pts2d) -> d_results / d_inliers
-int vo_run_triangulate(vo_ctx* ctx, const View& v, const float2* pts_l, const float2* pts_r, const int* n, float4* X4 = nullptr);
-int vo_run_pnp(vo_ctx* ctx, const View& v, const float2* pts2d, const int* n, const float* K9);
+// triangulate pts_l/pts_r ([units][cap], counts n) -> d_X ; PnP on (d_X, pts2d) -> d_results / d_inliers.  Unit u reads
+// the camera cal[u] (ctx->d_cal, or the stage calls' single entry with v.u0 = 0).
+int vo_run_triangulate(vo_ctx* ctx, const View& v, const float2* pts_l, const float2* pts_r, const int* n, const CamCalib* cal,
+                       float4* X4 = nullptr);
+int vo_run_pnp(vo_ctx* ctx, const View& v, const float2* pts2d, const int* n, const CamCalib* cal);

@@ -49,6 +49,7 @@ static __device__ __forceinline__ EssArgs ess_prob(const EssArgs& a0, int p)
     EssArgs a = a0;
     const size_t so = (size_t)p * a0.scratch_stride;
     a.n += (size_t)p * a0.n_stride;
+    a.cal += (size_t)p * a0.cal_stride;
     a.pts0 += (size_t)p * a0.pts_stride; a.pts1 += (size_t)p * a0.pts_stride;
     a.q0 = ess_at(a0.q0, so); a.q1 = ess_at(a0.q1, so); a.state = ess_at(a0.state, so);
     a.subsets = ess_at(a0.subsets, so); a.models = ess_at(a0.models, so); a.nmodels = ess_at(a0.nmodels, so);
@@ -81,8 +82,9 @@ __global__ void k_ess_init(const EssArgs a0)
     }
     if (i >= n) return;
     const float2 p0 = a.pts0[i], p1 = a.pts1[i];
-    a.q0[i] = make_double2(((double)p0.x - a.ppx) / a.focal, ((double)p0.y - a.ppy) / a.focal);
-    a.q1[i] = make_double2(((double)p1.x - a.ppx) / a.focal, ((double)p1.y - a.ppy) / a.focal);
+    const double focal = a.cal->focal, ppx = a.cal->ppx, ppy = a.cal->ppy;
+    a.q0[i] = make_double2(((double)p0.x - ppx) / focal, ((double)p0.y - ppy) / focal);
+    a.q1[i] = make_double2(((double)p1.x - ppx) / focal, ((double)p1.y - ppy) / focal);
 }
 
 __global__ void k_ess_subsets(const EssArgs a0, int it0, int it1)
@@ -140,10 +142,11 @@ __global__ void __launch_bounds__(128) k_ess_count(const EssArgs a0, int it0, in
     if (threadIdx.x == 0) total = 0;
     __syncthreads();
     const int n = ess_n(a);
+    const float thr2 = a.cal->thr2;
     int c = 0;
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
         const double2 u = a.q0[i], v = a.q1[i];
-        c += sampson_err(E, u.x, u.y, v.x, v.y) <= a.thr2;
+        c += sampson_err(E, u.x, u.y, v.x, v.y) <= thr2;
     }
     for (int d = 16; d > 0; d >>= 1) c += __shfl_xor_sync(0xffffffffu, c, d);
     if ((threadIdx.x & 31) == 0) atomicAdd(&total, c);
@@ -204,7 +207,7 @@ __global__ void k_ess_mask(const EssArgs a0)
     if (s.best_it < 0) { a.mask[i] = 0; return; }
     const double* E = a.models + (size_t)s.best_it * 90 + s.best_cand * 9;
     const double2 u = a.q0[i], v = a.q1[i];
-    a.mask[i] = (n == 5 || sampson_err(E, u.x, u.y, v.x, v.y) <= a.thr2) ? 1 : 0;
+    a.mask[i] = (n == 5 || sampson_err(E, u.x, u.y, v.x, v.y) <= a.cal->thr2) ? 1 : 0;
 }
 
 __global__ void k_ess_decompose(const EssArgs a0)
@@ -287,7 +290,8 @@ void vo_ess_bind(EssArgs& a, void* scratch, int n_max, int max_iters)
     uint8_t* b = (uint8_t*)scratch;
     auto take = [&](size_t bytes) { uint8_t* p = b; b += ess_up(bytes); return p; };
     a.n_max = n_max; a.max_iters = max_iters;
-    a.n_prob = 1; a.scratch_stride = 0; a.pts_stride = 0; a.n_stride = 0; a.result_stride = 0;
+    a.n_prob = 1; a.scratch_stride = 0; a.pts_stride = 0; a.n_stride = 0; a.result_stride = 0; a.cal_stride = 0;
+    a.prob = 0.999;
     a.q0 = (double2*)take(n * sizeof(double2)); a.q1 = (double2*)take(n * sizeof(double2));
     a.state = (EssState*)take(sizeof(EssState));
     a.subsets = (int*)take(it * 5 * sizeof(int));

@@ -35,7 +35,8 @@ __global__ void k_triangulate(const TriArgs a)
     const float2 pl = a.pts_l[(size_t)unit * a.cap + i];
     const float2 pr = a.pts_r[(size_t)unit * a.cap + i];
     float o[3], o4[4];
-    triangulate_dlt(a.Pl, a.Pr, pl.x, pl.y, pr.x, pr.y, o, o4);
+    const CamCalib& c = a.cal[unit];
+    triangulate_dlt(c.Pl, c.Pr, pl.x, pl.y, pr.x, pr.y, o, o4);
     a.X[(size_t)unit * a.cap + i] = make_float3(o[0], o[1], o[2]);
     if (a.X4) a.X4[(size_t)unit * a.cap + i] = make_float4(o4[0], o4[1], o4[2], o4[3]);
 }
@@ -54,7 +55,8 @@ __device__ __noinline__ void pnp_five_points(const PnpArgs& a, int unit)
         uv[2 * i] = x[i].x; uv[2 * i + 1] = x[i].y;
     }
     double rv[3], t[3], R[9];
-    epnp5(Xw, uv, a.fu, a.fv, a.uc, a.vc, rv, t, R);      // R = Rodrigues(rvec), the caller's conversion
+    const CamCalib& c = a.cal[unit];
+    epnp5(Xw, uv, c.fu, c.fv, c.uc, c.vc, rv, t, R);      // R = Rodrigues(rvec), the caller's conversion
     vo_unit_result_dev& res = a.results[unit];
     int* inl = a.inliers + (size_t)unit * a.cap;
     res.ransac_iters = 0;
@@ -198,7 +200,8 @@ __global__ void __launch_bounds__(32 * 1) k_pnp_hypotheses(const PnpArgs a, int 
             Xs[3 * i] = P.x; Xs[3 * i + 1] = P.y; Xs[3 * i + 2] = P.z;
             xs[2 * i] = p.x; xs[2 * i + 1] = p.y;
         }
-        epnp5_front(Xs, xs, a.fu, a.fv, a.uc, a.vc, sm_st[g], sm_mtm[g]);
+        const CamCalib& c = a.cal[unit];
+        epnp5_front(Xs, xs, c.fu, c.fv, c.uc, c.vc, sm_st[g], sm_mtm[g]);
     }
     __syncwarp();
     if (work) {          // uniform per 16-lane group
@@ -297,15 +300,16 @@ __global__ void __launch_bounds__(128) k_pnp_count(const PnpArgs a, int it0, int
     const int it = it0 + blockIdx.x;
     const PnpState& s = a.state[unit];
     if (s.done || it >= it1 || it >= s.niters) return;
-    __shared__ double m[12];
+    __shared__ double m[12], cam[4];         // the model; the unit's fu, fv, uc, vc
     __shared__ int total;
     if (threadIdx.x < 12) m[threadIdx.x] = a.models[((size_t)unit * a.iterations + it) * 12 + threadIdx.x];
+    else if (threadIdx.x < 16) cam[threadIdx.x - 12] = (&a.cal[unit].fu)[threadIdx.x - 12];
     if (threadIdx.x == 0) total = 0;
     __syncthreads();
     const int n = a.n_pts[unit];
     int c = 0;
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        const float e = reproj_err(m, a.X[(size_t)unit * a.cap + i], a.x[(size_t)unit * a.cap + i], a.fu, a.fv, a.uc, a.vc);
+        const float e = reproj_err(m, a.X[(size_t)unit * a.cap + i], a.x[(size_t)unit * a.cap + i], cam[0], cam[1], cam[2], cam[3]);
         c += (e <= a.thr2) ? 1 : 0;
     }
 #pragma unroll
@@ -398,7 +402,7 @@ __global__ void __launch_bounds__(FIN_T, 1) k_pnp_finalize(const PnpArgs a)
     const float2* x = a.x + (size_t)unit * a.cap;
     int* inl = a.inliers + (size_t)unit * a.cap;
 
-    __shared__ double sm_model[12];
+    __shared__ double sm_model[12], cam[4];      // the best model; the unit's fu, fv, uc, vc
     __shared__ int wcnt[FIN_T / 32];
     __shared__ int base;
     __shared__ double red[28];
@@ -417,7 +421,8 @@ __global__ void __launch_bounds__(FIN_T, 1) k_pnp_finalize(const PnpArgs a)
                 uv[2 * i] = x[i].x; uv[2 * i + 1] = x[i].y;
             }
             double R[9], t[3], rv[3];
-            const bool ok = p3p_four_points(Xw, uv, a.fu, a.fv, a.uc, a.vc, R, t);
+            const CamCalib& c = a.cal[unit];
+            const bool ok = p3p_four_points(Xw, uv, c.fu, c.fv, c.uc, c.vc, R, t);
             res.ransac_iters = 0;
             if (ok) {
                 rodrigues_inv(R, rv);
@@ -449,14 +454,16 @@ __global__ void __launch_bounds__(FIN_T, 1) k_pnp_finalize(const PnpArgs a)
         return;
     }
     if (threadIdx.x < 12) sm_model[threadIdx.x] = a.models[((size_t)unit * a.iterations + st.best_it) * 12 + threadIdx.x];
+    else if (threadIdx.x < 16) cam[threadIdx.x - 12] = (&a.cal[unit].fu)[threadIdx.x - 12];
     if (threadIdx.x == 0) base = 0;
     __syncthreads();
+    const double fu = cam[0], fv = cam[1], uc = cam[2], vc = cam[3];
     // ---- inlier mask of the best model, ordered compaction -----------------------------------
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int c0 = 0; c0 < n; c0 += FIN_T) {
         const int i = c0 + threadIdx.x;
         bool keep = false;
-        if (i < n) keep = reproj_err(sm_model, X[i], x[i], a.fu, a.fv, a.uc, a.vc) <= a.thr2;
+        if (i < n) keep = reproj_err(sm_model, X[i], x[i], fu, fv, uc, vc) <= a.thr2;
         const unsigned b = __ballot_sync(0xffffffffu, keep);
         if (lane == 0) wcnt[warp] = __popc(b);
         __syncthreads();
@@ -495,7 +502,7 @@ __global__ void __launch_bounds__(FIN_T, 1) k_pnp_finalize(const PnpArgs a)
             double zc = R[6] * Xw + R[7] * Yw + R[8] * Zw + param[5];
             const double z = zc ? 1. / zc : 1.;
             const double xn = xc * z, yn = yc * z;
-            const double ex = xn * a.fu + a.uc - (double)p.x, ey = yn * a.fv + a.vc - (double)p.y;
+            const double ex = xn * fu + uc - (double)p.x, ey = yn * fv + vc - (double)p.y;
             acc[27] += ex * ex + ey * ey;
             if (with_jac) {
                 double jx[6], jy[6];
@@ -504,11 +511,11 @@ __global__ void __launch_bounds__(FIN_T, 1) k_pnp_finalize(const PnpArgs a)
                     const double dx = dR[0] * Xw + dR[1] * Yw + dR[2] * Zw;
                     const double dy = dR[3] * Xw + dR[4] * Yw + dR[5] * Zw;
                     const double dz = dR[6] * Xw + dR[7] * Yw + dR[8] * Zw;
-                    jx[j] = a.fu * z * (dx - xn * dz);
-                    jy[j] = a.fv * z * (dy - yn * dz);
+                    jx[j] = fu * z * (dx - xn * dz);
+                    jy[j] = fv * z * (dy - yn * dz);
                 }
-                jx[3] = a.fu * z; jx[4] = 0; jx[5] = -a.fu * xn * z;
-                jy[3] = 0; jy[4] = a.fv * z; jy[5] = -a.fv * yn * z;
+                jx[3] = fu * z; jx[4] = 0; jx[5] = -fu * xn * z;
+                jy[3] = 0; jy[4] = fv * z; jy[5] = -fv * yn * z;
                 int q2 = 0;
                 for (int r = 0; r < 6; r++)
                     for (int c = r; c < 6; c++) acc[q2++] += jx[r] * jx[c] + jy[r] * jy[c];

@@ -27,7 +27,7 @@ struct TriArgs {
     const float2* pts_r;     // [units][cap]
     float3* X;               // [units][cap]
     float4* X4;              // optional [units][cap]: homogeneous points as cv::triangulatePoints returns them
-    double Pl[12], Pr[12];   // float projection matrices widened to double
+    const CamCalib* cal;     // [units]: Pl / Pr of each unit
 };
 
 struct PnpArgs {
@@ -35,7 +35,7 @@ struct PnpArgs {
     const int* n_pts;        // [units]
     const float3* X;         // [units][cap]
     const float2* x;         // [units][cap]   image points (pointsLeft_t1)
-    double fu, fv, uc, vc;   // float intrinsics widened to double
+    const CamCalib* cal;     // [units]: fu, fv, uc, vc of each unit
     float thr2;              // (float)(reprojectionError^2)
     double confidence;
     const double* t_prev;    // [units][3]

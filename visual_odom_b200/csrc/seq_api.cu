@@ -14,7 +14,8 @@
 // nor the previous frame reads, so the H2D of frame k+1 also runs under the kernels of frame k (double-buffered
 // upload).  Each stage is one CUDA graph (per image-slot pair / buffer unit / input format).
 //
-// vo_mseq_* runs n_seq independent sequences of one image size and calibration in lockstep through the same two stages:
+// vo_mseq_* runs n_seq independent sequences of one image size (each with its own calibration: the kernels read unit u's
+// camera from the calibration table, and sequence q's entries are those of units q and n_seq + q) in lockstep through the same two stages:
 // every stage kernel takes the n_seq units of a buffer parity (sequence q at parity p is unit p * n_seq + q) in ONE launch,
 // and vo_seq_* is the same code with n_seq = 1.  The image ring is slot-major: slot s holds the pairs of all sequences,
 // planes 2 * n_seq * s + 2q (left) and + 1 (right), so the new pairs of a frame are one contiguous run of planes (one
@@ -103,13 +104,12 @@ static void seq_ess_args(vo_ctx* ctx, int unit, int n_prob, EssArgs& a)
 {
     memset(&a, 0, sizeof(a));
     const size_t uo = (size_t)unit * ctx->cap, cs = (size_t)ctx->units * ctx->cap;
-    // `double focal = projMatrl.at<float>(0, 0)`, principle_point(projMatrl.at<float>(0, 2), projMatrl.at<float>(1, 2))
-    vo_ess_set_camera(a, (double)ctx->P_l[0], (double)ctx->P_l[2], (double)ctx->P_l[6]);
     vo_ess_bind(a, (uint8_t*)ctx->d_seq_ess + (size_t)unit * ctx->seq_ess_bytes, ctx->seq_ess_cap, VO_ESS_ITERS);
     a.n = ctx->d_n5 + unit;
+    a.cal = ctx->d_cal + unit;                                // focal / pp / threshold of each unit's P_l
     a.pts0 = ctx->d_valid4 + uo; a.pts1 = ctx->d_valid4 + 2 * cs + uo;
     a.n_prob = n_prob;
-    a.scratch_stride = a.result_stride = ctx->seq_ess_bytes; a.pts_stride = ctx->cap; a.n_stride = 1;
+    a.scratch_stride = a.result_stride = ctx->seq_ess_bytes; a.pts_stride = ctx->cap; a.n_stride = 1; a.cal_stride = 1;
 }
 
 // per-unit scratch of the mono branch for the 2 * n units of n sequences, sized for the bucket grid (outside any capture:
@@ -164,7 +164,7 @@ static int seq_front(vo_ctx* ctx, int s0, int s1, int p, bool bgr)
     // state carry: features.points = pointsLeft_t1, ages keep their A3 length
     ctx->launches += vo_launch_seq_carry(a, n, ctx->stream);
     const size_t cs = (size_t)ctx->units * ctx->cap;
-    if ((rc = vo_run_triangulate(ctx, v, ctx->d_valid4, ctx->d_valid4 + cs, ctx->d_n5))) return rc;
+    if ((rc = vo_run_triangulate(ctx, v, ctx->d_valid4, ctx->d_valid4 + cs, ctx->d_n5, ctx->d_cal))) return rc;
     if (ctx->seq_mono) VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->seq_mono_ev[1], 0));
     VO_CUDA_CHECK(cudaGetLastError());
     return VO_OK;
@@ -177,9 +177,8 @@ static int seq_back(vo_ctx* ctx, int p)
     const int n = ctx->seq_n, unit = p * n;
     const View v{unit, n, st, 0};
     const size_t cs = (size_t)ctx->units * ctx->cap;
-    float K9[9] = {ctx->P_l[0], ctx->P_l[1], ctx->P_l[2], ctx->P_l[4], ctx->P_l[5], ctx->P_l[6], ctx->P_l[8], ctx->P_l[9], ctx->P_l[10]};
     int rc;
-    if ((rc = vo_run_pnp(ctx, v, ctx->d_valid4 + 2 * cs, ctx->d_n5, K9))) return rc;
+    if ((rc = vo_run_pnp(ctx, v, ctx->d_valid4 + 2 * cs, ctx->d_n5, ctx->d_cal))) return rc;
     SeqArgs a;
     seq_args(ctx, p, a);
     ctx->launches += vo_launch_seq_finish(a, n, st);
@@ -252,12 +251,12 @@ extern "C" int vo_seq_begin(vo_ctx* ctx, int w, int h, const float P_l[12], cons
     return vo_seq_begin_ex(ctx, w, h, P_l, P_r, left0, right0, pitch, 1);
 }
 
-// n new sequences (multi: begun by vo_mseq_begin) whose first pairs `fill_slot0` enqueues into image slot 0 on ctx->stream
-// (arguments already checked); mono: every frame also runs the mono_rotation branch (the option "mono_rotation" for
-// vo_seq_begin*, the flag VO_MSEQ_MONO_ROTATION for vo_mseq_begin_ex).  A running sequence mode of the same kind is
-// drained and ended; one of the other kind only when it is idle.
+// n new sequences (multi: begun by vo_mseq_begin*) whose first pairs `fill_slot0` enqueues into image slot 0 on ctx->stream
+// (arguments already checked); sequence q runs with the matrices P_l + 12q / P_r + 12q; mono: every frame also runs the
+// mono_rotation branch (the option "mono_rotation" for vo_seq_begin*, the flag VO_MSEQ_MONO_ROTATION for vo_mseq_begin_ex /
+// _calib).  A running sequence mode of the same kind is drained and ended; one of the other kind only when it is idle.
 template <typename F>
-static int seq_begin(vo_ctx* ctx, int n, bool multi, bool mono, int w, int h, const float P_l[12], const float P_r[12], F fill_slot0)
+static int seq_begin(vo_ctx* ctx, int n, bool multi, bool mono, int w, int h, const float* P_l, const float* P_r, F fill_slot0)
 {
     const char* who = multi ? "vo_mseq_begin" : "vo_seq_begin";
     if (ctx->seq_active && ctx->seq_multi != multi && ctx->seq_inflight > 0) {
@@ -279,7 +278,8 @@ static int seq_begin(vo_ctx* ctx, int n, bool multi, bool mono, int w, int h, co
     if (ctx->seq_mono != mono) { vo_drop_graphs(ctx); ctx->seq_mono = mono; }
     if (ctx->seq_mono && (rc = seq_mono_scratch(ctx, n))) return rc;
     if ((rc = vo_ensure_pinned(ctx, seq_pinned(ctx, n).bytes))) return rc;
-    vo_set_calibration(ctx, P_l, P_r);
+    // sequence q owns the buffer units q and n + q (both parities): both entries carry its camera
+    if ((rc = vo_set_calibration(ctx, 0, 2 * n, P_l, P_r, n))) return rc;
     ctx->seq_slot = 0;
     ctx->seq_frames = 0;
     ctx->seq_submitted = 0;
@@ -608,10 +608,25 @@ extern "C" int vo_mseq_begin(vo_ctx* ctx, int n_seq, int w, int h, const float P
     return vo_mseq_begin_ex(ctx, n_seq, w, h, P_l, P_r, left0, right0, pitch, channels, 0);
 }
 
-// the mono_rotation branch is asked for with the flag only: the context option, which vo_seq_begin* take, would otherwise
-// silently pick (or drop) the branch for a whole set of sequences
+// one calibration for every sequence: vo_mseq_begin_calib with the matrices repeated
 extern "C" int vo_mseq_begin_ex(vo_ctx* ctx, int n_seq, int w, int h, const float P_l[12], const float P_r[12],
                                 const uint8_t* const* left0, const uint8_t* const* right0, size_t pitch, int channels, int flags)
+{
+    if (!ctx) return VO_E_INVALID;
+    if (!P_l || !P_r || n_seq < 1 || n_seq > VO_MSEQ_MAX)        // refused below with its message
+        return vo_mseq_begin_calib(ctx, n_seq, w, h, P_l, P_r, left0, right0, pitch, channels, flags);
+    std::vector<float> Pl(12 * (size_t)n_seq), Pr(12 * (size_t)n_seq);
+    for (int q = 0; q < n_seq; q++) {
+        memcpy(Pl.data() + 12 * q, P_l, 12 * sizeof(float));
+        memcpy(Pr.data() + 12 * q, P_r, 12 * sizeof(float));
+    }
+    return vo_mseq_begin_calib(ctx, n_seq, w, h, Pl.data(), Pr.data(), left0, right0, pitch, channels, flags);
+}
+
+// the mono_rotation branch is asked for with the flag only: the context option, which vo_seq_begin* take, would otherwise
+// silently pick (or drop) the branch for a whole set of sequences
+extern "C" int vo_mseq_begin_calib(vo_ctx* ctx, int n_seq, int w, int h, const float* P_l, const float* P_r,
+                                   const uint8_t* const* left0, const uint8_t* const* right0, size_t pitch, int channels, int flags)
 {
     if (!ctx) return VO_E_INVALID;
     if (flags & ~VO_MSEQ_MONO_ROTATION) { vo_set_error(ctx, "vo_mseq_begin: unknown flag bits 0x%x", (unsigned)(flags & ~VO_MSEQ_MONO_ROTATION)); return VO_E_INVALID; }
