@@ -298,7 +298,9 @@ VO_API int vo_dist_gather_wait(vo_ctx* ctx, vo_unit_result* all, int cap_records
  *   out      counts + pose of this frame pair
  *   pts4     optional: 4 arrays of pts_cap points (L0, R0, L1, R1 after the circular check); the first
  *            out->n_valid entries of each are meaningful, the rest of the arrays is scratch
- * The per-frame kernel sequence is replayed as two CUDA graphs (front half / pose solve; option "graphs"). */
+ * The per-frame kernel sequence is replayed as two CUDA graphs (front half / pose solve; option "graphs").
+ * vo_seq_begin* and vo_mseq_begin* are refused (VO_E_INVALID) while a vo_batch_submit submission has not been waited for,
+ * before they change anything: a sequence reuses the buffers and the pinned staging that submission still uses. */
 VO_API int vo_seq_begin(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], const uint8_t* left0,
                         const uint8_t* right0, size_t pitch);
 VO_API int vo_seq_push(vo_ctx* ctx, const uint8_t* left1, const uint8_t* right1, size_t pitch, vo_unit_result* out,

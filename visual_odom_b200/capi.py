@@ -458,6 +458,23 @@ class Context:
                     n_inliers=r.n_inliers, ransac_iters=r.ransac_iters, pnp_status=r.pnp_status,
                     rvec=np.array(r.rvec[:]), tvec=np.array(r.tvec[:]), R=np.array(r.R[:]).reshape(3, 3))
 
+    @classmethod
+    def _record(cls, r, cap, pts4=None, mono=None, mask=None, status=None):
+        """A sequence frame's record as a dict: _result_dict's keys, with pts4 ((4, cap, 2) point lists) l0 / r0 / l1 / r1,
+        with mono (a VoMonoResult) "mono" and the essential mask `mask` as "ess_mask", with status "status" (the first
+        n_valid entries of the lists, none for a retired sequence)."""
+        d = cls._result_dict(r)
+        n = 0 if status == VO_MSEQ_RETIRED else min(d["n_valid"], cap)
+        if status is not None:
+            d["status"] = int(status)
+        if pts4 is not None:
+            d.update(l0=pts4[0, :n].copy(), r0=pts4[1, :n].copy(), l1=pts4[2, :n].copy(), r1=pts4[3, :n].copy())
+        if mono is not None:
+            d["mono"] = dict(status=mono.status, n_inliers=mono.n_inliers, ransac_iters=mono.ransac_iters, n_good=mono.n_good,
+                             R=np.array(mono.R[:]).reshape(3, 3), t=np.array(mono.t[:]))
+            d["ess_mask"] = mask[:n].astype(bool)
+        return d
+
     @staticmethod
     def records_to_dicts(arr):
         """A RESULT_DTYPE array (batch_wait / dist_gather_wait with raw=True) as the list of dicts the other calls return."""
@@ -527,15 +544,9 @@ class Context:
             self._check(self.lib.vo_seq_submit(self.h, _p(l), _p(r), l.strides[0], 1))
             return self.seq_wait(pts_cap, want_points, mono=True)
         res = VoUnitResult()
-        if not want_points:
-            self._check(self.lib.vo_seq_push(self.h, _p(l), _p(r), l.strides[0], C.byref(res), None, 0))
-            return self._result_dict(res)
-        pts4 = np.zeros((4, pts_cap, 2), np.float32)
-        self._check(self.lib.vo_seq_push(self.h, _p(l), _p(r), l.strides[0], C.byref(res), _p(pts4), pts_cap))
-        d = self._result_dict(res)
-        n = min(d["n_valid"], pts_cap)
-        d.update(l0=pts4[0, :n].copy(), r0=pts4[1, :n].copy(), l1=pts4[2, :n].copy(), r1=pts4[3, :n].copy())
-        return d
+        pts4 = np.zeros((4, pts_cap, 2), np.float32) if want_points else None
+        self._check(self.lib.vo_seq_push(self.h, _p(l), _p(r), l.strides[0], C.byref(res), _p(pts4), pts_cap if want_points else 0))
+        return self._record(res, pts_cap, pts4)
 
     def seq_begin_bgr(self, left0, right0, P_l, P_r):
         """Colour (H x W x 3, BGR) inputs: converted on the device like cv::cvtColor(BGR2GRAY)."""
@@ -549,10 +560,7 @@ class Context:
         res = VoUnitResult()
         pts4 = np.zeros((4, pts_cap, 2), np.float32)
         self._check(self.lib.vo_seq_push_ex(self.h, _p(l), _p(r), l.strides[0], 3, C.byref(res), _p(pts4), pts_cap))
-        d = self._result_dict(res)
-        n = min(d["n_valid"], pts_cap)
-        d.update(l0=pts4[0, :n].copy(), r0=pts4[1, :n].copy(), l1=pts4[2, :n].copy(), r1=pts4[3, :n].copy())
-        return d
+        return self._record(res, pts_cap, pts4)
 
     def seq_push_ptr(self, left_ptr, right_ptr, pitch, channels=1):
         """Raw host pointers (e.g. the pinned buffers a SequenceReader hands out); returns counts + pose only."""
@@ -668,29 +676,15 @@ class Context:
         """mono=True: also "mono" (dict: status, n_inliers, ransac_iters, n_good, R 3x3, t) and "ess_mask" (bool, aligned
         with the point lists) of the same frame (vo_seq_wait_mono)."""
         res = VoUnitResult()
-        if mono:
-            m = VoMonoResult()
-            mask = np.zeros(pts_cap, np.uint8)
-            pts4 = np.zeros((4, pts_cap, 2), np.float32) if want_points else None
-            self._check(self.lib.vo_seq_wait_mono(self.h, C.byref(res), C.byref(m), _p(mask), pts_cap, _p(pts4),
-                                                  pts_cap if want_points else 0))
-            d = self._result_dict(res)
-            n = min(d["n_valid"], pts_cap)
-            if want_points:
-                d.update(l0=pts4[0, :n].copy(), r0=pts4[1, :n].copy(), l1=pts4[2, :n].copy(), r1=pts4[3, :n].copy())
-            d["mono"] = dict(status=m.status, n_inliers=m.n_inliers, ransac_iters=m.ransac_iters, n_good=m.n_good,
-                             R=np.array(m.R[:]).reshape(3, 3), t=np.array(m.t[:]))
-            d["ess_mask"] = mask[:n].astype(bool)
-            return d
-        if not want_points:
-            self._check(self.lib.vo_seq_wait(self.h, C.byref(res), None, 0))
-            return self._result_dict(res)
-        pts4 = np.zeros((4, pts_cap, 2), np.float32)
-        self._check(self.lib.vo_seq_wait(self.h, C.byref(res), _p(pts4), pts_cap))
-        d = self._result_dict(res)
-        n = min(d["n_valid"], pts_cap)
-        d.update(l0=pts4[0, :n].copy(), r0=pts4[1, :n].copy(), l1=pts4[2, :n].copy(), r1=pts4[3, :n].copy())
-        return d
+        pts4 = np.zeros((4, pts_cap, 2), np.float32) if want_points else None
+        npts = pts_cap if want_points else 0
+        if not mono:
+            self._check(self.lib.vo_seq_wait(self.h, C.byref(res), _p(pts4), npts))
+            return self._record(res, pts_cap, pts4)
+        m = VoMonoResult()
+        mask = np.zeros(pts_cap, np.uint8)
+        self._check(self.lib.vo_seq_wait_mono(self.h, C.byref(res), C.byref(m), _p(mask), pts_cap, _p(pts4), npts))
+        return self._record(res, pts_cap, pts4, m, mask)
 
     def seq_state(self, cap=1 << 17):
         pts = np.zeros((cap, 2), np.float32); ages = np.zeros(cap, np.int32); t = np.zeros(3)
@@ -795,20 +789,8 @@ class Context:
             self._check(self.lib.vo_mseq_wait_mono(self.h, res, _p(st), ms, _p(mask), pts_cap, _p(pts4), npts), ok=(VO_OK, VO_E_CAPACITY))
         else:
             self._check(self.lib.vo_mseq_wait(self.h, res, _p(st), _p(pts4), npts), ok=(VO_OK, VO_E_CAPACITY))
-        out = []
-        for q in range(n):
-            d = self._result_dict(res[q])
-            d["status"] = int(st[q])
-            m = min(d["n_valid"], pts_cap) if d["status"] != VO_MSEQ_RETIRED else 0
-            if want_points:
-                d.update(l0=pts4[q, 0, :m].copy(), r0=pts4[q, 1, :m].copy(), l1=pts4[q, 2, :m].copy(), r1=pts4[q, 3, :m].copy())
-            if mono:
-                r = ms[q]
-                d["mono"] = dict(status=r.status, n_inliers=r.n_inliers, ransac_iters=r.ransac_iters, n_good=r.n_good,
-                                 R=np.array(r.R[:]).reshape(3, 3), t=np.array(r.t[:]))
-                d["ess_mask"] = mask[q, :m].astype(bool)
-            out.append(d)
-        return out
+        return [self._record(res[q], pts_cap, None if pts4 is None else pts4[q], ms[q] if mono else None,
+                             mask[q] if mono else None, st[q]) for q in range(n)]
 
     def mseq_pose(self, q):
         pose = np.zeros((4, 4))

@@ -187,9 +187,8 @@ static int upload_range(vo_ctx* ctx, const vo_unit* units, int u0, int n, size_t
         const vo_unit& U = units[u - u0 + src0];
         const uint8_t* imgs[4] = {U.l0, U.r0, U.l1, U.r1};
         for (int k = 0; k < 4; k++) {
-            uint8_t* dst = ctx->d_raw + ((size_t)u * 4 + k) * w * h;
-            if (pitch == (size_t)w) VO_CUDA_CHECK(cudaMemcpyAsync(dst, imgs[k], (size_t)w * h, cudaMemcpyHostToDevice, st));
-            else VO_CUDA_CHECK(cudaMemcpy2DAsync(dst, w, imgs[k], pitch, w, h, cudaMemcpyHostToDevice, st));
+            const int rc = vo_upload_plane(ctx, ctx->d_raw + ((size_t)u * 4 + k) * w * h, imgs[k], w, h, pitch, st);
+            if (rc) return rc;
         }
     }
     return stage_inputs(ctx, units, u0, n, st, detect, src0);

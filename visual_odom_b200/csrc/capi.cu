@@ -4,9 +4,7 @@
 
 static int upload_image(vo_ctx* ctx, int plane, const uint8_t* img, int w, int h, size_t pitch)
 {
-    VO_CUDA_CHECK(cudaMemcpy2DAsync(ctx->d_raw + (size_t)plane * w * h, w, img, pitch, w, h,
-                                    cudaMemcpyHostToDevice, ctx->stream));
-    return VO_OK;
+    return vo_upload_plane(ctx, ctx->d_raw + (size_t)plane * w * h, img, w, h, pitch, ctx->stream);
 }
 
 static int check_common(vo_ctx* ctx, int w, int h, size_t pitch, int n)

@@ -175,18 +175,31 @@ int vo_ensure_pinned(vo_ctx* ctx, size_t bytes)
     return VO_OK;
 }
 
+int vo_upload_plane(vo_ctx* ctx, uint8_t* dst, const uint8_t* src, size_t row_bytes, int h, size_t pitch, cudaStream_t st)
+{
+    if (pitch == row_bytes) VO_CUDA_CHECK(cudaMemcpyAsync(dst, src, row_bytes * h, cudaMemcpyHostToDevice, st));
+    else VO_CUDA_CHECK(cudaMemcpy2DAsync(dst, row_bytes, src, pitch, row_bytes, h, cudaMemcpyHostToDevice, st));
+    return VO_OK;
+}
+
+int vo_refuse_pending_batches(vo_ctx* ctx, const char* who)
+{
+    for (auto& p : ctx->pending)
+        if (p.active) {
+            vo_set_error(ctx, "%s: the vo_batch_submit submission of slots [%d, %d) has not been waited for", who, p.u0, p.u0 + p.n);
+            return VO_E_INVALID;
+        }
+    return VO_OK;
+}
+
 int vo_claim_buffers(vo_ctx* ctx, const char* who, bool allow_pending_batches)
 {
     if (ctx->seq_inflight > 0) {
         vo_set_error(ctx, "%s: %d frame(s) submitted with vo_seq_submit have not been waited for (this call would overwrite their buffers)", who, ctx->seq_inflight);
         return VO_E_INVALID;
     }
-    if (!allow_pending_batches)
-        for (auto& p : ctx->pending)
-            if (p.active) {
-                vo_set_error(ctx, "%s: the vo_batch_submit submission of slots [%d, %d) has not been waited for", who, p.u0, p.u0 + p.n);
-                return VO_E_INVALID;
-            }
+    int rc;
+    if (!allow_pending_batches && (rc = vo_refuse_pending_batches(ctx, who))) return rc;
     ctx->seq_active = false;        // the sequence's image planes and per-frame buffers are reused from here on: vo_seq_begin again
     return VO_OK;
 }

@@ -101,9 +101,7 @@ struct vo_ctx {
                                         // 2 * seq_n * slot + 2q (left), + 1 (right) of sequence q
     int seq_inflight = 0;               // frames submitted and not yet waited for (<= 2)
     long long seq_submitted = 0;        // frames submitted since vo_seq_begin (frame k uses buffer parity k & 1)
-    int seq_channels[2] = {1, 1};
     cudaEvent_t seq_front_ev[2] = {nullptr, nullptr}, seq_back_ev[2] = {nullptr, nullptr};
-    long long seq_frames = 0;
     std::vector<double> seq_pose;       // [seq_n][16] frame_pose of main.cpp:90, integrated per push
     std::vector<char> seq_retired;      // [seq_n] retired by a NULL pair (vo_mseq_submit)
     std::vector<char> seq_live;         // [2 * seq_n] host copy of d_seq_live as the frame in flight in each parity saw it
@@ -225,7 +223,12 @@ void vo_partition_destroy(vo_ctx* ctx);
 int vo_dist_order_after_gathers(vo_ctx* ctx, cudaStream_t st);
 void vo_dist_shutdown(vo_ctx* ctx);
 int vo_claim_buffers(vo_ctx* ctx, const char* who, bool allow_pending_batches = false);
+// VO_E_INVALID + message while a vo_batch_submit submission has not been waited for
+int vo_refuse_pending_batches(vo_ctx* ctx, const char* who);
 int vo_ensure_pinned(vo_ctx* ctx, size_t bytes);
+// H2D of a host image (h rows of row_bytes, pitch bytes apart) into a packed device plane on st: one 1-D copy when the
+// rows are contiguous, else a 2-D copy
+int vo_upload_plane(vo_ctx* ctx, uint8_t* dst, const uint8_t* src, size_t row_bytes, int h, size_t pitch, cudaStream_t st);
 int vo_ensure_bgr(vo_ctx* ctx, size_t bytes);
 // k_bgr_to_gray: images tab[0 .. n_img) (device table), or with d_tab == nullptr `packed` advanced by packed_stride per image,
 // into gray planes img_stride_out apart

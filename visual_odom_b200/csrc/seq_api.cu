@@ -31,31 +31,24 @@
 #include "ctx.h"
 #include <string.h>
 
-// the new pairs of image slot `slot` (sequence q: lefts[q], rights[q]; a NULL pair is skipped)
+// the new host pairs of image slot `slot` (sequence q: lefts[q], rights[q]; a NULL pair is skipped): gray into the raw
+// planes, colour (BGR) bytes into the staging area, converted inside the frame's graph
 static int upload_pairs(vo_ctx* ctx, int slot, const uint8_t* const* lefts, const uint8_t* const* rights, size_t pitch, int channels,
                         cudaStream_t st)
 {
     const int w = ctx->w, h = ctx->h, n = ctx->seq_n;
-    if (channels == 3) {                 // colour input: BGR bytes to the staging area, converted inside the frame's graph
-        const size_t img = (size_t)3 * w * h;
-        int rc = vo_ensure_bgr(ctx, 2 * (size_t)n * img);
-        if (rc) return rc;
-        for (int q = 0; q < n; q++) {
-            if (!lefts[q]) continue;
-            const uint8_t* imgs[2] = {lefts[q], rights[q]};
-            for (int k = 0; k < 2; k++)
-                VO_CUDA_CHECK(cudaMemcpy2DAsync(ctx->d_bgr + (2 * q + k) * img, (size_t)3 * w, imgs[k], pitch, (size_t)3 * w, h, cudaMemcpyHostToDevice, st));
-        }
-        return VO_OK;
+    const size_t img = (size_t)channels * w * h;
+    uint8_t* dst = ctx->d_raw + (size_t)(2 * n * slot) * w * h;
+    int rc;
+    if (channels == 3) {
+        if ((rc = vo_ensure_bgr(ctx, 2 * (size_t)n * img))) return rc;
+        dst = ctx->d_bgr;
     }
     for (int q = 0; q < n; q++) {
         if (!lefts[q]) continue;
         const uint8_t* imgs[2] = {lefts[q], rights[q]};
-        for (int k = 0; k < 2; k++) {
-            uint8_t* dst = ctx->d_raw + (size_t)(2 * n * slot + 2 * q + k) * w * h;
-            if (pitch == (size_t)w) VO_CUDA_CHECK(cudaMemcpyAsync(dst, imgs[k], (size_t)w * h, cudaMemcpyHostToDevice, st));
-            else VO_CUDA_CHECK(cudaMemcpy2DAsync(dst, w, imgs[k], pitch, w, h, cudaMemcpyHostToDevice, st));
-        }
+        for (int k = 0; k < 2; k++)
+            if ((rc = vo_upload_plane(ctx, dst + (2 * q + k) * img, imgs[k], (size_t)channels * w, h, pitch, st))) return rc;
     }
     return VO_OK;
 }
@@ -203,7 +196,6 @@ static SeqPinned seq_pinned(vo_ctx* ctx, int n)
     uint8_t* b = (uint8_t*)ctx->h_pinned;
     return SeqPinned{(vo_unit_result_dev*)b, (int*)(b + o_err), (EssResult*)(b + o_ess), (vo_dimage*)(b + o_tab), end};
 }
-static vo_dimage* seq_pinned_tab(vo_ctx* ctx) { return seq_pinned(ctx, ctx->seq_n).tab; }
 
 // the per-sequence device state (FeatureSet, bucket scratch, error and live words) for n sequences, in one allocation that
 // lives until the batch state is re-allocated (outside any capture: vo_seq_begin / vo_mseq_begin)
@@ -245,27 +237,85 @@ static int seq_drain(vo_ctx* ctx)
     return VO_OK;
 }
 
-extern "C" int vo_seq_begin(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], const uint8_t* left0,
-                            const uint8_t* right0, size_t pitch)
+// where the new pairs of a begin or submit call come from: host images (gray or BGR, `pitch` bytes per row; in a
+// multi-sequence submission a NULL pair retires its sequence) or one device pair (vo_seq_*_device)
+struct SeqPairs {
+    const uint8_t* const* lefts; const uint8_t* const* rights; size_t pitch; int channels;
+    bool device; const vo_dimage* dl; const vo_dimage* dr;
+    bool bgr() const { return !device && channels == 3; }
+};
+static SeqPairs host_pairs(const uint8_t* const* lefts, const uint8_t* const* rights, size_t pitch, int channels)
 {
-    return vo_seq_begin_ex(ctx, w, h, P_l, P_r, left0, right0, pitch, 1);
+    return SeqPairs{lefts, rights, pitch, channels, false, nullptr, nullptr};
+}
+static SeqPairs device_pair(const vo_dimage* left, const vo_dimage* right) { return SeqPairs{nullptr, nullptr, 0, 1, true, left, right}; }
+
+// the new pairs' own checks (w: the image width; begin: the first pairs, which every sequence needs)
+static int seq_pairs_check(vo_ctx* ctx, const char* who, bool multi, int n, int w, const SeqPairs& in, bool begin)
+{
+    int rc;
+    if (in.device) {
+        if ((rc = vo_check_dimage(ctx, who, begin ? "left0" : "left1", in.dl, w)) ||
+            (rc = vo_check_dimage(ctx, who, begin ? "right0" : "right1", in.dr, w))) return rc;
+        return VO_OK;
+    }
+    if (in.channels != 1 && in.channels != 3) { vo_set_error(ctx, "%s: channels must be 1 (gray) or 3 (BGR)", who); return VO_E_INVALID; }
+    if (!in.lefts || !in.rights || in.pitch < (size_t)w * in.channels || (!multi && (!in.lefts[0] || !in.rights[0]))) {
+        vo_set_error(ctx, "%s: bad argument", who);
+        return VO_E_INVALID;
+    }
+    for (int q = 0; multi && q < n; q++) {
+        const bool l = in.lefts[q] != nullptr, r = in.rights[q] != nullptr;
+        if (begin && !(l && r)) { vo_set_error(ctx, "%s: sequence %d has no first pair", who, q); return VO_E_INVALID; }
+        if (!begin && l != r) { vo_set_error(ctx, "%s: sequence %d has only one image (a NULL pair retires it)", who, q); return VO_E_INVALID; }
+        if (!begin && l && ctx->seq_retired[q]) { vo_set_error(ctx, "%s: sequence %d was retired", who, q); return VO_E_INVALID; }
+    }
+    return VO_OK;
 }
 
-// n new sequences (multi: begun by vo_mseq_begin*) whose first pairs `fill_slot0` enqueues into image slot 0 on ctx->stream
-// (arguments already checked); sequence q runs with the matrices P_l + 12q / P_r + 12q; mono: every frame also runs the
-// mono_rotation branch (the option "mono_rotation" for vo_seq_begin*, the flag VO_MSEQ_MONO_ROTATION for vo_mseq_begin_ex /
-// _calib).  A running sequence mode of the same kind is drained and ended; one of the other kind only when it is idle.
-template <typename F>
-static int seq_begin(vo_ctx* ctx, int n, bool multi, bool mono, int w, int h, const float* P_l, const float* P_r, F fill_slot0)
+// the new pairs into image slot `slot` on st: host pairs as upload_pairs writes them, a device pair converted into the
+// slot's two raw planes through the slot's entries of the pinned descriptor table
+static int stage_pairs(vo_ctx* ctx, int slot, const SeqPairs& in, cudaStream_t st)
 {
-    const char* who = multi ? "vo_mseq_begin" : "vo_seq_begin";
+    if (!in.device) return upload_pairs(ctx, slot, in.lefts, in.rights, in.pitch, in.channels, st);
+    vo_dimage* tab = seq_pinned(ctx, ctx->seq_n).tab + 2 * slot;
+    tab[0] = *in.dl; tab[1] = *in.dr;
+    return vo_ingest_device(ctx, tab, 2, 2 * slot, st);
+}
+
+// n new sequences (multi: begun by vo_mseq_begin*) from their first pairs `in`; sequence q runs with the matrices
+// P_l + 12q / P_r + 12q; every frame also runs the mono_rotation branch with the option "mono_rotation" (vo_seq_begin*) or
+// the flag VO_MSEQ_MONO_ROTATION (vo_mseq_begin_ex / _calib).  Refused, before anything changes, while a batch submission
+// has not been waited for: it still uses the unit buffers and the pinned block.  A running sequence mode of the same kind
+// is drained and ended; one of the other kind only when it is idle.
+static int seq_begin(vo_ctx* ctx, const char* who, bool multi, int n, int flags, int w, int h, const float* P_l, const float* P_r,
+                     const SeqPairs& in)
+{
+    if (!ctx) return VO_E_INVALID;
+    if (multi) {
+        if (flags & ~VO_MSEQ_MONO_ROTATION) { vo_set_error(ctx, "%s: unknown flag bits 0x%x", who, (unsigned)(flags & ~VO_MSEQ_MONO_ROTATION)); return VO_E_INVALID; }
+        if (n < 1) { vo_set_error(ctx, "%s: n_seq = %d, need at least one sequence", who, n); return VO_E_INVALID; }
+        if (n > VO_MSEQ_MAX) { vo_set_error(ctx, "%s: n_seq = %d, a context holds at most %d sequences", who, n, VO_MSEQ_MAX); return VO_E_CAPACITY; }
+    }
+    if (!P_l || !P_r || w <= 0 || h <= 0) { vo_set_error(ctx, "%s: bad argument", who); return VO_E_INVALID; }
+    int rc;
+    if ((rc = seq_pairs_check(ctx, who, multi, n, w, in, true))) return rc;
+    if (h / 10 <= 0) { vo_set_error(ctx, "%s: image too small for the rows/10 bucket size", who); return VO_E_UNSUPPORTED; }
+    // the mono_rotation branch of several sequences is asked for with the flag only: the context option, which
+    // vo_seq_begin* take, would otherwise silently pick (or drop) the branch for a whole set of sequences
+    if (multi && ctx->mono_opt) {
+        vo_set_error(ctx, "%s: the option \"mono_rotation\" is not supported with several sequences (use the flag "
+                          "VO_MSEQ_MONO_ROTATION of vo_mseq_begin_ex)", who);
+        return VO_E_UNSUPPORTED;
+    }
+    if ((rc = vo_refuse_pending_batches(ctx, who))) return rc;
     if (ctx->seq_active && ctx->seq_multi != multi && ctx->seq_inflight > 0) {
         vo_set_error(ctx, "%s: %d frame(s) submitted with %s have not been waited for", who, ctx->seq_inflight,
                      multi ? "vo_seq_submit" : "vo_mseq_submit");
         return VO_E_INVALID;
     }
+    const bool mono = multi ? (flags & VO_MSEQ_MONO_ROTATION) != 0 : ctx->mono_opt;
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
-    int rc;
     if (ctx->seq_active && (rc = seq_drain(ctx))) return rc;
     ctx->seq_inflight = 0;
     ctx->seq_active = false;
@@ -281,7 +331,6 @@ static int seq_begin(vo_ctx* ctx, int n, bool multi, bool mono, int w, int h, co
     // sequence q owns the buffer units q and n + q (both parities): both entries carry its camera
     if ((rc = vo_set_calibration(ctx, 0, 2 * n, P_l, P_r, n))) return rc;
     ctx->seq_slot = 0;
-    ctx->seq_frames = 0;
     ctx->seq_submitted = 0;
     ctx->seq_pose.assign(16 * (size_t)n, 0.0);
     for (int q = 0; q < n; q++)
@@ -292,7 +341,9 @@ static int seq_begin(vo_ctx* ctx, int n, bool multi, bool mono, int w, int h, co
     VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_seq_err, 0, (1 + 2 * (size_t)n) * sizeof(int), ctx->stream));
     VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_seq_live, 1, 2 * (size_t)n * sizeof(int), ctx->stream));   // any non-zero word is live
     VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_tprev, 0, 6 * (size_t)n * sizeof(double), ctx->stream));   // translation = zeros (main.cpp:82)
-    if ((rc = fill_slot0())) return rc;
+    // the first pairs into image slot 0 on the caller's stream, after the work already enqueued there (the synchronise
+    // below is the release of device images)
+    if ((rc = stage_pairs(ctx, 0, in, ctx->stream)) || (in.bgr() && (rc = convert_pairs(ctx, 0)))) return rc;
     if ((rc = vo_run_pyramid(ctx, 0, 2 * n, ctx->stream))) return rc;
     // both event pairs start out signalled, so the first two frames do not wait for a predecessor
     for (int k = 0; k < 2; k++) {
@@ -304,61 +355,54 @@ static int seq_begin(vo_ctx* ctx, int n, bool multi, bool mono, int w, int h, co
     return VO_OK;
 }
 
-extern "C" int vo_seq_begin_ex(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], const uint8_t* left0,
-                               const uint8_t* right0, size_t pitch, int channels)
-{
-    if (!ctx) return VO_E_INVALID;
-    if (channels != 1 && channels != 3) { vo_set_error(ctx, "vo_seq_begin: channels must be 1 (gray) or 3 (BGR)"); return VO_E_INVALID; }
-    if (!P_l || !P_r || !left0 || !right0 || w <= 0 || h <= 0 || pitch < (size_t)w * channels) { vo_set_error(ctx, "vo_seq_begin: bad argument"); return VO_E_INVALID; }
-    if (h / 10 <= 0) { vo_set_error(ctx, "vo_seq_begin: image too small for the rows/10 bucket size"); return VO_E_UNSUPPORTED; }
-    return seq_begin(ctx, 1, false, ctx->mono_opt, w, h, P_l, P_r, [&] {
-        int rc = upload_pairs(ctx, 0, &left0, &right0, pitch, channels, ctx->stream);
-        return rc ? rc : channels == 3 ? convert_pairs(ctx, 0) : VO_OK;
-    });
-}
+enum SeqCall { SEQ_SUBMIT, SEQ_WAIT, SEQ_QUERY };
 
-extern "C" int vo_seq_begin_device(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], const vo_dimage* left0,
-                                   const vo_dimage* right0)
+// the checks every frame call starts with: the sequences run, begun by this mode (multi: vo_mseq_begin*; the frame calls
+// of one mode are refused while the other one runs), and the frames in flight allow the call (a submission: fewer than
+// two; a wait: at least one)
+static int seq_frame_check(vo_ctx* ctx, const char* who, bool multi, SeqCall call)
 {
-    if (!ctx) return VO_E_INVALID;
-    if (!P_l || !P_r || w <= 0 || h <= 0) { vo_set_error(ctx, "vo_seq_begin_device: bad argument"); return VO_E_INVALID; }
-    int rc;
-    if ((rc = vo_check_dimage(ctx, "vo_seq_begin_device", "left0", left0, w)) || (rc = vo_check_dimage(ctx, "vo_seq_begin_device", "right0", right0, w))) return rc;
-    if (h / 10 <= 0) { vo_set_error(ctx, "vo_seq_begin_device: image too small for the rows/10 bucket size"); return VO_E_UNSUPPORTED; }
-    // on the caller's stream, after the work already enqueued there; vo_seq_begin ends with a synchronise (the release)
-    return seq_begin(ctx, 1, false, ctx->mono_opt, w, h, P_l, P_r, [&] {
-        vo_dimage* tab = seq_pinned_tab(ctx);
-        tab[0] = *left0; tab[1] = *right0;
-        return vo_ingest_device(ctx, tab, 2, 0, ctx->stream);
-    });
-}
-
-// the frame calls of one sequence mode are refused while the other one runs
-static int seq_mode_check(vo_ctx* ctx, const char* who, bool multi)
-{
-    if (!ctx->seq_active) { vo_set_error(ctx, "%s: call %s first", who, multi ? "vo_mseq_begin" : "vo_seq_begin"); return VO_E_INVALID; }
-    if (ctx->seq_multi != multi) {
+    const char* begin = multi ? "vo_mseq_begin" : "vo_seq_begin";
+    if (ctx->seq_active && ctx->seq_multi != multi) {
         vo_set_error(ctx, "%s: the running sequences were begun with %s", who, multi ? "vo_seq_begin" : "vo_mseq_begin");
+        return VO_E_INVALID;
+    }
+    if (!ctx->seq_active) {
+        vo_set_error(ctx, call == SEQ_WAIT ? "%s: no frame in flight; call %s first" : "%s: call %s first", who, begin);
+        return VO_E_INVALID;
+    }
+    if (call == SEQ_WAIT && ctx->seq_inflight <= 0) { vo_set_error(ctx, "%s: no frame in flight", who); return VO_E_INVALID; }
+    if (call == SEQ_SUBMIT && ctx->seq_inflight >= 2) {
+        vo_set_error(ctx, "%s: two frames are in flight already; call %s", who, multi ? "vo_mseq_wait" : "vo_seq_wait");
         return VO_E_INVALID;
     }
     return VO_OK;
 }
 
-static int seq_enqueue(vo_ctx* ctx, int p, int s0, int s1, bool bgr);
-
-// host pairs of every sequence (lefts[q] == NULL: sequence q is retired or being retired, already checked)
-static int seq_submit(vo_ctx* ctx, const uint8_t* const* lefts, const uint8_t* const* rights, size_t pitch, int channels)
+// One frame of every sequence (a NULL pair retires its sequence): the new pairs into the image slot s1 that neither the
+// running nor the previous frame reads, the front stage (gray frames replay the gray graph whatever their source), the
+// back stage, the record copies
+static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& in)
 {
+    if (!ctx) return VO_E_INVALID;
+    int rc;
+    if ((rc = seq_frame_check(ctx, who, multi, SEQ_SUBMIT)) || (rc = seq_pairs_check(ctx, who, multi, ctx->seq_n, ctx->w, in, false)))
+        return rc;
+    const int n = ctx->seq_n;
+    for (int q = 0; multi && q < n; q++)
+        if (!in.lefts[q]) ctx->seq_retired[q] = 1;
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
     const int p = (int)(ctx->seq_submitted & 1);
     const int s0 = ctx->seq_slot, s1 = (s0 + 1) % 3;
-    const bool bgr = channels == 3;
-    int rc;
+    const bool bgr = in.bgr();
+    // Producer ordering of device images: the conversion reads them after the caller's work enqueued so far.  The event is
+    // recorded BEFORE the front stream waits for frame k-2's back stage below, so that the conversion does not queue
+    // behind that pose solve.
+    if (in.device) VO_CUDA_CHECK(cudaEventRecord(ctx->fork_ev, ctx->stream));
     // the per-frame buffers of parity p were last read by the back stage of frame k-2
     VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->seq_back_ev[p], 0));
     // a sequence retired by this or an earlier submission: its units of parity p stop working from this frame on (the
     // other parity's word is still read by the frame in flight, and is cleared by the next submission)
-    const int n = ctx->seq_n;
     for (int q = 0; q < n; q++)
         if (ctx->seq_retired[q] && ctx->seq_live[p * n + q]) {
             VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_seq_live + p * n + q, 0, sizeof(int), ctx->stream));
@@ -366,38 +410,24 @@ static int seq_submit(vo_ctx* ctx, const uint8_t* const* lefts, const uint8_t* c
         }
     if (bgr) {
         // colour frames share one staging buffer: upload + convert stay on the front stream
-        if ((rc = upload_pairs(ctx, s1, lefts, rights, pitch, channels, ctx->stream))) return rc;
+        if ((rc = stage_pairs(ctx, s1, in, ctx->stream))) return rc;
     } else {
         // image slot s1 (of three) was last read, as the previous pair, by the front stage of the frame before the one
         // now running: that frame has this frame's buffer parity, and its seq_front_ev[p] record is still the
-        // current one (it is re-recorded below).  So this copy runs under the front stage of the frame in flight.
-        // (No ordering against the caller's stream is needed: vo_seq_begin synchronises, and every later access to
-        // the image slots is made by this file and ordered through these events.)
+        // current one (it is re-recorded below).  So this copy (or the conversion of a device pair, launched outside the
+        // frame graph because its source pointers change every frame) runs under the front stage of the frame in flight.
+        // (No ordering against the caller's stream is needed for host pairs: vo_seq_begin synchronises, and every later
+        // access to the image slots is made by this file and ordered through these events.  A host upload must not wait
+        // for fork_ev: that would queue its H2D behind the previous front stage.)
         cudaStream_t sc = ctx->lane[1].side;
         VO_CUDA_CHECK(cudaStreamWaitEvent(sc, ctx->seq_front_ev[p], 0));
-        if ((rc = upload_pairs(ctx, s1, lefts, rights, pitch, channels, sc))) return rc;
+        if (in.device) VO_CUDA_CHECK(cudaStreamWaitEvent(sc, ctx->fork_ev, 0));
+        if ((rc = stage_pairs(ctx, s1, in, sc))) return rc;
+        // The join is also the release of device images: the caller's later work on ctx->stream is ordered after the
+        // conversion, the last read of the images.
         VO_CUDA_CHECK(cudaEventRecord(ctx->lane[1].join, sc));
         VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->lane[1].join, 0));
     }
-    return seq_enqueue(ctx, p, s0, s1, bgr);
-}
-
-extern "C" int vo_seq_submit(vo_ctx* ctx, const uint8_t* left1, const uint8_t* right1, size_t pitch, int channels)
-{
-    if (!ctx) return VO_E_INVALID;
-    if (channels != 1 && channels != 3) { vo_set_error(ctx, "vo_seq_submit: channels must be 1 (gray) or 3 (BGR)"); return VO_E_INVALID; }
-    int rc;
-    if ((rc = seq_mode_check(ctx, "vo_seq_submit", false))) return rc;
-    if (!left1 || !right1 || pitch < (size_t)ctx->w * channels) { vo_set_error(ctx, "vo_seq_submit: bad argument"); return VO_E_INVALID; }
-    if (ctx->seq_inflight >= 2) { vo_set_error(ctx, "vo_seq_submit: two frames are in flight already; call vo_seq_wait"); return VO_E_INVALID; }
-    return seq_submit(ctx, &left1, &right1, pitch, channels);
-}
-
-// The rest of a submission once the new pairs are (being) written into image slot s1: the front stage (gray frames
-// replay the gray graph whatever their source), the back stage, the record copies
-static int seq_enqueue(vo_ctx* ctx, int p, int s0, int s1, bool bgr)
-{
-    int rc;
     GraphKey key{};
     key.kind = GraphKey::SEQ_FRONT; key.s = ctx->stream; key.tma = ctx->lk_use_tma;
     key.slot = s0; key.parity = p; key.bgr = bgr;
@@ -409,7 +439,7 @@ static int seq_enqueue(vo_ctx* ctx, int p, int s0, int s1, bool bgr)
     key = GraphKey{};
     key.kind = GraphKey::SEQ_BACK; key.s = sb; key.tma = ctx->lk_use_tma; key.parity = p;
     if ((rc = vo_run_graph(ctx, key, [&] { return seq_back(ctx, p); }))) return rc;
-    const int n = ctx->seq_n, u0 = p * n;
+    const int u0 = p * n;
     const SeqPinned pin = seq_pinned(ctx, n);
     VO_CUDA_CHECK(cudaMemcpyAsync(pin.rec + u0, ctx->d_results + u0, n * sizeof(vo_unit_result_dev), cudaMemcpyDeviceToHost, sb));
     VO_CUDA_CHECK(cudaMemcpyAsync(pin.err + u0, ctx->d_seq_err + 1 + u0, n * sizeof(int), cudaMemcpyDeviceToHost, sb));
@@ -421,62 +451,39 @@ static int seq_enqueue(vo_ctx* ctx, int p, int s0, int s1, bool bgr)
     }
     VO_CUDA_CHECK(cudaEventRecord(ctx->seq_back_ev[p], sb));
     ctx->seq_slot = s1;                 // imageLeft_t0 = imageLeft_t1 (main.cpp:157-158)
-    ctx->seq_channels[p] = bgr ? 3 : 1;
     ctx->seq_submitted++;
     ctx->seq_inflight++;
     return VO_OK;
 }
 
-extern "C" int vo_seq_submit_device(vo_ctx* ctx, const vo_dimage* left1, const vo_dimage* right1)
+// Waits for the oldest submission (who / multi: the calling entry point; want_mono: vo_[m]seq_wait_mono); per sequence q:
+// out[q], status[q] (multi only: VO_OK, VO_E_CAPACITY for glue error bits, VO_MSEQ_RETIRED), frame_pose integrated, with
+// pts4 the four point lists at pts4 + 4 * pts_cap * q, and with want_mono mono[q] and the essential mask at
+// ess_mask + mask_cap * q.  Returns the first status that is an error (the single-sequence mode reports its frame this
+// way), else VO_OK.
+static int seq_wait(vo_ctx* ctx, const char* who, bool multi, bool want_mono, vo_unit_result* out, int* status, vo_mono_result* mono,
+                    uint8_t* ess_mask, int mask_cap, vo_point2f* pts4, int pts_cap)
 {
     if (!ctx) return VO_E_INVALID;
     int rc;
-    if ((rc = seq_mode_check(ctx, "vo_seq_submit_device", false))) return rc;
-    if ((rc = vo_check_dimage(ctx, "vo_seq_submit_device", "left1", left1, ctx->w)) ||
-        (rc = vo_check_dimage(ctx, "vo_seq_submit_device", "right1", right1, ctx->w))) return rc;
-    if (ctx->seq_inflight >= 2) { vo_set_error(ctx, "vo_seq_submit_device: two frames are in flight already; call vo_seq_wait"); return VO_E_INVALID; }
-    VO_CUDA_CHECK(cudaSetDevice(ctx->device));
-    const int unit = (int)(ctx->seq_submitted & 1);
-    const int s0 = ctx->seq_slot, s1 = (s0 + 1) % 3;
-    // Producer ordering: the conversion reads the images after the caller's work enqueued so far.  The event is recorded
-    // BEFORE the front stream waits for frame k-2's back stage below, so that the conversion does not queue behind that
-    // pose solve.
-    VO_CUDA_CHECK(cudaEventRecord(ctx->fork_ev, ctx->stream));
-    VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->seq_back_ev[unit], 0));
-    // As the host gray upload: on the copy stream, into slot s1 once the frame that last read it has finished its front
-    // stage, so the conversion runs under the frame in flight; it is launched outside the frame graph (its source pointers
-    // change every frame), and the frame replays the gray front graph.
-    cudaStream_t sc = ctx->lane[1].side;
-    VO_CUDA_CHECK(cudaStreamWaitEvent(sc, ctx->seq_front_ev[unit], 0));
-    VO_CUDA_CHECK(cudaStreamWaitEvent(sc, ctx->fork_ev, 0));
-    vo_dimage* tab = seq_pinned_tab(ctx) + 2 * s1;
-    tab[0] = *left1; tab[1] = *right1;
-    if ((rc = vo_ingest_device(ctx, tab, 2, 2 * s1, sc))) return rc;
-    // The join is also the release: the caller's later work on ctx->stream is ordered after the conversion, the last read
-    // of the images.
-    VO_CUDA_CHECK(cudaEventRecord(ctx->lane[1].join, sc));
-    VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->lane[1].join, 0));
-    return seq_enqueue(ctx, unit, s0, s1, false);
-}
-
-// Waits for the oldest submission; per sequence q: out[q], status[q] (VO_OK, VO_E_CAPACITY for glue error bits,
-// VO_MSEQ_RETIRED), frame_pose integrated, with pts4 the four point lists at pts4 + 4 * pts_cap * q, and with mono (a mono
-// run) mono[q] and the essential mask at ess_mask + mask_cap * q.  Returns the first status that is an error (the
-// single-sequence mode reports its frame this way), else VO_OK.
-static int seq_wait(vo_ctx* ctx, vo_unit_result* out, int* status, vo_mono_result* mono, uint8_t* ess_mask, int mask_cap,
-                    vo_point2f* pts4, int pts_cap)
-{
+    if ((rc = seq_frame_check(ctx, who, multi, SEQ_WAIT))) return rc;
+    if (!out || (multi && !status) || (want_mono && !mono)) { vo_set_error(ctx, "%s: null result", who); return VO_E_INVALID; }
+    if (want_mono && !ctx->seq_mono) {
+        vo_set_error(ctx, multi ? "%s: the sequences were begun without the flag VO_MSEQ_MONO_ROTATION"
+                                : "%s: the sequence was begun without the option \"mono_rotation\"", who);
+        return VO_E_INVALID;
+    }
+    int single_status;
+    if (!multi) status = &single_status;
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
     const int p = (int)((ctx->seq_submitted - ctx->seq_inflight) & 1);      // the parity of the oldest frame in flight
     VO_CUDA_CHECK(cudaEventSynchronize(ctx->seq_back_ev[p]));
     const int n = ctx->seq_n, u0 = p * n;
     const SeqPinned pin = seq_pinned(ctx, n);
     ctx->seq_inflight--;
-    ctx->seq_frames++;
     const size_t cs = (size_t)ctx->units * ctx->cap;
     cudaStream_t sb = ctx->lane[0].side;
     bool copies = false;
-    int rc = VO_OK;
     for (int q = 0; q < n; q++) {
         if (!ctx->seq_live[u0 + q]) {                   // retired by this submission or an earlier one: nothing ran
             memset(&out[q], 0, sizeof(out[q]));
@@ -532,26 +539,69 @@ static int seq_wait(vo_ctx* ctx, vo_unit_result* out, int* status, vo_mono_resul
     return rc;
 }
 
-extern "C" int vo_seq_wait(vo_ctx* ctx, vo_unit_result* out, vo_point2f* pts4, int pts_cap)
+// currentVOFeatures and the carried translation of sequence q (after the frames in flight)
+static int seq_state(vo_ctx* ctx, const char* who, bool multi, int q, vo_point2f* points, int32_t* ages, int cap, int* n_points,
+                     int* n_ages, double t_out[3])
 {
     if (!ctx) return VO_E_INVALID;
-    if (ctx->seq_active && ctx->seq_multi) return seq_mode_check(ctx, "vo_seq_wait", false);
-    if (!ctx->seq_active || ctx->seq_inflight <= 0) { vo_set_error(ctx, "vo_seq_wait: no frame in flight"); return VO_E_INVALID; }
-    if (!out) { vo_set_error(ctx, "vo_seq_wait: null result"); return VO_E_INVALID; }
-    int status;
-    return seq_wait(ctx, out, &status, nullptr, nullptr, 0, pts4, pts_cap);
+    int rc;
+    if ((rc = seq_frame_check(ctx, who, multi, SEQ_QUERY))) return rc;
+    if (q < 0 || q >= ctx->seq_n) { vo_set_error(ctx, "%s: bad sequence index %d", who, q); return VO_E_INVALID; }
+    VO_CUDA_CHECK(cudaSetDevice(ctx->device));
+    if ((rc = seq_drain(ctx))) return rc;
+    int cnt[2] = {0, 0};
+    VO_CUDA_CHECK(cudaMemcpyAsync(cnt, ctx->d_feat_cnt + 2 * q, 2 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    // the translation the NEXT frame will start from lives in the next frame's buffer parity
+    const size_t next = (size_t)(ctx->seq_submitted & 1) * ctx->seq_n + q;
+    if (t_out) VO_CUDA_CHECK(cudaMemcpyAsync(t_out, ctx->d_tprev + 3 * next, 3 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+    if (n_points) *n_points = cnt[0];
+    if (n_ages) *n_ages = cnt[1];
+    const size_t fo = (size_t)q * ctx->feat_cap;
+    if (points && cnt[0] > 0) VO_CUDA_CHECK(cudaMemcpyAsync(points, ctx->d_feat_pts + fo, (size_t)(cnt[0] < cap ? cnt[0] : cap) * sizeof(float2), cudaMemcpyDeviceToHost, ctx->stream));
+    if (ages && cnt[1] > 0) VO_CUDA_CHECK(cudaMemcpyAsync(ages, ctx->d_feat_ages + fo, (size_t)(cnt[1] < cap ? cnt[1] : cap) * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+    return VO_OK;
+}
+
+// ---- one sequence (vo_seq_*) ---------------------------------------------------------------------------------------
+extern "C" int vo_seq_begin(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], const uint8_t* left0,
+                            const uint8_t* right0, size_t pitch)
+{
+    return vo_seq_begin_ex(ctx, w, h, P_l, P_r, left0, right0, pitch, 1);
+}
+
+extern "C" int vo_seq_begin_ex(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], const uint8_t* left0,
+                               const uint8_t* right0, size_t pitch, int channels)
+{
+    return seq_begin(ctx, "vo_seq_begin", false, 1, 0, w, h, P_l, P_r, host_pairs(&left0, &right0, pitch, channels));
+}
+
+extern "C" int vo_seq_begin_device(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], const vo_dimage* left0,
+                                   const vo_dimage* right0)
+{
+    return seq_begin(ctx, "vo_seq_begin_device", false, 1, 0, w, h, P_l, P_r, device_pair(left0, right0));
+}
+
+extern "C" int vo_seq_submit(vo_ctx* ctx, const uint8_t* left1, const uint8_t* right1, size_t pitch, int channels)
+{
+    return seq_submit(ctx, "vo_seq_submit", false, host_pairs(&left1, &right1, pitch, channels));
+}
+
+extern "C" int vo_seq_submit_device(vo_ctx* ctx, const vo_dimage* left1, const vo_dimage* right1)
+{
+    return seq_submit(ctx, "vo_seq_submit_device", false, device_pair(left1, right1));
+}
+
+extern "C" int vo_seq_wait(vo_ctx* ctx, vo_unit_result* out, vo_point2f* pts4, int pts_cap)
+{
+    return seq_wait(ctx, "vo_seq_wait", false, false, out, nullptr, nullptr, nullptr, 0, pts4, pts_cap);
 }
 
 extern "C" int vo_seq_wait_mono(vo_ctx* ctx, vo_unit_result* out, vo_mono_result* mono, uint8_t* ess_mask, int mask_cap,
                                 vo_point2f* pts4, int pts_cap)
 {
-    if (!ctx) return VO_E_INVALID;
-    if (ctx->seq_active && ctx->seq_multi) return seq_mode_check(ctx, "vo_seq_wait_mono", false);
-    if (!ctx->seq_active || ctx->seq_inflight <= 0) { vo_set_error(ctx, "vo_seq_wait_mono: no frame in flight"); return VO_E_INVALID; }
-    if (!out || !mono) { vo_set_error(ctx, "vo_seq_wait_mono: null result"); return VO_E_INVALID; }
-    if (!ctx->seq_mono) { vo_set_error(ctx, "vo_seq_wait_mono: the sequence was begun without the option \"mono_rotation\""); return VO_E_INVALID; }
-    int status;
-    return seq_wait(ctx, out, &status, mono, ess_mask, mask_cap, pts4, pts_cap);
+    return seq_wait(ctx, "vo_seq_wait_mono", false, true, out, nullptr, mono, ess_mask, mask_cap, pts4, pts_cap);
 }
 
 extern "C" int vo_seq_push(vo_ctx* ctx, const uint8_t* left1, const uint8_t* right1, size_t pitch, vo_unit_result* out,
@@ -572,33 +622,9 @@ extern "C" int vo_seq_push_ex(vo_ctx* ctx, const uint8_t* left1, const uint8_t* 
     return vo_seq_wait(ctx, out, pts4, pts_cap);
 }
 
-// currentVOFeatures and the carried translation of sequence q (after the frames in flight)
-static int seq_state(vo_ctx* ctx, int q, vo_point2f* points, int32_t* ages, int cap, int* n_points, int* n_ages, double t_out[3])
-{
-    VO_CUDA_CHECK(cudaSetDevice(ctx->device));
-    int rc = seq_drain(ctx);
-    if (rc) return rc;
-    int cnt[2] = {0, 0};
-    VO_CUDA_CHECK(cudaMemcpyAsync(cnt, ctx->d_feat_cnt + 2 * q, 2 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    // the translation the NEXT frame will start from lives in the next frame's buffer parity
-    const size_t next = (size_t)(ctx->seq_submitted & 1) * ctx->seq_n + q;
-    if (t_out) VO_CUDA_CHECK(cudaMemcpyAsync(t_out, ctx->d_tprev + 3 * next, 3 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-    if (n_points) *n_points = cnt[0];
-    if (n_ages) *n_ages = cnt[1];
-    const size_t fo = (size_t)q * ctx->feat_cap;
-    if (points && cnt[0] > 0) VO_CUDA_CHECK(cudaMemcpyAsync(points, ctx->d_feat_pts + fo, (size_t)(cnt[0] < cap ? cnt[0] : cap) * sizeof(float2), cudaMemcpyDeviceToHost, ctx->stream));
-    if (ages && cnt[1] > 0) VO_CUDA_CHECK(cudaMemcpyAsync(ages, ctx->d_feat_ages + fo, (size_t)(cnt[1] < cap ? cnt[1] : cap) * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-    return VO_OK;
-}
-
 extern "C" int vo_seq_state(vo_ctx* ctx, vo_point2f* points, int32_t* ages, int cap, int* n_points, int* n_ages, double t_out[3])
 {
-    if (!ctx || !ctx->seq_active) return VO_E_INVALID;
-    int rc;
-    if ((rc = seq_mode_check(ctx, "vo_seq_state", false))) return rc;
-    return seq_state(ctx, 0, points, ages, cap, n_points, n_ages, t_out);
+    return seq_state(ctx, "vo_seq_state", false, 0, points, ages, cap, n_points, n_ages, t_out);
 }
 
 // ---- several sequences in lockstep (vo_mseq_*) ---------------------------------------------------------------------
@@ -623,77 +649,33 @@ extern "C" int vo_mseq_begin_ex(vo_ctx* ctx, int n_seq, int w, int h, const floa
     return vo_mseq_begin_calib(ctx, n_seq, w, h, Pl.data(), Pr.data(), left0, right0, pitch, channels, flags);
 }
 
-// the mono_rotation branch is asked for with the flag only: the context option, which vo_seq_begin* take, would otherwise
-// silently pick (or drop) the branch for a whole set of sequences
 extern "C" int vo_mseq_begin_calib(vo_ctx* ctx, int n_seq, int w, int h, const float* P_l, const float* P_r,
                                    const uint8_t* const* left0, const uint8_t* const* right0, size_t pitch, int channels, int flags)
 {
-    if (!ctx) return VO_E_INVALID;
-    if (flags & ~VO_MSEQ_MONO_ROTATION) { vo_set_error(ctx, "vo_mseq_begin: unknown flag bits 0x%x", (unsigned)(flags & ~VO_MSEQ_MONO_ROTATION)); return VO_E_INVALID; }
-    if (n_seq < 1) { vo_set_error(ctx, "vo_mseq_begin: n_seq = %d, need at least one sequence", n_seq); return VO_E_INVALID; }
-    if (n_seq > VO_MSEQ_MAX) { vo_set_error(ctx, "vo_mseq_begin: n_seq = %d, a context holds at most %d sequences", n_seq, VO_MSEQ_MAX); return VO_E_CAPACITY; }
-    if (channels != 1 && channels != 3) { vo_set_error(ctx, "vo_mseq_begin: channels must be 1 (gray) or 3 (BGR)"); return VO_E_INVALID; }
-    if (!P_l || !P_r || !left0 || !right0 || w <= 0 || h <= 0 || pitch < (size_t)w * channels) { vo_set_error(ctx, "vo_mseq_begin: bad argument"); return VO_E_INVALID; }
-    for (int q = 0; q < n_seq; q++)
-        if (!left0[q] || !right0[q]) { vo_set_error(ctx, "vo_mseq_begin: sequence %d has no first pair", q); return VO_E_INVALID; }
-    if (h / 10 <= 0) { vo_set_error(ctx, "vo_mseq_begin: image too small for the rows/10 bucket size"); return VO_E_UNSUPPORTED; }
-    if (ctx->mono_opt) {
-        vo_set_error(ctx, "vo_mseq_begin: the option \"mono_rotation\" is not supported with several sequences (use the flag "
-                          "VO_MSEQ_MONO_ROTATION of vo_mseq_begin_ex)");
-        return VO_E_UNSUPPORTED;
-    }
-    return seq_begin(ctx, n_seq, true, (flags & VO_MSEQ_MONO_ROTATION) != 0, w, h, P_l, P_r, [&] {
-        int rc = upload_pairs(ctx, 0, left0, right0, pitch, channels, ctx->stream);
-        return rc ? rc : channels == 3 ? convert_pairs(ctx, 0) : VO_OK;
-    });
+    return seq_begin(ctx, "vo_mseq_begin", true, n_seq, flags, w, h, P_l, P_r, host_pairs(left0, right0, pitch, channels));
 }
 
 extern "C" int vo_mseq_submit(vo_ctx* ctx, const uint8_t* const* left1, const uint8_t* const* right1, size_t pitch, int channels)
 {
-    if (!ctx) return VO_E_INVALID;
-    if (channels != 1 && channels != 3) { vo_set_error(ctx, "vo_mseq_submit: channels must be 1 (gray) or 3 (BGR)"); return VO_E_INVALID; }
-    int rc;
-    if ((rc = seq_mode_check(ctx, "vo_mseq_submit", true))) return rc;
-    if (!left1 || !right1 || pitch < (size_t)ctx->w * channels) { vo_set_error(ctx, "vo_mseq_submit: bad argument"); return VO_E_INVALID; }
-    if (ctx->seq_inflight >= 2) { vo_set_error(ctx, "vo_mseq_submit: two submissions are in flight already; call vo_mseq_wait"); return VO_E_INVALID; }
-    const int n = ctx->seq_n;
-    for (int q = 0; q < n; q++) {
-        const bool none = !left1[q] && !right1[q];
-        if (!none && (!left1[q] || !right1[q])) { vo_set_error(ctx, "vo_mseq_submit: sequence %d has only one image (a NULL pair retires it)", q); return VO_E_INVALID; }
-        if (!none && ctx->seq_retired[q]) { vo_set_error(ctx, "vo_mseq_submit: sequence %d was retired", q); return VO_E_INVALID; }
-    }
-    for (int q = 0; q < n; q++)
-        if (!left1[q]) ctx->seq_retired[q] = 1;
-    return seq_submit(ctx, left1, right1, pitch, channels);
+    return seq_submit(ctx, "vo_mseq_submit", true, host_pairs(left1, right1, pitch, channels));
 }
 
 extern "C" int vo_mseq_wait(vo_ctx* ctx, vo_unit_result* out, int* status, vo_point2f* pts4, int pts_cap)
 {
-    if (!ctx) return VO_E_INVALID;
-    int rc;
-    if ((rc = seq_mode_check(ctx, "vo_mseq_wait", true))) return rc;
-    if (ctx->seq_inflight <= 0) { vo_set_error(ctx, "vo_mseq_wait: no submission in flight"); return VO_E_INVALID; }
-    if (!out || !status) { vo_set_error(ctx, "vo_mseq_wait: null result"); return VO_E_INVALID; }
-    return seq_wait(ctx, out, status, nullptr, nullptr, 0, pts4, pts_cap);
+    return seq_wait(ctx, "vo_mseq_wait", true, false, out, status, nullptr, nullptr, 0, pts4, pts_cap);
 }
 
 extern "C" int vo_mseq_wait_mono(vo_ctx* ctx, vo_unit_result* out, int* status, vo_mono_result* mono, uint8_t* ess_mask, int mask_cap,
                                  vo_point2f* pts4, int pts_cap)
 {
-    if (!ctx) return VO_E_INVALID;
-    int rc;
-    if ((rc = seq_mode_check(ctx, "vo_mseq_wait_mono", true))) return rc;
-    if (ctx->seq_inflight <= 0) { vo_set_error(ctx, "vo_mseq_wait_mono: no submission in flight"); return VO_E_INVALID; }
-    if (!out || !status || !mono) { vo_set_error(ctx, "vo_mseq_wait_mono: null result"); return VO_E_INVALID; }
-    if (!ctx->seq_mono) { vo_set_error(ctx, "vo_mseq_wait_mono: the sequences were begun without the flag VO_MSEQ_MONO_ROTATION"); return VO_E_INVALID; }
-    return seq_wait(ctx, out, status, mono, ess_mask, mask_cap, pts4, pts_cap);
+    return seq_wait(ctx, "vo_mseq_wait_mono", true, true, out, status, mono, ess_mask, mask_cap, pts4, pts_cap);
 }
 
 extern "C" int vo_mseq_pose(vo_ctx* ctx, int q, double frame_pose[16])
 {
     if (!ctx) return VO_E_INVALID;
     int rc;
-    if ((rc = seq_mode_check(ctx, "vo_mseq_pose", true))) return rc;
+    if ((rc = seq_frame_check(ctx, "vo_mseq_pose", true, SEQ_QUERY))) return rc;
     if (q < 0 || q >= ctx->seq_n || !frame_pose) { vo_set_error(ctx, "vo_mseq_pose: bad argument"); return VO_E_INVALID; }
     memcpy(frame_pose, ctx->seq_pose.data() + 16 * (size_t)q, 16 * sizeof(double));
     return VO_OK;
@@ -701,9 +683,5 @@ extern "C" int vo_mseq_pose(vo_ctx* ctx, int q, double frame_pose[16])
 
 extern "C" int vo_mseq_state(vo_ctx* ctx, int q, vo_point2f* points, int32_t* ages, int cap, int* n_points, int* n_ages, double t_out[3])
 {
-    if (!ctx) return VO_E_INVALID;
-    int rc;
-    if ((rc = seq_mode_check(ctx, "vo_mseq_state", true))) return rc;
-    if (q < 0 || q >= ctx->seq_n) { vo_set_error(ctx, "vo_mseq_state: bad sequence index %d", q); return VO_E_INVALID; }
-    return seq_state(ctx, q, points, ages, cap, n_points, n_ages, t_out);
+    return seq_state(ctx, "vo_mseq_state", true, q, points, ages, cap, n_points, n_ages, t_out);
 }
