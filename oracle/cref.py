@@ -15,6 +15,13 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_build", "liboracle.so")
 _lib = None
 
+# lk_track's event log (lk_ref.c: lk_event_t and the LK_EV_* kinds)
+LK_EVENT = np.dtype([("pt", "<i4"), ("level", "<i4"), ("iter", "<i4"), ("kind", "<i4"),
+                     ("min_eig", "<f4"), ("D", "<f4"), ("dx", "<f4"), ("dy", "<f4"), ("sdx", "<f4"), ("sdy", "<f4"),
+                     ("ipx", "<i4"), ("ipy", "<i4"), ("inx", "<i4"), ("iny", "<i4"),
+                     ("d2", "<f8"), ("d2f", "<f4"), ("pad_", "<i4"), ("sabs", "<i8", (10,))])
+EV_ITER, EV_EPS, EV_HALF, EV_CAP, EV_JOUT, EV_SETUP, EV_REJECT, EV_IOUT, EV_FINAL = range(9)
+
 
 def lib():
     global _lib
@@ -34,6 +41,9 @@ def lib():
         L.lk_track.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_void_p]
         L.lk_set_sum_mode.argtypes = [C.c_int]
+        L.lk_log_enable.argtypes = [C.c_void_p, C.c_longlong]
+        L.lk_log_count.restype = C.c_longlong
+        assert L.lk_log_record_size() == LK_EVENT.itemsize
         L.pyr_down_u8.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int]
         L.scharr_deriv.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int]
         L.fast_detect.restype = C.c_int
@@ -91,19 +101,38 @@ class Pyramid:
 
 
 def lk_track(prev, nxt, pts, win=21, max_level=3, max_count=30, epsilon=0.01, min_eig=1e-3,
-             prev_pyr=None, next_pyr=None, return_iters=False):
-    """One calcOpticalFlowPyrLK call (flags=0, err requested) on the C restatement."""
+             prev_pyr=None, next_pyr=None, return_iters=False, return_log=False):
+    """One calcOpticalFlowPyrLK call (flags=0, err requested) on the C restatement.  return_log: also the event log
+    (a LK_EVENT array in the order the oracle made the decisions: levels coarse to fine, points, iterations)."""
     pp = prev_pyr or Pyramid(prev, win, max_level, True)
     np_ = next_pyr or Pyramid(nxt, win, max_level, False)
     pts = np.ascontiguousarray(pts, np.float32).reshape(-1, 2)
     n = len(pts)
     out = np.zeros((n, 2), np.float32); st = np.zeros(n, np.uint8); err = np.zeros(n, np.float32)
     it = np.zeros(n, np.int32)
-    if n:
+    log = np.zeros(0, LK_EVENT)
+
+    def run():
         lib().lk_track(pp.h, np_.h, _p(pts), _p(out), _p(st), _p(err), n, win, max_count, epsilon, min_eig, _p(it))
-    if return_iters:
-        return out, st, err, it
-    return out, st, err
+
+    if n and return_log:
+        cap = n * pp.nlevels() * 8
+        while True:                     # the oracle counts the records it could not store: re-run with that size
+            log = np.zeros(cap, LK_EVENT)
+            lib().lk_log_enable(_p(log), cap)
+            try:
+                run()
+                cnt = lib().lk_log_count()
+            finally:
+                lib().lk_log_enable(None, 0)
+            if cnt <= cap:
+                break
+            cap = cnt
+        log = log[:cnt]
+    elif n:
+        run()
+    res = (out, st, err) + ((it,) if return_iters else ()) + ((log,) if return_log else ())
+    return res
 
 
 def fast_detect(img, threshold=20, nms=True, cap=None):

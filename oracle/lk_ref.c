@@ -239,6 +239,66 @@ static void lk_chain_stats(const int *diffs_all, const int16_t *dIbuf, int win)
     g_stats[0]++; g_stats[1] += ok_old; g_stats[2] += ok_strip; g_stats[3] += ok_true;
 }
 
+/* Optional per-point event log (off by default; tests/test_oracle_lk_edges.py and tests/golden/make_lk_edges.py read it
+ * to find and check the inputs that sit on the decision edges of a level-solve).  One record per level-solve set-up
+ * (minEig, D, the I window origin) and one per Newton iteration (the step, the half-step sums, the J window origin,
+ * ||delta||^2 in double and in float, sum |addend| of the ten b chains as the kernel bounds them), plus one for the
+ * level-0 final re-check when it clears the status.  The layout is mirrored by oracle/cref.py:LK_EVENT. */
+enum {
+    LK_EV_ITER = 0,     /* an iteration after which the solve goes on                                   */
+    LK_EV_EPS = 1,      /* ended by delta.ddot(delta) <= eps^2                                          */
+    LK_EV_HALF = 2,     /* ended by |dx + pdx| < 0.01 && |dy + pdy| < 0.01 (the half-step exit)         */
+    LK_EV_CAP = 3,      /* the max_count-th iteration, none of the exits taken                          */
+    LK_EV_JOUT = 4,     /* the J window left the image before iteration `iter` (no step computed)       */
+    LK_EV_SETUP = 5,    /* level-solve set up: minEig >= threshold and D >= FLT_EPSILON                 */
+    LK_EV_REJECT = 6,   /* level-solve rejected: minEig < threshold or D < FLT_EPSILON                  */
+    LK_EV_IOUT = 7,     /* the I window is out of the image: the level is skipped                       */
+    LK_EV_FINAL = 8,    /* level 0 final re-check: the end position's window is out of the image        */
+};
+typedef struct {
+    int32_t pt, level, iter, kind;
+    float min_eig, D, dx, dy, sdx, sdy;     /* sdx = dx + pdx, sdy = dy + pdy (pdx = pdy = 0 at iteration 0) */
+    int32_t ipx, ipy, inx, iny;             /* floored window origins: I (level set-up), J (this iteration)  */
+    double d2;                              /* (double)dx*dx + (double)dy*dy                                  */
+    float d2f;                              /* dx*dx + dy*dy in float                                         */
+    int32_t pad_;
+    int64_t sabs[10];                       /* b1 chains 0..3, b1 tail, b2 chains 0..3, b2 tail               */
+} lk_event_t;
+static lk_event_t *g_log = NULL;
+static long long g_log_cap = 0, g_log_n = 0;
+void lk_log_enable(void *buf, long long cap) { g_log = (lk_event_t *)buf; g_log_cap = buf ? cap : 0; g_log_n = 0; }
+long long lk_log_count(void) { return g_log_n; }
+int lk_log_record_size(void) { return (int)sizeof(lk_event_t); }
+
+static lk_event_t *lk_log_add(int pt, int level, int iter, int kind)
+{
+    static lk_event_t sink;
+    lk_event_t *e = g_log_n < g_log_cap ? &g_log[g_log_n] : &sink;    /* counted even when full: the caller re-runs */
+    g_log_n++;
+    memset(e, 0, sizeof(*e));
+    e->pt = pt; e->level = level; e->iter = iter; e->kind = kind;
+    return e;
+}
+
+/* sum |addend| of each b chain as k_lk_ring bounds it: |v0| + |v1| for the pair addends of the SIMD chains */
+static void lk_chain_sabs(const int *diffs_all, const int16_t *dIbuf, int win, int64_t out[10])
+{
+    for (int comp = 0; comp < 2; comp++) {
+        for (int q = 0; q < 4; q++) {
+            long long s = 0;
+            for (int y = 0; y < win; y++)
+                for (int x = q; x < (win / 8) * 8; x += 4)
+                    s += llabs((long long)diffs_all[y * win + x] * dIbuf[(y * win + x) * 2 + comp]);
+            out[comp * 5 + q] = s;
+        }
+        long long s = 0;
+        for (int y = 0; y < win; y++)
+            for (int x = (win / 8) * 8; x < win; x++)
+                s += llabs((long long)diffs_all[y * win + x] * dIbuf[(y * win + x) * 2 + comp]);
+        out[comp * 5 + 4] = s;
+    }
+}
+
 static inline float reduce4(const float q[4])
 {
     switch (g_sum_mode) {
@@ -293,6 +353,7 @@ void lk_track(const lk_pyr_t *prev, const lk_pyr_t *next,
             px -= half; py -= half;
             int ipx = cv_floor(px), ipy = cv_floor(py);
             if (ipx < -win || ipx >= I->w || ipy < -win || ipy >= I->h) {
+                if (g_log) { lk_event_t *e = lk_log_add(pi, level, -1, LK_EV_IOUT); e->ipx = ipx; e->ipy = ipy; }
                 if (level == 0) { status[pi] = 0; if (err) err[pi] = 0.f; }
                 continue;
             }
@@ -336,6 +397,10 @@ void lk_track(const lk_pyr_t *prev, const lk_pyr_t *next,
             float A11 = iA11 * FLT_SCALE, A12 = iA12 * FLT_SCALE, A22 = iA22 * FLT_SCALE;
             float D = A11 * A22 - A12 * A12;
             float minEig = (A22 + A11 - sqrtf((A11 - A22) * (A11 - A22) + 4.f * A12 * A12)) / (2 * win * win);
+            if (g_log) {
+                lk_event_t *e = lk_log_add(pi, level, -1, (minEig < min_eig_thr || D < FLT_EPSILON) ? LK_EV_REJECT : LK_EV_SETUP);
+                e->min_eig = minEig; e->D = D; e->ipx = ipx; e->ipy = ipy;
+            }
             if (minEig < min_eig_thr || D < FLT_EPSILON) {
                 if (level == 0) status[pi] = 0;
                 continue;
@@ -347,6 +412,10 @@ void lk_track(const lk_pyr_t *prev, const lk_pyr_t *next,
             for (int j = 0; j < max_count; j++) {
                 int inx = cv_floor(npx), iny = cv_floor(npy);
                 if (inx < -win || inx >= J->w || iny < -win || iny >= J->h) {
+                    if (g_log) {
+                        lk_event_t *e = lk_log_add(pi, level, j, LK_EV_JOUT);
+                        e->min_eig = minEig; e->ipx = ipx; e->ipy = ipy; e->inx = inx; e->iny = iny;
+                    }
                     if (level == 0) status[pi] = 0;
                     break;
                 }
@@ -400,8 +469,17 @@ void lk_track(const lk_pyr_t *prev, const lk_pyr_t *next,
                 float dy = (float)((A12 * b1 - A11 * b2) * D);
                 npx += dx; npy += dy;
                 next_pts[2 * pi] = npx + half; next_pts[2 * pi + 1] = npy + half;
-                if ((double)dx * dx + (double)dy * dy <= eps2) break;
+                lk_event_t *ev = NULL;
+                if (g_log) {
+                    ev = lk_log_add(pi, level, j, j == max_count - 1 ? LK_EV_CAP : LK_EV_ITER);
+                    ev->min_eig = minEig; ev->D = D; ev->dx = dx; ev->dy = dy; ev->sdx = dx + pdx; ev->sdy = dy + pdy;
+                    ev->ipx = ipx; ev->ipy = ipy; ev->inx = inx; ev->iny = iny;
+                    ev->d2 = (double)dx * dx + (double)dy * dy; ev->d2f = dx * dx + dy * dy;
+                    lk_chain_sabs(diffs_all, dIbuf, win, ev->sabs);
+                }
+                if ((double)dx * dx + (double)dy * dy <= eps2) { if (ev) ev->kind = LK_EV_EPS; break; }
                 if (j > 0 && fabs(dx + pdx) < 0.01 && fabs(dy + pdy) < 0.01) {
+                    if (ev) ev->kind = LK_EV_HALF;
                     next_pts[2 * pi] -= dx * 0.5f;
                     next_pts[2 * pi + 1] -= dy * 0.5f;
                     break;
@@ -413,6 +491,7 @@ void lk_track(const lk_pyr_t *prev, const lk_pyr_t *next,
                 float fx = next_pts[2 * pi] - half, fy = next_pts[2 * pi + 1] - half;
                 int inx = cv_floor(fx), iny = cv_floor(fy);
                 if (inx < -win || inx >= J->w || iny < -win || iny >= J->h) {
+                    if (g_log) { lk_event_t *e = lk_log_add(pi, 0, -1, LK_EV_FINAL); e->inx = inx; e->iny = iny; }
                     status[pi] = 0;
                     continue;
                 }
