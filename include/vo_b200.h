@@ -350,8 +350,8 @@ VO_API int vo_seq_wait_mono(vo_ctx* ctx, vo_unit_result* out, vo_mono_result* mo
 VO_API int vo_seq_state(vo_ctx* ctx, vo_point2f* points, int32_t* ages, int cap, int* n_points, int* n_ages, double t_out[3]);
 
 /* ---- several independent sequences through the streaming sequence mode ----------------------------------------------
- * n_seq sequences of one image size, each with its own calibration (vo_mseq_begin_calib) or all with one, advance in
- * lockstep, one frame each per submission, through the
+ * n_seq sequences, each with its own calibration (vo_mseq_begin_calib) or all with one, and each with its own image size
+ * (vo_mseq_begin_sized) or all with one, advance in lockstep, one frame each per submission, through the
  * stages of the sequence mode above; every stage is ONE kernel launch for all of them, so a submission costs the launches
  * of one vo_seq_submit whatever n_seq is.  Each sequence's records, point lists, carried state and frame_pose are those of
  * running it alone through vo_seq_begin / vo_seq_push (the same kernels on its own units), bit for bit.
@@ -399,7 +399,23 @@ VO_API int vo_mseq_begin_ex(vo_ctx* ctx, int n_seq, int w, int h, const float P_
  * submission costs the same launches as with one calibration.  vo_mseq_begin_ex is this call with its matrices repeated. */
 VO_API int vo_mseq_begin_calib(vo_ctx* ctx, int n_seq, int w, int h, const float* P_l, const float* P_r,
                                const uint8_t* const* left0, const uint8_t* const* right0, size_t pitch, int channels, int flags);
+/* vo_mseq_begin_calib with one image size and one row pitch per sequence: sequence q is w[q] x h[q], its images are read
+ * pitch[q] bytes per row.  Each sequence's results are those of vo_seq_begin at its own size and calibration, bit for bit
+ * (its own pyramid borders, FAST raster, LK image bounds and rows/10 bucket grid), and a submission costs the same launches
+ * as with one size.  The image planes are allocated at the envelope of the sizes (the largest width, the largest height),
+ * so a later run whose sizes have the same envelope reuses them, and the frame graphs of any earlier run with the same
+ * largest rows/10 bucket grid.  vo_mseq_begin_calib is this call
+ * with w / h / pitch repeated.  Refused with VO_E_INVALID: NULL w, h or pitch, a size <= 0, pitch[q] < channels * w[q]
+ * (and every refusal of vo_mseq_begin_calib); VO_E_UNSUPPORTED: h[q] / 10 == 0, or sizes with different pyramid depths
+ * (every size above about 170 pixels on each side has the full depth of lk_max_level = 3).  A refusal changes nothing. */
+VO_API int vo_mseq_begin_sized(vo_ctx* ctx, int n_seq, const int* w, const int* h, const float* P_l, const float* P_r,
+                               const uint8_t* const* left0, const uint8_t* const* right0, const size_t* pitch,
+                               int channels, int flags);
+/* vo_mseq_submit with one row pitch per sequence (pitch[q] is not read for a retiring sequence); vo_mseq_submit is this
+ * call with its pitch repeated, so with several sizes it needs a pitch that covers every live sequence's width. */
 VO_API int vo_mseq_submit(vo_ctx* ctx, const uint8_t* const* left1, const uint8_t* const* right1, size_t pitch, int channels);
+VO_API int vo_mseq_submit_sized(vo_ctx* ctx, const uint8_t* const* left1, const uint8_t* const* right1,
+                                const size_t* pitch, int channels);
 VO_API int vo_mseq_wait(vo_ctx* ctx, vo_unit_result* out, int* status, vo_point2f* pts4, int pts_cap);
 VO_API int vo_mseq_wait_mono(vo_ctx* ctx, vo_unit_result* out, int* status, vo_mono_result* mono,
                              uint8_t* ess_mask, int mask_cap, vo_point2f* pts4, int pts_cap);

@@ -2,7 +2,7 @@
 """Scaling of the multi-sequence streaming mode (vo_mseq_*) with the number of sequences, measured on the GPU.
 
     python tools/mseq_timing.py [--frames 40] [--rounds 5] [--counts 1,2,4,8,16,32] [--mono-rotation] [--mixed-calibration]
-                                [--json out.json]
+                                [--mixed-sizes] [--json out.json]
 
 Synthetic 1241x376 drives (synth.stereo_unit; eight seeds, each with its own motion) of `--frames` frames each;
 sequence q replays drive q % 8, forwards for even q // 8 and backwards for odd, so up to 16 sequences are distinct and
@@ -16,7 +16,11 @@ mono_rotation branch (the option "mono_rotation" for vo_seq_*, the flag VO_MSEQ_
 reports both.  `--mixed-calibration` also runs every vo_mseq_* count with one calibration per sequence
 (vo_mseq_begin_calib): sequence q is then rendered with, and run with, its own camera (focal length, principal point and
 baseline spread over +-10 %, +-20 px and +-15 %), so that no two sequences share a calibration; the motions are those
-of the one-calibration run.  Both are timed in the same rounds, alternated.  The card's name, power limit and max SM clock, read in the same run, are printed with the numbers;
+of the one-calibration run.  Both are timed in the same rounds, alternated.  `--mixed-sizes` (counts 3, 11 and 32 unless
+--counts is given) also runs every vo_mseq_* count with sequence q at the image size of KITTI odometry training sequence
+q mod 11 (1241x376 for 00-02, 1242x375 for 03, 1226x370 for 04-10: the 3 : 1 : 7 mix of the training set, through
+vo_mseq_begin_sized), the drives rendered at those sizes with the motions of the one-size run, timed against the same
+count all at 1241x376 in the same rounds, alternated.  The card's name, power limit and max SM clock, read in the same run, are printed with the numbers;
 they are part of them."""
 import argparse
 import json
@@ -30,6 +34,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 
 W, H, DRIVES = 1241, 376, 8
+KITTI_SIZES = [(1241, 376)] * 3 + [(1242, 375)] + [(1226, 370)] * 7      # training sequences 00 .. 10
 
 
 def card():
@@ -57,17 +62,17 @@ def calibration(q, n):
 
 def render(job):
     from visual_odom_b200 import synth
-    d, k, cal = job
+    d, k, cal, (w, h) = job
     r, t = motion(d)
-    u = synth.stereo_unit(W, H, 50 + d, rvec=r * k, tvec=t * k, **({} if cal is None else dict(cal=cal)))
+    u = synth.stereo_unit(w, h, 50 + d, rvec=r * k, tvec=t * k, **({} if cal is None else dict(cal=cal)))
     return (u["l0"], u["r0"]) if k == 0 else (u["l1"], u["r1"])
 
 
-def drives(n_frames, cals=None):
-    """[drive][frame] = (left, right), rendered in parallel (one synth call per frame).  cals: one calibration per drive
-    (drive i then replays the motion of drive i % DRIVES), else DRIVES drives at KITTI 00's."""
+def drives(n_frames, cals=None, size=(W, H)):
+    """[drive][frame] = (left, right) of size w x h, rendered in parallel (one synth call per frame).  cals: one
+    calibration per drive (drive i then replays the motion of drive i % DRIVES), else DRIVES drives at KITTI 00's."""
     ids = [(d, None) for d in range(DRIVES)] if cals is None else [(i % DRIVES, c) for i, c in enumerate(cals)]
-    jobs = [(d, k, c) for d, c in ids for k in range(n_frames)]
+    jobs = [(d, k, c, size) for d, c in ids for k in range(n_frames)]
     with ProcessPoolExecutor(max_workers=min(32, os.cpu_count() or 1)) as ex:
         pairs = list(ex.map(render, jobs, chunksize=4))
     return [pairs[i * n_frames:(i + 1) * n_frames] for i in range(len(ids))]
@@ -118,8 +123,12 @@ def main():
     ap.add_argument("--mono-rotation", action="store_true", help="also time every mode with the mono_rotation branch")
     ap.add_argument("--mixed-calibration", action="store_true",
                     help="also time every vo_mseq_* count with a distinct calibration per sequence")
+    ap.add_argument("--mixed-sizes", action="store_true",
+                    help="also time every vo_mseq_* count with the KITTI training set's three image sizes")
     ap.add_argument("--json", help="also write the result here")
     a = ap.parse_args()
+    if a.mixed_sizes and a.counts == ap.get_default("counts"):
+        a.counts = "3,11,32"
     counts = [int(c) for c in a.counts.split(",")]
     from visual_odom_b200 import capi, synth
     P_l, P_r = synth.proj_matrices()
@@ -129,6 +138,8 @@ def main():
     monos = (False, True) if a.mono_rotation else (False,)
     mixes = (False, True) if a.mixed_calibration else (False,)
     modes = [(m, mono, mix) for m in ["seq"] + counts for mono in monos for mix in mixes if not (m == "seq" and mix)]
+    if a.mixed_sizes:
+        modes += [(m, mono, "sizes") for m in counts for mono in monos]
     seqs = {n: [sequence(dr, q) for q in range(n)] for n in counts}
     mixed = {}
     if a.mixed_calibration:              # per count n: sequence q rendered with calibration(q, n), played like sequence(dr, q)
@@ -139,6 +150,13 @@ def main():
             mixed[n] = ([md[q] if (q // DRIVES) % 2 == 0 else md[q][::-1] for q in range(n)],
                         np.stack([synth.proj_matrices(c)[0] for c in cals]), np.stack([synth.proj_matrices(c)[1] for c in cals]))
         print(f"rendered the mixed-calibration sequences in {time.perf_counter() - t0:.0f} s", flush=True)
+    sized = {}
+    if a.mixed_sizes:                    # per count n: sequence q at KITTI_SIZES[q % 11], played like sequence(dr, q)
+        t0 = time.perf_counter()
+        by_size = {sz: (dr if sz == (W, H) else drives(a.frames + 1, size=sz)) for sz in set(KITTI_SIZES)}
+        for n in counts:
+            sized[n] = [sequence(by_size[KITTI_SIZES[q % len(KITTI_SIZES)]], q) for q in range(n)]
+        print(f"rendered the drives at {len(by_size)} image sizes in {time.perf_counter() - t0:.0f} s", flush=True)
     ctx = capi.Context(0, max_features=4096)
     res = {m: dict(fps=[], lat=[], launches=[]) for m in modes}
 
@@ -147,7 +165,7 @@ def main():
         if m == "seq":
             fr = dr[0] if fr_cut is None else dr[0][:fr_cut]
             return run_seq(ctx, P_l, P_r, fr, mono)
-        s, Pl, Pr = mixed[m] if mix else (seqs[m], P_l, P_r)
+        s, Pl, Pr = (sized[m], P_l, P_r) if mix == "sizes" else (mixed[m] if mix else (seqs[m], P_l, P_r))
         s = s if fr_cut is None else [x[:fr_cut] for x in s]
         return run_mseq(ctx, Pl, Pr, s, mono)
 
@@ -165,9 +183,9 @@ def main():
                  aggregate_fps_max=float(np.max(r["fps"])), step_latency_ms=1e3 * float(np.median(r["lat"])),
                  launches_per_submission=float(np.median(r["launches"])))
         m, mono, mix = mode
-        out["modes"][str(m) + ("+mono" if mono else "") + ("+mixed" if mix else "")] = o
+        out["modes"][str(m) + ("+mono" if mono else "") + ("+sizes" if mix == "sizes" else "+mixed" if mix else "")] = o
         name = ("vo_seq (1 sequence)" if m == "seq" else f"vo_mseq n_seq = {m:2d}") + (", mono" if mono else "") + \
-            (", mixed cal." if mix else "")
+            (", KITTI sizes" if mix == "sizes" else ", mixed cal." if mix else "")
         print(f"{name:40s}: {o['aggregate_fps']:8.0f} frames/s [{o['aggregate_fps_min']:.0f}, {o['aggregate_fps_max']:.0f}], "
               f"step {o['step_latency_ms']:.3f} ms, {o['launches_per_submission']:.1f} launches / submission")
     print(json.dumps(out))

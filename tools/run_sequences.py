@@ -9,7 +9,9 @@ submission advances every sequence by one frame (two submissions in flight), and
 frame, so sequences of unequal length share the run.  frame_pose of each is integrated with the reference's Euler and
 scale gates (src/main.cpp:196-208), written to OUTDIR/<name>.txt in the KITTI text format (<name> = the dataset
 directory's name) and, with --gt, scored against GTDIR/<name>.txt with the KITTI segment metric.  All sequences must
-have the image size of the first.  The positional calibration applies to every sequence that no
+have the image size of the first, unless `--mixed-sizes` runs each at its own size (vo_mseq_begin_sized: KITTI's
+training sequences come in three sizes, 1241x376, 1242x375 and 1226x370), which needs one pyramid depth for all of them
+(every size above about 170 pixels on each side has the full depth).  The positional calibration applies to every sequence that no
 `--calibration-for NAME=YAML` names (NAME = the dataset directory's name); each sequence runs with the matrices built from
 its own file, as the reference's main() builds them (src/main.cpp:67-74).  `--mono-rotation` runs trackingFrame2Frame
 as its header default does, for every sequence (mono_rotation = true: the rotation from findEssentialMat + recoverPose,
@@ -26,6 +28,23 @@ import numpy as np
 from run_sequence import count_frames, read_calibration
 
 
+def pyramid_depth(w, h):
+    """pyramid images of a w x h image as the library builds them (vo_pyr_depth, csrc/common.cuh): levels up to the
+    default vo_params.lk_max_level, a level dropped once it is not larger than the lk_win window.  Both values are read
+    from the library's vo_default_params, which the run's context is created with."""
+    import ctypes as C
+    from visual_odom_b200 import capi
+    p = capi.VoParams()
+    capi.load_library().vo_default_params(C.byref(p))
+    n = 1
+    for _ in range(p.lk_max_level):
+        w, h = (w + 1) // 2, (h + 1) // 2
+        if w <= p.lk_win or h <= p.lk_win:
+            break
+        n += 1
+    return n
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("datasets", nargs="+", metavar="DIR")
@@ -38,6 +57,8 @@ def main():
                     help="rotation from findEssentialMat + recoverPose (trackingFrame2Frame's header default)")
     ap.add_argument("--calibration-for", action="append", default=[], metavar="NAME=YAML",
                     help="calibration of the dataset named NAME (repeatable; the others use the positional one)")
+    ap.add_argument("--mixed-sizes", action="store_true",
+                    help="run sequences of different image sizes together, each at its own size")
     ap.add_argument("--check", action="store_true")
     a = ap.parse_args()
     from visual_odom_b200 import capi, synth
@@ -65,9 +86,16 @@ def main():
         if n < 2:
             raise SystemExit(f"{d}: need at least two stereo pairs (image_0/%06d.png, image_1/%06d.png from 0)")
         w, h, ctype, depth = capi.png_info(open(os.path.join(d, "image_0", "%06d.png" % 0), "rb").read())
-        if seqs and (w, h) != (seqs[0]["w"], seqs[0]["h"]):
+        if seqs and (w, h) != (seqs[0]["w"], seqs[0]["h"]) and not a.mixed_sizes:
             raise SystemExit(f"{d}: {w}x{h} images, {a.datasets[0]} has {seqs[0]['w']}x{seqs[0]['h']}: "
-                             "one context runs one image size (group the sequences by size)")
+                             "one context runs one image size (group the sequences by size, or run them together with "
+                             "--mixed-sizes)")
+        if a.mixed_sizes and h // 10 == 0:
+            raise SystemExit(f"{d}: {w}x{h} images are too small for the rows/10 bucket size")
+        if a.mixed_sizes and seqs and pyramid_depth(w, h) != pyramid_depth(seqs[0]["w"], seqs[0]["h"]):
+            raise SystemExit(f"{d}: {w}x{h} images have {pyramid_depth(w, h)} pyramid levels, {a.datasets[0]} "
+                             f"({seqs[0]['w']}x{seqs[0]['h']}) has {pyramid_depth(seqs[0]['w'], seqs[0]['h'])}: "
+                             "one context runs one pyramid depth")
         gt = os.path.join(a.gt, name + ".txt") if a.gt else None
         if gt and not os.path.exists(gt):
             raise SystemExit(f"{gt}: no ground truth for sequence {name}")
@@ -76,6 +104,8 @@ def main():
         seqs.append(dict(dir=d, name=name, n=n, w=w, h=h, gray=ctype == 0, gt=gt, P_l=P_l, P_r=P_r))
         print(f"{name}: {n} stereo pairs of {w}x{h} (PNG colour type {ctype}, {depth} bit), calibration {cal_path}")
         print(f"  P_left =\n{P_l}\n  P_right =\n{P_r}")
+    if a.mixed_sizes:
+        print("image sizes: " + ", ".join(f"{s['name']} {s['w']}x{s['h']}" for s in seqs))
     print("rotation: " + ("findEssentialMat + recoverPose (mono_rotation = true)" if a.mono_rotation else
                           "Rodrigues of the PnP rvec (mono_rotation = false)"))
     if a.check:
@@ -87,22 +117,30 @@ def main():
     rds = [capi.SequenceReader(s["dir"], 0, s["n"], threads=a.threads, depth=a.threads + 3, force_channels=force) for s in seqs]
 
     def pairs(k):
-        """pointers of frame k of every sequence (None past a sequence's last frame), pitch, channels"""
-        lp, rp, fmt = [], [], set()
+        """pointers of frame k of every sequence (None past a sequence's last frame), pitch (one per sequence with
+        --mixed-sizes: its reader's), channels"""
+        lp, rp, fmt, pitches, chs = [], [], set(), [], set()
         for s, rd in zip(seqs, rds):
             if k >= s["n"]:
-                lp.append(None); rp.append(None)
+                lp.append(None); rp.append(None); pitches.append(s["w"])
                 continue
             l, r, _, _, pitch, ch, _ = rd.next_ptr()
-            lp.append(l); rp.append(r); fmt.add((pitch, ch))
-        if len(fmt) > 1:
+            lp.append(l); rp.append(r); fmt.add((pitch, ch)); pitches.append(pitch); chs.add(ch)
+        if len(chs) > 1 or (len(fmt) > 1 and not a.mixed_sizes):
             raise SystemExit(f"frame {k}: the readers deliver different layouts {sorted(fmt)}")
-        pitch, ch = fmt.pop() if fmt else (seqs[0]["w"], 1)
+        ch = chs.pop() if chs else 1
+        if a.mixed_sizes:
+            return lp, rp, pitches, ch
+        pitch = fmt.pop()[0] if fmt else seqs[0]["w"]
         return lp, rp, pitch, ch
 
     lp, rp, pitch, ch = pairs(0)
     P_l = np.stack([s["P_l"] for s in seqs]); P_r = np.stack([s["P_r"] for s in seqs])
-    ctx.mseq_begin_ptr(seqs[0]["w"], seqs[0]["h"], lp, rp, pitch, P_l, P_r, ch, mono_rotation=a.mono_rotation)
+    if a.mixed_sizes:
+        ctx.mseq_begin_ptr([s["w"] for s in seqs], [s["h"] for s in seqs], lp, rp, pitch, P_l, P_r, ch,
+                           mono_rotation=a.mono_rotation)
+    else:
+        ctx.mseq_begin_ptr(seqs[0]["w"], seqs[0]["h"], lp, rp, pitch, P_l, P_r, ch, mono_rotation=a.mono_rotation)
     poses = [[np.eye(4)] for _ in seqs]
     aborted = [0] * len(seqs)
     steps = max(s["n"] for s in seqs)

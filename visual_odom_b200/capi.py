@@ -182,7 +182,10 @@ SIGNATURES = {
     "vo_mseq_begin_calib": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_size_t, C.c_int, C.c_int]),
     "vo_batch_calibrate": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vo_mseq_begin_sized": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     "vo_mseq_submit": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
+    "vo_mseq_submit_sized": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "vo_mseq_wait": (C.c_int, [C.c_void_p, C.POINTER(VoUnitResult), C.c_void_p, C.c_void_p, C.c_int]),
     "vo_mseq_wait_mono": (C.c_int, [C.c_void_p, C.POINTER(VoUnitResult), C.c_void_p, C.POINTER(VoMonoResult), C.c_void_p,
                                     C.c_int, C.c_void_p, C.c_int]),
@@ -701,13 +704,15 @@ class Context:
     # ---- several sequences in lockstep (vo_mseq_*) --------------------------------------------------------------------
     @staticmethod
     def _pairs(lefts, rights, allow_none):
-        """(left pointer table, right pointer table, pitch, channels, keep-alive) of one image per sequence: gray H x W or
-        BGR H x W x 3, all of one shape and pitch; a None pair (allow_none) is passed as two NULL pointers."""
+        """(left pointer table, right pointer table, pitch, channels, keep-alive, shape, shapes) of one image per sequence:
+        gray H x W or BGR H x W x 3, one channel count for all; a pair's two images have one shape, the sequences may
+        differ.  pitch is the packed row length when every shape is equal (None otherwise); shapes[q] is sequence q's
+        shape (None for a None pair, which allow_none passes as two NULL pointers)."""
         if len(lefts) != len(rights):
             raise ValueError(f"{len(lefts)} left and {len(rights)} right images")
         n = len(lefts)
         lp, rp = (C.c_void_p * n)(), (C.c_void_p * n)()
-        keep, geom = [], None
+        keep, shapes = [], [None] * n
         for q, (l, r) in enumerate(zip(lefts, rights)):
             if l is None and r is None and allow_none:
                 continue
@@ -717,22 +722,43 @@ class Context:
             if l.dtype != np.uint8 or l.ndim not in (2, 3) or (l.ndim == 3 and l.shape[2] != 3):
                 raise ValueError(f"sequence {q}: images must be uint8 H x W (gray) or H x W x 3 (BGR)")
             l = np.ascontiguousarray(l); r = np.ascontiguousarray(r)
-            if geom is None:
-                geom = l.shape
-            if l.shape != geom or r.shape != geom:
-                raise ValueError(f"sequence {q}: image shape {l.shape} / {r.shape}, expected {geom}")
+            if r.shape != l.shape:
+                raise ValueError(f"sequence {q}: image shape {l.shape} / {r.shape}, expected one shape per pair")
+            first = next((g for g in shapes if g is not None), None)
+            if first is not None and len(first) != l.ndim:
+                raise ValueError(f"sequence {q}: image shape {l.shape}, expected {'gray' if len(first) == 2 else 'BGR'} images")
+            shapes[q] = l.shape
             keep += [l, r]
             lp[q], rp[q] = l.ctypes.data, r.ctypes.data
-        if geom is None:
-            return lp, rp, 0, 1, keep, None
+        live = [g for g in shapes if g is not None]
+        if not live:
+            return lp, rp, 0, 1, keep, None, shapes
+        geom = live[0]
         ch = 1 if len(geom) == 2 else 3
-        return lp, rp, geom[1] * ch, ch, keep, geom
+        uniform = all(g == geom for g in live)
+        return lp, rp, (geom[1] * ch if uniform else None), ch, keep, (geom if uniform else None), shapes
 
     def _mseq_begin(self, n, w, h, lp, rp, pitch, ch, P_l, P_r, mono_rotation):
         """P_l / P_r (3, 4): one calibration for every sequence (vo_mseq_begin_ex); (n, 3, 4): sequence q runs with
-        P_l[q] / P_r[q] (vo_mseq_begin_calib)."""
+        P_l[q] / P_r[q] (vo_mseq_begin_calib).  w / h / pitch: one value for all, or one per sequence
+        (vo_mseq_begin_sized, which takes the calibrations per sequence)."""
         P_l = np.ascontiguousarray(P_l, np.float32); P_r = np.ascontiguousarray(P_r, np.float32)
         flags = VO_MSEQ_MONO_ROTATION if mono_rotation else 0
+        if any(np.ndim(v) > 0 for v in (w, h, pitch)):
+            ws, hs, ps = (np.broadcast_to(np.asarray(v), (n,)) for v in (w, h, pitch))
+            wa = np.ascontiguousarray(ws, np.int32); ha = np.ascontiguousarray(hs, np.int32)
+            pa = np.ascontiguousarray(ps, np.uint64)
+            if P_l.ndim == 2:
+                P_l = np.ascontiguousarray(np.broadcast_to(P_l, (n, 3, 4)))
+            if P_r.ndim == 2:
+                P_r = np.ascontiguousarray(np.broadcast_to(P_r, (n, 3, 4)))
+            if P_l.shape != (n, 3, 4) or P_r.shape != (n, 3, 4):
+                raise ValueError(f"per-sequence calibrations must be ({n}, 3, 4), got {P_l.shape} / {P_r.shape}")
+            self._check(self.lib.vo_mseq_begin_sized(self.h, n, _p(wa), _p(ha), _p(P_l), _p(P_r), lp, rp, _p(pa), ch, flags))
+            self._mseq_n, self._mseq_pitch = n, pa.copy()
+            self._mseq_sizes = [(int(a), int(b)) for a, b in zip(ha, wa)]
+            self._mseq_keep = [None, None]
+            return
         if P_l.ndim == 3 or P_r.ndim == 3:
             if P_l.shape != (n, 3, 4) or P_r.shape != (n, 3, 4):
                 raise ValueError(f"per-sequence calibrations must be ({n}, 3, 4), got {P_l.shape} / {P_r.shape}")
@@ -744,34 +770,53 @@ class Context:
         self._mseq_keep = [None, None]
 
     def mseq_begin(self, lefts, rights, P_l, P_r, mono_rotation=False):
-        """Start len(lefts) sequences (one image size) from their first stereo pairs.  P_l / P_r: (3, 4) for one calibration,
-        or (n_seq, 3, 4) for one per sequence.  mono_rotation=True: every sequence runs trackingFrame2Frame(mono_rotation =
+        """Start len(lefts) sequences from their first stereo pairs.  The sequences may differ in image size (gray or BGR
+        for all): each then runs at its own size (vo_mseq_begin_sized).  P_l / P_r: (3, 4) for one calibration, or
+        (n_seq, 3, 4) for one per sequence.  mono_rotation=True: every sequence runs trackingFrame2Frame(mono_rotation =
         true) (flag VO_MSEQ_MONO_ROTATION; see mseq_wait(mono=True))."""
-        lp, rp, pitch, ch, keep, geom = self._pairs(lefts, rights, False)
-        h, w = (geom or (0, 0))[:2]
+        lp, rp, pitch, ch, keep, geom, shapes = self._pairs(lefts, rights, False)
+        if geom is None and shapes and shapes[0] is not None:         # several sizes
+            w = [g[1] for g in shapes]; h = [g[0] for g in shapes]
+            pitch = [g[1] * ch for g in shapes]
+        else:
+            h, w = (geom or (0, 0))[:2]
         self._mseq_begin(len(lefts), w, h, lp, rp, pitch, ch, P_l, P_r, mono_rotation)
 
     def mseq_begin_ptr(self, w, h, left_ptrs, right_ptrs, pitch, P_l, P_r, channels=1, mono_rotation=False):
         """Raw host pointers, one pair per sequence (e.g. the pinned buffers of one SequenceReader each); P_l / P_r as for
-        mseq_begin."""
+        mseq_begin.  w / h / pitch: one value for every sequence, or a sequence of one per sequence (vo_mseq_begin_sized)."""
         n = len(left_ptrs)
         lp, rp = (C.c_void_p * n)(*left_ptrs), (C.c_void_p * n)(*right_ptrs)
         self._mseq_begin(n, w, h, lp, rp, pitch, channels, P_l, P_r, mono_rotation)
 
     def mseq_submit_ptr(self, left_ptrs, right_ptrs, pitch, channels=1):
-        """Raw host pointers; None in both lists retires that sequence.  The memory must stay valid until the wait."""
+        """Raw host pointers; None in both lists retires that sequence.  The memory must stay valid until the wait.
+        pitch: one row pitch for every image, or a sequence of one per sequence (vo_mseq_submit_sized)."""
         n = len(left_ptrs)
         lp, rp = (C.c_void_p * n)(*left_ptrs), (C.c_void_p * n)(*right_ptrs)
-        self._check(self.lib.vo_mseq_submit(self.h, lp, rp, pitch, channels))
+        if np.ndim(pitch) > 0:
+            pa = np.ascontiguousarray(np.broadcast_to(np.asarray(pitch), (n,)), np.uint64)
+            self._check(self.lib.vo_mseq_submit_sized(self.h, lp, rp, _p(pa), channels))
+        else:
+            self._check(self.lib.vo_mseq_submit(self.h, lp, rp, pitch, channels))
 
     def mseq_submit(self, lefts, rights):
         """Asynchronous: one frame of every sequence; a (None, None) pair retires that sequence.  At most two submissions
         in flight.  The arrays are kept alive by the context until their submission has been waited for."""
-        lp, rp, pitch, ch, keep, _ = self._pairs(lefts, rights, True)
+        lp, rp, pitch, ch, keep, geom, shapes = self._pairs(lefts, rights, True)
         if len(lefts) != getattr(self, "_mseq_n", len(lefts)):
             raise ValueError(f"{len(lefts)} pairs for {self._mseq_n} sequences")
-        # with every sequence retired no image is read: the pitch of the first pairs passes the width check
-        self._check(self.lib.vo_mseq_submit(self.h, lp, rp, pitch or self._mseq_pitch, ch))
+        if np.ndim(self._mseq_pitch) > 0:           # begun with several sizes: one packed pitch per live pair
+            for q, g in enumerate(shapes):
+                if g is not None and tuple(g[:2]) != self._mseq_sizes[q]:
+                    raise ValueError(f"sequence {q}: image shape {g}, the sequence is {self._mseq_sizes[q]}")
+            pa = np.array([g[1] * ch if g is not None else 0 for g in shapes], np.uint64)
+            self._check(self.lib.vo_mseq_submit_sized(self.h, lp, rp, _p(pa), ch))
+        else:
+            if pitch is None:
+                raise ValueError("the sequences were begun with one image size: every pair needs that shape")
+            # with every sequence retired no image is read: the pitch of the first pairs passes the width check
+            self._check(self.lib.vo_mseq_submit(self.h, lp, rp, pitch or self._mseq_pitch, ch))
         self._mseq_keep = [self._mseq_keep[1], keep]
 
     def mseq_wait(self, pts_cap=4096, want_points=True, mono=False):

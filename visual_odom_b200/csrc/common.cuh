@@ -7,6 +7,10 @@
 //   with hp_l = h_l + 2*PAD, pitch_l = roundup(w_l + 2*PAD, 64).  The u8 border is REFLECT_101
 //   filled (what OpenCV's LK pyramid pads with), the derivative border is zero (BORDER_CONSTANT),
 //   so the LK kernel needs no border logic and 3-D TMA boxes never leave the allocation.
+//   With images of several sizes in one run (PlaneGeom below), w_l / h_l are the envelope: a smaller
+//   image's u8 plane is REFLECT_101 padded at its own size over the whole envelope plane, and the
+//   derivative pass writes zeros over the envelope area outside the image, so the zero border holds
+//   whatever size the plane held before.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda.h>
@@ -31,6 +35,28 @@ struct PyrGeom {
     int n_img;
     LevelGeom lv[VO_MAX_LEVELS];
 };
+
+// One raw image plane's own size, where a run holds images of several sizes (vo_mseq_begin_sized).  The planes are then
+// allocated at the envelope (PyrGeom: the largest width and height per level), and the kernels that must see an image's
+// own border, raster or bucket grid read its entry of the context's geometry table (ctx.h vo_ctx::d_geo) instead of the
+// launch-wide size.  A null table pointer means "every plane is the launch-wide size" (every other path).
+struct PlaneGeom {
+    int w[VO_MAX_LEVELS], h[VO_MAX_LEVELS];   // image size per pyramid level: level l + 1 is ((w_l + 1) / 2, (h_l + 1) / 2)
+    int pitch;                                // raw plane row pitch in bytes (rows are packed: w[0])
+    int pad_;
+};
+
+// effective pyramid depth (maxLevel + 1) of a w x h image: OpenCV stops adding levels once one is not larger than the window
+static inline int vo_pyr_depth(int w, int h, int max_level)
+{
+    int n = 1;
+    for (int l = 1; l <= max_level; l++) {
+        const int nw = (w + 1) / 2, nh = (h + 1) / 2;
+        if (nw <= VO_WIN || nh <= VO_WIN) break;
+        w = nw; h = nh; n++;
+    }
+    return n;
+}
 
 // One camera as the triangulation, PnP and five-point kernels read it: one entry per buffer unit in the context's
 // calibration table (ctx.h vo_ctx::d_cal).  Every value is computed on the host with the expressions of the reference's

@@ -387,6 +387,7 @@ void vo_free_state(vo_ctx* ctx)
     ctx->d_feat_pts = nullptr; ctx->d_feat_ages = nullptr; ctx->d_feat_cnt = ctx->d_bucket = ctx->d_seq_err = ctx->d_seq_live = nullptr;
     ctx->d_out = nullptr; ctx->out_stride = 0; ctx->out_per = 0;
     ctx->d_cal_tab = ctx->d_cal = nullptr;
+    ctx->d_geo = nullptr;
     ctx->w = ctx->h = ctx->units = 0;
 }
 
@@ -445,10 +446,12 @@ static int encode_maps(vo_ctx* ctx)
     return VO_OK;
 }
 
-int vo_ensure_state(vo_ctx* ctx, int w, int h, int units)
+int vo_ensure_state(vo_ctx* ctx, int w, int h, int units, int levels)
 {
     if (w <= 0 || h <= 0 || units <= 0) { vo_set_error(ctx, "bad geometry %dx%d units=%d", w, h, units); return VO_E_INVALID; }
-    if (ctx->w == w && ctx->h == h && ctx->units >= units) return VO_OK;
+    const int depth = vo_pyr_depth(w, h, ctx->p.lk_max_level);
+    if (levels <= 0 || levels > depth) levels = depth;
+    if (ctx->w == w && ctx->h == h && ctx->units >= units && ctx->pg.nlevels == levels) return VO_OK;
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
     { int drc = vo_drain_pending(ctx); if (drc) return drc; }
     VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
@@ -459,12 +462,8 @@ int vo_ensure_state(vo_ctx* ctx, int w, int h, int units)
     PyrGeom& pg = ctx->pg;
     memset(&pg, 0, sizeof(pg));
     int cw = w, ch = h;
-    for (int l = 0; l <= ctx->p.lk_max_level; l++) {
-        if (l > 0) {
-            int nw = (cw + 1) / 2, nh = (ch + 1) / 2;
-            if (nw <= VO_WIN || nh <= VO_WIN) break;
-            cw = nw; ch = nh;
-        }
+    for (int l = 0; l < levels; l++) {
+        if (l > 0) { cw = (cw + 1) / 2; ch = (ch + 1) / 2; }
         LevelGeom& g = pg.lv[l];
         g.w = cw; g.h = ch;
         g.pitch = ((cw + 2 * VO_PAD) + 63) / 64 * 64;
@@ -539,15 +538,39 @@ int vo_ensure_state(vo_ctx* ctx, int w, int h, int units)
     VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_results, 0, (size_t)units * sizeof(vo_unit_result_dev), ctx->stream));
     VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_tprev, 0, (size_t)units * 3 * sizeof(double), ctx->stream));
     ctx->w = w; ctx->h = h; ctx->units = units;
+    // geometry table: every plane w x h until a run of several sizes writes its planes' entries
+    VO_CUDA_CHECK(dalloc(ctx, &ctx->d_geo, (size_t)n_img));
+    ctx->geo.assign((size_t)n_img, vo_plane_geom(ctx, w, h));
+    VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_geo, ctx->geo.data(), (size_t)n_img * sizeof(PlaneGeom), cudaMemcpyHostToDevice, ctx->stream));
     int rc = encode_maps(ctx);
     if (rc != VO_OK) { vo_free_state(ctx); return rc; }
     VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
     return VO_OK;
 }
 
+PlaneGeom vo_plane_geom(const vo_ctx* ctx, int w, int h)
+{
+    PlaneGeom g;
+    memset(&g, 0, sizeof(g));
+    for (int l = 0; l < ctx->pg.nlevels; l++) {
+        g.w[l] = w; g.h[l] = h;
+        w = (w + 1) / 2; h = (h + 1) / 2;
+    }
+    g.pitch = g.w[0];
+    return g;
+}
+
+int vo_write_geo(vo_ctx* ctx, int p0, int n, const PlaneGeom* g)
+{
+    if (memcmp(ctx->geo.data() + p0, g, n * sizeof(PlaneGeom)) == 0) return VO_OK;
+    memcpy(ctx->geo.data() + p0, g, n * sizeof(PlaneGeom));
+    VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_geo + p0, ctx->geo.data() + p0, n * sizeof(PlaneGeom), cudaMemcpyHostToDevice, ctx->stream));
+    return VO_OK;
+}
+
 // ---------------------------------------------------------------------------------------------
 // pyramids (u8 + Scharr derivative, all levels) of the raw planes [plane0, plane0 + nplanes)
-int vo_run_pyramid(vo_ctx* ctx, int plane0, int nplanes, cudaStream_t s)
+int vo_run_pyramid(vo_ctx* ctx, int plane0, int nplanes, cudaStream_t s, bool sized)
 {
     PyrGeom pg = ctx->pg;
     pg.n_img = nplanes;
@@ -555,7 +578,7 @@ int vo_run_pyramid(vo_ctx* ctx, int plane0, int nplanes, cudaStream_t s)
         pg.lv[l].img += (size_t)plane0 * pg.lv[l].plane;
         pg.lv[l].der += (size_t)plane0 * pg.lv[l].plane;
     }
-    ctx->launches += vo_launch_pyramid(pg, ctx->d_raw_tab + plane0, ctx->w, s);
+    ctx->launches += vo_launch_pyramid(pg, ctx->d_raw_tab + plane0, ctx->w, sized ? ctx->d_geo + plane0 : nullptr, s);
     VO_CUDA_CHECK(cudaGetLastError());
     return VO_OK;
 }
@@ -584,6 +607,7 @@ int vo_run_lk_ring(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, 
     for (int c = 0; c < ncalls; c++) { a.img_prev[c] = img_prev[c]; a.img_next[c] = img_next[c]; }
     a.nlevels = pg.nlevels;
     for (int l = 0; l < pg.nlevels; l++) { a.lw[l] = pg.lv[l].w; a.lh[l] = pg.lv[l].h; }
+    a.geo = v.sized ? ctx->d_geo : nullptr;
     a.max_iters = ctx->p.lk_max_iters;
     double eps = ctx->p.lk_epsilon;
     if (eps < 0.) eps = 0.; if (eps > 10.) eps = 10.;
@@ -677,6 +701,7 @@ int vo_run_fast(vo_ctx* ctx, const View& v, int plane_in_unit, bool want_resp)
     a.corners = ctx->d_corners + (size_t)v.u0 * ctx->corner_cap;
     a.resp = want_resp ? ctx->d_resp + (size_t)v.u0 * ctx->corner_cap : nullptr;
     a.corner_cap = ctx->corner_cap;
+    a.geo = v.sized ? ctx->d_geo + (a.img_tab - ctx->d_raw_tab) : nullptr;
     ctx->launches += vo_launch_fast(a, v.s);
     VO_CUDA_CHECK(cudaGetLastError());
     return VO_OK;

@@ -23,6 +23,7 @@ struct GraphKey {
     cudaStream_t s;
     bool tma;
     int u0, n, max_pts; bool detect;        // BATCH_RANGE: the unit range, its feature bound, on-GPU detection
+                                            // (SEQ_FRONT: max_pts = the LK launch bound, the sequences' largest bucket grid)
     int slot, parity; bool bgr;             // SEQ_FRONT / SEQ_BACK: image slot of the previous pairs, buffer parity, colour input
 };
 
@@ -46,9 +47,14 @@ struct vo_ctx {
     CamCalib* d_cal_tab = nullptr;      // [1 + units]
     CamCalib* d_cal = nullptr;          // d_cal_tab + 1: indexed by buffer unit
     std::vector<CamCalib> cal;          // [1 + units] host copy (kept across re-allocations of the batch state)
+    // geometry table (the same life as d_cal_tab): one entry per raw image plane, its own size per level and raw pitch.
+    // w / h above are then the envelope of the sizes; only runs of several sizes (vo_mseq_begin_sized) point kernels at
+    // it, every other path uses the launch-wide sizes.  Entries start out as w x h.  geo mirrors it.
+    PlaneGeom* d_geo = nullptr;         // [units * 4]
+    std::vector<PlaneGeom> geo;
 
     // ---- device buffers ---------------------------------------------------------------------
-    uint8_t* d_raw = nullptr;           // [units*4][h*w] raw images
+    uint8_t* d_raw = nullptr;           // [units*4][h*w] raw images (a smaller image: its own rows packed from the plane start)
     const uint8_t** d_raw_tab = nullptr;// [units*4] pointers into d_raw
     vo_dimage* d_ingest_tab = nullptr;  // [units*4] descriptors of caller device images, per raw plane (staged per submission)
     float2* d_pts_in = nullptr;         // [units][cap]
@@ -97,6 +103,8 @@ struct vo_ctx {
     bool seq_active = false;
     bool seq_multi = false;             // begun with vo_mseq_begin (the vo_seq_* frame calls are refused, and vice versa)
     int seq_n = 1;                      // sequences of the running sequence mode
+    bool seq_sized = false;             // the sequences' image sizes differ (planes are envelope-sized, kernels read d_geo)
+    std::vector<int> seq_w, seq_h;      // [seq_n] each sequence's image size
     int seq_slot = 0;                   // image slot holding the previous stereo pairs: raw/pyramid planes
                                         // 2 * seq_n * slot + 2q (left), + 1 (right) of sequence q
     int seq_inflight = 0;               // frames submitted and not yet waited for (<= 2)
@@ -200,7 +208,12 @@ struct vo_ctx {
 };
 
 void vo_set_error(vo_ctx* ctx, const char* fmt, ...);
-int vo_ensure_state(vo_ctx* ctx, int w, int h, int units);
+// levels > 0: that pyramid depth (the common depth of a run's image sizes, which their envelope w x h may exceed)
+int vo_ensure_state(vo_ctx* ctx, int w, int h, int units, int levels = 0);
+// geometry table entries [p0, p0 + n) = g[0 .. n), written on ctx->stream only where they change (as vo_write_calib)
+int vo_write_geo(vo_ctx* ctx, int p0, int n, const PlaneGeom* g);
+// the geometry of a w x h image in the allocated pyramid's levels (raw rows packed)
+PlaneGeom vo_plane_geom(const vo_ctx* ctx, int w, int h);
 void vo_free_state(vo_ctx* ctx);
 void vo_drop_graphs(vo_ctx* ctx);
 // replays the graph cached for `key` on key.s, or captures what `launch` enqueues there, caches and replays it (plain
@@ -231,9 +244,9 @@ int vo_ensure_pinned(vo_ctx* ctx, size_t bytes);
 int vo_upload_plane(vo_ctx* ctx, uint8_t* dst, const uint8_t* src, size_t row_bytes, int h, size_t pitch, cudaStream_t st);
 int vo_ensure_bgr(vo_ctx* ctx, size_t bytes);
 // k_bgr_to_gray: images tab[0 .. n_img) (device table), or with d_tab == nullptr `packed` advanced by packed_stride per image,
-// into gray planes img_stride_out apart
+// into gray planes img_stride_out apart; geo: the images' geometry table entries (packed input only; nullptr: all w x h)
 int vo_launch_bgr_to_gray(const vo_dimage* d_tab, const vo_dimage& packed, size_t packed_stride, uint8_t* d_gray, size_t img_stride_out,
-                          int w, int h, int n_img, cudaStream_t s);
+                          int w, int h, int n_img, cudaStream_t s, const PlaneGeom* geo = nullptr);
 vo_dimage vo_packed_bgr(const uint8_t* d_bgr, int w);      // the descriptor of w-pixel packed BGR rows
 // VO_E_INVALID + message unless `im` can be read as an image `w` pixels wide in device memory of the context's GPU
 int vo_check_dimage(vo_ctx* ctx, const char* who, const char* name, const vo_dimage* im, int w);
@@ -245,10 +258,12 @@ int vo_ingest_device(vo_ctx* ctx, const vo_dimage* h_tab, int n, int plane0, cud
 // between two buffer parities while both address the same image ring.  imgs: image planes per unit (4: a stereo pair at
 // t0 and t1; 2: one LK call, or one sequence's pair in the sequence mode).  max_pts: live features per unit at most
 // (0 = cap), which sizes the LK launch.
-struct View { int u0, n; cudaStream_t s; int plane0 = -1; int imgs = 4; int max_pts = 0; };
+// sized: the image planes hold images of several sizes; FAST and the LK ring read each one's from the geometry table.
+struct View { int u0, n; cudaStream_t s; int plane0 = -1; int imgs = 4; int max_pts = 0; bool sized = false; };
 // run pyramids + LK (ncalls chained) for the units of `v`; images must already be in d_raw/d_raw_tab
 int vo_run_lk(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, const int* img_next, bool want_err);
-int vo_run_pyramid(vo_ctx* ctx, int plane0, int nplanes, cudaStream_t s);
+// sized: the planes hold images of several sizes, read from the geometry table (vo_mseq_begin_sized)
+int vo_run_pyramid(vo_ctx* ctx, int plane0, int nplanes, cudaStream_t s, bool sized = false);
 int vo_run_lk_ring(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, const int* img_next, bool want_err);
 int vo_run_filter(vo_ctx* ctx, const View& v, bool with_ages);
 // FAST on raw plane `plane_in_unit` of each unit -> d_corners / d_ndet ; stride selection -> d_pts_in / d_npts

@@ -20,9 +20,12 @@
 #include "common.cuh"
 #include "fast.h"
 
+// With a geometry table (geo[unit * img_stride_idx]: images of several sizes) every kernel takes the image's own size for
+// its border, raster and score map; w / h are then the envelope and only lay out the per-row buffers.
 __global__ void __launch_bounds__(256) k_fast_score(const uint8_t* const* __restrict__ img_tab, int img_stride_idx,
                                                     int w, int h, int pitch, int threshold, int nonmax,
-                                                    uint8_t* __restrict__ score, size_t score_plane)
+                                                    uint8_t* __restrict__ score, size_t score_plane,
+                                                    const PlaneGeom* __restrict__ geo)
 {
     // the 16-pixel Bresenham ring, compile-time: the unrolled loop below folds the offsets into immediates
     constexpr int ring_dx[16] = {0, 1, 2, 3, 3, 3, 2, 1, 0, -1, -2, -3, -3, -3, -2, -1};
@@ -30,6 +33,7 @@ __global__ void __launch_bounds__(256) k_fast_score(const uint8_t* const* __rest
     const int unit = blockIdx.z;
     const uint8_t* __restrict__ img = img_tab[unit * img_stride_idx];
     uint8_t* __restrict__ sc = score + (size_t)unit * score_plane;
+    if (geo) { const PlaneGeom& g = geo[unit * img_stride_idx]; w = g.w[0]; h = g.h[0]; pitch = g.pitch; }
     const int x = blockIdx.x * 32 + (threadIdx.x & 31);
     const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
     if (x >= w || y >= h) return;
@@ -82,29 +86,32 @@ __global__ void __launch_bounds__(256) k_fast_score(const uint8_t* const* __rest
 #define NMS_NC 8                 // chunks of NMS_T pixels handled per pass: one pass covers rows up to 2048 pixels
 __global__ void __launch_bounds__(NMS_T) k_fast_nms_row(const uint8_t* __restrict__ score, size_t score_plane, int w, int h,
                                                         int nonmax, uint16_t* __restrict__ rowbuf, int rowcap,
-                                                        int* __restrict__ rowcount)
+                                                        int* __restrict__ rowcount, const PlaneGeom* __restrict__ geo,
+                                                        int geo_stride)
 {
     const int y = blockIdx.x, unit = blockIdx.y;
+    int iw = w, ih = h;                                 // the image's own size (h lays out the row buffers)
+    if (geo) { iw = geo[unit * geo_stride].w[0]; ih = geo[unit * geo_stride].h[0]; }
     const uint8_t* __restrict__ sc = score + (size_t)unit * score_plane;
     uint16_t* __restrict__ out = rowbuf + ((size_t)unit * h + y) * rowcap;
     __shared__ uint8_t rows[3][NMS_T * NMS_NC + 2];
     __shared__ int wcnt[NMS_NC * (NMS_T / 32)];         // survivors per (chunk, warp), then their exclusive prefix
     __shared__ int base;
-    if (y < 3 || y >= h - 3) {                     // border rows hold no corners
+    if (y < 3 || y >= ih - 3) {                    // border rows (and rows below the image) hold no corners
         if (threadIdx.x == 0) rowcount[unit * h + y] = 0;
         return;
     }
     if (threadIdx.x == 0) base = 0;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     constexpr int NW = NMS_T / 32, SPAN = NMS_T * NMS_NC;
-    for (int x0 = 0; x0 < w; x0 += SPAN) {
+    for (int x0 = 0; x0 < iw; x0 += SPAN) {
         // stage the three score rows (with a 1-pixel halo) in shared memory: the whole pass at once
         for (int i = threadIdx.x; i < SPAN + 2; i += NMS_T) {
             const int x = x0 - 1 + i;
-            const bool in = (x >= 0 && x < w);
-            rows[0][i] = in ? sc[(size_t)(y - 1) * w + x] : 0;
-            rows[1][i] = in ? sc[(size_t)y * w + x] : 0;
-            rows[2][i] = in ? sc[(size_t)(y + 1) * w + x] : 0;
+            const bool in = (x >= 0 && x < iw);
+            rows[0][i] = in ? sc[(size_t)(y - 1) * iw + x] : 0;
+            rows[1][i] = in ? sc[(size_t)y * iw + x] : 0;
+            rows[2][i] = in ? sc[(size_t)(y + 1) * iw + x] : 0;
         }
         __syncthreads();
         unsigned bal[NMS_NC];
@@ -112,7 +119,7 @@ __global__ void __launch_bounds__(NMS_T) k_fast_nms_row(const uint8_t* __restric
         for (int c = 0; c < NMS_NC; c++) {
             const int x = x0 + c * NMS_T + threadIdx.x, i = c * NMS_T + threadIdx.x + 1;
             bool keep = false;
-            if (x < w) {
+            if (x < iw) {
                 const int s = rows[1][i];
                 if (s > 0) {
                     keep = !nonmax ||
@@ -197,9 +204,11 @@ __global__ void __launch_bounds__(1024) k_fast_scan(const int* __restrict__ rowc
 __global__ void __launch_bounds__(128) k_fast_gather(const uint16_t* __restrict__ rowbuf, int rowcap,
                                                      const int* __restrict__ rowcount, const int* __restrict__ rowoff,
                                                      int h, const uint8_t* __restrict__ score, size_t score_plane, int w,
-                                                     int nonmax, float2* __restrict__ out, float* __restrict__ resp, int cap)
+                                                     int nonmax, float2* __restrict__ out, float* __restrict__ resp, int cap,
+                                                     const PlaneGeom* __restrict__ geo, int geo_stride)
 {
     const int y = blockIdx.x, unit = blockIdx.y;
+    if (geo) w = geo[unit * geo_stride].w[0];           // the score map's row length
     const int n = rowcount[unit * h + y], off = rowoff[unit * h + y];
     const uint16_t* src = rowbuf + ((size_t)unit * h + y) * rowcap;
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
@@ -235,12 +244,13 @@ int vo_launch_fast(const FastArgs& a, cudaStream_t stream)
 {
     dim3 g1((a.w + 31) / 32, (a.h + 7) / 8, a.n_units);
     k_fast_score<<<g1, 256, 0, stream>>>(a.img_tab, a.img_stride_idx, a.w, a.h, a.pitch, a.threshold, a.nonmax, a.score,
-                                          a.score_plane);
+                                          a.score_plane, a.geo);
     dim3 g2(a.h, a.n_units);
-    k_fast_nms_row<<<g2, NMS_T, 0, stream>>>(a.score, a.score_plane, a.w, a.h, a.nonmax, a.rowbuf, a.rowcap, a.rowcount);
+    k_fast_nms_row<<<g2, NMS_T, 0, stream>>>(a.score, a.score_plane, a.w, a.h, a.nonmax, a.rowbuf, a.rowcap, a.rowcount, a.geo,
+                                              a.img_stride_idx);
     k_fast_scan<<<a.n_units, 1024, 0, stream>>>(a.rowcount, a.h, a.rowoff, a.n_det);
     k_fast_gather<<<g2, 128, 0, stream>>>(a.rowbuf, a.rowcap, a.rowcount, a.rowoff, a.h, a.score, a.score_plane, a.w,
-                                           a.nonmax, a.corners, a.resp, a.corner_cap);
+                                           a.nonmax, a.corners, a.resp, a.corner_cap, a.geo, a.img_stride_idx);
     return 4;
 }
 

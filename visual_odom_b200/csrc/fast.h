@@ -18,6 +18,8 @@ struct FastArgs {
     float2* corners;                 // [units][corner_cap]
     float* resp;                     // optional [units][corner_cap]
     int corner_cap;
+    const PlaneGeom* geo;            // geometry table entries of the images, indexed like img_tab (nullptr: all w x h); w / h
+                                     // are then the envelope, which lays out score, rowbuf, rowcount and rowoff
 };
 
 int vo_launch_fast(const FastArgs& a, cudaStream_t stream);

@@ -348,13 +348,16 @@ extern "C" void vo_reader_close(vo_reader* rd)
 // `packed` advanced by z * packed_stride (the packed BGR staging of host colour input, whose graph-captured launch
 // cannot take a per-frame table).  Sources may have any alignment, pitch and strides: every pixel is read with byte
 // loads.  Colour: cv::cvtColor(BGR2GRAY / RGB2GRAY)'s fixed point; gray: the identity (which the formula is on b=g=r).
+// With a geometry table (geo[img]: images of several sizes, w x h the envelope) image z is geo[z]'s own size, its packed
+// source rows 3 * w[0] bytes apart and its gray rows w[0].
 __global__ void k_bgr_to_gray(const vo_dimage* __restrict__ tab, vo_dimage packed, size_t packed_stride, uint8_t* __restrict__ gray,
-                              size_t img_stride_out, int w, int h)
+                              size_t img_stride_out, int w, int h, const PlaneGeom* __restrict__ geo)
 {
     const int img = blockIdx.z, y = blockIdx.y;
     const int x0 = 4 * (blockIdx.x * blockDim.x + threadIdx.x);
-    if (x0 >= w) return;
     vo_dimage src = packed;
+    if (geo) { w = geo[img].w[0]; h = geo[img].h[0]; src.row_pitch = (size_t)3 * w; }
+    if (x0 >= w || y >= h) return;
     if (tab) src = tab[img];
     else src.data += (size_t)img * packed_stride;
     const uint8_t* s = src.data + (size_t)y * src.row_pitch + (size_t)x0 * src.pixel_stride;
@@ -380,10 +383,10 @@ __global__ void k_bgr_to_gray(const vo_dimage* __restrict__ tab, vo_dimage packe
 }
 
 int vo_launch_bgr_to_gray(const vo_dimage* d_tab, const vo_dimage& packed, size_t packed_stride, uint8_t* d_gray, size_t img_stride_out,
-                          int w, int h, int n_img, cudaStream_t s)
+                          int w, int h, int n_img, cudaStream_t s, const PlaneGeom* geo)
 {
     dim3 grid(((w + 3) / 4 + 127) / 128, h, n_img);
-    k_bgr_to_gray<<<grid, 128, 0, s>>>(d_tab, packed, packed_stride, d_gray, img_stride_out, w, h);
+    k_bgr_to_gray<<<grid, 128, 0, s>>>(d_tab, packed, packed_stride, d_gray, img_stride_out, w, h, geo);
     return 1;
 }
 

@@ -220,7 +220,9 @@ __device__ __forceinline__ float combine_chains(float acc)
 } // namespace
 
 // ---------------------------------------------------------------------------------------------
-template <bool USE_TMA>
+// SIZED: the units' images have sizes of their own (args.geo); the other instantiation is the launch-wide-size kernel
+// exactly, so runs of one image size pay nothing for the table
+template <bool USE_TMA, bool SIZED>
 __global__ void __launch_bounds__(LK_WARPS_PER_CTA * 32, LK_CTAS_PER_SM)
 k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
 {
@@ -310,7 +312,8 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
             const int img_prev = args.img_plane0 + unit * args.imgs_per_unit + args.img_prev[call];
             const int img_next = args.img_plane0 + unit * args.imgs_per_unit + args.img_next[call];
             do {                                // one level-solve; `break` = the reference's `continue`
-                const int lw = args.lw[level], lh = args.lh[level];
+                int lw = args.lw[level], lh = args.lh[level];
+                if (SIZED) { lw = __ldg(&args.geo[img_prev].w[level]); lh = __ldg(&args.geo[img_prev].h[level]); }
                 const float sc = 1.f / (float)(1 << level);
                 float px = pt.x * sc, py = pt.y * sc;
                 if (level == max_level) { nxt.x = px; nxt.y = py; }
@@ -641,16 +644,18 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
 // ---------------------------------------------------------------------------------------------
 size_t vo_lk_smem_bytes() { return sizeof(WarpSmem) * LK_WARPS_PER_CTA; }
 
-template <bool T>
+template <bool T, bool S>
 static cudaError_t prep()
 {
-    return cudaFuncSetAttribute(k_lk_ring<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)vo_lk_smem_bytes());
+    return cudaFuncSetAttribute(k_lk_ring<T, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)vo_lk_smem_bytes());
 }
 
 cudaError_t vo_lk_prepare()
 {
-    cudaError_t e = prep<false>();
-    return e != cudaSuccess ? e : prep<true>();
+    cudaError_t e = prep<false, false>();
+    if (e == cudaSuccess) e = prep<true, false>();
+    if (e == cudaSuccess) e = prep<false, true>();
+    return e != cudaSuccess ? e : prep<true, true>();
 }
 
 cudaError_t vo_launch_lk_ring(const LkMaps& maps, const LkArgs& args, int sm_count, cudaStream_t stream)
@@ -662,7 +667,10 @@ cudaError_t vo_launch_lk_ring(const LkMaps& maps, const LkArgs& args, int sm_cou
     if (ctas > resident) ctas = resident;
     const int thr = LK_WARPS_PER_CTA * 32;
     const size_t sh = vo_lk_smem_bytes();
-    if (args.use_tma) k_lk_ring<true><<<(int)ctas, thr, sh, stream>>>(maps, args);
-    else k_lk_ring<false><<<(int)ctas, thr, sh, stream>>>(maps, args);
+    if (args.geo) {
+        if (args.use_tma) k_lk_ring<true, true><<<(int)ctas, thr, sh, stream>>>(maps, args);
+        else k_lk_ring<false, true><<<(int)ctas, thr, sh, stream>>>(maps, args);
+    } else if (args.use_tma) k_lk_ring<true, false><<<(int)ctas, thr, sh, stream>>>(maps, args);
+    else k_lk_ring<false, false><<<(int)ctas, thr, sh, stream>>>(maps, args);
     return cudaGetLastError();
 }

@@ -23,6 +23,7 @@ struct LkArgs {
     int img_next[4];        // plane index of next image per call
     int nlevels;            // pyramid images (effective maxLevel + 1)
     int lw[VO_MAX_LEVELS], lh[VO_MAX_LEVELS];
+    const PlaneGeom* geo;   // geometry table indexed by absolute plane (images of several sizes), or nullptr = lw / lh
     int max_iters;          // 30
     double eps2;            // epsilon^2 (0.01^2)
     double min_eig;         // 1e-3
@@ -49,4 +50,4 @@ size_t vo_lk_smem_bytes();
 cudaError_t vo_lk_prepare();
 // sm_count sizes the persistent grid (CTAs = min(needed, sm_count * LK_CTAS_PER_SM))
 cudaError_t vo_launch_lk_ring(const LkMaps& maps, const LkArgs& args, int sm_count, cudaStream_t stream);
-int vo_launch_pyramid(const PyrGeom& pg, const uint8_t* const* src_tab_dev, int src_pitch, cudaStream_t stream);
+int vo_launch_pyramid(const PyrGeom& pg, const uint8_t* const* src_tab_dev, int src_pitch, const PlaneGeom* geo, cudaStream_t stream);

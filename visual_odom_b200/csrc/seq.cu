@@ -45,9 +45,13 @@ __global__ void __launch_bounds__(1024) k_seq_bucket(const float2* __restrict__ 
                                                      int feat_cap, const int* __restrict__ cnt, int rows, int cols, int bucket_size,
                                                      int* bucket /* [nb] scratch */, int nb_cap,
                                                      float2* out_pts, int* out_ages, int* out_n, int out_cap, int* err,
-                                                     const int* __restrict__ live)
+                                                     const int* __restrict__ live, const PlaneGeom* __restrict__ geo, int geo_stride)
 {
     const int q = blockIdx.y;
+    if (geo) {             // the sequence's own grid: the stride-nw aliasing below depends on nw
+        rows = geo[q * geo_stride].h[0]; cols = geo[q * geo_stride].w[0];
+        bucket_size = rows / 10;
+    }
     feat_pts += (size_t)q * feat_cap; feat_ages += (size_t)q * feat_cap; cnt += 2 * q; bucket += (size_t)q * nb_cap;
     out_pts += (size_t)q * out_cap; out_ages += (size_t)q * out_cap; out_n += q; err += q;
     if (!live[q]) { if (threadIdx.x == 0) *out_n = 0; return; }        // retired: no features, so no work downstream
@@ -156,7 +160,8 @@ int vo_launch_seq_append(const SeqArgs& a, int n_seq, cudaStream_t s)
 int vo_launch_seq_bucket(const SeqArgs& a, int n_seq, cudaStream_t s)
 {
     k_seq_bucket<<<dim3(1, n_seq), 1024, 0, s>>>(a.feat_pts, a.feat_ages, a.feat_cap, a.cnt, a.rows, a.cols, a.bucket_size,
-                                                 a.bucket, a.bucket_cap, a.out_pts, a.out_ages, a.out_n, a.out_cap, a.err, a.live);
+                                                 a.bucket, a.bucket_cap, a.out_pts, a.out_ages, a.out_n, a.out_cap, a.err, a.live,
+                                                 a.geo, a.geo_stride);
     return 1;
 }
 int vo_launch_seq_carry(const SeqArgs& a, int n_seq, cudaStream_t s)

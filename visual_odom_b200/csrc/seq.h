@@ -13,6 +13,8 @@ struct SeqArgs {
     float2* feat_pts; int* feat_ages; int* cnt /* [2]: points, ages */; int feat_cap; int refill_below;
     // bucketing
     int rows, cols, bucket_size; int* bucket; int bucket_cap;
+    // images of several sizes: sequence q's rows / cols (and bucket_size = rows / 10) are those of geo[q * geo_stride]
+    const PlaneGeom* geo; int geo_stride;
     float2* out_pts; int* out_ages; int* out_n; int out_cap;
     // update
     const float2* valid_l1; const int* n5; const int* ages_out; const int* n3;

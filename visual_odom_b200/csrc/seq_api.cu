@@ -14,12 +14,17 @@
 // nor the previous frame reads, so the H2D of frame k+1 also runs under the kernels of frame k (double-buffered
 // upload).  Each stage is one CUDA graph (per image-slot pair / buffer unit / input format).
 //
-// vo_mseq_* runs n_seq independent sequences of one image size (each with its own calibration: the kernels read unit u's
-// camera from the calibration table, and sequence q's entries are those of units q and n_seq + q) in lockstep through the same two stages:
+// vo_mseq_* runs n_seq independent sequences (each with its own calibration: the kernels read unit u's camera from the
+// calibration table, and sequence q's entries are those of units q and n_seq + q; and each with its own image size:
+// vo_mseq_begin_sized) in lockstep through the same two stages:
 // every stage kernel takes the n_seq units of a buffer parity (sequence q at parity p is unit p * n_seq + q) in ONE launch,
 // and vo_seq_* is the same code with n_seq = 1.  The image ring is slot-major: slot s holds the pairs of all sequences,
 // planes 2 * n_seq * s + 2q (left) and + 1 (right), so the new pairs of a frame are one contiguous run of planes (one
 // pyramid launch, one BGR conversion) and FAST / the LK ring address sequence q's planes with an image stride of 2.
+// Sequences of several image sizes share planes allocated at the envelope of the sizes (the largest width and height);
+// each image's rows are packed from its plane's start, the geometry table (vo_ctx::d_geo) holds every plane's own size,
+// and the pyramid, FAST, LK ring, BGR conversion and bucketing kernels read it (View::sized, SeqArgs::geo).  The table
+// lives with the batch state, so the frame graphs carry no sizes; with one size the kernels take no table at all.
 //
 // With the option "mono_rotation" (vo_seq_*) or the flag VO_MSEQ_MONO_ROTATION (vo_mseq_begin_ex) -- trackingFrame2Frame's
 // header default, reference src/visualOdometry.cpp:146-157 -- the front stage also forks the essential-matrix RANSAC +
@@ -30,15 +35,18 @@
 // (k_seq_mono); rvec / tvec / inliers stay the PnP's.
 #include "ctx.h"
 #include <string.h>
+#include <algorithm>
 
 // the new host pairs of image slot `slot` (sequence q: lefts[q], rights[q]; a NULL pair is skipped): gray into the raw
 // planes, colour (BGR) bytes into the staging area, converted inside the frame's graph
-static int upload_pairs(vo_ctx* ctx, int slot, const uint8_t* const* lefts, const uint8_t* const* rights, size_t pitch, int channels,
-                        cudaStream_t st)
+// planes (a staging image holds an envelope plane's pixels); every image goes with its own rows of its own width, pitch[q]
+// bytes apart in host memory
+static int upload_pairs(vo_ctx* ctx, int slot, const uint8_t* const* lefts, const uint8_t* const* rights, const size_t* pitch,
+                        int channels, cudaStream_t st)
 {
-    const int w = ctx->w, h = ctx->h, n = ctx->seq_n;
-    const size_t img = (size_t)channels * w * h;
-    uint8_t* dst = ctx->d_raw + (size_t)(2 * n * slot) * w * h;
+    const int n = ctx->seq_n;
+    const size_t img = (size_t)channels * ctx->w * ctx->h;
+    uint8_t* dst = ctx->d_raw + (size_t)(2 * n * slot) * ctx->w * ctx->h;
     int rc;
     if (channels == 3) {
         if ((rc = vo_ensure_bgr(ctx, 2 * (size_t)n * img))) return rc;
@@ -48,7 +56,8 @@ static int upload_pairs(vo_ctx* ctx, int slot, const uint8_t* const* lefts, cons
         if (!lefts[q]) continue;
         const uint8_t* imgs[2] = {lefts[q], rights[q]};
         for (int k = 0; k < 2; k++)
-            if ((rc = vo_upload_plane(ctx, dst + (2 * q + k) * img, imgs[k], (size_t)channels * w, h, pitch, st))) return rc;
+            if ((rc = vo_upload_plane(ctx, dst + (2 * q + k) * img, imgs[k], (size_t)channels * ctx->seq_w[q], ctx->seq_h[q], pitch[q], st)))
+                return rc;
     }
     return VO_OK;
 }
@@ -58,7 +67,7 @@ static int convert_pairs(vo_ctx* ctx, int slot)
 {
     const int w = ctx->w, h = ctx->h, n = ctx->seq_n;
     ctx->launches += vo_launch_bgr_to_gray(nullptr, vo_packed_bgr(ctx->d_bgr, w), (size_t)3 * w * h, ctx->d_raw + (size_t)(2 * n * slot) * w * h,
-                                           (size_t)w * h, w, h, 2 * n, ctx->stream);
+                                           (size_t)w * h, w, h, 2 * n, ctx->stream, ctx->seq_sized ? ctx->d_geo + 2 * n * slot : nullptr);
     VO_CUDA_CHECK(cudaGetLastError());
     return VO_OK;
 }
@@ -73,6 +82,7 @@ static void seq_args(vo_ctx* ctx, int p, SeqArgs& a)
     a.feat_pts = ctx->d_feat_pts; a.feat_ages = ctx->d_feat_ages; a.cnt = ctx->d_feat_cnt; a.feat_cap = ctx->feat_cap;
     a.refill_below = 2000;                                   // visualOdometry.cpp:95
     a.rows = ctx->h; a.cols = ctx->w; a.bucket_size = ctx->h / 10;      // visualOdometry.cpp:106 (features_per_bucket = 1)
+    a.geo = ctx->seq_sized ? ctx->d_geo : nullptr; a.geo_stride = 2;    // sequence q: plane 2q (image slot 0)
     a.bucket = ctx->d_bucket; a.bucket_cap = ctx->bucket_cap;
     a.out_pts = ctx->d_pts_in + uo; a.out_ages = ctx->d_ages_in + uo; a.out_n = ctx->d_npts + u0; a.out_cap = ctx->cap;
     a.valid_l1 = ctx->d_valid4 + 2 * cs + uo; a.n5 = ctx->d_n5 + u0; a.ages_out = ctx->d_ages_out + uo; a.n3 = ctx->d_n3 + u0;
@@ -84,11 +94,17 @@ static void seq_args(vo_ctx* ctx, int p, SeqArgs& a)
 }
 
 // bucketingFeatures() reads back (rows/bs + 1) x (cols/bs + 1) slots at most (feature.cpp:242-249): the bound of every
-// per-frame point count
+// per-frame point count (the largest over the sequences' sizes)
+static int seq_grid(int w, int h)
+{
+    const int bs = h / 10 > 0 ? h / 10 : 1;
+    return (h / bs + 1) * (w / bs + 1);
+}
 static int seq_grid(const vo_ctx* ctx)
 {
-    const int bs = ctx->h / 10 > 0 ? ctx->h / 10 : 1;
-    return (ctx->h / bs + 1) * (ctx->w / bs + 1);
+    int g = 0;
+    for (int q = 0; q < ctx->seq_n; q++) g = std::max(g, seq_grid(ctx->seq_w[q], ctx->seq_h[q]));
+    return g;
 }
 
 // the mono branch of buffer units unit .. unit + n_prob - 1 (one problem each): pointsLeft_t0 / pointsLeft_t1 = the
@@ -131,11 +147,11 @@ static int seq_front(vo_ctx* ctx, int s0, int s1, int p, bool bgr)
     const int n = ctx->seq_n, unit = p * n;
     const int L0 = 2 * n * s0, R0 = L0 + 1, L1 = 2 * n * s1, R1 = L1 + 1;
     // image planes are addressed from plane 0 whatever the parity; sequence q's pair of a slot is planes 2q, 2q + 1 of it
-    const View v{unit, n, ctx->stream, 0, 2, seq_grid(ctx)};
+    const View v{unit, n, ctx->stream, 0, 2, seq_grid(ctx), ctx->seq_sized};
     int rc;
     if (bgr && (rc = convert_pairs(ctx, s1))) return rc;
     // the new pairs' pyramids (the previous pairs' are already resident)
-    if ((rc = vo_run_pyramid(ctx, L1, 2 * n, ctx->stream))) return rc;
+    if ((rc = vo_run_pyramid(ctx, L1, 2 * n, ctx->stream, ctx->seq_sized))) return rc;
     // matchingFeatures(): FAST refill on the t0 left image -> bucketing -> circular matching -> filters
     if ((rc = vo_run_fast(ctx, v, L0, false))) return rc;
     SeqArgs a;
@@ -237,33 +253,39 @@ static int seq_drain(vo_ctx* ctx)
     return VO_OK;
 }
 
-// where the new pairs of a begin or submit call come from: host images (gray or BGR, `pitch` bytes per row; in a
-// multi-sequence submission a NULL pair retires its sequence) or one device pair (vo_seq_*_device)
+// where the new pairs of a begin or submit call come from: host images (gray or BGR, sequence q's pitch[q] bytes per row;
+// in a multi-sequence submission a NULL pair retires its sequence) or one device pair (vo_seq_*_device)
 struct SeqPairs {
-    const uint8_t* const* lefts; const uint8_t* const* rights; size_t pitch; int channels;
+    const uint8_t* const* lefts; const uint8_t* const* rights; const size_t* pitch; int channels;
     bool device; const vo_dimage* dl; const vo_dimage* dr;
     bool bgr() const { return !device && channels == 3; }
 };
-static SeqPairs host_pairs(const uint8_t* const* lefts, const uint8_t* const* rights, size_t pitch, int channels)
+static SeqPairs host_pairs(const uint8_t* const* lefts, const uint8_t* const* rights, const size_t* pitch, int channels)
 {
     return SeqPairs{lefts, rights, pitch, channels, false, nullptr, nullptr};
 }
-static SeqPairs device_pair(const vo_dimage* left, const vo_dimage* right) { return SeqPairs{nullptr, nullptr, 0, 1, true, left, right}; }
+static SeqPairs device_pair(const vo_dimage* left, const vo_dimage* right) { return SeqPairs{nullptr, nullptr, nullptr, 1, true, left, right}; }
 
-// the new pairs' own checks (w: the image width; begin: the first pairs, which every sequence needs)
-static int seq_pairs_check(vo_ctx* ctx, const char* who, bool multi, int n, int w, const SeqPairs& in, bool begin)
+// the new pairs' own checks (w[q]: sequence q's image width; begin: the first pairs, which every sequence needs).  A pitch
+// is checked only where a pair is read: a retiring sequence's is not.
+static int seq_pairs_check(vo_ctx* ctx, const char* who, bool multi, int n, const int* w, const SeqPairs& in, bool begin)
 {
     int rc;
     if (in.device) {
-        if ((rc = vo_check_dimage(ctx, who, begin ? "left0" : "left1", in.dl, w)) ||
-            (rc = vo_check_dimage(ctx, who, begin ? "right0" : "right1", in.dr, w))) return rc;
+        if ((rc = vo_check_dimage(ctx, who, begin ? "left0" : "left1", in.dl, w[0])) ||
+            (rc = vo_check_dimage(ctx, who, begin ? "right0" : "right1", in.dr, w[0]))) return rc;
         return VO_OK;
     }
     if (in.channels != 1 && in.channels != 3) { vo_set_error(ctx, "%s: channels must be 1 (gray) or 3 (BGR)", who); return VO_E_INVALID; }
-    if (!in.lefts || !in.rights || in.pitch < (size_t)w * in.channels || (!multi && (!in.lefts[0] || !in.rights[0]))) {
+    if (!in.lefts || !in.rights || !in.pitch || (!multi && (!in.lefts[0] || !in.rights[0]))) {
         vo_set_error(ctx, "%s: bad argument", who);
         return VO_E_INVALID;
     }
+    for (int q = 0; q < n; q++)
+        if (in.lefts[q] && in.pitch[q] < (size_t)w[q] * in.channels) {
+            vo_set_error(ctx, "%s: bad argument (sequence %d: pitch %zu < %d pixels x %d channel(s))", who, q, in.pitch[q], w[q], in.channels);
+            return VO_E_INVALID;
+        }
     for (int q = 0; multi && q < n; q++) {
         const bool l = in.lefts[q] != nullptr, r = in.rights[q] != nullptr;
         if (begin && !(l && r)) { vo_set_error(ctx, "%s: sequence %d has no first pair", who, q); return VO_E_INVALID; }
@@ -283,13 +305,13 @@ static int stage_pairs(vo_ctx* ctx, int slot, const SeqPairs& in, cudaStream_t s
     return vo_ingest_device(ctx, tab, 2, 2 * slot, st);
 }
 
-// n new sequences (multi: begun by vo_mseq_begin*) from their first pairs `in`; sequence q runs with the matrices
-// P_l + 12q / P_r + 12q; every frame also runs the mono_rotation branch with the option "mono_rotation" (vo_seq_begin*) or
-// the flag VO_MSEQ_MONO_ROTATION (vo_mseq_begin_ex / _calib).  Refused, before anything changes, while a batch submission
-// has not been waited for: it still uses the unit buffers and the pinned block.  A running sequence mode of the same kind
-// is drained and ended; one of the other kind only when it is idle.
-static int seq_begin(vo_ctx* ctx, const char* who, bool multi, int n, int flags, int w, int h, const float* P_l, const float* P_r,
-                     const SeqPairs& in)
+// n new sequences (multi: begun by vo_mseq_begin*) from their first pairs `in`; sequence q is w[q] x h[q] and runs with
+// the matrices P_l + 12q / P_r + 12q; every frame also runs the mono_rotation branch with the option "mono_rotation"
+// (vo_seq_begin*) or the flag VO_MSEQ_MONO_ROTATION (vo_mseq_begin_ex / _calib / _sized).  Refused, before anything
+// changes, while a batch submission has not been waited for: it still uses the unit buffers and the pinned block.  A
+// running sequence mode of the same kind is drained and ended; one of the other kind only when it is idle.
+static int seq_begin(vo_ctx* ctx, const char* who, bool multi, int n, int flags, const int* w, const int* h, const float* P_l,
+                     const float* P_r, const SeqPairs& in)
 {
     if (!ctx) return VO_E_INVALID;
     if (multi) {
@@ -297,10 +319,25 @@ static int seq_begin(vo_ctx* ctx, const char* who, bool multi, int n, int flags,
         if (n < 1) { vo_set_error(ctx, "%s: n_seq = %d, need at least one sequence", who, n); return VO_E_INVALID; }
         if (n > VO_MSEQ_MAX) { vo_set_error(ctx, "%s: n_seq = %d, a context holds at most %d sequences", who, n, VO_MSEQ_MAX); return VO_E_CAPACITY; }
     }
-    if (!P_l || !P_r || w <= 0 || h <= 0) { vo_set_error(ctx, "%s: bad argument", who); return VO_E_INVALID; }
+    if (!P_l || !P_r || !w || !h) { vo_set_error(ctx, "%s: bad argument", who); return VO_E_INVALID; }
+    for (int q = 0; q < n; q++)
+        if (w[q] <= 0 || h[q] <= 0) { vo_set_error(ctx, "%s: bad argument (sequence %d is %d x %d)", who, q, w[q], h[q]); return VO_E_INVALID; }
     int rc;
     if ((rc = seq_pairs_check(ctx, who, multi, n, w, in, true))) return rc;
-    if (h / 10 <= 0) { vo_set_error(ctx, "%s: image too small for the rows/10 bucket size", who); return VO_E_UNSUPPORTED; }
+    // the envelope of the sizes (the planes' allocation) and the one pyramid depth they must share
+    int W = 0, H = 0;
+    const int depth = vo_pyr_depth(w[0], h[0], ctx->p.lk_max_level);
+    for (int q = 0; q < n; q++) {
+        if (h[q] / 10 <= 0) { vo_set_error(ctx, "%s: image too small for the rows/10 bucket size", who); return VO_E_UNSUPPORTED; }
+        if (vo_pyr_depth(w[q], h[q], ctx->p.lk_max_level) != depth) {
+            vo_set_error(ctx, "%s: sequence 0 (%d x %d) has %d pyramid levels, sequence %d (%d x %d) %d: one run needs one pyramid depth",
+                         who, w[0], h[0], depth, q, w[q], h[q], vo_pyr_depth(w[q], h[q], ctx->p.lk_max_level));
+            return VO_E_UNSUPPORTED;
+        }
+        W = std::max(W, w[q]); H = std::max(H, h[q]);
+    }
+    bool sized = false;
+    for (int q = 0; q < n; q++) sized = sized || w[q] != W || h[q] != H;
     // the mono_rotation branch of several sequences is asked for with the flag only: the context option, which
     // vo_seq_begin* take, would otherwise silently pick (or drop) the branch for a whole set of sequences
     if (multi && ctx->mono_opt) {
@@ -319,13 +356,24 @@ static int seq_begin(vo_ctx* ctx, const char* who, bool multi, int n, int flags,
     if (ctx->seq_active && (rc = seq_drain(ctx))) return rc;
     ctx->seq_inflight = 0;
     ctx->seq_active = false;
-    if ((rc = vo_ensure_state(ctx, w, h, 2 * n))) return rc;      // two per-frame buffer units per sequence (frames in flight)
+    // two per-frame buffer units per sequence (frames in flight)
+    if ((rc = vo_ensure_state(ctx, W, H, 2 * n, depth))) return rc;
     if ((rc = seq_state_alloc(ctx, n))) return rc;
     if ((rc = seq_events(ctx))) return rc;
-    // the frame graphs are captured for one sequence count, and with or without the mono branch (which a sequence keeps)
+    // the frame graphs are captured for one sequence count, with or without the mono branch (which a sequence keeps),
+    // and with or without the geometry table (not for the sizes in it)
     if (ctx->seq_n != n) { vo_drop_graphs(ctx); ctx->seq_n = n; }
     ctx->seq_multi = multi;
     if (ctx->seq_mono != mono) { vo_drop_graphs(ctx); ctx->seq_mono = mono; }
+    if (ctx->seq_sized != sized) { vo_drop_graphs(ctx); ctx->seq_sized = sized; }
+    ctx->seq_w.assign(w, w + n);
+    ctx->seq_h.assign(h, h + n);
+    if (sized) {        // sequence q's planes 2q, 2q + 1 of each of the three image slots
+        std::vector<PlaneGeom> g(6 * (size_t)n);
+        for (int s = 0; s < 3; s++)
+            for (int q = 0; q < n; q++) g[2 * n * s + 2 * q] = g[2 * n * s + 2 * q + 1] = vo_plane_geom(ctx, w[q], h[q]);
+        if ((rc = vo_write_geo(ctx, 0, 6 * n, g.data()))) return rc;
+    }
     if (ctx->seq_mono && (rc = seq_mono_scratch(ctx, n))) return rc;
     if ((rc = vo_ensure_pinned(ctx, seq_pinned(ctx, n).bytes))) return rc;
     // sequence q owns the buffer units q and n + q (both parities): both entries carry its camera
@@ -344,7 +392,7 @@ static int seq_begin(vo_ctx* ctx, const char* who, bool multi, int n, int flags,
     // the first pairs into image slot 0 on the caller's stream, after the work already enqueued there (the synchronise
     // below is the release of device images)
     if ((rc = stage_pairs(ctx, 0, in, ctx->stream)) || (in.bgr() && (rc = convert_pairs(ctx, 0)))) return rc;
-    if ((rc = vo_run_pyramid(ctx, 0, 2 * n, ctx->stream))) return rc;
+    if ((rc = vo_run_pyramid(ctx, 0, 2 * n, ctx->stream, sized))) return rc;
     // both event pairs start out signalled, so the first two frames do not wait for a predecessor
     for (int k = 0; k < 2; k++) {
         VO_CUDA_CHECK(cudaEventRecord(ctx->seq_front_ev[k], ctx->stream));
@@ -386,7 +434,8 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
 {
     if (!ctx) return VO_E_INVALID;
     int rc;
-    if ((rc = seq_frame_check(ctx, who, multi, SEQ_SUBMIT)) || (rc = seq_pairs_check(ctx, who, multi, ctx->seq_n, ctx->w, in, false)))
+    if ((rc = seq_frame_check(ctx, who, multi, SEQ_SUBMIT)) ||
+        (rc = seq_pairs_check(ctx, who, multi, ctx->seq_n, ctx->seq_w.data(), in, false)))
         return rc;
     const int n = ctx->seq_n;
     for (int q = 0; multi && q < n; q++)
@@ -431,6 +480,9 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
     GraphKey key{};
     key.kind = GraphKey::SEQ_FRONT; key.s = ctx->stream; key.tma = ctx->lk_use_tma;
     key.slot = s0; key.parity = p; key.bgr = bgr;
+    // the LK launch bound: the largest bucket grid of the sequences' sizes, which a new set of sizes inside the same
+    // envelope can raise (the sizes themselves are in the geometry table, not in the graph)
+    key.max_pts = seq_grid(ctx);
     if ((rc = vo_run_graph(ctx, key, [&] { return seq_front(ctx, s0, s1, p, bgr); }))) return rc;
     VO_CUDA_CHECK(cudaEventRecord(ctx->seq_front_ev[p], ctx->stream));
     // back stage: after this frame's front stage; after the previous frame's back stage by stream order
@@ -574,18 +626,18 @@ extern "C" int vo_seq_begin(vo_ctx* ctx, int w, int h, const float P_l[12], cons
 extern "C" int vo_seq_begin_ex(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], const uint8_t* left0,
                                const uint8_t* right0, size_t pitch, int channels)
 {
-    return seq_begin(ctx, "vo_seq_begin", false, 1, 0, w, h, P_l, P_r, host_pairs(&left0, &right0, pitch, channels));
+    return seq_begin(ctx, "vo_seq_begin", false, 1, 0, &w, &h, P_l, P_r, host_pairs(&left0, &right0, &pitch, channels));
 }
 
 extern "C" int vo_seq_begin_device(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], const vo_dimage* left0,
                                    const vo_dimage* right0)
 {
-    return seq_begin(ctx, "vo_seq_begin_device", false, 1, 0, w, h, P_l, P_r, device_pair(left0, right0));
+    return seq_begin(ctx, "vo_seq_begin_device", false, 1, 0, &w, &h, P_l, P_r, device_pair(left0, right0));
 }
 
 extern "C" int vo_seq_submit(vo_ctx* ctx, const uint8_t* left1, const uint8_t* right1, size_t pitch, int channels)
 {
-    return seq_submit(ctx, "vo_seq_submit", false, host_pairs(&left1, &right1, pitch, channels));
+    return seq_submit(ctx, "vo_seq_submit", false, host_pairs(&left1, &right1, &pitch, channels));
 }
 
 extern "C" int vo_seq_submit_device(vo_ctx* ctx, const vo_dimage* left1, const vo_dimage* right1)
@@ -649,15 +701,34 @@ extern "C" int vo_mseq_begin_ex(vo_ctx* ctx, int n_seq, int w, int h, const floa
     return vo_mseq_begin_calib(ctx, n_seq, w, h, Pl.data(), Pr.data(), left0, right0, pitch, channels, flags);
 }
 
+// one image size and row pitch for every sequence: vo_mseq_begin_sized with them repeated
 extern "C" int vo_mseq_begin_calib(vo_ctx* ctx, int n_seq, int w, int h, const float* P_l, const float* P_r,
                                    const uint8_t* const* left0, const uint8_t* const* right0, size_t pitch, int channels, int flags)
 {
-    return seq_begin(ctx, "vo_mseq_begin", true, n_seq, flags, w, h, P_l, P_r, host_pairs(left0, right0, pitch, channels));
+    const int n = n_seq >= 1 && n_seq <= VO_MSEQ_MAX ? n_seq : 1;     // other counts are refused with their message
+    const std::vector<int> ws(n, w), hs(n, h);
+    const std::vector<size_t> ps(n, pitch);
+    return seq_begin(ctx, "vo_mseq_begin", true, n_seq, flags, ws.data(), hs.data(), P_l, P_r, host_pairs(left0, right0, ps.data(), channels));
 }
 
+extern "C" int vo_mseq_begin_sized(vo_ctx* ctx, int n_seq, const int* w, const int* h, const float* P_l, const float* P_r,
+                                   const uint8_t* const* left0, const uint8_t* const* right0, const size_t* pitch, int channels,
+                                   int flags)
+{
+    return seq_begin(ctx, "vo_mseq_begin_sized", true, n_seq, flags, w, h, P_l, P_r, host_pairs(left0, right0, pitch, channels));
+}
+
+// one row pitch for every image: vo_mseq_submit_sized with it repeated (it must cover every live sequence's width)
 extern "C" int vo_mseq_submit(vo_ctx* ctx, const uint8_t* const* left1, const uint8_t* const* right1, size_t pitch, int channels)
 {
-    return seq_submit(ctx, "vo_mseq_submit", true, host_pairs(left1, right1, pitch, channels));
+    const std::vector<size_t> ps(ctx && ctx->seq_active && ctx->seq_multi ? ctx->seq_n : 1, pitch);
+    return seq_submit(ctx, "vo_mseq_submit", true, host_pairs(left1, right1, ps.data(), channels));
+}
+
+extern "C" int vo_mseq_submit_sized(vo_ctx* ctx, const uint8_t* const* left1, const uint8_t* const* right1, const size_t* pitch,
+                                    int channels)
+{
+    return seq_submit(ctx, "vo_mseq_submit_sized", true, host_pairs(left1, right1, pitch, channels));
 }
 
 extern "C" int vo_mseq_wait(vo_ctx* ctx, vo_unit_result* out, int* status, vo_point2f* pts4, int pts_cap)
