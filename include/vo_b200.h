@@ -416,6 +416,38 @@ VO_API int vo_mseq_begin_sized(vo_ctx* ctx, int n_seq, const int* w, const int* 
 VO_API int vo_mseq_submit(vo_ctx* ctx, const uint8_t* const* left1, const uint8_t* const* right1, size_t pitch, int channels);
 VO_API int vo_mseq_submit_sized(vo_ctx* ctx, const uint8_t* const* left1, const uint8_t* const* right1,
                                 const size_t* pitch, int channels);
+/* Sequences that start while others run (a service whose streams come and go, or a queue of drives of unequal length).
+ *   vo_mseq_open          ends a running sequence mode as vo_mseq_begin* do and opens a run of n_slots EMPTY slots whose
+ *                         image planes, per-slot state, mono scratch (flag VO_MSEQ_MONO_ROTATION) and pinned block are
+ *                         allocated once, at the envelope max_w x max_h.  An empty slot's wait status is VO_MSEQ_RETIRED
+ *                         (zeroed record), its pose the identity, its state empty.
+ *   vo_mseq_submit_start  vo_mseq_submit_sized plus n_start starts: starts[i].slot's pair of this call is the FIRST pair of
+ *                         a new sequence of size w x h with the matrices P_l / P_r.  The slot may be empty, retired, or
+ *                         live (its sequence then ends at its previous frame).  This submission only stages the pair and
+ *                         builds its pyramids, as vo_seq_begin does; its wait reports VO_MSEQ_STARTED with a zeroed record
+ *                         (and mono), and from that wait on the slot's pose is the identity and its state empty.  Waits
+ *                         for earlier submissions still report the slot's previous sequence.  From the next submission
+ *                         on the slot's pairs are plain pairs (a NULL pair retires it).  vo_mseq_submit_sized is this call
+ *                         with n_start = 0.
+ * A started sequence gives what vo_seq_begin(first pair) + vo_seq_push with its matrices gives on a fresh context, bit for
+ * bit, and every other sequence what it gives without the start.  A start costs no kernel launch, and never allocates,
+ * drains or synchronises; the front graph is recaptured only for a larger bucket grid than the run has seen.  Starts work
+ * in runs of vo_mseq_begin* too (vo_mseq_begin / _ex / _calib runs: at the run's one size only).
+ * Refused, changing nothing: VO_E_INVALID for a slot out of range, two starts in one slot, a start without both images,
+ * pitch[slot] < channels * w, w or h <= 0, a third submission in flight, and vo_mseq_open with n_slots outside
+ * 1 .. VO_MSEQ_MAX or while the other sequence mode has frames in flight or a batch submission has not been waited for;
+ * VO_E_UNSUPPORTED for a size outside the envelope, of another pyramid depth, with h / 10 == 0, or other than the one size
+ * of a run begun with one size; VO_E_CAPACITY for a size whose bucket grid exceeds the bucketing scratch (4096 cells) or,
+ * with VO_MSEQ_MONO_ROTATION, the mono scratch (sized for the bucket grid of the envelope, or of the begun sizes). */
+#define VO_MSEQ_STARTED 3        /* vo_mseq_wait status: this submission started the slot's sequence from its first pair */
+typedef struct vo_mseq_start {
+    int slot;                /* 0 <= slot < n_seq; the first pair is left1[slot] / right1[slot] of the same call */
+    int w, h;                /* the new sequence's image size */
+    float P_l[12], P_r[12];  /* its matrices, row-major 3 x 4, built as the reference's main() builds them (src/main.cpp:67-74) */
+} vo_mseq_start;
+VO_API int vo_mseq_open(vo_ctx* ctx, int n_slots, int max_w, int max_h, int flags);
+VO_API int vo_mseq_submit_start(vo_ctx* ctx, const uint8_t* const* left1, const uint8_t* const* right1, const size_t* pitch,
+                                int channels, int n_start, const vo_mseq_start* starts);
 VO_API int vo_mseq_wait(vo_ctx* ctx, vo_unit_result* out, int* status, vo_point2f* pts4, int pts_cap);
 VO_API int vo_mseq_wait_mono(vo_ctx* ctx, vo_unit_result* out, int* status, vo_mono_result* mono,
                              uint8_t* ess_mask, int mask_cap, vo_point2f* pts4, int pts_cap);

@@ -15,7 +15,11 @@ training sequences come in three sizes, 1241x376, 1242x375 and 1226x370), which 
 `--calibration-for NAME=YAML` names (NAME = the dataset directory's name); each sequence runs with the matrices built from
 its own file, as the reference's main() builds them (src/main.cpp:67-74).  `--mono-rotation` runs trackingFrame2Frame
 as its header default does, for every sequence (mono_rotation = true: the rotation from findEssentialMat + recoverPose,
-the translation from the PnP; frames where that branch would abort are reported and not integrated).  `--check` only validates the inputs (no GPU needed)."""
+the translation from the PnP; frames where that branch would abort are reported and not integrated).  `--slots N` runs
+the datasets as a queue through N slots (vo_mseq_open + vo_mseq_submit_start): the first N start together, and each
+next one starts in the first slot that frees (the lowest slot on a tie), in the order given, so any number of datasets
+runs through one context; their sizes may differ (one pyramid depth, the envelope of all of them), and every pose file
+is the same for every N.  `--check` only validates the inputs and prints the schedule of --slots (no GPU needed)."""
 import argparse
 import os
 import sys
@@ -45,6 +49,25 @@ def pyramid_depth(w, h):
     return n
 
 
+def queue_schedule(lengths, n_slots):
+    """(slot, first submission) of each sequence of the given lengths (frames) run as a queue through n_slots slots: a
+    sequence occupies its slot from the submission of its first pair to that of its last, and the next one starts in the
+    first slot that frees (lowest index on a tie) at the submission after."""
+    free_at = [1] * n_slots
+    out = []
+    for n in lengths:
+        q = min(range(n_slots), key=lambda s: (free_at[s], s))
+        out.append((q, free_at[q]))
+        free_at[q] += n
+    return out
+
+
+def bucket_grid(w, h):
+    """bucketingFeatures' (rows/bs + 1) x (cols/bs + 1) cells, bs = rows / 10 (the library's seq_grid)"""
+    bs = max(h // 10, 1)
+    return (h // bs + 1) * (w // bs + 1)
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("datasets", nargs="+", metavar="DIR")
@@ -59,11 +82,16 @@ def main():
                     help="calibration of the dataset named NAME (repeatable; the others use the positional one)")
     ap.add_argument("--mixed-sizes", action="store_true",
                     help="run sequences of different image sizes together, each at its own size")
+    ap.add_argument("--slots", type=int, metavar="N",
+                    help="run the datasets as a queue through N slots, each starting in the first slot that frees")
     ap.add_argument("--check", action="store_true")
     a = ap.parse_args()
     from visual_odom_b200 import capi, synth
     default_cal = read_calibration(a.calibration)
-    if len(a.datasets) > capi.VO_MSEQ_MAX:
+    if a.slots is not None and not 1 <= a.slots <= capi.VO_MSEQ_MAX:
+        raise SystemExit(f"--slots {a.slots}: one context holds 1 to {capi.VO_MSEQ_MAX} slots")
+    sized = a.mixed_sizes or a.slots is not None
+    if a.slots is None and len(a.datasets) > capi.VO_MSEQ_MAX:
         raise SystemExit(f"{len(a.datasets)} sequences: one context runs at most {capi.VO_MSEQ_MAX}")
     names = [os.path.basename(os.path.normpath(d)) for d in a.datasets]
     if len(set(names)) != len(names):
@@ -86,13 +114,13 @@ def main():
         if n < 2:
             raise SystemExit(f"{d}: need at least two stereo pairs (image_0/%06d.png, image_1/%06d.png from 0)")
         w, h, ctype, depth = capi.png_info(open(os.path.join(d, "image_0", "%06d.png" % 0), "rb").read())
-        if seqs and (w, h) != (seqs[0]["w"], seqs[0]["h"]) and not a.mixed_sizes:
+        if seqs and (w, h) != (seqs[0]["w"], seqs[0]["h"]) and not sized:
             raise SystemExit(f"{d}: {w}x{h} images, {a.datasets[0]} has {seqs[0]['w']}x{seqs[0]['h']}: "
                              "one context runs one image size (group the sequences by size, or run them together with "
                              "--mixed-sizes)")
-        if a.mixed_sizes and h // 10 == 0:
+        if sized and h // 10 == 0:
             raise SystemExit(f"{d}: {w}x{h} images are too small for the rows/10 bucket size")
-        if a.mixed_sizes and seqs and pyramid_depth(w, h) != pyramid_depth(seqs[0]["w"], seqs[0]["h"]):
+        if sized and seqs and pyramid_depth(w, h) != pyramid_depth(seqs[0]["w"], seqs[0]["h"]):
             raise SystemExit(f"{d}: {w}x{h} images have {pyramid_depth(w, h)} pyramid levels, {a.datasets[0]} "
                              f"({seqs[0]['w']}x{seqs[0]['h']}) has {pyramid_depth(seqs[0]['w'], seqs[0]['h'])}: "
                              "one context runs one pyramid depth")
@@ -104,12 +132,29 @@ def main():
         seqs.append(dict(dir=d, name=name, n=n, w=w, h=h, gray=ctype == 0, gt=gt, P_l=P_l, P_r=P_r))
         print(f"{name}: {n} stereo pairs of {w}x{h} (PNG colour type {ctype}, {depth} bit), calibration {cal_path}")
         print(f"  P_left =\n{P_l}\n  P_right =\n{P_r}")
-    if a.mixed_sizes:
+    if sized:
         print("image sizes: " + ", ".join(f"{s['name']} {s['w']}x{s['h']}" for s in seqs))
+    if a.slots is not None:
+        W, H = max(s["w"] for s in seqs), max(s["h"] for s in seqs)
+        if pyramid_depth(W, H) != pyramid_depth(seqs[0]["w"], seqs[0]["h"]):
+            raise SystemExit(f"the envelope {W}x{H} of the sizes has {pyramid_depth(W, H)} pyramid levels, the sizes "
+                             f"{pyramid_depth(seqs[0]['w'], seqs[0]['h'])}: one context runs one pyramid depth")
+        for s in seqs:
+            if a.mono_rotation and bucket_grid(s["w"], s["h"]) > bucket_grid(W, H):
+                raise SystemExit(f"{s['dir']}: {s['w']}x{s['h']} has {bucket_grid(s['w'], s['h'])} buckets, more than "
+                                 f"the {bucket_grid(W, H)} of the envelope {W}x{H} the mono scratch is sized for")
+        sched = queue_schedule([s["n"] for s in seqs], a.slots)
+        steps = max(k0 + s["n"] - 1 for s, (_, k0) in zip(seqs, sched))
+        print(f"schedule: {len(seqs)} sequences through {a.slots} slots of {W}x{H}, {steps} submissions")
+        for s, (q, k0) in zip(seqs, sched):
+            s["slot"], s["k0"] = q, k0
+            print(f"  {s['name']}: slot {q}, submissions {k0}..{k0 + s['n'] - 1}")
     print("rotation: " + ("findEssentialMat + recoverPose (mono_rotation = true)" if a.mono_rotation else
                           "Rodrigues of the PnP rvec (mono_rotation = false)"))
     if a.check:
         return
+    if a.slots is not None:
+        return run_queue(a, capi, seqs, sched, W, H)
     # one pitch and one channel count per submission: colour files are read as BGR (converted on the device) unless the
     # sequences mix gray and colour files, then all are converted to gray while decoding
     force = 0 if len({s["gray"] for s in seqs}) == 1 else 1
@@ -164,6 +209,72 @@ def main():
             print(f"step {k}: {done} sequence-frames, {done / (time.perf_counter() - t0):.0f} frames/s")
     for rd in rds:
         rd.close()
+    ctx.close()
+    os.makedirs(a.poses, exist_ok=True)
+    for s, p, n_abort in zip(seqs, poses, aborted):
+        path = os.path.join(a.poses, s["name"] + ".txt")
+        capi.poses_save(path, p)
+        line = f"{s['name']}: {len(p)} poses -> {path}"
+        if a.mono_rotation:
+            line += f", {n_abort} frames where findEssentialMat / recoverPose would abort (reported, not integrated)"
+        if s["gt"]:
+            gt = capi.poses_load(s["gt"])[:len(p)]
+            seg, t_err, r_err = capi.eval_segments(gt, p[:len(gt)])
+            line += (", ground-truth path shorter than the 100 m minimum segment" if len(seg) == 0 else
+                     f", KITTI metric over {len(seg)} segments: t_err {100 * t_err:.2f} %, r_err {r_err * 180 / np.pi * 100:.4f} deg / 100 m")
+        print(line)
+
+
+def run_queue(a, capi, seqs, sched, W, H):
+    """--slots: every dataset starts in its scheduled slot (vo_mseq_submit_start) and retires after its last frame."""
+    force = 0 if len({s["gray"] for s in seqs}) == 1 else 1
+    ctx = capi.Context(a.device, max_features=4096)
+    ctx.mseq_open(a.slots, W, H, mono_rotation=a.mono_rotation)
+    steps = max(s["k0"] + s["n"] - 1 for s in seqs)
+    rds = {}                   # dataset index -> its reader, opened at its first pair, closed after its last wait
+    by_step = {}
+    for i, s in enumerate(seqs):
+        for k in range(s["k0"], s["k0"] + s["n"]):
+            by_step.setdefault(k, []).append(i)
+
+    def submit(k):
+        lp, rp, pitches, chs, start = [None] * a.slots, [None] * a.slots, [0] * a.slots, set(), {}
+        for i in by_step.get(k, []):
+            s = seqs[i]
+            if k == s["k0"]:
+                rds[i] = capi.SequenceReader(s["dir"], 0, s["n"], threads=a.threads, depth=a.threads + 3, force_channels=force)
+                start[s["slot"]] = (s["w"], s["h"], s["P_l"], s["P_r"])
+            l, r, _, _, pitch, ch, _ = rds[i].next_ptr()
+            lp[s["slot"]], rp[s["slot"]], pitches[s["slot"]] = l, r, pitch
+            chs.add(ch)
+        if len(chs) > 1:
+            raise SystemExit(f"submission {k}: the readers deliver different channel counts {sorted(chs)}")
+        ctx.mseq_submit_ptr(lp, rp, pitches, chs.pop() if chs else 1, start=start)
+
+    poses = [[np.eye(4)] for _ in seqs]
+    aborted = [0] * len(seqs)
+    t0 = time.perf_counter()
+    done = 0
+    submit(1)
+    for k in range(1, steps + 1):
+        if k + 1 <= steps:
+            submit(k + 1)
+        recs = ctx.mseq_wait(want_points=False, mono=a.mono_rotation)
+        for i in by_step.get(k, []):
+            s = seqs[i]
+            r = recs[s["slot"]]
+            if k == s["k0"]:
+                continue                     # VO_MSEQ_STARTED: the first pair
+            if r["status"] != capi.VO_OK:
+                print(f"{s['name']} frame {k - s['k0']}: status {r['status']} ({ctx.lib.vo_last_error(ctx.h).decode()})")
+            if a.mono_rotation and r["mono"]["status"] != capi.VO_OK:
+                aborted[i] += 1
+            poses[i].append(ctx.mseq_pose(s["slot"]))
+            done += 1
+            if k == s["k0"] + s["n"] - 1:
+                rds.pop(i).close()           # its last submission has been waited for
+        if k % 100 == 0 or k == steps:
+            print(f"step {k}: {done} sequence-frames, {done / (time.perf_counter() - t0):.0f} frames/s")
     ctx.close()
     os.makedirs(a.poses, exist_ok=True)
     for s, p, n_abort in zip(seqs, poses, aborted):

@@ -22,6 +22,7 @@ VO_E_CAPACITY = -5
 VO_MSEQ_MAX = 64           # sequences one vo_mseq_begin may start (include/vo_b200.h)
 VO_MSEQ_RETIRED = 2        # vo_mseq_wait status of a retired sequence
 VO_MSEQ_MONO_ROTATION = 1  # vo_mseq_begin_ex flag: every sequence runs trackingFrame2Frame(mono_rotation = true)
+VO_MSEQ_STARTED = 3        # vo_mseq_wait status of the submission that started a slot's sequence
 
 
 class VoParams(C.Structure):
@@ -91,6 +92,11 @@ class VoUnitResult(C.Structure):
         ("n_inliers", C.c_int), ("ransac_iters", C.c_int), ("pnp_status", C.c_int),
         ("rvec", C.c_double * 3), ("tvec", C.c_double * 3), ("R", C.c_double * 9),
     ]
+
+
+class VoMseqStart(C.Structure):
+    """vo_mseq_start: the slot, image size and matrices of a sequence that vo_mseq_submit_start starts."""
+    _fields_ = [("slot", C.c_int), ("w", C.c_int), ("h", C.c_int), ("P_l", C.c_float * 12), ("P_r", C.c_float * 12)]
 
 
 class VoMonoResult(C.Structure):
@@ -186,6 +192,8 @@ SIGNATURES = {
                                       C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     "vo_mseq_submit": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
     "vo_mseq_submit_sized": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
+    "vo_mseq_open": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "vo_mseq_submit_start": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(VoMseqStart)]),
     "vo_mseq_wait": (C.c_int, [C.c_void_p, C.POINTER(VoUnitResult), C.c_void_p, C.c_void_p, C.c_int]),
     "vo_mseq_wait_mono": (C.c_int, [C.c_void_p, C.POINTER(VoUnitResult), C.c_void_p, C.POINTER(VoMonoResult), C.c_void_p,
                                     C.c_int, C.c_void_p, C.c_int]),
@@ -789,29 +797,69 @@ class Context:
         lp, rp = (C.c_void_p * n)(*left_ptrs), (C.c_void_p * n)(*right_ptrs)
         self._mseq_begin(n, w, h, lp, rp, pitch, channels, P_l, P_r, mono_rotation)
 
-    def mseq_submit_ptr(self, left_ptrs, right_ptrs, pitch, channels=1):
+    def mseq_open(self, n_slots, max_w, max_h, mono_rotation=False):
+        """n_slots empty slots for sequences of any size inside max_w x max_h with that size's pyramid depth
+        (vo_mseq_open); sequences come in through mseq_submit(start=...).  mono_rotation=True: every sequence started in
+        the run runs trackingFrame2Frame(mono_rotation = true)."""
+        flags = VO_MSEQ_MONO_ROTATION if mono_rotation else 0
+        self._check(self.lib.vo_mseq_open(self.h, int(n_slots), int(max_w), int(max_h), flags))
+        self._mseq_n, self._mseq_pitch = int(n_slots), np.zeros(int(n_slots), np.uint64)
+        self._mseq_sizes = [None] * int(n_slots)
+        self._mseq_keep = [None, None]
+
+    @staticmethod
+    def _starts(start):
+        """{slot: (w, h, P_l, P_r)} as a vo_mseq_start array and its length."""
+        arr = (VoMseqStart * max(len(start), 1))()
+        for s, (q, (w, h, P_l, P_r)) in zip(arr, start.items()):
+            s.slot, s.w, s.h = int(q), int(w), int(h)
+            s.P_l[:] = np.asarray(P_l, np.float32).reshape(12).tolist()
+            s.P_r[:] = np.asarray(P_r, np.float32).reshape(12).tolist()
+        return arr, len(start)
+
+    def mseq_submit_ptr(self, left_ptrs, right_ptrs, pitch, channels=1, start=None):
         """Raw host pointers; None in both lists retires that sequence.  The memory must stay valid until the wait.
-        pitch: one row pitch for every image, or a sequence of one per sequence (vo_mseq_submit_sized)."""
+        pitch: one row pitch for every image, or a sequence of one per sequence (vo_mseq_submit_sized).
+        start = {slot: (w, h, P_l, P_r)}: those slots' pairs are the first pairs of new sequences (vo_mseq_submit_start)."""
         n = len(left_ptrs)
         lp, rp = (C.c_void_p * n)(*left_ptrs), (C.c_void_p * n)(*right_ptrs)
-        if np.ndim(pitch) > 0:
+        if start:
+            pa = np.ascontiguousarray(np.broadcast_to(np.asarray(pitch), (n,)), np.uint64)
+            arr, ns = self._starts(start)
+            self._check(self.lib.vo_mseq_submit_start(self.h, lp, rp, _p(pa), channels, ns, arr))
+        elif np.ndim(pitch) > 0:
             pa = np.ascontiguousarray(np.broadcast_to(np.asarray(pitch), (n,)), np.uint64)
             self._check(self.lib.vo_mseq_submit_sized(self.h, lp, rp, _p(pa), channels))
         else:
             self._check(self.lib.vo_mseq_submit(self.h, lp, rp, pitch, channels))
 
-    def mseq_submit(self, lefts, rights):
+    def mseq_submit(self, lefts, rights, start=None):
         """Asynchronous: one frame of every sequence; a (None, None) pair retires that sequence.  At most two submissions
-        in flight.  The arrays are kept alive by the context until their submission has been waited for."""
+        in flight.  The arrays are kept alive by the context until their submission has been waited for.
+        start = {slot: (P_l, P_r)}: those slots' pairs are the first pairs of new sequences with these matrices, at the
+        pairs' sizes (vo_mseq_submit_start; the wait of this submission reports VO_MSEQ_STARTED for them)."""
         lp, rp, pitch, ch, keep, geom, shapes = self._pairs(lefts, rights, True)
         if len(lefts) != getattr(self, "_mseq_n", len(lefts)):
             raise ValueError(f"{len(lefts)} pairs for {self._mseq_n} sequences")
-        if np.ndim(self._mseq_pitch) > 0:           # begun with several sizes: one packed pitch per live pair
+        start = dict(start or {})
+        for q in start:
+            if not 0 <= q < len(shapes) or shapes[q] is None:
+                raise ValueError(f"slot {q}: a start needs its first pair")
+        sized = np.ndim(self._mseq_pitch) > 0
+        if sized or start:                          # several sizes or starts: one packed pitch per live pair
             for q, g in enumerate(shapes):
-                if g is not None and tuple(g[:2]) != self._mseq_sizes[q]:
+                if sized and g is not None and q not in start and self._mseq_sizes[q] is not None \
+                        and tuple(g[:2]) != self._mseq_sizes[q]:
                     raise ValueError(f"sequence {q}: image shape {g}, the sequence is {self._mseq_sizes[q]}")
             pa = np.array([g[1] * ch if g is not None else 0 for g in shapes], np.uint64)
-            self._check(self.lib.vo_mseq_submit_sized(self.h, lp, rp, _p(pa), ch))
+            if start:
+                arr, ns = self._starts({q: (shapes[q][1], shapes[q][0], P[0], P[1]) for q, P in start.items()})
+                self._check(self.lib.vo_mseq_submit_start(self.h, lp, rp, _p(pa), ch, ns, arr))
+                if sized:
+                    for q in start:
+                        self._mseq_sizes[q] = tuple(shapes[q][:2])
+            else:
+                self._check(self.lib.vo_mseq_submit_sized(self.h, lp, rp, _p(pa), ch))
         else:
             if pitch is None:
                 raise ValueError("the sequences were begun with one image size: every pair needs that shape")

@@ -15,6 +15,7 @@
 #define VO_DIST_BUCKET 4       // posted steps per collective
 #define VO_DIST_NB 4           // buckets (ring)
 #define VO_LANES 3            // submissions in flight, each with its own side stream / partition streams / events
+#define SEQ_STARTED 2         // vo_ctx::seq_live: the slot's sequence started in this submission (stages skip it)
 
 // what a cached CUDA graph was captured for: its kind, the stream (the LK work queue is that stream's), the LK staging,
 // and the kind's own fields (the others stay zero)
@@ -111,8 +112,14 @@ struct vo_ctx {
     long long seq_submitted = 0;        // frames submitted since vo_seq_begin (frame k uses buffer parity k & 1)
     cudaEvent_t seq_front_ev[2] = {nullptr, nullptr}, seq_back_ev[2] = {nullptr, nullptr};
     std::vector<double> seq_pose;       // [seq_n][16] frame_pose of main.cpp:90, integrated per push
-    std::vector<char> seq_retired;      // [seq_n] retired by a NULL pair (vo_mseq_submit)
-    std::vector<char> seq_live;         // [2 * seq_n] host copy of d_seq_live as the frame in flight in each parity saw it
+    std::vector<char> seq_retired;      // [seq_n] no sequence runs in the slot: retired by a NULL pair (vo_mseq_submit), or
+                                        // never started (vo_mseq_open)
+    std::vector<char> seq_live;         // [2 * seq_n] d_seq_live as the frame in flight in each parity saw it: 0 not running,
+                                        // 1 running, SEQ_STARTED (host only, the device word is 0) its sequence started there
+    int seq_lk_bound = 0;               // the LK launch bound: the largest bucket grid of the run's sizes (raised by starts)
+    std::vector<CamCalib> seq_cal_next; // [2 * seq_n] calibration entries of started sequences that the frame in flight
+    std::vector<char> seq_cal_due;      // still reads: written by the next submission of that buffer parity
+    std::vector<char> seq_geo_due;      // [seq_n] image slots whose geometry entries still hold the slot's previous size
     uint8_t* d_bgr = nullptr;           // staging of colour (BGR) inputs, converted by k_bgr_to_gray (ingest.cu)
     size_t bgr_bytes = 0;
     // SM partition (green contexts, ctx.cu vo_partition_enable): the LK ring kernel -- persistent, 100 % of the registers of

@@ -72,8 +72,9 @@ static int convert_pairs(vo_ctx* ctx, int slot)
     return VO_OK;
 }
 
-// the glue kernels' arguments for the n_seq units of buffer parity p (units u0 .. u0 + n_seq - 1)
-static void seq_args(vo_ctx* ctx, int p, SeqArgs& a)
+// the glue kernels' arguments for the n_seq units of buffer parity p (units u0 .. u0 + n_seq - 1); s0 = the image slot of
+// the frame's previous pairs, whose geometry entries give each sequence's bucket grid
+static void seq_args(vo_ctx* ctx, int p, SeqArgs& a, int s0 = 0)
 {
     memset(&a, 0, sizeof(a));
     const int n = ctx->seq_n, u0 = p * n;
@@ -82,7 +83,8 @@ static void seq_args(vo_ctx* ctx, int p, SeqArgs& a)
     a.feat_pts = ctx->d_feat_pts; a.feat_ages = ctx->d_feat_ages; a.cnt = ctx->d_feat_cnt; a.feat_cap = ctx->feat_cap;
     a.refill_below = 2000;                                   // visualOdometry.cpp:95
     a.rows = ctx->h; a.cols = ctx->w; a.bucket_size = ctx->h / 10;      // visualOdometry.cpp:106 (features_per_bucket = 1)
-    a.geo = ctx->seq_sized ? ctx->d_geo : nullptr; a.geo_stride = 2;    // sequence q: plane 2q (image slot 0)
+    // sequence q: plane 2q of image slot s0 (a started sequence's size reaches the three slots one staged pair at a time)
+    a.geo = ctx->seq_sized ? ctx->d_geo + 2 * n * s0 : nullptr; a.geo_stride = 2;
     a.bucket = ctx->d_bucket; a.bucket_cap = ctx->bucket_cap;
     a.out_pts = ctx->d_pts_in + uo; a.out_ages = ctx->d_ages_in + uo; a.out_n = ctx->d_npts + u0; a.out_cap = ctx->cap;
     a.valid_l1 = ctx->d_valid4 + 2 * cs + uo; a.n5 = ctx->d_n5 + u0; a.ages_out = ctx->d_ages_out + uo; a.n3 = ctx->d_n3 + u0;
@@ -147,7 +149,7 @@ static int seq_front(vo_ctx* ctx, int s0, int s1, int p, bool bgr)
     const int n = ctx->seq_n, unit = p * n;
     const int L0 = 2 * n * s0, R0 = L0 + 1, L1 = 2 * n * s1, R1 = L1 + 1;
     // image planes are addressed from plane 0 whatever the parity; sequence q's pair of a slot is planes 2q, 2q + 1 of it
-    const View v{unit, n, ctx->stream, 0, 2, seq_grid(ctx), ctx->seq_sized};
+    const View v{unit, n, ctx->stream, 0, 2, ctx->seq_lk_bound, ctx->seq_sized};
     int rc;
     if (bgr && (rc = convert_pairs(ctx, s1))) return rc;
     // the new pairs' pyramids (the previous pairs' are already resident)
@@ -155,7 +157,7 @@ static int seq_front(vo_ctx* ctx, int s0, int s1, int p, bool bgr)
     // matchingFeatures(): FAST refill on the t0 left image -> bucketing -> circular matching -> filters
     if ((rc = vo_run_fast(ctx, v, L0, false))) return rc;
     SeqArgs a;
-    seq_args(ctx, p, a);
+    seq_args(ctx, p, a, s0);
     ctx->launches += vo_launch_seq_append(a, n, ctx->stream);
     ctx->launches += vo_launch_seq_bucket(a, n, ctx->stream);
     const int ip[4] = {L0, R0, R1, L1}, in[4] = {R0, R1, L1, L0};
@@ -266,9 +268,11 @@ static SeqPairs host_pairs(const uint8_t* const* lefts, const uint8_t* const* ri
 }
 static SeqPairs device_pair(const vo_dimage* left, const vo_dimage* right) { return SeqPairs{nullptr, nullptr, nullptr, 1, true, left, right}; }
 
-// the new pairs' own checks (w[q]: sequence q's image width; begin: the first pairs, which every sequence needs).  A pitch
-// is checked only where a pair is read: a retiring sequence's is not.
-static int seq_pairs_check(vo_ctx* ctx, const char* who, bool multi, int n, const int* w, const SeqPairs& in, bool begin)
+// the new pairs' own checks (w[q]: sequence q's image width; begin: the first pairs, which every sequence needs; starting[q]:
+// the pair starts a new sequence in slot q of a running submission, so it needs both images and may follow a retirement).
+// A pitch is checked only where a pair is read: a retiring sequence's is not.
+static int seq_pairs_check(vo_ctx* ctx, const char* who, bool multi, int n, const int* w, const SeqPairs& in, bool begin,
+                           const char* starting = nullptr)
 {
     int rc;
     if (in.device) {
@@ -288,9 +292,10 @@ static int seq_pairs_check(vo_ctx* ctx, const char* who, bool multi, int n, cons
         }
     for (int q = 0; multi && q < n; q++) {
         const bool l = in.lefts[q] != nullptr, r = in.rights[q] != nullptr;
-        if (begin && !(l && r)) { vo_set_error(ctx, "%s: sequence %d has no first pair", who, q); return VO_E_INVALID; }
+        const bool first = begin || (starting && starting[q]);
+        if (first && !(l && r)) { vo_set_error(ctx, "%s: sequence %d has no first pair", who, q); return VO_E_INVALID; }
         if (!begin && l != r) { vo_set_error(ctx, "%s: sequence %d has only one image (a NULL pair retires it)", who, q); return VO_E_INVALID; }
-        if (!begin && l && ctx->seq_retired[q]) { vo_set_error(ctx, "%s: sequence %d was retired", who, q); return VO_E_INVALID; }
+        if (!first && l && ctx->seq_retired[q]) { vo_set_error(ctx, "%s: sequence %d was retired", who, q); return VO_E_INVALID; }
     }
     return VO_OK;
 }
@@ -310,20 +315,26 @@ static int stage_pairs(vo_ctx* ctx, int slot, const SeqPairs& in, cudaStream_t s
 // (vo_seq_begin*) or the flag VO_MSEQ_MONO_ROTATION (vo_mseq_begin_ex / _calib / _sized).  Refused, before anything
 // changes, while a batch submission has not been waited for: it still uses the unit buffers and the pinned block.  A
 // running sequence mode of the same kind is drained and ended; one of the other kind only when it is idle.
+// in == nullptr (vo_mseq_open): n empty slots at the envelope w[q] x h[q] (one value repeated), no matrices, no pairs; the
+// run reads the geometry table whatever sizes its sequences get.
 static int seq_begin(vo_ctx* ctx, const char* who, bool multi, int n, int flags, const int* w, const int* h, const float* P_l,
-                     const float* P_r, const SeqPairs& in)
+                     const float* P_r, const SeqPairs* in)
 {
     if (!ctx) return VO_E_INVALID;
+    const bool open = in == nullptr;
     if (multi) {
         if (flags & ~VO_MSEQ_MONO_ROTATION) { vo_set_error(ctx, "%s: unknown flag bits 0x%x", who, (unsigned)(flags & ~VO_MSEQ_MONO_ROTATION)); return VO_E_INVALID; }
         if (n < 1) { vo_set_error(ctx, "%s: n_seq = %d, need at least one sequence", who, n); return VO_E_INVALID; }
-        if (n > VO_MSEQ_MAX) { vo_set_error(ctx, "%s: n_seq = %d, a context holds at most %d sequences", who, n, VO_MSEQ_MAX); return VO_E_CAPACITY; }
+        if (n > VO_MSEQ_MAX) {
+            vo_set_error(ctx, "%s: %s = %d, a context holds at most %d sequences", who, open ? "n_slots" : "n_seq", n, VO_MSEQ_MAX);
+            return open ? VO_E_INVALID : VO_E_CAPACITY;
+        }
     }
-    if (!P_l || !P_r || !w || !h) { vo_set_error(ctx, "%s: bad argument", who); return VO_E_INVALID; }
+    if ((!open && (!P_l || !P_r)) || !w || !h) { vo_set_error(ctx, "%s: bad argument", who); return VO_E_INVALID; }
     for (int q = 0; q < n; q++)
         if (w[q] <= 0 || h[q] <= 0) { vo_set_error(ctx, "%s: bad argument (sequence %d is %d x %d)", who, q, w[q], h[q]); return VO_E_INVALID; }
     int rc;
-    if ((rc = seq_pairs_check(ctx, who, multi, n, w, in, true))) return rc;
+    if (!open && (rc = seq_pairs_check(ctx, who, multi, n, w, *in, true))) return rc;
     // the envelope of the sizes (the planes' allocation) and the one pyramid depth they must share
     int W = 0, H = 0;
     const int depth = vo_pyr_depth(w[0], h[0], ctx->p.lk_max_level);
@@ -336,7 +347,7 @@ static int seq_begin(vo_ctx* ctx, const char* who, bool multi, int n, int flags,
         }
         W = std::max(W, w[q]); H = std::max(H, h[q]);
     }
-    bool sized = false;
+    bool sized = open;
     for (int q = 0; q < n; q++) sized = sized || w[q] != W || h[q] != H;
     // the mono_rotation branch of several sequences is asked for with the flag only: the context option, which
     // vo_seq_begin* take, would otherwise silently pick (or drop) the branch for a whole set of sequences
@@ -374,25 +385,32 @@ static int seq_begin(vo_ctx* ctx, const char* who, bool multi, int n, int flags,
             for (int q = 0; q < n; q++) g[2 * n * s + 2 * q] = g[2 * n * s + 2 * q + 1] = vo_plane_geom(ctx, w[q], h[q]);
         if ((rc = vo_write_geo(ctx, 0, 6 * n, g.data()))) return rc;
     }
+    // the LK launch bound (and the mono scratch): the begun sizes' largest bucket grid, or the envelope's for an open run
+    ctx->seq_lk_bound = seq_grid(ctx);
     if (ctx->seq_mono && (rc = seq_mono_scratch(ctx, n))) return rc;
     if ((rc = vo_ensure_pinned(ctx, seq_pinned(ctx, n).bytes))) return rc;
-    // sequence q owns the buffer units q and n + q (both parities): both entries carry its camera
-    if ((rc = vo_set_calibration(ctx, 0, 2 * n, P_l, P_r, n))) return rc;
+    // sequence q owns the buffer units q and n + q (both parities): both entries carry its camera (a start writes them)
+    if (!open && (rc = vo_set_calibration(ctx, 0, 2 * n, P_l, P_r, n))) return rc;
     ctx->seq_slot = 0;
     ctx->seq_submitted = 0;
     ctx->seq_pose.assign(16 * (size_t)n, 0.0);
     for (int q = 0; q < n; q++)
         for (int i = 0; i < 4; i++) ctx->seq_pose[16 * q + 5 * i] = 1.0;
-    ctx->seq_retired.assign(n, 0);
-    ctx->seq_live.assign(2 * (size_t)n, 1);
+    ctx->seq_retired.assign(n, open ? 1 : 0);
+    ctx->seq_live.assign(2 * (size_t)n, open ? 0 : 1);
+    ctx->seq_cal_next.assign(2 * (size_t)n, CamCalib{});
+    ctx->seq_cal_due.assign(2 * (size_t)n, 0);
+    ctx->seq_geo_due.assign(n, 0);
     VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_feat_cnt, 0, 2 * (size_t)n * sizeof(int), ctx->stream));
     VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_seq_err, 0, (1 + 2 * (size_t)n) * sizeof(int), ctx->stream));
-    VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_seq_live, 1, 2 * (size_t)n * sizeof(int), ctx->stream));   // any non-zero word is live
+    VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_seq_live, open ? 0 : 1, 2 * (size_t)n * sizeof(int), ctx->stream));   // any non-zero word is live
     VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_tprev, 0, 6 * (size_t)n * sizeof(double), ctx->stream));   // translation = zeros (main.cpp:82)
     // the first pairs into image slot 0 on the caller's stream, after the work already enqueued there (the synchronise
     // below is the release of device images)
-    if ((rc = stage_pairs(ctx, 0, in, ctx->stream)) || (in.bgr() && (rc = convert_pairs(ctx, 0)))) return rc;
-    if ((rc = vo_run_pyramid(ctx, 0, 2 * n, ctx->stream, sized))) return rc;
+    if (!open) {
+        if ((rc = stage_pairs(ctx, 0, *in, ctx->stream)) || (in->bgr() && (rc = convert_pairs(ctx, 0)))) return rc;
+        if ((rc = vo_run_pyramid(ctx, 0, 2 * n, ctx->stream, sized))) return rc;
+    }
     // both event pairs start out signalled, so the first two frames do not wait for a predecessor
     for (int k = 0; k < 2; k++) {
         VO_CUDA_CHECK(cudaEventRecord(ctx->seq_front_ev[k], ctx->stream));
@@ -430,16 +448,108 @@ static int seq_frame_check(vo_ctx* ctx, const char* who, bool multi, SeqCall cal
 // One frame of every sequence (a NULL pair retires its sequence): the new pairs into the image slot s1 that neither the
 // running nor the previous frame reads, the front stage (gray frames replay the gray graph whatever their source), the
 // back stage, the record copies
-static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& in)
+// The checks of a submission's starts (vo_mseq_submit_start), before anything changes: starting[q] marks slot q's pair as
+// the first pair of a new sequence, w[q] is then its width (for the pitch check).
+static int seq_starts_check(vo_ctx* ctx, const char* who, int n_start, const vo_mseq_start* starts, std::vector<char>& starting,
+                            std::vector<int>& w)
+{
+    const int n = ctx->seq_n;
+    if (n_start < 0 || (n_start > 0 && !starts)) { vo_set_error(ctx, "%s: bad argument (n_start = %d)", who, n_start); return VO_E_INVALID; }
+    for (int i = 0; i < n_start; i++) {
+        const vo_mseq_start& s = starts[i];
+        if (s.slot < 0 || s.slot >= n) { vo_set_error(ctx, "%s: start %d: slot %d of %d", who, i, s.slot, n); return VO_E_INVALID; }
+        if (starting[s.slot]) { vo_set_error(ctx, "%s: start %d: slot %d is started twice", who, i, s.slot); return VO_E_INVALID; }
+        if (s.w <= 0 || s.h <= 0) { vo_set_error(ctx, "%s: start %d: bad size %d x %d", who, i, s.w, s.h); return VO_E_INVALID; }
+        starting[s.slot] = 1;
+        w[s.slot] = s.w;
+    }
+    return VO_OK;
+}
+
+// the sizes a run can start: the run's planes, pyramid depth, bucketing scratch and mono scratch are those of its begin
+static int seq_starts_fit(vo_ctx* ctx, const char* who, int n_start, const vo_mseq_start* starts)
+{
+    for (int i = 0; i < n_start; i++) {
+        const int w = starts[i].w, h = starts[i].h, q = starts[i].slot;
+        if (!ctx->seq_sized && (w != ctx->w || h != ctx->h)) {
+            vo_set_error(ctx, "%s: slot %d: %d x %d in a run of the one size %d x %d (a run begun with vo_mseq_open or "
+                              "vo_mseq_begin_sized starts other sizes)", who, q, w, h, ctx->w, ctx->h);
+            return VO_E_UNSUPPORTED;
+        }
+        if (w > ctx->w || h > ctx->h) {
+            vo_set_error(ctx, "%s: slot %d: %d x %d is outside the run's envelope %d x %d", who, q, w, h, ctx->w, ctx->h);
+            return VO_E_UNSUPPORTED;
+        }
+        if (h / 10 <= 0) { vo_set_error(ctx, "%s: slot %d: image too small for the rows/10 bucket size", who, q); return VO_E_UNSUPPORTED; }
+        const int depth = vo_pyr_depth(w, h, ctx->p.lk_max_level);
+        if (depth != ctx->pg.nlevels) {
+            vo_set_error(ctx, "%s: slot %d: %d x %d has %d pyramid levels, the run %d", who, q, w, h, depth, ctx->pg.nlevels);
+            return VO_E_UNSUPPORTED;
+        }
+        const int grid = seq_grid(w, h);
+        if (grid > ctx->bucket_cap) {
+            vo_set_error(ctx, "%s: slot %d: %d x %d has %d buckets, the run holds %d", who, q, w, h, grid, ctx->bucket_cap);
+            return VO_E_CAPACITY;
+        }
+        if (ctx->seq_mono && std::min(grid, ctx->cap) > ctx->seq_ess_cap) {
+            vo_set_error(ctx, "%s: slot %d: %d x %d needs mono scratch for %d points, the run reserved %d", who, q, w, h,
+                         std::min(grid, ctx->cap), ctx->seq_ess_cap);
+            return VO_E_CAPACITY;
+        }
+    }
+    return VO_OK;
+}
+
+// One frame of every sequence (a NULL pair retires its sequence; starts: the listed slots' pairs begin new sequences,
+// vo_mseq_submit_start): the new pairs into the image slot s1 that neither the running nor the previous frame reads, the
+// front stage (gray frames replay the gray graph whatever their source), the back stage, the record copies.
+//
+// A start in slot q at submission k (parity p) resets the slot's state against the two frames that may be in flight:
+//   live word      unit p * n + q is 0 in frame k (its stages skip the slot, as for a retired one; the wait reports
+//                  VO_MSEQ_STARTED from the host copy) and 1 from frame k + 1 on.  Like a retirement, a unit's word is
+//                  written by the next submission of its parity, after the back stage that last read it.
+//   FeatureSet     d_feat_cnt of q zeroed on the front stream: after the carry of frame k - 1 (stream order), and frame k
+//                  skips the slot, so frame k + 1 refills from FAST on the first pair as vo_seq_begin's first push does.
+//   translation    the back stage of frame k - 1 (side stream) writes tprev[p n + q], and k_seq_finish of frame k copies
+//                  it into tprev[(1 - p) n + q] for the skipped slot: the zeroing goes on the side stream right after the
+//                  back stage of frame k, so frame k + 1 solves from zeros (main.cpp:82).
+//   calibration    unit p n + q was last read by frame k - 2 (the front stream has waited for its back stage): written
+//                  now.  Unit (1 - p) n + q may still be read by the triangulation / PnP / five-point kernels of frame
+//                  k - 1: written by submission k + 1, after seq_back_ev[1 - p].
+//   geometry       the entries of q's planes in image slot s are written when a pair of the new sequence is staged into
+//                  s (s1 of frames k, k + 1, k + 2): s1 was last read by frame k - 2, and slot s0 of frame k is still being
+//                  written by the pyramid launch of frame k - 1.
+//   frame_pose     reset by the wait of frame k: the waits of frames k - 2 and k - 1 still integrate the old sequence.
+static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& in, int n_start = 0, const vo_mseq_start* starts = nullptr)
 {
     if (!ctx) return VO_E_INVALID;
     int rc;
-    if ((rc = seq_frame_check(ctx, who, multi, SEQ_SUBMIT)) ||
-        (rc = seq_pairs_check(ctx, who, multi, ctx->seq_n, ctx->seq_w.data(), in, false)))
-        return rc;
+    if ((rc = seq_frame_check(ctx, who, multi, SEQ_SUBMIT))) return rc;
     const int n = ctx->seq_n;
+    // a submission without starts checks its pairs against the running sizes, with no per-slot copies
+    std::vector<char> starting;
+    std::vector<int> wq;
+    const int* w = ctx->seq_w.data();
+    const char* st = nullptr;
+    if (n_start || starts) {
+        starting.assign(n, 0);
+        wq = ctx->seq_w;
+        if ((rc = seq_starts_check(ctx, who, n_start, starts, starting, wq))) return rc;
+        w = wq.data(); st = starting.data();
+    }
+    if ((rc = seq_pairs_check(ctx, who, multi, n, w, in, false, st)) ||
+        (rc = seq_starts_fit(ctx, who, n_start, starts)))
+        return rc;
     for (int q = 0; multi && q < n; q++)
         if (!in.lefts[q]) ctx->seq_retired[q] = 1;
+    for (int i = 0; i < n_start; i++) {
+        const vo_mseq_start& s = starts[i];
+        ctx->seq_retired[s.slot] = 0;
+        ctx->seq_w[s.slot] = s.w; ctx->seq_h[s.slot] = s.h;
+        ctx->seq_geo_due[s.slot] = 3;
+        // a larger bucket grid is a front graph of its own; the bound never shrinks within a run
+        ctx->seq_lk_bound = std::max(ctx->seq_lk_bound, seq_grid(s.w, s.h));
+    }
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
     const int p = (int)(ctx->seq_submitted & 1);
     const int s0 = ctx->seq_slot, s1 = (s0 + 1) % 3;
@@ -450,12 +560,35 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
     if (in.device) VO_CUDA_CHECK(cudaEventRecord(ctx->fork_ev, ctx->stream));
     // the per-frame buffers of parity p were last read by the back stage of frame k-2
     VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->seq_back_ev[p], 0));
-    // a sequence retired by this or an earlier submission: its units of parity p stop working from this frame on (the
-    // other parity's word is still read by the frame in flight, and is cleared by the next submission)
+    // calibration entries of parity p deferred by a start in the previous submission, then this submission's starts
     for (int q = 0; q < n; q++)
-        if (ctx->seq_retired[q] && ctx->seq_live[p * n + q]) {
-            VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_seq_live + p * n + q, 0, sizeof(int), ctx->stream));
-            ctx->seq_live[p * n + q] = 0;
+        if (ctx->seq_cal_due[p * n + q]) {
+            if ((rc = vo_write_calib(ctx, p * n + q, 1, &ctx->seq_cal_next[p * n + q]))) return rc;
+            ctx->seq_cal_due[p * n + q] = 0;
+        }
+    for (int i = 0; i < n_start; i++) {
+        const int q = starts[i].slot;
+        const CamCalib c = vo_calib_from(starts[i].P_l, starts[i].P_r);
+        if ((rc = vo_write_calib(ctx, p * n + q, 1, &c))) return rc;
+        ctx->seq_cal_next[(1 - p) * n + q] = c;
+        ctx->seq_cal_due[(1 - p) * n + q] = 1;
+        VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_feat_cnt + 2 * q, 0, 2 * sizeof(int), ctx->stream));
+    }
+    // the live words of parity p: a sequence retired by this or an earlier submission (or started by this one) stops
+    // working from this frame on, a started one works from the next; the other parity's word is still read by the frame
+    // in flight, and is written by the next submission
+    for (int q = 0; q < n; q++) {
+        const char want = st && st[q] ? SEQ_STARTED : ctx->seq_retired[q] ? 0 : 1;
+        if ((ctx->seq_live[p * n + q] == 1) != (want == 1))
+            VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_seq_live + p * n + q, want == 1 ? 1 : 0, sizeof(int), ctx->stream));
+        ctx->seq_live[p * n + q] = want;
+    }
+    // geometry entries of the image slot s1 for the pairs of started sequences staged into it
+    for (int q = 0; ctx->seq_sized && !in.device && q < n; q++)
+        if (ctx->seq_geo_due[q] && in.lefts[q]) {
+            const PlaneGeom g = vo_plane_geom(ctx, ctx->seq_w[q], ctx->seq_h[q]), gg[2] = {g, g};
+            if ((rc = vo_write_geo(ctx, 2 * n * s1 + 2 * q, 2, gg))) return rc;
+            ctx->seq_geo_due[q]--;
         }
     if (bgr) {
         // colour frames share one staging buffer: upload + convert stay on the front stream
@@ -481,8 +614,8 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
     key.kind = GraphKey::SEQ_FRONT; key.s = ctx->stream; key.tma = ctx->lk_use_tma;
     key.slot = s0; key.parity = p; key.bgr = bgr;
     // the LK launch bound: the largest bucket grid of the sequences' sizes, which a new set of sizes inside the same
-    // envelope can raise (the sizes themselves are in the geometry table, not in the graph)
-    key.max_pts = seq_grid(ctx);
+    // envelope, or a start, can raise (the sizes themselves are in the geometry table, not in the graph)
+    key.max_pts = ctx->seq_lk_bound;
     if ((rc = vo_run_graph(ctx, key, [&] { return seq_front(ctx, s0, s1, p, bgr); }))) return rc;
     VO_CUDA_CHECK(cudaEventRecord(ctx->seq_front_ev[p], ctx->stream));
     // back stage: after this frame's front stage; after the previous frame's back stage by stream order
@@ -491,6 +624,9 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
     key = GraphKey{};
     key.kind = GraphKey::SEQ_BACK; key.s = sb; key.tma = ctx->lk_use_tma; key.parity = p;
     if ((rc = vo_run_graph(ctx, key, [&] { return seq_back(ctx, p); }))) return rc;
+    // a started sequence's next frame solves from zeros: after k_seq_finish of this frame copied the slot's translation
+    for (int i = 0; i < n_start; i++)
+        VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_tprev + 3 * (size_t)((1 - p) * n + starts[i].slot), 0, 3 * sizeof(double), sb));
     const int u0 = p * n;
     const SeqPinned pin = seq_pinned(ctx, n);
     VO_CUDA_CHECK(cudaMemcpyAsync(pin.rec + u0, ctx->d_results + u0, n * sizeof(vo_unit_result_dev), cudaMemcpyDeviceToHost, sb));
@@ -537,10 +673,15 @@ static int seq_wait(vo_ctx* ctx, const char* who, bool multi, bool want_mono, vo
     cudaStream_t sb = ctx->lane[0].side;
     bool copies = false;
     for (int q = 0; q < n; q++) {
-        if (!ctx->seq_live[u0 + q]) {                   // retired by this submission or an earlier one: nothing ran
+        if (ctx->seq_live[u0 + q] != 1) {               // retired (or never started), or started by this submission: nothing ran
             memset(&out[q], 0, sizeof(out[q]));
             if (mono) memset(&mono[q], 0, sizeof(mono[q]));
             status[q] = VO_MSEQ_RETIRED;
+            if (ctx->seq_live[u0 + q] == SEQ_STARTED) {     // the new sequence's frame_pose starts here (main.cpp:90)
+                status[q] = VO_MSEQ_STARTED;
+                double* pose = ctx->seq_pose.data() + 16 * q;
+                for (int i = 0; i < 16; i++) pose[i] = i % 5 == 0 ? 1.0 : 0.0;
+            }
             continue;
         }
         const vo_unit_result_dev r = pin.rec[u0 + q];
@@ -626,13 +767,15 @@ extern "C" int vo_seq_begin(vo_ctx* ctx, int w, int h, const float P_l[12], cons
 extern "C" int vo_seq_begin_ex(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], const uint8_t* left0,
                                const uint8_t* right0, size_t pitch, int channels)
 {
-    return seq_begin(ctx, "vo_seq_begin", false, 1, 0, &w, &h, P_l, P_r, host_pairs(&left0, &right0, &pitch, channels));
+    const SeqPairs in = host_pairs(&left0, &right0, &pitch, channels);
+    return seq_begin(ctx, "vo_seq_begin", false, 1, 0, &w, &h, P_l, P_r, &in);
 }
 
 extern "C" int vo_seq_begin_device(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], const vo_dimage* left0,
                                    const vo_dimage* right0)
 {
-    return seq_begin(ctx, "vo_seq_begin_device", false, 1, 0, &w, &h, P_l, P_r, device_pair(left0, right0));
+    const SeqPairs in = device_pair(left0, right0);
+    return seq_begin(ctx, "vo_seq_begin_device", false, 1, 0, &w, &h, P_l, P_r, &in);
 }
 
 extern "C" int vo_seq_submit(vo_ctx* ctx, const uint8_t* left1, const uint8_t* right1, size_t pitch, int channels)
@@ -708,14 +851,16 @@ extern "C" int vo_mseq_begin_calib(vo_ctx* ctx, int n_seq, int w, int h, const f
     const int n = n_seq >= 1 && n_seq <= VO_MSEQ_MAX ? n_seq : 1;     // other counts are refused with their message
     const std::vector<int> ws(n, w), hs(n, h);
     const std::vector<size_t> ps(n, pitch);
-    return seq_begin(ctx, "vo_mseq_begin", true, n_seq, flags, ws.data(), hs.data(), P_l, P_r, host_pairs(left0, right0, ps.data(), channels));
+    const SeqPairs in = host_pairs(left0, right0, ps.data(), channels);
+    return seq_begin(ctx, "vo_mseq_begin", true, n_seq, flags, ws.data(), hs.data(), P_l, P_r, &in);
 }
 
 extern "C" int vo_mseq_begin_sized(vo_ctx* ctx, int n_seq, const int* w, const int* h, const float* P_l, const float* P_r,
                                    const uint8_t* const* left0, const uint8_t* const* right0, const size_t* pitch, int channels,
                                    int flags)
 {
-    return seq_begin(ctx, "vo_mseq_begin_sized", true, n_seq, flags, w, h, P_l, P_r, host_pairs(left0, right0, pitch, channels));
+    const SeqPairs in = host_pairs(left0, right0, pitch, channels);
+    return seq_begin(ctx, "vo_mseq_begin_sized", true, n_seq, flags, w, h, P_l, P_r, &in);
 }
 
 // one row pitch for every image: vo_mseq_submit_sized with it repeated (it must cover every live sequence's width)
@@ -729,6 +874,20 @@ extern "C" int vo_mseq_submit_sized(vo_ctx* ctx, const uint8_t* const* left1, co
                                     int channels)
 {
     return seq_submit(ctx, "vo_mseq_submit_sized", true, host_pairs(left1, right1, pitch, channels));
+}
+
+// n_slots empty slots at the envelope max_w x max_h; sequences come in through vo_mseq_submit_start
+extern "C" int vo_mseq_open(vo_ctx* ctx, int n_slots, int max_w, int max_h, int flags)
+{
+    const int n = n_slots >= 1 && n_slots <= VO_MSEQ_MAX ? n_slots : 1;     // other counts are refused with their message
+    const std::vector<int> ws(n, max_w), hs(n, max_h);
+    return seq_begin(ctx, "vo_mseq_open", true, n_slots, flags, ws.data(), hs.data(), nullptr, nullptr, nullptr);
+}
+
+extern "C" int vo_mseq_submit_start(vo_ctx* ctx, const uint8_t* const* left1, const uint8_t* const* right1, const size_t* pitch,
+                                    int channels, int n_start, const vo_mseq_start* starts)
+{
+    return seq_submit(ctx, "vo_mseq_submit_start", true, host_pairs(left1, right1, pitch, channels), n_start, starts);
 }
 
 extern "C" int vo_mseq_wait(vo_ctx* ctx, vo_unit_result* out, int* status, vo_point2f* pts4, int pts_cap)
