@@ -370,7 +370,7 @@ VO_API int vo_seq_state(vo_ctx* ctx, vo_point2f* points, int32_t* ages, int cap,
  * Refused with VO_E_INVALID: n_seq < 1, a third submission in flight, a wait with nothing in flight, a pair with one NULL
  * image, a pair for a retired sequence, unknown flag bits.  VO_E_UNSUPPORTED: the option "mono_rotation" is on (in this
  * mode the branch is asked for with the flag below, for every sequence at once).  VO_E_CAPACITY: n_seq above VO_MSEQ_MAX.
- * Device-memory inputs (vo_dimage) are not accepted in this mode.
+ * Frames already in device memory: vo_mseq_begin_device / vo_mseq_submit_device below.
  * trackingFrame2Frame(mono_rotation = true) for every sequence: vo_mseq_begin_ex with the flag VO_MSEQ_MONO_ROTATION
  * (vo_mseq_begin is vo_mseq_begin_ex with flags = 0).  Each sequence then gets what vo_seq_wait_mono gives a single
  * sequence begun with the option "mono_rotation" -- the record's R is recoverPose's rotation, rvec / tvec / n_inliers /
@@ -448,6 +448,31 @@ typedef struct vo_mseq_start {
 VO_API int vo_mseq_open(vo_ctx* ctx, int n_slots, int max_w, int max_h, int flags);
 VO_API int vo_mseq_submit_start(vo_ctx* ctx, const uint8_t* const* left1, const uint8_t* const* right1, const size_t* pitch,
                                 int channels, int n_start, const vo_mseq_start* starts);
+/* Frames already in device memory (vo_dimage, see vo_seq_begin_device), one descriptor pair per sequence.  Stream contract
+ * as for the *_device calls above: the images are read after the work already enqueued on the context's stream, and work
+ * the caller enqueues there after the call returns is ordered after the library's last read of them.  Each image has its
+ * own format, pitch, strides and alignment (gray, BGR / RGB interleaved or planar), so the sequences of one call may
+ * differ in layout; sequence q's images are read as its own w x h (its begun size, or its start's size).
+ *   vo_mseq_begin_device   vo_mseq_begin_sized with left0[q] / right0[q] in place of host pointers, pitches and channels:
+ *                          sequence q is w[q] x h[q] with the matrices P_l + 12 q / P_r + 12 q; flags takes
+ *                          VO_MSEQ_MONO_ROTATION.  Synchronous, as vo_seq_begin_device: when it returns the first pairs
+ *                          have been read.
+ *   vo_mseq_submit_device  vo_mseq_submit_start with left1[q] / right1[q] in place of host pointers, pitches and channels
+ *                          (n_start = 0: a plain submission).  A pair whose two data pointers are NULL retires its
+ *                          sequence, as a NULL host pair does.  Results through vo_mseq_wait[_mono], vo_mseq_pose and
+ *                          vo_mseq_state.
+ * Both work in every multi-sequence run (begun with any vo_mseq_begin*, with vo_mseq_begin_device or with vo_mseq_open),
+ * and host and device submissions may alternate within a run.  Each sequence's results are those of the same pixels (as
+ * cv::cvtColor(BGR2GRAY / RGB2GRAY) converts colour) through the host entry points, bit for bit.  The 2 * n_seq images of a
+ * submission are converted by ONE kernel launch on the sequence mode's copy stream under the frame in flight, outside the
+ * front stage's graph, so a device submission costs one launch more than a host gray submission whatever n_seq is; each
+ * image is checked with one cudaPointerGetAttributes.  Refused with VO_E_INVALID, changing nothing: NULL left / right
+ * tables, an image that vo_seq_begin_device refuses (at its sequence's width), one NULL image in a pair, a pair for a
+ * retired sequence, and every refusal of vo_mseq_begin_sized / vo_mseq_submit_start (with their codes). */
+VO_API int vo_mseq_begin_device(vo_ctx* ctx, int n_seq, const int* w, const int* h, const float* P_l, const float* P_r,
+                                const vo_dimage* left0, const vo_dimage* right0, int flags);
+VO_API int vo_mseq_submit_device(vo_ctx* ctx, const vo_dimage* left1, const vo_dimage* right1, int n_start,
+                                 const vo_mseq_start* starts);
 VO_API int vo_mseq_wait(vo_ctx* ctx, vo_unit_result* out, int* status, vo_point2f* pts4, int pts_cap);
 VO_API int vo_mseq_wait_mono(vo_ctx* ctx, vo_unit_result* out, int* status, vo_mono_result* mono,
                              uint8_t* ess_mask, int mask_cap, vo_point2f* pts4, int pts_cap);

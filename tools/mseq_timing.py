@@ -2,7 +2,7 @@
 """Scaling of the multi-sequence streaming mode (vo_mseq_*) with the number of sequences, measured on the GPU.
 
     python tools/mseq_timing.py [--frames 40] [--rounds 5] [--counts 1,2,4,8,16,32] [--mono-rotation] [--mixed-calibration]
-                                [--mixed-sizes] [--json out.json]
+                                [--mixed-sizes] [--device-input] [--json out.json]
 
 Synthetic 1241x376 drives (synth.stereo_unit; eight seeds, each with its own motion) of `--frames` frames each;
 sequence q replays drive q % 8, forwards for even q // 8 and backwards for odd, so up to 16 sequences are distinct and
@@ -20,7 +20,11 @@ of the one-calibration run.  Both are timed in the same rounds, alternated.  `--
 --counts is given) also runs every vo_mseq_* count with sequence q at the image size of KITTI odometry training sequence
 q mod 11 (1241x376 for 00-02, 1242x375 for 03, 1226x370 for 04-10: the 3 : 1 : 7 mix of the training set, through
 vo_mseq_begin_sized), the drives rendered at those sizes with the motions of the one-size run, timed against the same
-count all at 1241x376 in the same rounds, alternated.  The card's name, power limit and max SM clock, read in the same run, are printed with the numbers;
+count all at 1241x376 in the same rounds, alternated.  `--device-input` (counts 1, 8, 16 and 32 unless --counts is given)
+times every vo_mseq_* count three ways in the same rounds, alternated: host gray images (vo_mseq_submit, the loop above),
+and every frame made resident as CUDA tensors before the timed window and fed through vo_mseq_submit_device as gray
+(H, W) and as BGR (H, W, 3) tensors; it also times the host side of one vo_mseq_submit_device call (the binding, and the
+C call alone) at 32 and 64 sequences.  The card's name, power limit and max SM clock, read in the same run, are printed with the numbers;
 they are part of them."""
 import argparse
 import json
@@ -115,6 +119,44 @@ def run_mseq(ctx, P_l, P_r, seqs, mono=False):
     return n * steps / dt, dt / steps, (ctx.kernel_launches() - l0) / steps
 
 
+def run_mseq_device(ctx, P_l, P_r, seqs, order=None):
+    """run_mseq with every frame a CUDA tensor (resident before the timed window) through vo_mseq_submit_device"""
+    n, nf = len(seqs), len(seqs[0])
+    ctx.mseq_begin_device([s[0][0] for s in seqs], [s[0][1] for s in seqs], P_l, P_r, order=order)
+    frame = [([s[k][0] for s in seqs], [s[k][1] for s in seqs]) for k in range(nf)]
+    l0 = ctx.kernel_launches()
+    t0 = time.perf_counter()
+    ctx.mseq_submit_device(*frame[1], order=order)
+    for k in range(1, nf):
+        if k + 1 < nf:
+            ctx.mseq_submit_device(*frame[k + 1], order=order)
+        ctx.mseq_wait(want_points=False)
+    dt = time.perf_counter() - t0
+    steps = nf - 1
+    return n * steps / dt, dt / steps, (ctx.kernel_launches() - l0) / steps
+
+
+def submit_host_cost(ctx, P_l, P_r, seqs, reps=50):
+    """median host time of one vo_mseq_submit_device call [us]: through the binding, and the C call alone (descriptor
+    tables built beforehand); each call is waited for outside the timed region"""
+    n = len(seqs)
+    ctx.mseq_begin_device([s[0][0] for s in seqs], [s[0][1] for s in seqs], P_l, P_r)
+    lefts, rights = [s[1][0] for s in seqs], [s[1][1] for s in seqs]
+    lt, rt, _ = ctx._device_pairs(lefts, rights, None, n, False)
+    binding, call = [], []
+    for _ in range(reps):
+        t0 = time.perf_counter()
+        ctx.mseq_submit_device(lefts, rights)
+        binding.append(time.perf_counter() - t0)
+        ctx.mseq_wait(want_points=False)
+        t0 = time.perf_counter()
+        rc = ctx.lib.vo_mseq_submit_device(ctx.h, lt, rt, 0, None)
+        call.append(time.perf_counter() - t0)
+        ctx._check(rc)
+        ctx.mseq_wait(want_points=False)
+    return 1e6 * float(np.median(binding)), 1e6 * float(np.median(call))
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--frames", type=int, default=40)
@@ -125,10 +167,14 @@ def main():
                     help="also time every vo_mseq_* count with a distinct calibration per sequence")
     ap.add_argument("--mixed-sizes", action="store_true",
                     help="also time every vo_mseq_* count with the KITTI training set's three image sizes")
+    ap.add_argument("--device-input", action="store_true",
+                    help="also time every vo_mseq_* count with frames resident in GPU memory (gray and BGR tensors)")
     ap.add_argument("--json", help="also write the result here")
     a = ap.parse_args()
     if a.mixed_sizes and a.counts == ap.get_default("counts"):
         a.counts = "3,11,32"
+    if a.device_input and a.counts == ap.get_default("counts"):
+        a.counts = "1,8,16,32"
     counts = [int(c) for c in a.counts.split(",")]
     from visual_odom_b200 import capi, synth
     P_l, P_r = synth.proj_matrices()
@@ -140,6 +186,8 @@ def main():
     modes = [(m, mono, mix) for m in ["seq"] + counts for mono in monos for mix in mixes if not (m == "seq" and mix)]
     if a.mixed_sizes:
         modes += [(m, mono, "sizes") for m in counts for mono in monos]
+    if a.device_input:
+        modes += [(m, False, kind) for m in counts for kind in ("dev-gray", "dev-bgr")]
     seqs = {n: [sequence(dr, q) for q in range(n)] for n in counts}
     mixed = {}
     if a.mixed_calibration:              # per count n: sequence q rendered with calibration(q, n), played like sequence(dr, q)
@@ -157,6 +205,15 @@ def main():
         for n in counts:
             sized[n] = [sequence(by_size[KITTI_SIZES[q % len(KITTI_SIZES)]], q) for q in range(n)]
         print(f"rendered the drives at {len(by_size)} image sizes in {time.perf_counter() - t0:.0f} s", flush=True)
+    dev = {}
+    if a.device_input:                   # every frame of every drive resident on the GPU, gray and BGR, before any timing
+        import torch
+        for kind in ("dev-gray", "dev-bgr"):
+            t = [[tuple(torch.from_numpy(np.ascontiguousarray(x if kind == "dev-gray" else np.repeat(x[:, :, None], 3, axis=2)))
+                        .cuda() for x in pair) for pair in fr] for fr in dr]
+            dev[kind] = {n: [sequence(t, q) for q in range(n)] for n in set(counts) | {32, 64}}
+        torch.cuda.synchronize()
+        print(f"resident on the GPU: {torch.cuda.memory_allocated() / 2**30:.2f} GiB", flush=True)
     ctx = capi.Context(0, max_features=4096)
     res = {m: dict(fps=[], lat=[], launches=[]) for m in modes}
 
@@ -165,6 +222,9 @@ def main():
         if m == "seq":
             fr = dr[0] if fr_cut is None else dr[0][:fr_cut]
             return run_seq(ctx, P_l, P_r, fr, mono)
+        if mix in ("dev-gray", "dev-bgr"):
+            s = dev[mix][m] if fr_cut is None else [x[:fr_cut] for x in dev[mix][m]]
+            return run_mseq_device(ctx, P_l, P_r, s, "bgr" if mix == "dev-bgr" else None)
         s, Pl, Pr = (sized[m], P_l, P_r) if mix == "sizes" else (mixed[m] if mix else (seqs[m], P_l, P_r))
         s = s if fr_cut is None else [x[:fr_cut] for x in s]
         return run_mseq(ctx, Pl, Pr, s, mono)
@@ -174,8 +234,11 @@ def main():
             run(m, 4)                     # warm-up: (re-)captures the mode's graphs, untimed
             fps, lat, launches = run(m)
             res[m]["fps"].append(fps); res[m]["lat"].append(lat); res[m]["launches"].append(launches)
+    host_cost = {n: submit_host_cost(ctx, P_l, P_r, dev["dev-gray"][n]) for n in (32, 64)} if a.device_input else {}
     ctx.close()
     out = dict(card=card(), image=f"{W}x{H}", frames=a.frames, rounds=a.rounds, in_flight=2, modes={})
+    if host_cost:
+        out["submit_device_host_us"] = {str(n): dict(binding=b, c_call=c) for n, (b, c) in host_cost.items()}
     print(f"card (name, power limit, max SM clock): {out['card']}")
     for mode in modes:
         r = res[mode]
@@ -183,11 +246,15 @@ def main():
                  aggregate_fps_max=float(np.max(r["fps"])), step_latency_ms=1e3 * float(np.median(r["lat"])),
                  launches_per_submission=float(np.median(r["launches"])))
         m, mono, mix = mode
-        out["modes"][str(m) + ("+mono" if mono else "") + ("+sizes" if mix == "sizes" else "+mixed" if mix else "")] = o
+        out["modes"][str(m) + ("+mono" if mono else "") + ("+sizes" if mix == "sizes" else f"+{mix}" if mix in ("dev-gray", "dev-bgr")
+                               else "+mixed" if mix else "")] = o
         name = ("vo_seq (1 sequence)" if m == "seq" else f"vo_mseq n_seq = {m:2d}") + (", mono" if mono else "") + \
-            (", KITTI sizes" if mix == "sizes" else ", mixed cal." if mix else "")
+            (", KITTI sizes" if mix == "sizes" else ", device gray" if mix == "dev-gray" else ", device BGR" if mix == "dev-bgr"
+             else ", mixed cal." if mix else "")
         print(f"{name:40s}: {o['aggregate_fps']:8.0f} frames/s [{o['aggregate_fps_min']:.0f}, {o['aggregate_fps_max']:.0f}], "
               f"step {o['step_latency_ms']:.3f} ms, {o['launches_per_submission']:.1f} launches / submission")
+    for n, (b, c) in host_cost.items():
+        print(f"one vo_mseq_submit_device, n_seq = {n:2d}: host {b:.1f} us through the binding, {c:.1f} us in the C call")
     print(json.dumps(out))
     if a.json:
         os.makedirs(os.path.dirname(os.path.abspath(a.json)), exist_ok=True)

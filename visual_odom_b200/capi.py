@@ -194,6 +194,9 @@ SIGNATURES = {
     "vo_mseq_submit_sized": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "vo_mseq_open": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]),
     "vo_mseq_submit_start": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(VoMseqStart)]),
+    "vo_mseq_begin_device": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(VoDImage),
+                                       C.POINTER(VoDImage), C.c_int]),
+    "vo_mseq_submit_device": (C.c_int, [C.c_void_p, C.POINTER(VoDImage), C.POINTER(VoDImage), C.c_int, C.POINTER(VoMseqStart)]),
     "vo_mseq_wait": (C.c_int, [C.c_void_p, C.POINTER(VoUnitResult), C.c_void_p, C.c_void_p, C.c_int]),
     "vo_mseq_wait_mono": (C.c_int, [C.c_void_p, C.POINTER(VoUnitResult), C.c_void_p, C.POINTER(VoMonoResult), C.c_void_p,
                                     C.c_int, C.c_void_p, C.c_int]),
@@ -775,6 +778,7 @@ class Context:
             P_l = P_l.reshape(12); P_r = P_r.reshape(12)
             self._check(self.lib.vo_mseq_begin_ex(self.h, n, w, h, _p(P_l), _p(P_r), lp, rp, pitch, ch, flags))
         self._mseq_n, self._mseq_pitch = n, pitch
+        self._mseq_sizes = [(int(h), int(w))] * n
         self._mseq_keep = [None, None]
 
     def mseq_begin(self, lefts, rights, P_l, P_r, mono_rotation=False):
@@ -866,6 +870,66 @@ class Context:
             # with every sequence retired no image is read: the pitch of the first pairs passes the width check
             self._check(self.lib.vo_mseq_submit(self.h, lp, rp, pitch or self._mseq_pitch, ch))
         self._mseq_keep = [self._mseq_keep[1], keep]
+
+    # ---- several sequences from images already on the GPU (vo_mseq_begin_device / vo_mseq_submit_device) ------------------
+    def _device_pairs(self, lefts, rights, order, n, allow_none):
+        """(left descriptor table, right descriptor table, sizes) of one pair of CUDA uint8 tensors per sequence, as
+        _device_image reads them; sizes[q] = (h, w) of sequence q's pair, None for a (None, None) pair (allow_none: NULL
+        descriptors, which retire the sequence).  order: one string for every colour pair, or one per sequence."""
+        if len(lefts) != n or len(rights) != n:
+            raise ValueError(f"{len(lefts)} left and {len(rights)} right images for {n} sequences")
+        orders = [order] * n if order is None or isinstance(order, str) else list(order)
+        if len(orders) != n:
+            raise ValueError(f"{len(orders)} orders for {n} sequences")
+        lt, rt = (VoDImage * n)(), (VoDImage * n)()
+        sizes = [None] * n
+        for q, (l, r) in enumerate(zip(lefts, rights)):
+            if l is None and r is None and allow_none:
+                continue
+            if l is None or r is None:
+                raise ValueError(f"sequence {q}: a pair needs both images (None, None retires a sequence)")
+            (dl, w, h), (dr, wr, hr) = self._device_image(l, orders[q]), self._device_image(r, orders[q])
+            if (wr, hr) != (w, h):
+                raise ValueError(f"sequence {q}: left image {w} x {h}, right image {wr} x {hr}")
+            lt[q], rt[q], sizes[q] = dl, dr, (h, w)
+        return lt, rt, sizes
+
+    def mseq_begin_device(self, lefts, rights, P_l, P_r, order=None, mono_rotation=False):
+        """mseq_begin from CUDA uint8 tensors (H, W), (H, W, 3) or (3, H, W), one pair per sequence, each sequence at its
+        pair's size and in its own layout (vo_mseq_begin_device; synchronous).  order: "bgr" / "rgb" for colour pairs, one
+        string or one per sequence.  P_l / P_r: (3, 4) for one calibration, or (n_seq, 3, 4)."""
+        n = len(lefts)
+        lt, rt, sizes = self._device_pairs(lefts, rights, order, n, False)
+        P_l = np.ascontiguousarray(np.broadcast_to(np.asarray(P_l, np.float32), (n, 3, 4)))
+        P_r = np.ascontiguousarray(np.broadcast_to(np.asarray(P_r, np.float32), (n, 3, 4)))
+        wa = np.array([g[1] for g in sizes], np.int32); ha = np.array([g[0] for g in sizes], np.int32)
+        flags = VO_MSEQ_MONO_ROTATION if mono_rotation else 0
+        self._device_call(self.lib.vo_mseq_begin_device, n, _p(wa), _p(ha), _p(P_l), _p(P_r), lt, rt, flags)
+        # host submissions may follow: the pitch state mseq_begin leaves for these sizes
+        uniform = all(g == sizes[0] for g in sizes)
+        self._mseq_n, self._mseq_pitch = n, (int(wa[0]) if uniform else wa.astype(np.uint64))
+        self._mseq_sizes = list(sizes)
+        self._mseq_keep = [None, None]
+
+    def mseq_submit_device(self, lefts, rights, start=None, order=None):
+        """mseq_submit from CUDA uint8 tensors (vo_mseq_submit_device): one frame of every sequence, a (None, None) pair
+        retires that sequence; start = {slot: (P_l, P_r)} starts new sequences at their pairs' sizes.  Each pair must have
+        its sequence's size.  The tensors may be overwritten or freed stream-ordered as soon as the call returns."""
+        n = self._mseq_n
+        lt, rt, sizes = self._device_pairs(lefts, rights, order, n, True)
+        start = dict(start or {})
+        for q in start:
+            if not 0 <= q < n or sizes[q] is None:
+                raise ValueError(f"slot {q}: a start needs its first pair")
+        known = getattr(self, "_mseq_sizes", [None] * n)
+        for q, g in enumerate(sizes):
+            if g is not None and q not in start and known[q] is not None and g != known[q]:
+                raise ValueError(f"sequence {q}: image size {g[1]} x {g[0]}, the sequence is {known[q][1]} x {known[q][0]}")
+        arr, ns = self._starts({q: (sizes[q][1], sizes[q][0], P[0], P[1]) for q, P in start.items()}) if start else (None, 0)
+        self._device_call(self.lib.vo_mseq_submit_device, lt, rt, ns, arr)
+        for q in start:
+            self._mseq_sizes[q] = sizes[q]
+        self._mseq_keep = [self._mseq_keep[1], None]        # a host submission still in flight keeps its arrays
 
     def mseq_wait(self, pts_cap=4096, want_points=True, mono=False):
         """The oldest submission: one dict per sequence with seq_wait's keys plus "status" (VO_OK, VO_E_CAPACITY or

@@ -560,11 +560,12 @@ PlaneGeom vo_plane_geom(const vo_ctx* ctx, int w, int h)
     return g;
 }
 
-int vo_write_geo(vo_ctx* ctx, int p0, int n, const PlaneGeom* g)
+int vo_write_geo(vo_ctx* ctx, int p0, int n, const PlaneGeom* g, cudaStream_t st)
 {
     if (memcmp(ctx->geo.data() + p0, g, n * sizeof(PlaneGeom)) == 0) return VO_OK;
     memcpy(ctx->geo.data() + p0, g, n * sizeof(PlaneGeom));
-    VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_geo + p0, ctx->geo.data() + p0, n * sizeof(PlaneGeom), cudaMemcpyHostToDevice, ctx->stream));
+    VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_geo + p0, ctx->geo.data() + p0, n * sizeof(PlaneGeom), cudaMemcpyHostToDevice,
+                                  st ? st : ctx->stream));
     return VO_OK;
 }
 

@@ -217,8 +217,9 @@ struct vo_ctx {
 void vo_set_error(vo_ctx* ctx, const char* fmt, ...);
 // levels > 0: that pyramid depth (the common depth of a run's image sizes, which their envelope w x h may exceed)
 int vo_ensure_state(vo_ctx* ctx, int w, int h, int units, int levels = 0);
-// geometry table entries [p0, p0 + n) = g[0 .. n), written on ctx->stream only where they change (as vo_write_calib)
-int vo_write_geo(vo_ctx* ctx, int p0, int n, const PlaneGeom* g);
+// geometry table entries [p0, p0 + n) = g[0 .. n), written on st (nullptr: ctx->stream) only where they change (as
+// vo_write_calib)
+int vo_write_geo(vo_ctx* ctx, int p0, int n, const PlaneGeom* g, cudaStream_t st = nullptr);
 // the geometry of a w x h image in the allocated pyramid's levels (raw rows packed)
 PlaneGeom vo_plane_geom(const vo_ctx* ctx, int w, int h);
 void vo_free_state(vo_ctx* ctx);
@@ -251,15 +252,17 @@ int vo_ensure_pinned(vo_ctx* ctx, size_t bytes);
 int vo_upload_plane(vo_ctx* ctx, uint8_t* dst, const uint8_t* src, size_t row_bytes, int h, size_t pitch, cudaStream_t st);
 int vo_ensure_bgr(vo_ctx* ctx, size_t bytes);
 // k_bgr_to_gray: images tab[0 .. n_img) (device table), or with d_tab == nullptr `packed` advanced by packed_stride per image,
-// into gray planes img_stride_out apart; geo: the images' geometry table entries (packed input only; nullptr: all w x h)
+// into gray planes img_stride_out apart; geo: the images' geometry table entries (nullptr: all w x h).  A table entry
+// with data == NULL is skipped.
 int vo_launch_bgr_to_gray(const vo_dimage* d_tab, const vo_dimage& packed, size_t packed_stride, uint8_t* d_gray, size_t img_stride_out,
                           int w, int h, int n_img, cudaStream_t s, const PlaneGeom* geo = nullptr);
 vo_dimage vo_packed_bgr(const uint8_t* d_bgr, int w);      // the descriptor of w-pixel packed BGR rows
 // VO_E_INVALID + message unless `im` can be read as an image `w` pixels wide in device memory of the context's GPU
 int vo_check_dimage(vo_ctx* ctx, const char* who, const char* name, const vo_dimage* im, int w);
 // caller device images h_tab[0 .. n) (pinned staging, untouched until the copy has run on st) -> raw planes
-// [plane0, plane0 + n): one descriptor copy into d_ingest_tab + plane0 and one k_bgr_to_gray launch on st
-int vo_ingest_device(vo_ctx* ctx, const vo_dimage* h_tab, int n, int plane0, cudaStream_t st);
+// [plane0, plane0 + n): one descriptor copy into d_ingest_tab + plane0 and one k_bgr_to_gray launch on st.  geo: the
+// planes' geometry table entries (images of several sizes, each written packed from its plane's start; nullptr: all w x h)
+int vo_ingest_device(vo_ctx* ctx, const vo_dimage* h_tab, int n, int plane0, cudaStream_t st, const PlaneGeom* geo = nullptr);
 // a contiguous range of resident work units processed on one stream
 // plane0 >= 0 overrides the image-plane base (default u0 * imgs): the sequence mode ping-pongs its per-frame buffers
 // between two buffer parities while both address the same image ring.  imgs: image planes per unit (4: a stereo pair at

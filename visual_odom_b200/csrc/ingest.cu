@@ -349,7 +349,8 @@ extern "C" void vo_reader_close(vo_reader* rd)
 // cannot take a per-frame table).  Sources may have any alignment, pitch and strides: every pixel is read with byte
 // loads.  Colour: cv::cvtColor(BGR2GRAY / RGB2GRAY)'s fixed point; gray: the identity (which the formula is on b=g=r).
 // With a geometry table (geo[img]: images of several sizes, w x h the envelope) image z is geo[z]'s own size, its packed
-// source rows 3 * w[0] bytes apart and its gray rows w[0].
+// source rows 3 * w[0] bytes apart (a table source keeps its own pitch) and its gray rows w[0].  A table entry with
+// data == NULL (a retired or empty slot of the multi-sequence mode) is skipped: its plane keeps what it held.
 __global__ void k_bgr_to_gray(const vo_dimage* __restrict__ tab, vo_dimage packed, size_t packed_stride, uint8_t* __restrict__ gray,
                               size_t img_stride_out, int w, int h, const PlaneGeom* __restrict__ geo)
 {
@@ -358,8 +359,10 @@ __global__ void k_bgr_to_gray(const vo_dimage* __restrict__ tab, vo_dimage packe
     vo_dimage src = packed;
     if (geo) { w = geo[img].w[0]; h = geo[img].h[0]; src.row_pitch = (size_t)3 * w; }
     if (x0 >= w || y >= h) return;
-    if (tab) src = tab[img];
-    else src.data += (size_t)img * packed_stride;
+    if (tab) {
+        src = tab[img];
+        if (!src.data) return;
+    } else src.data += (size_t)img * packed_stride;
     const uint8_t* s = src.data + (size_t)y * src.row_pitch + (size_t)x0 * src.pixel_stride;
     const size_t cs = src.channel_stride;
     uint8_t* d = gray + (size_t)img * img_stride_out + (size_t)y * w + x0;
@@ -424,12 +427,12 @@ int vo_check_dimage(vo_ctx* ctx, const char* who, const char* name, const vo_dim
     return VO_OK;
 }
 
-int vo_ingest_device(vo_ctx* ctx, const vo_dimage* h_tab, int n, int plane0, cudaStream_t st)
+int vo_ingest_device(vo_ctx* ctx, const vo_dimage* h_tab, int n, int plane0, cudaStream_t st, const PlaneGeom* geo)
 {
     const size_t plane = (size_t)ctx->w * ctx->h;
     VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_ingest_tab + plane0, h_tab, (size_t)n * sizeof(vo_dimage), cudaMemcpyHostToDevice, st));
     ctx->launches += vo_launch_bgr_to_gray(ctx->d_ingest_tab + plane0, vo_dimage{}, 0, ctx->d_raw + (size_t)plane0 * plane, plane,
-                                           ctx->w, ctx->h, n, st);
+                                           ctx->w, ctx->h, n, st, geo);
     VO_CUDA_CHECK(cudaGetLastError());
     return VO_OK;
 }

@@ -203,14 +203,16 @@ static int seq_back(vo_ctx* ctx, int p)
 }
 
 // pinned staging of the sequence mode: the records and error words of the 2 * n_seq units (both parities) |
-// EssResult[2 * n_seq] (mono sequences only) | vo_dimage[6] (device-image descriptors, one per raw plane of the three-slot ring; plane 2s + k
-// is restaged only after the frame that last used it has been waited for)
+// EssResult[2 * n_seq] (mono sequences only) | vo_dimage[6 * n_seq] (device-image descriptors, one per raw plane of the
+// three-slot ring, indexed by plane: entry 2 * n_seq * s + 2q + k is sequence q's image k of slot s).  Slot s's entries are
+// rewritten by the submission that stages into s, three submissions after the one that last copied them to the device;
+// with at most two submissions in flight that one has been waited for, so its copy has run.
 struct SeqPinned { vo_unit_result_dev* rec; int* err; EssResult* ess; vo_dimage* tab; size_t bytes; };
 static SeqPinned seq_pinned(vo_ctx* ctx, int n)
 {
     auto up = [](size_t b) { return (b + 255) / 256 * 256; };
     const size_t o_err = up(2 * (size_t)n * sizeof(vo_unit_result_dev)), o_ess = up(o_err + 2 * (size_t)n * sizeof(int));
-    const size_t o_tab = up(o_ess + 2 * (size_t)n * sizeof(EssResult)), end = up(o_tab + 6 * sizeof(vo_dimage));
+    const size_t o_tab = up(o_ess + 2 * (size_t)n * sizeof(EssResult)), end = up(o_tab + 6 * (size_t)n * sizeof(vo_dimage));
     uint8_t* b = (uint8_t*)ctx->h_pinned;
     return SeqPinned{(vo_unit_result_dev*)b, (int*)(b + o_err), (EssResult*)(b + o_ess), (vo_dimage*)(b + o_tab), end};
 }
@@ -255,18 +257,21 @@ static int seq_drain(vo_ctx* ctx)
     return VO_OK;
 }
 
-// where the new pairs of a begin or submit call come from: host images (gray or BGR, sequence q's pitch[q] bytes per row;
-// in a multi-sequence submission a NULL pair retires its sequence) or one device pair (vo_seq_*_device)
+// where the new pairs of a begin or submit call come from: host images (gray or BGR, sequence q's pitch[q] bytes per row)
+// or device images (vo_seq_*_device, vo_mseq_*_device: sequence q's pair is dl[q] / dr[q]).  In a multi-sequence
+// submission a NULL pair (host pointers, or descriptors whose data are NULL) retires its sequence.
 struct SeqPairs {
     const uint8_t* const* lefts; const uint8_t* const* rights; const size_t* pitch; int channels;
     bool device; const vo_dimage* dl; const vo_dimage* dr;
     bool bgr() const { return !device && channels == 3; }
+    bool left(int q) const { return device ? dl[q].data != nullptr : lefts[q] != nullptr; }
+    bool right(int q) const { return device ? dr[q].data != nullptr : rights[q] != nullptr; }
 };
 static SeqPairs host_pairs(const uint8_t* const* lefts, const uint8_t* const* rights, const size_t* pitch, int channels)
 {
     return SeqPairs{lefts, rights, pitch, channels, false, nullptr, nullptr};
 }
-static SeqPairs device_pair(const vo_dimage* left, const vo_dimage* right) { return SeqPairs{nullptr, nullptr, nullptr, 1, true, left, right}; }
+static SeqPairs device_pairs(const vo_dimage* lefts, const vo_dimage* rights) { return SeqPairs{nullptr, nullptr, nullptr, 1, true, lefts, rights}; }
 
 // the new pairs' own checks (w[q]: sequence q's image width; begin: the first pairs, which every sequence needs; starting[q]:
 // the pair starts a new sequence in slot q of a running submission, so it needs both images and may follow a retirement).
@@ -276,22 +281,31 @@ static int seq_pairs_check(vo_ctx* ctx, const char* who, bool multi, int n, cons
 {
     int rc;
     if (in.device) {
-        if ((rc = vo_check_dimage(ctx, who, begin ? "left0" : "left1", in.dl, w[0])) ||
-            (rc = vo_check_dimage(ctx, who, begin ? "right0" : "right1", in.dr, w[0]))) return rc;
-        return VO_OK;
-    }
-    if (in.channels != 1 && in.channels != 3) { vo_set_error(ctx, "%s: channels must be 1 (gray) or 3 (BGR)", who); return VO_E_INVALID; }
-    if (!in.lefts || !in.rights || !in.pitch || (!multi && (!in.lefts[0] || !in.rights[0]))) {
-        vo_set_error(ctx, "%s: bad argument", who);
-        return VO_E_INVALID;
-    }
-    for (int q = 0; q < n; q++)
-        if (in.lefts[q] && in.pitch[q] < (size_t)w[q] * in.channels) {
-            vo_set_error(ctx, "%s: bad argument (sequence %d: pitch %zu < %d pixels x %d channel(s))", who, q, in.pitch[q], w[q], in.channels);
+        if (!in.dl || !in.dr) { vo_set_error(ctx, "%s: bad argument", who); return VO_E_INVALID; }
+        // a single sequence's images, and every image of a pair that is read, as sequence q's w[q] pixels
+        char name[32];
+        for (int q = 0; q < n; q++)
+            for (int k = 0; k < 2; k++) {
+                const vo_dimage* im = k ? in.dr + q : in.dl + q;
+                if (multi && !in.left(q) && !in.right(q)) continue;
+                if (multi && !im->data) continue;             // one image of a pair: refused below
+                snprintf(name, sizeof(name), multi ? "%s%c[%d]" : "%s%c", k ? "right" : "left", begin ? '0' : '1', q);
+                if ((rc = vo_check_dimage(ctx, who, name, im, w[q]))) return rc;
+            }
+    } else {
+        if (in.channels != 1 && in.channels != 3) { vo_set_error(ctx, "%s: channels must be 1 (gray) or 3 (BGR)", who); return VO_E_INVALID; }
+        if (!in.lefts || !in.rights || !in.pitch || (!multi && (!in.lefts[0] || !in.rights[0]))) {
+            vo_set_error(ctx, "%s: bad argument", who);
             return VO_E_INVALID;
         }
+        for (int q = 0; q < n; q++)
+            if (in.lefts[q] && in.pitch[q] < (size_t)w[q] * in.channels) {
+                vo_set_error(ctx, "%s: bad argument (sequence %d: pitch %zu < %d pixels x %d channel(s))", who, q, in.pitch[q], w[q], in.channels);
+                return VO_E_INVALID;
+            }
+    }
     for (int q = 0; multi && q < n; q++) {
-        const bool l = in.lefts[q] != nullptr, r = in.rights[q] != nullptr;
+        const bool l = in.left(q), r = in.right(q);
         const bool first = begin || (starting && starting[q]);
         if (first && !(l && r)) { vo_set_error(ctx, "%s: sequence %d has no first pair", who, q); return VO_E_INVALID; }
         if (!begin && l != r) { vo_set_error(ctx, "%s: sequence %d has only one image (a NULL pair retires it)", who, q); return VO_E_INVALID; }
@@ -300,14 +314,17 @@ static int seq_pairs_check(vo_ctx* ctx, const char* who, bool multi, int n, cons
     return VO_OK;
 }
 
-// the new pairs into image slot `slot` on st: host pairs as upload_pairs writes them, a device pair converted into the
-// slot's two raw planes through the slot's entries of the pinned descriptor table
+// the new pairs into image slot `slot` on st: host pairs as upload_pairs writes them; device pairs converted into the
+// slot's 2 * n_seq raw planes by ONE k_bgr_to_gray launch through the slot's entries of the pinned descriptor table (a
+// retiring or empty slot's entries have data == NULL: its planes keep their stale contents, as a skipped host upload
+// leaves them), each image at its plane's own size from the geometry table in a run of several sizes
 static int stage_pairs(vo_ctx* ctx, int slot, const SeqPairs& in, cudaStream_t st)
 {
     if (!in.device) return upload_pairs(ctx, slot, in.lefts, in.rights, in.pitch, in.channels, st);
-    vo_dimage* tab = seq_pinned(ctx, ctx->seq_n).tab + 2 * slot;
-    tab[0] = *in.dl; tab[1] = *in.dr;
-    return vo_ingest_device(ctx, tab, 2, 2 * slot, st);
+    const int n = ctx->seq_n;
+    vo_dimage* tab = seq_pinned(ctx, n).tab + 2 * n * slot;
+    for (int q = 0; q < n; q++) { tab[2 * q] = in.dl[q]; tab[2 * q + 1] = in.dr[q]; }
+    return vo_ingest_device(ctx, tab, 2 * n, 2 * n * slot, st, ctx->seq_sized ? ctx->d_geo + 2 * n * slot : nullptr);
 }
 
 // n new sequences (multi: begun by vo_mseq_begin*) from their first pairs `in`; sequence q is w[q] x h[q] and runs with
@@ -541,7 +558,7 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
         (rc = seq_starts_fit(ctx, who, n_start, starts)))
         return rc;
     for (int q = 0; multi && q < n; q++)
-        if (!in.lefts[q]) ctx->seq_retired[q] = 1;
+        if (!in.left(q)) ctx->seq_retired[q] = 1;
     for (int i = 0; i < n_start; i++) {
         const vo_mseq_start& s = starts[i];
         ctx->seq_retired[s.slot] = 0;
@@ -583,13 +600,24 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
             VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_seq_live + p * n + q, want == 1 ? 1 : 0, sizeof(int), ctx->stream));
         ctx->seq_live[p * n + q] = want;
     }
-    // geometry entries of the image slot s1 for the pairs of started sequences staged into it
-    for (int q = 0; ctx->seq_sized && !in.device && q < n; q++)
-        if (ctx->seq_geo_due[q] && in.lefts[q]) {
-            const PlaneGeom g = vo_plane_geom(ctx, ctx->seq_w[q], ctx->seq_h[q]), gg[2] = {g, g};
-            if ((rc = vo_write_geo(ctx, 2 * n * s1 + 2 * q, 2, gg))) return rc;
-            ctx->seq_geo_due[q]--;
-        }
+    // geometry entries of the image slot s1 for the pairs of started sequences staged into it, on stream gs.  Host pairs:
+    // on the front stream here (their upload reads no entry; the front stage's kernels do).  Device pairs: the conversion
+    // on the copy stream reads them, and it is not ordered after this point of the front stream (it follows fork_ev,
+    // recorded before the wait for seq_back_ev[p] above, so that it does not queue behind frame k-2's pose solve); they are
+    // written on the copy stream after its waits below instead.  Either way every earlier reader of slot s1's entries (the
+    // front stage of frame k-2, which seq_front_ev[p] covers) is done, and every later one (the conversion, the front
+    // stage of this frame) follows the write.
+    auto write_geo = [&](cudaStream_t gs) {
+        for (int q = 0; ctx->seq_sized && q < n; q++)
+            if (ctx->seq_geo_due[q] && in.left(q)) {
+                const PlaneGeom g = vo_plane_geom(ctx, ctx->seq_w[q], ctx->seq_h[q]), gg[2] = {g, g};
+                const int rw = vo_write_geo(ctx, 2 * n * s1 + 2 * q, 2, gg, gs);
+                if (rw) return rw;
+                ctx->seq_geo_due[q]--;
+            }
+        return VO_OK;
+    };
+    if (!in.device && (rc = write_geo(ctx->stream))) return rc;
     if (bgr) {
         // colour frames share one staging buffer: upload + convert stay on the front stream
         if ((rc = stage_pairs(ctx, s1, in, ctx->stream))) return rc;
@@ -604,6 +632,7 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
         cudaStream_t sc = ctx->lane[1].side;
         VO_CUDA_CHECK(cudaStreamWaitEvent(sc, ctx->seq_front_ev[p], 0));
         if (in.device) VO_CUDA_CHECK(cudaStreamWaitEvent(sc, ctx->fork_ev, 0));
+        if (in.device && (rc = write_geo(sc))) return rc;
         if ((rc = stage_pairs(ctx, s1, in, sc))) return rc;
         // The join is also the release of device images: the caller's later work on ctx->stream is ordered after the
         // conversion, the last read of the images.
@@ -774,7 +803,7 @@ extern "C" int vo_seq_begin_ex(vo_ctx* ctx, int w, int h, const float P_l[12], c
 extern "C" int vo_seq_begin_device(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], const vo_dimage* left0,
                                    const vo_dimage* right0)
 {
-    const SeqPairs in = device_pair(left0, right0);
+    const SeqPairs in = device_pairs(left0, right0);
     return seq_begin(ctx, "vo_seq_begin_device", false, 1, 0, &w, &h, P_l, P_r, &in);
 }
 
@@ -785,7 +814,7 @@ extern "C" int vo_seq_submit(vo_ctx* ctx, const uint8_t* left1, const uint8_t* r
 
 extern "C" int vo_seq_submit_device(vo_ctx* ctx, const vo_dimage* left1, const vo_dimage* right1)
 {
-    return seq_submit(ctx, "vo_seq_submit_device", false, device_pair(left1, right1));
+    return seq_submit(ctx, "vo_seq_submit_device", false, device_pairs(left1, right1));
 }
 
 extern "C" int vo_seq_wait(vo_ctx* ctx, vo_unit_result* out, vo_point2f* pts4, int pts_cap)
@@ -888,6 +917,19 @@ extern "C" int vo_mseq_submit_start(vo_ctx* ctx, const uint8_t* const* left1, co
                                     int channels, int n_start, const vo_mseq_start* starts)
 {
     return seq_submit(ctx, "vo_mseq_submit_start", true, host_pairs(left1, right1, pitch, channels), n_start, starts);
+}
+
+extern "C" int vo_mseq_begin_device(vo_ctx* ctx, int n_seq, const int* w, const int* h, const float* P_l, const float* P_r,
+                                    const vo_dimage* left0, const vo_dimage* right0, int flags)
+{
+    const SeqPairs in = device_pairs(left0, right0);
+    return seq_begin(ctx, "vo_mseq_begin_device", true, n_seq, flags, w, h, P_l, P_r, &in);
+}
+
+extern "C" int vo_mseq_submit_device(vo_ctx* ctx, const vo_dimage* left1, const vo_dimage* right1, int n_start,
+                                     const vo_mseq_start* starts)
+{
+    return seq_submit(ctx, "vo_mseq_submit_device", true, device_pairs(left1, right1), n_start, starts);
 }
 
 extern "C" int vo_mseq_wait(vo_ctx* ctx, vo_unit_result* out, int* status, vo_point2f* pts4, int pts_cap)
