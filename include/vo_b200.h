@@ -48,23 +48,35 @@ typedef struct vo_ctx vo_ctx;
 typedef struct vo_point2f { float x, y; } vo_point2f;
 typedef struct vo_point3f { float x, y, z; } vo_point3f;
 
-/* All literals the reference hard-codes, as run-time parameters (SURVEY.md section 5, "Config"). */
+/* All literals the reference hard-codes, as run-time parameters (SURVEY.md section 5, "Config").  Away from the
+ * reference's values each one does what OpenCV does with it: clamped where OpenCV clamps, refused where it asserts. */
 typedef struct vo_params {
     int fast_threshold;      /* 20      reference src/feature.cpp:43; vo_create refuses values
                                         outside [0, 255] (VO_E_INVALID)                           */
     int fast_nonmax;         /* 1       reference src/feature.cpp:44; 0: every FAST corner is kept
                                         with response 0 (as cv::FAST).  Fixed at vo_create: the
                                         corner capacity of a frame depends on it                  */
-    int lk_win;              /* 21      reference src/feature.cpp:127 (only 21 is built)      */
-    int lk_max_level;        /* 3       reference src/feature.cpp:136 (0-based: 4 images)     */
-    int lk_max_iters;        /* 30      reference src/feature.cpp:128                         */
-    double lk_epsilon;       /* 0.01    reference src/feature.cpp:128                         */
-    double lk_min_eig;       /* 0.001   reference src/feature.cpp:136                         */
-    int circ_threshold;      /* 0       reference src/visualOdometry.cpp:120                  */
-    int pnp_iterations;      /* 500     reference src/visualOdometry.cpp:168                  */
-    float pnp_reproj_error;  /* 0.5     reference src/visualOdometry.cpp:169                  */
-    double pnp_confidence;   /* 0.999   reference src/visualOdometry.cpp:170                  */
-    int max_features;        /* per-unit feature capacity of the context (default 8192)       */
+    int lk_win;              /* 21      reference src/feature.cpp:127 (only 21 is built; vo_create
+                                        refuses others with VO_E_UNSUPPORTED)                     */
+    int lk_max_level;        /* 3       reference src/feature.cpp:136 (0-based: 4 images); 0..7,
+                                        vo_create refuses others (VO_E_UNSUPPORTED).  A pyramid
+                                        stops early where a level would not exceed the window     */
+    int lk_max_iters;        /* 30      reference src/feature.cpp:128; clamped to [0, 100] as
+                                        calcOpticalFlowPyrLK clamps TermCriteria::maxCount        */
+    double lk_epsilon;       /* 0.01    reference src/feature.cpp:128; clamped to [0, 10]         */
+    double lk_min_eig;       /* 0.001   reference src/feature.cpp:136; used as a float, as
+                                        OpenCV's tracker stores and compares it                   */
+    int circ_threshold;      /* 0       reference src/visualOdometry.cpp:120; any value (< 0
+                                        keeps no point)                                           */
+    int pnp_iterations;      /* 500     reference src/visualOdometry.cpp:168; <= 0 runs one
+                                        iteration, as cv::solvePnPRansac does                     */
+    float pnp_reproj_error;  /* 0.5     reference src/visualOdometry.cpp:169; squared, so a
+                                        negative value acts as its magnitude (as in OpenCV)       */
+    double pnp_confidence;   /* 0.999   reference src/visualOdometry.cpp:170; vo_create refuses
+                                        values outside (0, 1) and NaN (VO_E_INVALID: OpenCV
+                                        asserts 0 < confidence < 1)                               */
+    int max_features;        /* per-unit feature capacity of the context (default 8192); vo_create
+                                refuses values <= 0 (VO_E_INVALID)                                */
     int max_units;           /* work units the batched path can hold at once (default 1)      */
 } vo_params;
 

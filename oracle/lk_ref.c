@@ -329,8 +329,12 @@ void lk_track(const lk_pyr_t *prev, const lk_pyr_t *next,
     int max_level = nlev - 1;
     const float half = (win - 1) * 0.5f;
     const float FLT_SCALE = 1.f / (1 << 20);
+    /* calcOpticalFlowPyrLK clamps the criteria (maxCount to [0, 100], epsilon to [0, 10]), and LKTrackerInvoker keeps
+     * minEigThreshold as a float: minEig is compared with the float threshold, in float */
+    if (max_count < 0) max_count = 0; if (max_count > 100) max_count = 100;
     if (epsilon < 0.) epsilon = 0.; if (epsilon > 10.) epsilon = 10.;
     double eps2 = epsilon * epsilon;
+    const float min_eig_f = (float)min_eig_thr;
     int16_t *Ibuf = (int16_t *)malloc(sizeof(int16_t) * win * win * 3);
     int16_t *dIbuf = Ibuf + win * win;
     const int nsimd = (win / 8) * 8;   /* columns handled by the 8-wide SIMD body */
@@ -398,10 +402,10 @@ void lk_track(const lk_pyr_t *prev, const lk_pyr_t *next,
             float D = A11 * A22 - A12 * A12;
             float minEig = (A22 + A11 - sqrtf((A11 - A22) * (A11 - A22) + 4.f * A12 * A12)) / (2 * win * win);
             if (g_log) {
-                lk_event_t *e = lk_log_add(pi, level, -1, (minEig < min_eig_thr || D < FLT_EPSILON) ? LK_EV_REJECT : LK_EV_SETUP);
+                lk_event_t *e = lk_log_add(pi, level, -1, (minEig < min_eig_f || D < FLT_EPSILON) ? LK_EV_REJECT : LK_EV_SETUP);
                 e->min_eig = minEig; e->D = D; e->ipx = ipx; e->ipy = ipy;
             }
-            if (minEig < min_eig_thr || D < FLT_EPSILON) {
+            if (minEig < min_eig_f || D < FLT_EPSILON) {
                 if (level == 0) status[pi] = 0;
                 continue;
             }

@@ -881,9 +881,12 @@ def solve_pnp_ransac(X, x, K, rvec0, tvec0, iterations=500, reproj=0.5, confiden
         # pose is not finite (five identical points: rvec 0, tvec nan)
         m = model_fn(X, x, K64)
         return dict(ok=True, rvec=m[0], tvec=m[1], inliers=np.arange(5, dtype=np.int32), iters=0, model=m)
+    # RANSACPointSetRegistrator::run: CV_Assert(confidence > 0 && confidence < 1), then at least one iteration
+    if not (0 < confidence < 1):
+        raise ValueError(f"confidence={confidence} outside (0, 1): cv::solvePnPRansac asserts 0 < confidence < 1")
     rng = CvRNG(MASK64)
     thr = np.float32(np.float64(reproj) * np.float64(reproj))
-    niters = iterations
+    niters = max(int(iterations), 1)
     best_mask = None
     max_good = 0
     best_model = None

@@ -45,7 +45,9 @@ class FeatureSet:
 # ------------------------------------------------------------------------------------ OpenCV calls
 # `float confidence = 0.999;` (visualOdometry.cpp:170) reaches cv::solvePnPRansac as (double)0.999f
 PNP_CONFIDENCE = float(np.float32(0.999))
-LK_ARGS = dict(winSize=(21, 21), maxLevel=3, flags=0, minEigThreshold=0.001)
+# the literals of the reference's calcOpticalFlowPyrLK call (feature.cpp:127-139: 21 x 21 window, maxLevel 3, 30
+# iterations, epsilon 0.01, minEigThreshold 0.001) are the defaults of the LK keywords below (max_level, max_iters,
+# epsilon, min_eig); the window stays 21 x 21
 
 
 def fast_cv2(img, threshold=20, nonmax=True):
@@ -54,19 +56,19 @@ def fast_cv2(img, threshold=20, nonmax=True):
     return np.array([k.pt for k in kps], np.float32).reshape(-1, 2)
 
 
-def lk_cv2(prev, nxt, pts):
+def lk_cv2(prev, nxt, pts, max_level=3, max_iters=30, epsilon=0.01, min_eig=0.001, with_err=False):
     if len(pts) == 0:
-        return np.zeros((0, 2), np.float32), np.zeros((0,), np.uint8)
-    crit = (cv2.TERM_CRITERIA_COUNT + cv2.TERM_CRITERIA_EPS, 30, 0.01)
-    o, s, _ = cv2.calcOpticalFlowPyrLK(prev, nxt, np.ascontiguousarray(pts, np.float32).reshape(-1, 1, 2), None,
-                                       criteria=crit, **LK_ARGS)
-    return o.reshape(-1, 2), s.ravel()
+        return (np.zeros((0, 2), np.float32), np.zeros((0,), np.uint8)) + ((np.zeros((0,), np.float32),) if with_err else ())
+    crit = (cv2.TERM_CRITERIA_COUNT + cv2.TERM_CRITERIA_EPS, max_iters, epsilon)
+    o, s, e = cv2.calcOpticalFlowPyrLK(prev, nxt, np.ascontiguousarray(pts, np.float32).reshape(-1, 1, 2), None,
+                                       criteria=crit, winSize=(21, 21), maxLevel=max_level, flags=0, minEigThreshold=min_eig)
+    return (o.reshape(-1, 2), s.ravel()) + ((e.ravel(),) if with_err else ())
 
 
-def lk_c(prev, nxt, pts):
+def lk_c(prev, nxt, pts, max_level=3, max_iters=30, epsilon=0.01, min_eig=0.001, with_err=False):
     from . import cref
-    o, s, _ = cref.lk_track(prev, nxt, pts)
-    return o, s
+    o, s, e = cref.lk_track(prev, nxt, pts, max_level=max_level, max_count=max_iters, epsilon=epsilon, min_eig=min_eig)
+    return (o, s) + ((e,) if with_err else ())
 
 
 def fast_c(img, threshold=20, nonmax=True):
@@ -102,10 +104,12 @@ def delete_unmatch_features_circle(p0, p1, p2, p3, p0r, s0, s1, s2, s3, ages):
     return p0[keep], p1[keep], p2[keep], p3[keep], p0r[keep], s3, ages_out, keep.astype(np.int32)
 
 
-def circular_matching(l0, r0, l1, r1, pts_l0, features, backend="cv2"):
+def circular_matching(l0, r0, l1, r1, pts_l0, features, backend="cv2", max_level=3, max_iters=30, epsilon=0.01,
+                      min_eig=0.001):
     """feature.cpp:118-148: ring L0->R0->R1->L1->L0 then deleteUnmatchFeaturesCircle.
     Returns dict with the five compacted vectors, raw per-call outputs/status, kept indices."""
-    _, lk = _backend(backend)
+    _, lk_fn = _backend(backend)
+    lk = lambda a, b, p: lk_fn(a, b, p, max_level=max_level, max_iters=max_iters, epsilon=epsilon, min_eig=min_eig)
     pts_l0 = np.ascontiguousarray(pts_l0, np.float32).reshape(-1, 2)
     pr0, s0 = lk(l0, r0, pts_l0)
     pr1, s1 = lk(r0, r1, pr0)
@@ -182,15 +186,18 @@ def append_new_features(img, features, backend="cv2"):
     features.ages = np.concatenate([features.ages, np.zeros(len(new), np.int32)]).astype(np.int32)
 
 
-def matching_features(l0, r0, l1, r1, features, backend="cv2"):
-    """visualOdometry.cpp:81-129.  Returns (pL0, pR0, pL1, pR1, info)."""
+def matching_features(l0, r0, l1, r1, features, backend="cv2", max_level=3, max_iters=30, epsilon=0.01, min_eig=0.001,
+                      circ_threshold=0):
+    """visualOdometry.cpp:81-129.  Returns (pL0, pR0, pL1, pR1, info).  The keywords replace the reference's literals
+    (the LK call's, and checkValidMatch's threshold 0 at :120)."""
     if features.size() < 2000:
         append_new_features(l0, features, backend)
     bucket_size = l0.shape[0] // 10
     bucketing_features(l0.shape[0], l0.shape[1], features, bucket_size, 1)
     pts_l0 = features.points.copy()
-    cm = circular_matching(l0, r0, l1, r1, pts_l0, features, backend)
-    status = check_valid_match(cm["l0"], cm["l0_ret"], 0)
+    cm = circular_matching(l0, r0, l1, r1, pts_l0, features, backend, max_level=max_level, max_iters=max_iters,
+                           epsilon=epsilon, min_eig=min_eig)
+    status = check_valid_match(cm["l0"], cm["l0_ret"], circ_threshold)
     pL0 = remove_invalid_points(cm["l0"], status)
     pL1 = remove_invalid_points(cm["l1"], status)
     pR0 = remove_invalid_points(cm["r0"], status)
@@ -212,9 +219,10 @@ def triangulate(P_l, P_r, pts_l, pts_r, backend="cv2"):
     return pnp_ref.triangulate(P_l, P_r, pts_l, pts_r)
 
 
-def tracking_frame2frame(P_l, pts_l0, pts_l1, X, translation, backend="cv2"):
-    """visualOdometry.cpp:132-193 with mono_rotation=false (what main.cpp:181 passes).
-    Returns (rotation 3x3 f64, translation 3 f64, inlier indices int32)."""
+def tracking_frame2frame(P_l, pts_l0, pts_l1, X, translation, backend="cv2", iterations=500, reproj=0.5,
+                         confidence=PNP_CONFIDENCE):
+    """visualOdometry.cpp:132-193 with mono_rotation=false (what main.cpp:181 passes); the keywords replace the literals
+    of its solvePnPRansac call (:168-170).  Returns (rotation 3x3 f64, translation 3 f64, inlier indices int32, rvec)."""
     K = np.ascontiguousarray(P_l[:, :3], np.float32)
     if backend == "cv2":
         dist = np.zeros((4, 1), np.float64)
@@ -222,12 +230,13 @@ def tracking_frame2frame(P_l, pts_l0, pts_l1, X, translation, backend="cv2"):
         tvec = np.asarray(translation, np.float64).reshape(3, 1).copy()
         ok, rvec, tvec, inl = cv2.solvePnPRansac(
             np.ascontiguousarray(X, np.float32).reshape(-1, 1, 3), np.ascontiguousarray(pts_l1, np.float32).reshape(-1, 1, 2),
-            K, dist, rvec, tvec, True, 500, 0.5, PNP_CONFIDENCE, None, cv2.SOLVEPNP_ITERATIVE)
+            K, dist, rvec, tvec, True, iterations, reproj, confidence, None, cv2.SOLVEPNP_ITERATIVE)
         R, _ = cv2.Rodrigues(rvec)
         inl = np.zeros((0,), np.int32) if inl is None else inl.ravel().astype(np.int32)
         return R, tvec.ravel(), inl, rvec.ravel()
     from . import pnp_ref
-    res = pnp_ref.solve_pnp_ransac(X, pts_l1, K, np.zeros(3), translation, confidence=PNP_CONFIDENCE)
+    res = pnp_ref.solve_pnp_ransac(X, pts_l1, K, np.zeros(3), translation, iterations=iterations, reproj=reproj,
+                                   confidence=confidence)
     return pnp_ref.rodrigues(res["rvec"]), res["tvec"], res["inliers"], res["rvec"]
 
 

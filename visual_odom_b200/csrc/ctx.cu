@@ -42,6 +42,15 @@ extern "C" int vo_create(int device, const vo_params* params, vo_ctx** out)
         vo_set_error(ctx, "fast_threshold=%d outside [0,255]", ctx->p.fast_threshold);
         return VO_E_INVALID;
     }
+    if (!(ctx->p.pnp_confidence > 0.0 && ctx->p.pnp_confidence < 1.0)) {
+        // cv::solvePnPRansac asserts 0 < confidence < 1 (NaN included); outside it the iteration bound has no meaning
+        vo_set_error(ctx, "pnp_confidence=%g outside (0,1)", ctx->p.pnp_confidence);
+        return VO_E_INVALID;
+    }
+    if (ctx->p.max_features <= 0) {
+        vo_set_error(ctx, "max_features=%d: the per-unit feature capacity must be positive", ctx->p.max_features);
+        return VO_E_INVALID;
+    }
     if (ctx->p.lk_win != VO_WIN) {
         vo_set_error(ctx, "lk_win=%d unsupported: the LK kernel is built for the reference's 21x21 window", ctx->p.lk_win);
         return VO_E_UNSUPPORTED;
@@ -518,7 +527,7 @@ int vo_ensure_state(vo_ctx* ctx, int w, int h, int units, int levels)
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_resp, (size_t)units * ctx->corner_cap));
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_want, (size_t)units));
     // triangulation + PnP
-    const size_t its = (size_t)ctx->p.pnp_iterations;
+    const size_t its = (size_t)vo_pnp_iterations(ctx);
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_X, uc));
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_tprev, (size_t)units * 3));
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_pnp_state, (size_t)units));
@@ -609,11 +618,12 @@ int vo_run_lk_ring(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, 
     a.nlevels = pg.nlevels;
     for (int l = 0; l < pg.nlevels; l++) { a.lw[l] = pg.lv[l].w; a.lh[l] = pg.lv[l].h; }
     a.geo = v.sized ? ctx->d_geo : nullptr;
-    a.max_iters = ctx->p.lk_max_iters;
+    // calcOpticalFlowPyrLK clamps the criteria: maxCount to [0, 100], epsilon to [0, 10]
+    a.max_iters = ctx->p.lk_max_iters < 0 ? 0 : ctx->p.lk_max_iters > 100 ? 100 : ctx->p.lk_max_iters;
     double eps = ctx->p.lk_epsilon;
     if (eps < 0.) eps = 0.; if (eps > 10.) eps = 10.;
     a.eps2 = eps * eps;
-    a.min_eig = ctx->p.lk_min_eig;
+    a.min_eig = (float)ctx->p.lk_min_eig;          // LKTrackerInvoker keeps minEigThreshold as a float
     a.pts_in = ctx->d_pts_in + uo;
     a.pts_out = ctx->d_pts_out + uo;
     a.status_out = ctx->d_status + uo;
@@ -732,10 +742,11 @@ int vo_run_triangulate(vo_ctx* ctx, const View& v, const float2* pts_l, const fl
 
 int vo_run_pnp(vo_ctx* ctx, const View& v, const float2* pts2d, const int* n, const CamCalib* cal)
 {
-    const size_t uo = (size_t)v.u0 * ctx->cap, its = (size_t)ctx->p.pnp_iterations;
+    const int iterations = vo_pnp_iterations(ctx);
+    const size_t uo = (size_t)v.u0 * ctx->cap, its = (size_t)iterations;
     PnpArgs a;
     memset(&a, 0, sizeof(a));
-    a.n_units = v.n; a.cap = ctx->cap; a.iterations = ctx->p.pnp_iterations;
+    a.n_units = v.n; a.cap = ctx->cap; a.iterations = iterations;
     a.n_pts = n + v.u0; a.X = ctx->d_X + uo; a.x = pts2d + uo;
     a.cal = cal + v.u0;
     const double thr = (double)ctx->p.pnp_reproj_error;      // float -> double, squared in double, stored float

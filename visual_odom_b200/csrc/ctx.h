@@ -284,3 +284,5 @@ int vo_run_select(vo_ctx* ctx, const View& v);
 int vo_run_triangulate(vo_ctx* ctx, const View& v, const float2* pts_l, const float2* pts_r, const int* n, const CamCalib* cal,
                        float4* X4 = nullptr);
 int vo_run_pnp(vo_ctx* ctx, const View& v, const float2* pts2d, const int* n, const CamCalib* cal);
+// RANSAC iterations the PnP stage sizes and runs: cv::RANSACPointSetRegistrator runs at least one (max(maxIters, 1))
+inline int vo_pnp_iterations(const vo_ctx* ctx) { return ctx->p.pnp_iterations > 1 ? ctx->p.pnp_iterations : 1; }

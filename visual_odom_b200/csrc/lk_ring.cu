@@ -415,7 +415,7 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                     float dd = __fsub_rn(A11, A22);
                     float rad = __fadd_rn(__fmul_rn(dd, dd), __fmul_rn(__fmul_rn(4.f, A12), A12));
                     float minEig = __fdiv_rn(__fsub_rn(__fadd_rn(A22, A11), __fsqrt_rn(rad)), (float)(2 * VO_WIN * VO_WIN));
-                    if ((double)minEig < args.min_eig || D < 1.1920928955078125e-07f) {
+                    if (minEig < args.min_eig || D < 1.1920928955078125e-07f) {
                         if (level == 0) status = 0;
                         break;
                     }
