@@ -78,6 +78,26 @@ typedef struct vo_params {
     int max_features;        /* per-unit feature capacity of the context (default 8192); vo_create
                                 refuses values <= 0 (VO_E_INVALID)                                */
     int max_units;           /* work units the batched path can hold at once (default 1)      */
+    /* matchingFeatures()' feature bookkeeping (reference src/visualOdometry.cpp:95-107, src/bucket.cpp:16).  Only the
+     * sequence modes (vo_seq_*, vo_mseq_*) use them; the batched path (vo_frame_batch, vo_batch_*) selects features by
+     * stride and never buckets, so it ignores them.  They are context-wide, fixed at vo_create.  A sequence mode reads
+     * back at most (rows/bs + 1) * (cols/bs + 1) * features_per_bucket points per frame, bs = rows / bucket_rows_divisor
+     * (the bucket bound); a begin, open or start whose largest bound exceeds max_features is refused with
+     * VO_E_CAPACITY.  These four fields were appended in this order after max_units: callers compiled against a header
+     * without them pass a shorter struct and must be rebuilt. */
+    int refill_threshold;    /* 2000    reference src/visualOdometry.cpp:95: FAST corners are
+                                        appended while the live point count is < refill_threshold
+                                        (any value; <= 0 never refills)                           */
+    int bucket_rows_divisor; /* 10      reference src/visualOdometry.cpp:106: bucket_size = rows /
+                                        bucket_rows_divisor, per sequence from its own rows; vo_create
+                                        refuses <= 0 (VO_E_INVALID), a begin / open / start whose
+                                        rows / divisor is 0 is refused (VO_E_UNSUPPORTED: the
+                                        reference divides by zero)                                */
+    int features_per_bucket; /* 1       reference src/visualOdometry.cpp:107 (Bucket(max_size)); vo_create
+                                        refuses <= 0 (VO_E_INVALID: the reference reads ages[0] of an
+                                        empty bucket)                                             */
+    int bucket_age_threshold;/* 10      reference src/bucket.cpp:16: a bucket admits a feature whose
+                                        age is < bucket_age_threshold (any value)                 */
 } vo_params;
 
 VO_API void vo_default_params(vo_params* p);
@@ -186,7 +206,9 @@ typedef struct vo_unit {
 
 typedef struct vo_unit_result {
     int n_features;      /* features fed to the ring                                   */
-    int n_detected;      /* FAST corners found on l0 (0 when pts were given)           */
+    int n_detected;      /* FAST corners found on l0 (0 when pts were given); in the
+                            sequence modes whether or not they were appended (a frame
+                            with refill_threshold or more live points appends none)     */
     int n_tracked;       /* survivors of deleteUnmatchFeaturesCircle (A3)              */
     int n_valid;         /* survivors of checkValidMatch/removeInvalidPoints (A5/A6)   */
     int n_inliers;       /* RANSAC inliers                                             */

@@ -40,6 +40,34 @@ def count_frames(dataset, first):
     return n
 
 
+def bucket_grid(w, h, divisor=10, per_bucket=1):
+    """the points bucketingFeatures reads back at most: (rows/bs + 1) x (cols/bs + 1) cells of per_bucket slots,
+    bs = rows / divisor (the library's seq_grid)"""
+    bs = max(h // divisor, 1)
+    return (h // bs + 1) * (w // bs + 1) * per_bucket
+
+
+def add_bucket_args(ap):
+    """matchingFeatures' bookkeeping (vo_params; the reference's literals by default)"""
+    ap.add_argument("--features-per-bucket", type=int, default=1, help="Bucket(max_size) (default 1)")
+    ap.add_argument("--bucket-divisor", type=int, default=10, help="bucket_size = rows / DIVISOR (default 10)")
+    ap.add_argument("--age-threshold", type=int, default=10, help="buckets admit features aged < THRESHOLD (default 10)")
+    ap.add_argument("--refill-threshold", type=int, default=2000,
+                    help="FAST corners are appended while fewer than THRESHOLD features are tracked (default 2000)")
+
+
+def bucket_params(a, sizes):
+    """the Context keywords of the flags; max_features is raised from 4096 to the largest read-back bound of the sizes"""
+    if a.features_per_bucket < 1 or a.bucket_divisor < 1:
+        raise SystemExit("--features-per-bucket and --bucket-divisor must be positive")
+    for w, h in sizes:
+        if h // a.bucket_divisor == 0:
+            raise SystemExit(f"{w}x{h} images are too small for the rows/{a.bucket_divisor} bucket size")
+    bound = max(bucket_grid(w, h, a.bucket_divisor, a.features_per_bucket) for w, h in sizes)
+    return dict(max_features=max(4096, bound), refill_threshold=a.refill_threshold, bucket_rows_divisor=a.bucket_divisor,
+                features_per_bucket=a.features_per_bucket, bucket_age_threshold=a.age_threshold)
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("dataset"); ap.add_argument("calibration")
@@ -49,6 +77,7 @@ def main():
     ap.add_argument("--threads", type=int, default=8); ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--mono-rotation", action="store_true",
                     help="rotation from findEssentialMat + recoverPose (trackingFrame2Frame's header default)")
+    add_bucket_args(ap)
     ap.add_argument("--check", action="store_true")
     a = ap.parse_args()
     from visual_odom_b200 import capi, synth
@@ -63,9 +92,12 @@ def main():
     print(f"{n} stereo pairs of {w}x{h} (PNG colour type {ctype}, {depth} bit); P_left =\n{P_l}\nP_right =\n{P_r}")
     print("rotation: " + ("findEssentialMat + recoverPose (mono_rotation = true)" if a.mono_rotation else
                           "Rodrigues of the PnP rvec (mono_rotation = false)"))
+    prm = bucket_params(a, [(w, h)])
+    print(f"bucketing: {a.features_per_bucket} feature(s) per bucket of rows/{a.bucket_divisor}, ages < {a.age_threshold}, "
+          f"refill below {a.refill_threshold} features; max_features {prm['max_features']}")
     if a.check:
         return
-    ctx = capi.Context(a.device, max_features=4096, max_units=2)
+    ctx = capi.Context(a.device, max_units=2, **prm)
     ctx.set_option("mono_rotation", 1 if a.mono_rotation else 0)
     aborted = 0
     rd = capi.SequenceReader(a.dataset, a.first, n, threads=a.threads, depth=a.threads + 3)

@@ -29,7 +29,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import numpy as np
 
-from run_sequence import count_frames, read_calibration
+from run_sequence import add_bucket_args, bucket_grid, bucket_params, count_frames, read_calibration
 
 
 def pyramid_depth(w, h):
@@ -62,12 +62,6 @@ def queue_schedule(lengths, n_slots):
     return out
 
 
-def bucket_grid(w, h):
-    """bucketingFeatures' (rows/bs + 1) x (cols/bs + 1) cells, bs = rows / 10 (the library's seq_grid)"""
-    bs = max(h // 10, 1)
-    return (h // bs + 1) * (w // bs + 1)
-
-
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("datasets", nargs="+", metavar="DIR")
@@ -84,6 +78,7 @@ def main():
                     help="run sequences of different image sizes together, each at its own size")
     ap.add_argument("--slots", type=int, metavar="N",
                     help="run the datasets as a queue through N slots, each starting in the first slot that frees")
+    add_bucket_args(ap)
     ap.add_argument("--check", action="store_true")
     a = ap.parse_args()
     from visual_odom_b200 import capi, synth
@@ -118,8 +113,8 @@ def main():
             raise SystemExit(f"{d}: {w}x{h} images, {a.datasets[0]} has {seqs[0]['w']}x{seqs[0]['h']}: "
                              "one context runs one image size (group the sequences by size, or run them together with "
                              "--mixed-sizes)")
-        if sized and h // 10 == 0:
-            raise SystemExit(f"{d}: {w}x{h} images are too small for the rows/10 bucket size")
+        if sized and h // max(a.bucket_divisor, 1) == 0:
+            raise SystemExit(f"{d}: {w}x{h} images are too small for the rows/{a.bucket_divisor} bucket size")
         if sized and seqs and pyramid_depth(w, h) != pyramid_depth(seqs[0]["w"], seqs[0]["h"]):
             raise SystemExit(f"{d}: {w}x{h} images have {pyramid_depth(w, h)} pyramid levels, {a.datasets[0]} "
                              f"({seqs[0]['w']}x{seqs[0]['h']}) has {pyramid_depth(seqs[0]['w'], seqs[0]['h'])}: "
@@ -140,9 +135,10 @@ def main():
             raise SystemExit(f"the envelope {W}x{H} of the sizes has {pyramid_depth(W, H)} pyramid levels, the sizes "
                              f"{pyramid_depth(seqs[0]['w'], seqs[0]['h'])}: one context runs one pyramid depth")
         for s in seqs:
-            if a.mono_rotation and bucket_grid(s["w"], s["h"]) > bucket_grid(W, H):
-                raise SystemExit(f"{s['dir']}: {s['w']}x{s['h']} has {bucket_grid(s['w'], s['h'])} buckets, more than "
-                                 f"the {bucket_grid(W, H)} of the envelope {W}x{H} the mono scratch is sized for")
+            grid = lambda w, h: bucket_grid(w, h, a.bucket_divisor, a.features_per_bucket)
+            if a.mono_rotation and grid(s["w"], s["h"]) > grid(W, H):
+                raise SystemExit(f"{s['dir']}: {s['w']}x{s['h']} reads back {grid(s['w'], s['h'])} points, more than "
+                                 f"the {grid(W, H)} of the envelope {W}x{H} the mono scratch is sized for")
         sched = queue_schedule([s["n"] for s in seqs], a.slots)
         steps = max(k0 + s["n"] - 1 for s, (_, k0) in zip(seqs, sched))
         print(f"schedule: {len(seqs)} sequences through {a.slots} slots of {W}x{H}, {steps} submissions")
@@ -151,14 +147,18 @@ def main():
             print(f"  {s['name']}: slot {q}, submissions {k0}..{k0 + s['n'] - 1}")
     print("rotation: " + ("findEssentialMat + recoverPose (mono_rotation = true)" if a.mono_rotation else
                           "Rodrigues of the PnP rvec (mono_rotation = false)"))
+    prm = bucket_params(a, [(s["w"], s["h"]) for s in seqs] + ([(W, H)] if a.slots is not None else []))
+    print(f"bucketing: {a.features_per_bucket} feature(s) per bucket of rows/{a.bucket_divisor}, ages < {a.age_threshold}, "
+          f"refill below {a.refill_threshold} features; max_features {prm['max_features']}")
     if a.check:
         return
+    a.context_params = prm
     if a.slots is not None:
         return run_queue(a, capi, seqs, sched, W, H)
     # one pitch and one channel count per submission: colour files are read as BGR (converted on the device) unless the
     # sequences mix gray and colour files, then all are converted to gray while decoding
     force = 0 if len({s["gray"] for s in seqs}) == 1 else 1
-    ctx = capi.Context(a.device, max_features=4096)
+    ctx = capi.Context(a.device, **a.context_params)
     rds = [capi.SequenceReader(s["dir"], 0, s["n"], threads=a.threads, depth=a.threads + 3, force_channels=force) for s in seqs]
 
     def pairs(k):
@@ -228,7 +228,7 @@ def main():
 def run_queue(a, capi, seqs, sched, W, H):
     """--slots: every dataset starts in its scheduled slot (vo_mseq_submit_start) and retires after its last frame."""
     force = 0 if len({s["gray"] for s in seqs}) == 1 else 1
-    ctx = capi.Context(a.device, max_features=4096)
+    ctx = capi.Context(a.device, **a.context_params)
     ctx.mseq_open(a.slots, W, H, mono_rotation=a.mono_rotation)
     steps = max(s["k0"] + s["n"] - 1 for s in seqs)
     rds = {}                   # dataset index -> its reader, opened at its first pair, closed after its last wait

@@ -32,6 +32,9 @@ class VoParams(C.Structure):
         ("lk_min_eig", C.c_double), ("circ_threshold", C.c_int), ("pnp_iterations", C.c_int),
         ("pnp_reproj_error", C.c_float), ("pnp_confidence", C.c_double),
         ("max_features", C.c_int), ("max_units", C.c_int),
+        # the sequence modes' bookkeeping (matchingFeatures' literals); the batched path ignores them
+        ("refill_threshold", C.c_int), ("bucket_rows_divisor", C.c_int), ("features_per_bucket", C.c_int),
+        ("bucket_age_threshold", C.c_int),
     ]
 
 

@@ -27,6 +27,10 @@ extern "C" void vo_default_params(vo_params* p)
     p->pnp_confidence = (double)0.999f;   // the reference stores it in a float (visualOdometry.cpp:170)
     p->max_features = 8192;
     p->max_units = 1;
+    p->refill_threshold = 2000;           // visualOdometry.cpp:95
+    p->bucket_rows_divisor = 10;          // visualOdometry.cpp:106
+    p->features_per_bucket = 1;           // visualOdometry.cpp:107
+    p->bucket_age_threshold = 10;         // bucket.cpp:16
 }
 
 extern "C" int vo_create(int device, const vo_params* params, vo_ctx** out)
@@ -49,6 +53,15 @@ extern "C" int vo_create(int device, const vo_params* params, vo_ctx** out)
     }
     if (ctx->p.max_features <= 0) {
         vo_set_error(ctx, "max_features=%d: the per-unit feature capacity must be positive", ctx->p.max_features);
+        return VO_E_INVALID;
+    }
+    if (ctx->p.bucket_rows_divisor <= 0) {
+        vo_set_error(ctx, "bucket_rows_divisor=%d: bucket_size = rows / divisor needs a positive divisor", ctx->p.bucket_rows_divisor);
+        return VO_E_INVALID;
+    }
+    if (ctx->p.features_per_bucket <= 0) {
+        // Bucket::add_feature on a full bucket of max_size 0 reads ages[0] of an empty vector
+        vo_set_error(ctx, "features_per_bucket=%d: a bucket holds at least one feature", ctx->p.features_per_bucket);
         return VO_E_INVALID;
     }
     if (ctx->p.lk_win != VO_WIN) {
@@ -77,6 +90,7 @@ extern "C" int vo_create(int device, const vo_params* params, vo_ctx** out)
     ctx->stream = ctx->own_stream;
     VO_CUDA_CHECK(vo_lk_prepare());
     ctx->cap = ctx->p.max_features;
+    ctx->bucket_cap = (size_t)(ctx->cap / ctx->p.features_per_bucket) * ((size_t)ctx->p.features_per_bucket + 1);
     VO_CUDA_CHECK(cudaMalloc(&ctx->d_lk_queue, LK_QUEUES * 2 * sizeof(int)));
     VO_CUDA_CHECK(cudaMemset(ctx->d_lk_queue, 0, LK_QUEUES * 2 * sizeof(int)));
     {   // VO_LK_STAGING=ldg switches the LK window staging from TMA to plain loads (debug / A-B runs)

@@ -95,12 +95,15 @@ struct vo_ctx {
     float2* d_feat_pts = nullptr;       // [seq_n_cap][feat_cap] currentVOFeatures.points
     int* d_feat_ages = nullptr;         // [seq_n_cap][feat_cap] currentVOFeatures.ages (may be longer than points)
     int* d_feat_cnt = nullptr;          // [seq_n_cap][2] sizes of the two vectors
-    int* d_bucket = nullptr;            // [seq_n_cap][bucket_cap] scratch of bucketingFeatures
+    int* d_bucket = nullptr;            // [seq_n_cap][bucket_cap] scratch of bucketingFeatures (k_seq_bucket)
     int* d_seq_err = nullptr;           // [1 + 2 * seq_n_cap] error bits of the glue kernels, [1 + unit] per frame
     int* d_seq_live = nullptr;          // [2 * seq_n_cap] per unit: 0 once its sequence is retired (vo_mseq_submit)
     void* d_seq_state = nullptr;        // the one allocation behind the six arrays above (freed with the batch state)
     int seq_n_cap = 0;                  // sequences those arrays hold
-    int feat_cap = 0, bucket_cap = 4096;
+    int feat_cap = 0;
+    // ints of bucketing scratch per sequence: a grid of nb cells takes nb * (features_per_bucket + 1), and every run the
+    // begin and start calls accept has nb * features_per_bucket <= max_features (vo_create)
+    size_t bucket_cap = 0;
     bool seq_active = false;
     bool seq_multi = false;             // begun with vo_mseq_begin (the vo_seq_* frame calls are refused, and vice versa)
     int seq_n = 1;                      // sequences of the running sequence mode
