@@ -510,6 +510,47 @@ VO_API int vo_mseq_submit_device(vo_ctx* ctx, const vo_dimage* left1, const vo_d
 VO_API int vo_mseq_wait(vo_ctx* ctx, vo_unit_result* out, int* status, vo_point2f* pts4, int pts_cap);
 VO_API int vo_mseq_wait_mono(vo_ctx* ctx, vo_unit_result* out, int* status, vo_mono_result* mono,
                              uint8_t* ess_mask, int mask_cap, vo_point2f* pts4, int pts_cap);
+/* Results into GPU memory, without a host wait: a device-resident loop (frames in from GPU memory, results out to it, the
+ * host never touching pixels or waiting for a pose solve).  A run begun with the flag VO_MSEQ_DEVICE_RESULTS (any
+ * vo_mseq_begin*, vo_mseq_begin_device or vo_mseq_open; it combines with VO_MSEQ_MONO_ROTATION):
+ *   - takes its frames through vo_mseq_submit_device only, starts included (a begin with host pairs is synchronous and
+ *     accepted).  Host submissions are refused: a wait that does not block gives no point after which a pinned host image
+ *     is free again.
+ *   - returns its results through vo_mseq_wait_device only; vo_mseq_wait / vo_mseq_wait_mono are refused.
+ *   - keeps frame_pose on the device; vo_mseq_pose returns it after the last waited submission (it synchronises, as
+ *     vo_mseq_state does).
+ *   vo_mseq_wait_device  retires the oldest submission without blocking the host: ONE kernel launch on the context's
+ *                        stream, ordered after the work already enqueued there and after that submission's pose solve
+ *                        (never behind the next submission's), writes for every sequence q into the caller's device
+ *                        buffers below; work enqueued on the context's stream after the call sees the results.  Every
+ *                        pointer may be NULL (skipped); each must otherwise be device (or managed) memory of the context's
+ *                        GPU.  The point arrays hold pts_cap entries per sequence, of which the first n_valid (inliers:
+ *                        n_inliers) are defined; a retired or started sequence defines none.
+ *     status[q]      VO_OK, VO_E_CAPACITY (glue error bits, as vo_mseq_wait; no message, the call returns VO_OK),
+ *                    VO_MSEQ_RETIRED or VO_MSEQ_STARTED
+ *     records[q]     vo_mseq_wait's record (zeroed for a retired or started slot)
+ *     frame_pose     [n_seq][16] row-major: integrated in wait order under the main loop's gates, bit for bit as
+ *                    vo_pose_step integrates it in vo_mseq_wait (the identity from a start on)
+ *     pts4           [n_seq][4][pts_cap]: L0, R0, L1, R1, as vo_mseq_wait's pts4
+ *     points3d       [n_seq][pts_cap]: points3D_t0, the triangulated L0 / R0 (vo_triangulate with the sequence's matrices)
+ *     inliers        [n_seq][pts_cap]: solvePnPRansac's inliers, indices into the frame's n_valid list (vo_batch_outputs)
+ *     mono, ess_mask [n_seq], [n_seq][pts_cap]: vo_mseq_wait_mono's, in runs with VO_MSEQ_MONO_ROTATION only
+ *   Refused with VO_E_INVALID, changing nothing: a run without the flag, nothing in flight, pts_cap < 0, a point array
+ *   with pts_cap == 0, mono / ess_mask without VO_MSEQ_MONO_ROTATION, a pointer that is not device memory of the
+ *   context's GPU.  At most two submissions in flight, as ever. */
+#define VO_MSEQ_DEVICE_RESULTS 8 /* vo_mseq_begin* / vo_mseq_open flag: results through vo_mseq_wait_device (bits 2 and 4 stay unknown) */
+typedef struct vo_mseq_dresults {
+    int32_t* status;             /* [n_seq] */
+    vo_unit_result* records;     /* [n_seq] */
+    double* frame_pose;          /* [n_seq][16] */
+    int pts_cap;                 /* entries per sequence of pts4 (per list), points3d, inliers, ess_mask */
+    vo_point2f* pts4;            /* [n_seq][4][pts_cap] */
+    vo_point3f* points3d;        /* [n_seq][pts_cap] */
+    int32_t* inliers;            /* [n_seq][pts_cap] */
+    vo_mono_result* mono;        /* [n_seq] */
+    uint8_t* ess_mask;           /* [n_seq][pts_cap] */
+} vo_mseq_dresults;
+VO_API int vo_mseq_wait_device(vo_ctx* ctx, const vo_mseq_dresults* r);
 VO_API int vo_mseq_pose(vo_ctx* ctx, int q, double frame_pose[16]);
 VO_API int vo_mseq_state(vo_ctx* ctx, int q, vo_point2f* points, int32_t* ages, int cap, int* n_points, int* n_ages, double t_out[3]);
 
@@ -547,12 +588,16 @@ VO_API int vo_bgr_to_gray(vo_ctx* ctx, const uint8_t* bgr, size_t pitch, int w, 
  *                        [R|t;0 0 0 1]^-1; frame_pose *= rigid_inv iff 0.05 < |t| < 10.  Returns 1 when the
  *                        pose was advanced, 0 when the frame was skipped, <0 on a singular transform.
  *   vo_pose_step         the main loop's gate + integration    (src/main.cpp:196-208):  all |euler| < 0.1
- *   vo_seq_pose          frame_pose accumulated by vo_seq_push since vo_seq_begin */
+ *   vo_seq_pose          frame_pose accumulated by vo_seq_push since vo_seq_begin
+ *   vo_pose_step_device  vo_pose_step of n frames (frame_pose[16 i], R[9 i], t[3 i]; rc[i] its return value, rc may be
+ *                        NULL) computed by the device function vo_mseq_wait_device integrates with (stage-level entry
+ *                        point, for parity tests; synchronous) */
 VO_API int  vo_pose_is_rotation(const double R[9]);
 VO_API void vo_pose_euler(const double R[9], float euler_xyz[3]);
 VO_API int  vo_pose_integrate(double frame_pose[16], const double R[9], const double t[3], double rigid_inv[16]);
 VO_API int  vo_pose_step(double frame_pose[16], const double R[9], const double t[3]);
 VO_API int  vo_seq_pose(vo_ctx* ctx, double frame_pose[16]);
+VO_API int  vo_pose_step_device(vo_ctx* ctx, int n, double* frame_pose, const double* R, const double* t, int* rc);
 
 /* ---- KITTI accuracy evaluation (SURVEY.md 8f, row N4) -- host-only, offline -----------------------------
  * Poses are KITTI rows: 12 doubles = top 3 rows of the 4x4 camera-to-world matrix (what vo_seq_pose accumulates).

@@ -2,7 +2,7 @@
 """Scaling of the multi-sequence streaming mode (vo_mseq_*) with the number of sequences, measured on the GPU.
 
     python tools/mseq_timing.py [--frames 40] [--rounds 5] [--counts 1,2,4,8,16,32] [--mono-rotation] [--mixed-calibration]
-                                [--mixed-sizes] [--device-input] [--json out.json]
+                                [--mixed-sizes] [--device-input] [--device-results] [--json out.json]
 
 Synthetic 1241x376 drives (synth.stereo_unit; eight seeds, each with its own motion) of `--frames` frames each;
 sequence q replays drive q % 8, forwards for even q // 8 and backwards for odd, so up to 16 sequences are distinct and
@@ -24,7 +24,12 @@ count all at 1241x376 in the same rounds, alternated.  `--device-input` (counts 
 times every vo_mseq_* count three ways in the same rounds, alternated: host gray images (vo_mseq_submit, the loop above),
 and every frame made resident as CUDA tensors before the timed window and fed through vo_mseq_submit_device as gray
 (H, W) and as BGR (H, W, 3) tensors; it also times the host side of one vo_mseq_submit_device call (the binding, and the
-C call alone) at 32 and 64 sequences.  The card's name, power limit and max SM clock, read in the same run, are printed with the numbers;
+C call alone) at 32 and 64 sequences.  `--device-results` (counts 1, 8 and 32 unless --counts is given) times every
+vo_mseq_* count two ways in the same rounds, alternated, both with resident gray CUDA tensors through
+vo_mseq_submit_device: host waits that return the point lists (vo_mseq_wait with pts4), and a run begun with
+VO_MSEQ_DEVICE_RESULTS whose waits are vo_mseq_wait_device into one reused set of CUDA tensors, each followed by a trivial
+torch consumer of them on the same stream (the loop ends with a synchronise, inside the timed window).  It adds the host
+time per step spent inside the submit and wait calls, and the kernel launches per submission and per wait.  The card's name, power limit and max SM clock, read in the same run, are printed with the numbers;
 they are part of them."""
 import argparse
 import json
@@ -136,6 +141,44 @@ def run_mseq_device(ctx, P_l, P_r, seqs, order=None):
     return n * steps / dt, dt / steps, (ctx.kernel_launches() - l0) / steps
 
 
+def run_mseq_dres(ctx, P_l, P_r, seqs, device_results):
+    """device input, two submissions in flight; host waits with point lists, or vo_mseq_wait_device + a torch consumer.
+    Returns (aggregate frames/s, step time, host time per step in the calls, launches per submission, per wait)."""
+    import torch
+    n, nf = len(seqs), len(seqs[0])
+    ctx.mseq_begin_device([s[0][0] for s in seqs], [s[0][1] for s in seqs], P_l, P_r, device_results=device_results)
+    frame = [([s[k][0] for s in seqs], [s[k][1] for s in seqs]) for k in range(nf)]
+    out = ctx.mseq_dresults_alloc() if device_results else None
+    acc = torch.zeros((), dtype=torch.float64, device="cuda")
+    host, l_sub, l_wait = 0.0, 0, 0
+
+    def submit(k):
+        nonlocal host, l_sub
+        l, t = ctx.kernel_launches(), time.perf_counter()
+        ctx.mseq_submit_device(*frame[k])
+        host += time.perf_counter() - t
+        l_sub += ctx.kernel_launches() - l
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    submit(1)
+    for k in range(1, nf):
+        if k + 1 < nf:
+            submit(k + 1)
+        l, t = ctx.kernel_launches(), time.perf_counter()
+        if device_results:
+            ctx.mseq_wait_device(out=out)
+        else:
+            ctx.mseq_wait()
+        host += time.perf_counter() - t
+        l_wait += ctx.kernel_launches() - l
+        if device_results:              # the consumer: reads the poses and the inlier counts where they are
+            acc += out["frame_pose"][:, :3, 3].sum() + out["counts"][:, 4].sum()
+    torch.cuda.synchronize()
+    dt = time.perf_counter() - t0
+    steps = nf - 1
+    return n * steps / dt, dt / steps, host / steps, l_sub / steps, l_wait / steps
+
+
 def submit_host_cost(ctx, P_l, P_r, seqs, reps=50):
     """median host time of one vo_mseq_submit_device call [us]: through the binding, and the C call alone (descriptor
     tables built beforehand); each call is waited for outside the timed region"""
@@ -169,12 +212,16 @@ def main():
                     help="also time every vo_mseq_* count with the KITTI training set's three image sizes")
     ap.add_argument("--device-input", action="store_true",
                     help="also time every vo_mseq_* count with frames resident in GPU memory (gray and BGR tensors)")
+    ap.add_argument("--device-results", action="store_true",
+                    help="also time device input with host waits against vo_mseq_wait_device (VO_MSEQ_DEVICE_RESULTS)")
     ap.add_argument("--json", help="also write the result here")
     a = ap.parse_args()
     if a.mixed_sizes and a.counts == ap.get_default("counts"):
         a.counts = "3,11,32"
     if a.device_input and a.counts == ap.get_default("counts"):
         a.counts = "1,8,16,32"
+    if a.device_results and a.counts == ap.get_default("counts"):
+        a.counts = "1,8,32"
     counts = [int(c) for c in a.counts.split(",")]
     from visual_odom_b200 import capi, synth
     P_l, P_r = synth.proj_matrices()
@@ -188,6 +235,8 @@ def main():
         modes += [(m, mono, "sizes") for m in counts for mono in monos]
     if a.device_input:
         modes += [(m, False, kind) for m in counts for kind in ("dev-gray", "dev-bgr")]
+    if a.device_results:
+        modes += [(m, False, kind) for m in counts for kind in ("dres-host", "dres-dev")]
     seqs = {n: [sequence(dr, q) for q in range(n)] for n in counts}
     mixed = {}
     if a.mixed_calibration:              # per count n: sequence q rendered with calibration(q, n), played like sequence(dr, q)
@@ -206,22 +255,25 @@ def main():
             sized[n] = [sequence(by_size[KITTI_SIZES[q % len(KITTI_SIZES)]], q) for q in range(n)]
         print(f"rendered the drives at {len(by_size)} image sizes in {time.perf_counter() - t0:.0f} s", flush=True)
     dev = {}
-    if a.device_input:                   # every frame of every drive resident on the GPU, gray and BGR, before any timing
+    if a.device_input or a.device_results:  # every frame of every drive resident on the GPU, gray and BGR, before any timing
         import torch
-        for kind in ("dev-gray", "dev-bgr"):
+        for kind in ("dev-gray", "dev-bgr") if a.device_input else ("dev-gray",):
             t = [[tuple(torch.from_numpy(np.ascontiguousarray(x if kind == "dev-gray" else np.repeat(x[:, :, None], 3, axis=2)))
                         .cuda() for x in pair) for pair in fr] for fr in dr]
             dev[kind] = {n: [sequence(t, q) for q in range(n)] for n in set(counts) | {32, 64}}
         torch.cuda.synchronize()
         print(f"resident on the GPU: {torch.cuda.memory_allocated() / 2**30:.2f} GiB", flush=True)
     ctx = capi.Context(0, max_features=4096)
-    res = {m: dict(fps=[], lat=[], launches=[]) for m in modes}
+    res = {m: dict(fps=[], lat=[], launches=[], host=[], wait_launches=[]) for m in modes}
 
     def run(mode, fr_cut=None):
         m, mono, mix = mode
         if m == "seq":
             fr = dr[0] if fr_cut is None else dr[0][:fr_cut]
             return run_seq(ctx, P_l, P_r, fr, mono)
+        if mix in ("dres-host", "dres-dev"):
+            s = dev["dev-gray"][m] if fr_cut is None else [x[:fr_cut] for x in dev["dev-gray"][m]]
+            return run_mseq_dres(ctx, P_l, P_r, s, mix == "dres-dev")
         if mix in ("dev-gray", "dev-bgr"):
             s = dev[mix][m] if fr_cut is None else [x[:fr_cut] for x in dev[mix][m]]
             return run_mseq_device(ctx, P_l, P_r, s, "bgr" if mix == "dev-bgr" else None)
@@ -232,8 +284,11 @@ def main():
     for _ in range(a.rounds):
         for m in modes:
             run(m, 4)                     # warm-up: (re-)captures the mode's graphs, untimed
-            fps, lat, launches = run(m)
+            r = run(m)
+            fps, lat, launches = r[0], r[1], r[-2] if len(r) == 5 else r[2]
             res[m]["fps"].append(fps); res[m]["lat"].append(lat); res[m]["launches"].append(launches)
+            if len(r) == 5:
+                res[m]["host"].append(r[2]); res[m]["wait_launches"].append(r[4])
     host_cost = {n: submit_host_cost(ctx, P_l, P_r, dev["dev-gray"][n]) for n in (32, 64)} if a.device_input else {}
     ctx.close()
     out = dict(card=card(), image=f"{W}x{H}", frames=a.frames, rounds=a.rounds, in_flight=2, modes={})
@@ -245,14 +300,18 @@ def main():
         o = dict(aggregate_fps=float(np.median(r["fps"])), aggregate_fps_min=float(np.min(r["fps"])),
                  aggregate_fps_max=float(np.max(r["fps"])), step_latency_ms=1e3 * float(np.median(r["lat"])),
                  launches_per_submission=float(np.median(r["launches"])))
+        if r["host"]:
+            o.update(host_ms_per_step=1e3 * float(np.median(r["host"])), launches_per_wait=float(np.median(r["wait_launches"])))
         m, mono, mix = mode
-        out["modes"][str(m) + ("+mono" if mono else "") + ("+sizes" if mix == "sizes" else f"+{mix}" if mix in ("dev-gray", "dev-bgr")
+        out["modes"][str(m) + ("+mono" if mono else "") + ("+sizes" if mix == "sizes" else f"+{mix}" if mix in ("dev-gray", "dev-bgr", "dres-host", "dres-dev")
                                else "+mixed" if mix else "")] = o
         name = ("vo_seq (1 sequence)" if m == "seq" else f"vo_mseq n_seq = {m:2d}") + (", mono" if mono else "") + \
             (", KITTI sizes" if mix == "sizes" else ", device gray" if mix == "dev-gray" else ", device BGR" if mix == "dev-bgr"
+             else ", dev in, host wait" if mix == "dres-host" else ", dev in, dev results" if mix == "dres-dev"
              else ", mixed cal." if mix else "")
         print(f"{name:40s}: {o['aggregate_fps']:8.0f} frames/s [{o['aggregate_fps_min']:.0f}, {o['aggregate_fps_max']:.0f}], "
-              f"step {o['step_latency_ms']:.3f} ms, {o['launches_per_submission']:.1f} launches / submission")
+              f"step {o['step_latency_ms']:.3f} ms, {o['launches_per_submission']:.1f} launches / submission"
+              + (f", host {o['host_ms_per_step']:.3f} ms / step, {o['launches_per_wait']:.1f} launches / wait" if "host_ms_per_step" in o else ""))
     for n, (b, c) in host_cost.items():
         print(f"one vo_mseq_submit_device, n_seq = {n:2d}: host {b:.1f} us through the binding, {c:.1f} us in the C call")
     print(json.dumps(out))

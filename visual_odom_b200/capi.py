@@ -23,6 +23,7 @@ VO_MSEQ_MAX = 64           # sequences one vo_mseq_begin may start (include/vo_b
 VO_MSEQ_RETIRED = 2        # vo_mseq_wait status of a retired sequence
 VO_MSEQ_MONO_ROTATION = 1  # vo_mseq_begin_ex flag: every sequence runs trackingFrame2Frame(mono_rotation = true)
 VO_MSEQ_STARTED = 3        # vo_mseq_wait status of the submission that started a slot's sequence
+VO_MSEQ_DEVICE_RESULTS = 8 # vo_mseq_begin* / vo_mseq_open flag: results into device memory through vo_mseq_wait_device
 
 
 class VoParams(C.Structure):
@@ -107,6 +108,13 @@ class VoMonoResult(C.Structure):
         ("status", C.c_int), ("n_inliers", C.c_int), ("ransac_iters", C.c_int), ("n_good", C.c_int),
         ("R", C.c_double * 9), ("t", C.c_double * 3),
     ]
+
+
+class VoMseqDResults(C.Structure):
+    """vo_mseq_dresults: the caller's device buffers vo_mseq_wait_device writes (any pointer may be NULL)."""
+    _fields_ = [("status", C.c_void_p), ("records", C.c_void_p), ("frame_pose", C.c_void_p), ("pts_cap", C.c_int),
+                ("pts4", C.c_void_p), ("points3d", C.c_void_p), ("inliers", C.c_void_p), ("mono", C.c_void_p),
+                ("ess_mask", C.c_void_p)]
 
 
 # the same record as a numpy structured dtype (C layout, 152 bytes): arrays of records can be handed out without building
@@ -203,6 +211,8 @@ SIGNATURES = {
     "vo_mseq_wait": (C.c_int, [C.c_void_p, C.POINTER(VoUnitResult), C.c_void_p, C.c_void_p, C.c_int]),
     "vo_mseq_wait_mono": (C.c_int, [C.c_void_p, C.POINTER(VoUnitResult), C.c_void_p, C.POINTER(VoMonoResult), C.c_void_p,
                                     C.c_int, C.c_void_p, C.c_int]),
+    "vo_mseq_wait_device": (C.c_int, [C.c_void_p, C.POINTER(VoMseqDResults)]),
+    "vo_pose_step_device": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vo_mseq_pose": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     "vo_mseq_state": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
                                 C.c_void_p]),
@@ -769,6 +779,7 @@ class Context:
             if P_l.shape != (n, 3, 4) or P_r.shape != (n, 3, 4):
                 raise ValueError(f"per-sequence calibrations must be ({n}, 3, 4), got {P_l.shape} / {P_r.shape}")
             self._check(self.lib.vo_mseq_begin_sized(self.h, n, _p(wa), _p(ha), _p(P_l), _p(P_r), lp, rp, _p(pa), ch, flags))
+            self._mseq_mono = bool(mono_rotation)
             self._mseq_n, self._mseq_pitch = n, pa.copy()
             self._mseq_sizes = [(int(a), int(b)) for a, b in zip(ha, wa)]
             self._mseq_keep = [None, None]
@@ -781,6 +792,7 @@ class Context:
             P_l = P_l.reshape(12); P_r = P_r.reshape(12)
             self._check(self.lib.vo_mseq_begin_ex(self.h, n, w, h, _p(P_l), _p(P_r), lp, rp, pitch, ch, flags))
         self._mseq_n, self._mseq_pitch = n, pitch
+        self._mseq_mono = bool(mono_rotation)
         self._mseq_sizes = [(int(h), int(w))] * n
         self._mseq_keep = [None, None]
 
@@ -804,12 +816,14 @@ class Context:
         lp, rp = (C.c_void_p * n)(*left_ptrs), (C.c_void_p * n)(*right_ptrs)
         self._mseq_begin(n, w, h, lp, rp, pitch, channels, P_l, P_r, mono_rotation)
 
-    def mseq_open(self, n_slots, max_w, max_h, mono_rotation=False):
+    def mseq_open(self, n_slots, max_w, max_h, mono_rotation=False, device_results=False):
         """n_slots empty slots for sequences of any size inside max_w x max_h with that size's pyramid depth
         (vo_mseq_open); sequences come in through mseq_submit(start=...).  mono_rotation=True: every sequence started in
-        the run runs trackingFrame2Frame(mono_rotation = true)."""
-        flags = VO_MSEQ_MONO_ROTATION if mono_rotation else 0
+        the run runs trackingFrame2Frame(mono_rotation = true).  device_results=True: the run takes its frames through
+        mseq_submit_device and returns its results through mseq_wait_device (VO_MSEQ_DEVICE_RESULTS)."""
+        flags = (VO_MSEQ_MONO_ROTATION if mono_rotation else 0) | (VO_MSEQ_DEVICE_RESULTS if device_results else 0)
         self._check(self.lib.vo_mseq_open(self.h, int(n_slots), int(max_w), int(max_h), flags))
+        self._mseq_mono = bool(mono_rotation)
         self._mseq_n, self._mseq_pitch = int(n_slots), np.zeros(int(n_slots), np.uint64)
         self._mseq_sizes = [None] * int(n_slots)
         self._mseq_keep = [None, None]
@@ -897,17 +911,19 @@ class Context:
             lt[q], rt[q], sizes[q] = dl, dr, (h, w)
         return lt, rt, sizes
 
-    def mseq_begin_device(self, lefts, rights, P_l, P_r, order=None, mono_rotation=False):
+    def mseq_begin_device(self, lefts, rights, P_l, P_r, order=None, mono_rotation=False, device_results=False):
         """mseq_begin from CUDA uint8 tensors (H, W), (H, W, 3) or (3, H, W), one pair per sequence, each sequence at its
         pair's size and in its own layout (vo_mseq_begin_device; synchronous).  order: "bgr" / "rgb" for colour pairs, one
-        string or one per sequence.  P_l / P_r: (3, 4) for one calibration, or (n_seq, 3, 4)."""
+        string or one per sequence.  P_l / P_r: (3, 4) for one calibration, or (n_seq, 3, 4).  device_results=True: results
+        through mseq_wait_device only (VO_MSEQ_DEVICE_RESULTS)."""
         n = len(lefts)
         lt, rt, sizes = self._device_pairs(lefts, rights, order, n, False)
         P_l = np.ascontiguousarray(np.broadcast_to(np.asarray(P_l, np.float32), (n, 3, 4)))
         P_r = np.ascontiguousarray(np.broadcast_to(np.asarray(P_r, np.float32), (n, 3, 4)))
         wa = np.array([g[1] for g in sizes], np.int32); ha = np.array([g[0] for g in sizes], np.int32)
-        flags = VO_MSEQ_MONO_ROTATION if mono_rotation else 0
+        flags = (VO_MSEQ_MONO_ROTATION if mono_rotation else 0) | (VO_MSEQ_DEVICE_RESULTS if device_results else 0)
         self._device_call(self.lib.vo_mseq_begin_device, n, _p(wa), _p(ha), _p(P_l), _p(P_r), lt, rt, flags)
+        self._mseq_mono = bool(mono_rotation)
         # host submissions may follow: the pitch state mseq_begin leaves for these sizes
         uniform = all(g == sizes[0] for g in sizes)
         self._mseq_n, self._mseq_pitch = n, (int(wa[0]) if uniform else wa.astype(np.uint64))
@@ -951,6 +967,88 @@ class Context:
             self._check(self.lib.vo_mseq_wait(self.h, res, _p(st), _p(pts4), npts), ok=(VO_OK, VO_E_CAPACITY))
         return [self._record(res[q], pts_cap, None if pts4 is None else pts4[q], ms[q] if mono else None,
                              mask[q] if mono else None, st[q]) for q in range(n)]
+
+    def mseq_dresults_alloc(self, pts_cap=4096, points=True, points3d=True, inliers=True, mono=False):
+        """The CUDA tensors mseq_wait_device writes for the run's n_seq sequences (pass them back as out= to reuse them):
+        "records" (n, 19) float64 holds vo_unit_result records, viewed as "counts" (n, 7) int32 (n_features, n_detected,
+        n_tracked, n_valid, n_inliers, ransac_iters, pnp_status), "rvec" / "tvec" (n, 3) and "R" (n, 3, 3); "status" (n,)
+        int32; "frame_pose" (n, 4, 4) float64; "pts4" (n, 4, pts_cap, 2) float32 (L0, R0, L1, R1); "points3d"
+        (n, pts_cap, 3) float32; "inliers" (n, pts_cap) int32; with mono, "mono_raw" (n, 14) float64 holds vo_mono_result,
+        viewed as "mono_counts" (n, 4) int32 (status, n_inliers, ransac_iters, n_good), "mono_R" (n, 3, 3), "mono_t" (n, 3),
+        and "ess_mask" (n, pts_cap) uint8."""
+        import torch
+        n, dev = self._mseq_n, torch.device("cuda", self.device)
+        lists = points or points3d or inliers or mono
+        if lists and (not isinstance(pts_cap, (int, np.integer)) or pts_cap <= 0):
+            raise ValueError(f"pts_cap = {pts_cap!r}: point outputs need pts_cap > 0")
+        rec = torch.zeros((n, 19), dtype=torch.float64, device=dev)
+        out = dict(records=rec, counts=rec[:, :4].view(torch.int32)[:, :7], rvec=rec[:, 4:7], tvec=rec[:, 7:10],
+                   R=rec[:, 10:19].view(n, 3, 3), status=torch.zeros(n, dtype=torch.int32, device=dev),
+                   frame_pose=torch.zeros((n, 4, 4), dtype=torch.float64, device=dev), pts_cap=int(pts_cap) if lists else 0)
+        if points:
+            out["pts4"] = torch.zeros((n, 4, pts_cap, 2), dtype=torch.float32, device=dev)
+        if points3d:
+            out["points3d"] = torch.zeros((n, pts_cap, 3), dtype=torch.float32, device=dev)
+        if inliers:
+            out["inliers"] = torch.zeros((n, pts_cap), dtype=torch.int32, device=dev)
+        if mono:
+            m = torch.zeros((n, 14), dtype=torch.float64, device=dev)
+            out.update(mono_raw=m, mono_counts=m[:, :2].view(torch.int32), mono_R=m[:, 2:11].view(n, 3, 3), mono_t=m[:, 11:14],
+                       ess_mask=torch.zeros((n, pts_cap), dtype=torch.uint8, device=dev))
+        return out
+
+    _DRES_SHAPES = {"records": ("float64", (19,)), "status": ("int32", ()), "frame_pose": ("float64", (4, 4)),
+                    "pts4": ("float32", (4, None, 2)), "points3d": ("float32", (None, 3)), "inliers": ("int32", (None,)),
+                    "mono_raw": ("float64", (14,)), "ess_mask": ("uint8", (None,))}
+
+    def mseq_wait_device(self, pts_cap=4096, points=True, points3d=True, inliers=True, out=None):
+        """Retire the oldest submission of a run begun with device_results=True without blocking the host
+        (vo_mseq_wait_device): one kernel on torch.cuda.current_stream() writes every sequence's results into CUDA tensors,
+        which work queued on that stream afterwards may read at once.  Returns the dict of mseq_dresults_alloc (with
+        "mono_*" and "ess_mask" in runs begun with mono_rotation=True); out= such a dict, which is filled in place, so a
+        loop allocates nothing.  Only the first n_valid entries of a sequence's point lists (inliers: n_inliers) are
+        defined."""
+        mono = bool(getattr(self, "_mseq_mono", False))
+        if out is None:
+            out = self.mseq_dresults_alloc(pts_cap, points, points3d, inliers, mono)
+        else:
+            self._check_dresults(out)
+        r = VoMseqDResults()
+        r.pts_cap = int(out.get("pts_cap", 0))
+        for f, k in (("status", "status"), ("records", "records"), ("frame_pose", "frame_pose"), ("pts4", "pts4"),
+                     ("points3d", "points3d"), ("inliers", "inliers"), ("mono", "mono_raw"), ("ess_mask", "ess_mask")):
+            t = out.get(k)
+            setattr(r, f, None if t is None else t.data_ptr())
+        self._device_call(self.lib.vo_mseq_wait_device, C.byref(r))
+        return out
+
+    def _check_dresults(self, out):
+        """out= of mseq_wait_device: CUDA tensors on the context's GPU, contiguous, of the run's sequence count, the
+        dtypes mseq_dresults_alloc gives and one pts_cap."""
+        import torch
+        n = self._mseq_n
+        cap = out.get("pts_cap", 0)
+        for k, (dt, tail) in self._DRES_SHAPES.items():
+            t = out.get(k)
+            if t is None:
+                continue
+            want = (n,) + tuple(cap if d is None else d for d in tail)
+            if not isinstance(t, torch.Tensor):
+                raise TypeError(f"out[{k!r}] must be a CUDA tensor on cuda:{self.device}")
+            if str(t.dtype) != "torch." + dt or tuple(t.shape) != want or not t.is_contiguous():
+                raise ValueError(f"out[{k!r}]: {tuple(t.shape)} {t.dtype}, expected a contiguous {want} {dt}")
+            if not t.is_cuda or t.device.index != self.device:
+                raise TypeError(f"out[{k!r}] must be a CUDA tensor on cuda:{self.device}")
+
+    def pose_step_device(self, frame_pose, R, t):
+        """vo_pose_step of n frames by the device function vo_mseq_wait_device integrates with (vo_pose_step_device):
+        frame_pose (n, 4, 4), R (n, 3, 3), t (n, 3) -> (new poses, return codes)."""
+        pose = np.array(frame_pose, np.float64).reshape(-1, 16).copy()
+        n = len(pose)
+        R = np.ascontiguousarray(R, np.float64).reshape(n, 9); t = np.ascontiguousarray(t, np.float64).reshape(n, 3)
+        rc = np.zeros(n, np.int32)
+        self._check(self.lib.vo_pose_step_device(self.h, n, _p(pose), _p(R), _p(t), _p(rc)))
+        return pose.reshape(n, 4, 4), rc
 
     def mseq_pose(self, q):
         pose = np.zeros((4, 4))

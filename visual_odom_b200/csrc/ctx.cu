@@ -128,6 +128,8 @@ extern "C" void vo_destroy(vo_ctx* ctx)
     if (ctx->d_lk_queue) cudaFree(ctx->d_lk_queue);
     if (ctx->d_ess) cudaFree(ctx->d_ess);
     if (ctx->d_seq_ess) cudaFree(ctx->d_seq_ess);
+    if (ctx->d_seq_pose) cudaFree(ctx->d_seq_pose);
+    for (cudaEvent_t e : ctx->seq_tab_ev) if (e) cudaEventDestroy(e);
     for (int k = 0; k < 2; k++) if (ctx->seq_mono_ev[k]) cudaEventDestroy(ctx->seq_mono_ev[k]);
     if (ctx->seq_mono_stream) cudaStreamDestroy(ctx->seq_mono_stream);
     if (ctx->h_out) cudaFreeHost(ctx->h_out);

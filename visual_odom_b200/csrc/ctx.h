@@ -15,7 +15,6 @@
 #define VO_DIST_BUCKET 4       // posted steps per collective
 #define VO_DIST_NB 4           // buckets (ring)
 #define VO_LANES 3            // submissions in flight, each with its own side stream / partition streams / events
-#define SEQ_STARTED 2         // vo_ctx::seq_live: the slot's sequence started in this submission (stages skip it)
 
 // what a cached CUDA graph was captured for: its kind, the stream (the LK work queue is that stream's), the LK staging,
 // and the kind's own fields (the others stay zero)
@@ -119,6 +118,13 @@ struct vo_ctx {
                                         // never started (vo_mseq_open)
     std::vector<char> seq_live;         // [2 * seq_n] d_seq_live as the frame in flight in each parity saw it: 0 not running,
                                         // 1 running, SEQ_STARTED (host only, the device word is 0) its sequence started there
+    // results into device memory (flag VO_MSEQ_DEVICE_RESULTS, vo_mseq_wait_device): frame_pose lives in d_seq_pose
+    // ([VO_MSEQ_MAX][16], allocated at the first such begin) and k_seq_collect integrates it.  The host no longer waits for
+    // a submission, so the descriptor table entries of image slot s (pinned) are rewritten only after seq_tab_ev[s], recorded
+    // after their copy to the device.
+    bool seq_dres = false;
+    double* d_seq_pose = nullptr;
+    cudaEvent_t seq_tab_ev[3] = {nullptr, nullptr, nullptr};
     int seq_lk_bound = 0;               // the LK launch bound: the largest bucket grid of the run's sizes (raised by starts)
     std::vector<CamCalib> seq_cal_next; // [2 * seq_n] calibration entries of started sequences that the frame in flight
     std::vector<char> seq_cal_due;      // still reads: written by the next submission of that buffer parity

@@ -1,8 +1,10 @@
 // pose.cu -- host-side pose bookkeeping of the reference's main loop (SURVEY.md 8f row N2): the Euler-angle gate
 // (src/main.cpp:196-203, src/utils.cpp:93-131) and integrateOdometryStereo (src/utils.cpp:57-91).  O(1) per frame,
-// double precision, no device work: these are the C-ABI forms the facade's utils.h functions and the streaming
-// sequence mode call.
+// double precision, on the host: these are the C-ABI forms the facade's utils.h functions and the streaming sequence
+// mode call.  vo_pose_step_device runs the device form (pose_math.cuh, which k_seq_collect integrates frame_pose with)
+// on host arrays, for parity tests.
 #include "ctx.h"
+#include "pose_math.cuh"
 #include <cmath>
 #include <cstring>
 
@@ -34,54 +36,12 @@ extern "C" void vo_pose_euler(const double R[9], float e[3])
     }
 }
 
-// inverse of T = [R|t; 0 0 0 1] by Gauss-Jordan with partial pivoting (what cv::Mat::inv() defaults to)
-static bool invert_rigid4(const double R[9], const double t[3], double inv[16])
-{
-    double a[4][8];
-    for (int r = 0; r < 4; r++)
-        for (int c = 0; c < 8; c++) a[r][c] = (c >= 4 && c - 4 == r) ? 1.0 : 0.0;
-    for (int r = 0; r < 3; r++) {
-        for (int c = 0; c < 3; c++) a[r][c] = R[3 * r + c];
-        a[r][3] = t[r];
-    }
-    a[3][3] = 1.0;
-    for (int col = 0; col < 4; col++) {
-        int piv = col;
-        for (int r = col + 1; r < 4; r++)
-            if (std::fabs(a[r][col]) > std::fabs(a[piv][col])) piv = r;
-        if (a[piv][col] == 0.0) return false;
-        if (piv != col)
-            for (int c = 0; c < 8; c++) { const double x = a[piv][c]; a[piv][c] = a[col][c]; a[col][c] = x; }
-        const double d = a[col][col];
-        for (int c = 0; c < 8; c++) a[col][c] /= d;
-        for (int r = 0; r < 4; r++) {
-            if (r == col) continue;
-            const double f = a[r][col];
-            if (f != 0.0)
-                for (int c = 0; c < 8; c++) a[r][c] -= f * a[col][c];
-        }
-    }
-    for (int r = 0; r < 4; r++)
-        for (int c = 0; c < 4; c++) inv[4 * r + c] = a[r][4 + c];
-    return true;
-}
-
 extern "C" int vo_pose_integrate(double frame_pose[16], const double R[9], const double t[3], double rigid_inv[16])
 {
     double inv[16];
-    if (!invert_rigid4(R, t, inv)) return VO_E_INVALID;
+    if (!vo_invert_rigid4(R, t, inv)) return VO_E_INVALID;
     if (rigid_inv) memcpy(rigid_inv, inv, sizeof(inv));
-    const double scale = std::sqrt(t[0] * t[0] + t[1] * t[1] + t[2] * t[2]);
-    if (!(scale > 0.05 && scale < 10)) return 0;
-    double out[16];
-    for (int r = 0; r < 4; r++)
-        for (int c = 0; c < 4; c++) {
-            double s = 0;
-            for (int k = 0; k < 4; k++) s += frame_pose[4 * r + k] * inv[4 * k + c];
-            out[4 * r + c] = s;
-        }
-    memcpy(frame_pose, out, sizeof(out));
-    return 1;
+    return vo_integrate_rigid(frame_pose, t, inv);
 }
 
 extern "C" int vo_pose_step(double frame_pose[16], const double R[9], const double t[3])
@@ -97,5 +57,43 @@ extern "C" int vo_seq_pose(vo_ctx* ctx, double frame_pose[16])
     if (!ctx || !ctx->seq_active || !frame_pose) return VO_E_INVALID;
     if (ctx->seq_multi) { vo_set_error(ctx, "vo_seq_pose: the sequences were begun with vo_mseq_begin; use vo_mseq_pose"); return VO_E_INVALID; }
     memcpy(frame_pose, ctx->seq_pose.data(), 16 * sizeof(double));
+    return VO_OK;
+}
+
+__global__ void k_pose_step(int n, double* frame_pose, const double* __restrict__ R, const double* __restrict__ t, int* rc)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    double pose[16];
+    for (int k = 0; k < 16; k++) pose[k] = frame_pose[16 * (size_t)i + k];
+    const int r = vo_pose_step_dev(pose, R + 9 * (size_t)i, t + 3 * (size_t)i);
+    for (int k = 0; k < 16; k++) frame_pose[16 * (size_t)i + k] = pose[k];
+    rc[i] = r;
+}
+
+extern "C" int vo_pose_step_device(vo_ctx* ctx, int n, double* frame_pose, const double* R, const double* t, int* rc)
+{
+    if (!ctx) return VO_E_INVALID;
+    if (n < 0 || (n > 0 && (!frame_pose || !R || !t))) { vo_set_error(ctx, "vo_pose_step_device: bad argument"); return VO_E_INVALID; }
+    if (n == 0) return VO_OK;
+    VO_CUDA_CHECK(cudaSetDevice(ctx->device));
+    const size_t o_R = 16 * (size_t)n * sizeof(double), o_t = o_R + 9 * (size_t)n * sizeof(double);
+    const size_t o_rc = o_t + 3 * (size_t)n * sizeof(double), bytes = o_rc + (size_t)n * sizeof(int);
+    uint8_t* d = nullptr;
+    VO_CUDA_CHECK(cudaMalloc(&d, bytes));
+    cudaStream_t st = ctx->stream;
+    cudaError_t e = cudaMemcpyAsync(d, frame_pose, o_R, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d + o_R, R, o_t - o_R, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d + o_t, t, o_rc - o_t, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) {
+        k_pose_step<<<(n + 127) / 128, 128, 0, st>>>(n, (double*)d, (const double*)(d + o_R), (const double*)(d + o_t), (int*)(d + o_rc));
+        ctx->launches++;
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(frame_pose, d, o_R, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess && rc) e = cudaMemcpyAsync(rc, d + o_rc, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    cudaFree(d);
+    VO_CUDA_CHECK(e);
     return VO_OK;
 }

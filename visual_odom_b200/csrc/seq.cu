@@ -18,6 +18,7 @@
 // single-sequence mode launches them with n_seq = 1.
 #include "common.cuh"
 #include "seq.h"
+#include "pose_math.cuh"
 #include <climits>
 
 __global__ void __launch_bounds__(1024) k_seq_append(const float2* __restrict__ corners, const int* __restrict__ n_det,
@@ -192,6 +193,63 @@ __global__ void k_seq_mono(vo_unit_result_dev* res, const EssResult* __restrict_
     ess = (const EssResult*)((const char*)ess + (size_t)q * ess_stride);
     const int k = threadIdx.x;
     if (k < 9) res->R[k] = ess->status == ESS_OK ? ess->R[k] : (k % 4 == 0 ? 1.0 : 0.0);
+}
+
+// vo_mseq_wait_device (K7): one block per sequence retires the oldest submission into the caller's buffers -- what
+// seq_wait does on the host from the pinned copies, and the point lists, points3D and inliers it leaves in the units.
+// Thread 0 writes the status / record / mono result and integrates frame_pose (main.cpp:196-208: a frame is integrated
+// when its PnP ran (VO_OK or no model) and, with mono_rotation, the essential branch did not abort); the block copies the
+// lists.  Sequences are independent, so the launch is one grid however many of them there are.
+__global__ void __launch_bounds__(256) k_seq_collect(const CollectArgs a)
+{
+    const int q = blockIdx.x, mode = a.mode[q];
+    const vo_unit_result_dev* res = a.res + q;
+    const EssResult* ess = a.ess ? (const EssResult*)((const char*)a.ess + (size_t)q * a.ess_stride) : nullptr;
+    double* pose = a.pose + 16 * (size_t)q;
+    const int nv = mode == 1 ? min(res->n_valid, a.pts_cap) : 0;
+    const int ni = mode == 1 ? min(res->n_inliers, a.pts_cap) : 0;
+    if (threadIdx.x == 0) {
+        int status = mode == SEQ_STARTED ? VO_MSEQ_STARTED : VO_MSEQ_RETIRED;
+        vo_unit_result_dev r;
+        memset(&r, 0, sizeof(r));
+        vo_mono_result m;
+        memset(&m, 0, sizeof(m));
+        if (mode == 1) {
+            r = *res;
+            const bool mono_ok = !ess || ess->status == ESS_OK;
+            if ((r.pnp_status == VO_OK || r.pnp_status == VO_PNP_NO_MODEL) && mono_ok) vo_pose_step_dev(pose, r.R, r.tvec);
+            if (ess) {
+                m.status = mono_ok ? VO_OK : VO_E_TOO_FEW_POINTS;
+                m.n_inliers = ess->n_inliers; m.ransac_iters = ess->iters; m.n_good = ess->n_good;
+                for (int k = 0; k < 9; k++) m.R[k] = ess->R[k];
+                for (int k = 0; k < 3; k++) m.t[k] = ess->t[k];
+            }
+            // bit 8 (a tracked point outside the bucket grid) is not an error, as in seq_wait
+            status = (a.err[q] & ~8) ? VO_E_CAPACITY : VO_OK;
+        } else if (mode == SEQ_STARTED) {              // the new sequence's frame_pose starts here (main.cpp:90)
+            for (int i = 0; i < 16; i++) pose[i] = i % 5 == 0 ? 1.0 : 0.0;
+        }
+        if (a.status) a.status[q] = status;
+        if (a.records) a.records[q] = r;
+        if (a.mono) a.mono[q] = m;
+        if (a.pose_out)
+            for (int i = 0; i < 16; i++) a.pose_out[16 * (size_t)q + i] = pose[i];
+    }
+    const size_t src = (size_t)q * a.cap, dst = (size_t)q * a.pts_cap;
+    for (int i = threadIdx.x; i < nv; i += blockDim.x) {
+        if (a.pts4)
+            for (int k = 0; k < 4; k++) a.pts4[(4 * (size_t)q + k) * a.pts_cap + i] = a.valid4[k * a.plane_stride + src + i];
+        if (a.points3d) a.points3d[dst + i] = a.X[src + i];
+        if (a.mask_out) a.mask_out[dst + i] = a.ess_mask[(size_t)q * a.ess_stride + i];
+    }
+    if (a.inliers_out)
+        for (int i = threadIdx.x; i < ni; i += blockDim.x) a.inliers_out[dst + i] = a.inliers[src + i];
+}
+
+int vo_launch_seq_collect(const CollectArgs& a, int n_seq, cudaStream_t s)
+{
+    k_seq_collect<<<n_seq, 256, 0, s>>>(a);
+    return 1;
 }
 
 int vo_launch_seq_append(const SeqArgs& a, int n_seq, cudaStream_t s)

@@ -3,6 +3,8 @@
 #include "common.cuh"
 #include "pnp.h"
 #include "ess.h"
+#include "../../include/vo_b200.h"
+#define SEQ_STARTED 2         // vo_ctx::seq_live: the slot's sequence started in this submission (stages skip it)
 
 // The pointers are those of sequence 0; one launch covers n_seq sequences (blockIdx.y = q) and finds sequence q's part of
 // each array `stride` elements further on: corner_cap (corners), feat_cap (feat_pts, feat_ages), 2 (cnt), bucket_cap
@@ -33,3 +35,19 @@ int vo_launch_seq_finish(const SeqArgs& a, int n_seq, cudaStream_t s);
 // mono_rotation = true: each live sequence's record R becomes recoverPose's rotation (I where the branch aborted);
 // everything else in the record stays the PnP's.  ess: sequence 0's result, sequence q's ess_stride bytes further on.
 int vo_launch_seq_mono(const SeqArgs& a, const EssResult* ess, size_t ess_stride, int n_seq, cudaStream_t s);
+
+// vo_mseq_wait_device: the oldest submission's results (buffer units u0 .. u0 + n_seq - 1) into caller device buffers.
+// mode[q]: 1 the sequence ran in that submission, 0 retired or empty, SEQ_STARTED started by it.  Sources are
+// sequence 0's (the unit u0) with the strides of SeqArgs (cap for the point lists, ess_stride bytes for ess / ess_mask);
+// every destination may be NULL.
+struct CollectArgs {
+    const vo_unit_result_dev* res; const int* err; int cap;
+    const float2* valid4; size_t plane_stride;          // the four lists of unit u0: valid4 + k * plane_stride
+    const float3* X; const int* inliers;
+    const EssResult* ess; const uint8_t* ess_mask; size_t ess_stride;   // mono runs only (else NULL)
+    double* pose;                                       // [n_seq][16] device frame_pose, integrated here
+    int* status; vo_unit_result_dev* records; double* pose_out; int pts_cap;
+    float2* pts4; float3* points3d; int* inliers_out; vo_mono_result* mono; uint8_t* mask_out;
+    unsigned char mode[VO_MSEQ_MAX];
+};
+int vo_launch_seq_collect(const CollectArgs& a, int n_seq, cudaStream_t s);

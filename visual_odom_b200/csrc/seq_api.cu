@@ -229,7 +229,8 @@ static int seq_back(vo_ctx* ctx, int p)
 // EssResult[2 * n_seq] (mono sequences only) | vo_dimage[6 * n_seq] (device-image descriptors, one per raw plane of the
 // three-slot ring, indexed by plane: entry 2 * n_seq * s + 2q + k is sequence q's image k of slot s).  Slot s's entries are
 // rewritten by the submission that stages into s, three submissions after the one that last copied them to the device;
-// with at most two submissions in flight that one has been waited for, so its copy has run.
+// with at most two submissions in flight that one has been waited for, so its copy has run -- when the wait blocks.
+// vo_mseq_wait_device does not, so runs begun with VO_MSEQ_DEVICE_RESULTS wait for seq_tab_ev[s], recorded after the copy.
 struct SeqPinned { vo_unit_result_dev* rec; int* err; EssResult* ess; vo_dimage* tab; size_t bytes; };
 static SeqPinned seq_pinned(vo_ctx* ctx, int n)
 {
@@ -346,8 +347,11 @@ static int stage_pairs(vo_ctx* ctx, int slot, const SeqPairs& in, cudaStream_t s
     if (!in.device) return upload_pairs(ctx, slot, in.lefts, in.rights, in.pitch, in.channels, st);
     const int n = ctx->seq_n;
     vo_dimage* tab = seq_pinned(ctx, n).tab + 2 * n * slot;
+    if (ctx->seq_dres) VO_CUDA_CHECK(cudaEventSynchronize(ctx->seq_tab_ev[slot]));
     for (int q = 0; q < n; q++) { tab[2 * q] = in.dl[q]; tab[2 * q + 1] = in.dr[q]; }
-    return vo_ingest_device(ctx, tab, 2 * n, 2 * n * slot, st, ctx->seq_sized ? ctx->d_geo + 2 * n * slot : nullptr);
+    const int rc = vo_ingest_device(ctx, tab, 2 * n, 2 * n * slot, st, ctx->seq_sized ? ctx->d_geo + 2 * n * slot : nullptr);
+    if (!rc && ctx->seq_dres) VO_CUDA_CHECK(cudaEventRecord(ctx->seq_tab_ev[slot], st));
+    return rc;
 }
 
 // n new sequences (multi: begun by vo_mseq_begin*) from their first pairs `in`; sequence q is w[q] x h[q] and runs with
@@ -363,7 +367,8 @@ static int seq_begin(vo_ctx* ctx, const char* who, bool multi, int n, int flags,
     if (!ctx) return VO_E_INVALID;
     const bool open = in == nullptr;
     if (multi) {
-        if (flags & ~VO_MSEQ_MONO_ROTATION) { vo_set_error(ctx, "%s: unknown flag bits 0x%x", who, (unsigned)(flags & ~VO_MSEQ_MONO_ROTATION)); return VO_E_INVALID; }
+        const int known = VO_MSEQ_MONO_ROTATION | VO_MSEQ_DEVICE_RESULTS;
+        if (flags & ~known) { vo_set_error(ctx, "%s: unknown flag bits 0x%x", who, (unsigned)(flags & ~known)); return VO_E_INVALID; }
         if (n < 1) { vo_set_error(ctx, "%s: n_seq = %d, need at least one sequence", who, n); return VO_E_INVALID; }
         if (n > VO_MSEQ_MAX) {
             vo_set_error(ctx, "%s: %s = %d, a context holds at most %d sequences", who, open ? "n_slots" : "n_seq", n, VO_MSEQ_MAX);
@@ -431,6 +436,11 @@ static int seq_begin(vo_ctx* ctx, const char* who, bool multi, int n, int flags,
     ctx->seq_lk_bound = (int)seq_grid(ctx);
     if (ctx->seq_mono && (rc = seq_mono_scratch(ctx, n))) return rc;
     if ((rc = vo_ensure_pinned(ctx, seq_pinned(ctx, n).bytes))) return rc;
+    ctx->seq_dres = multi && (flags & VO_MSEQ_DEVICE_RESULTS);
+    if (ctx->seq_dres && !ctx->d_seq_pose) {
+        VO_CUDA_CHECK(cudaMalloc(&ctx->d_seq_pose, 16 * (size_t)VO_MSEQ_MAX * sizeof(double)));
+        for (int s = 0; s < 3; s++) VO_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->seq_tab_ev[s], cudaEventDisableTiming));
+    }
     // sequence q owns the buffer units q and n + q (both parities): both entries carry its camera (a start writes them)
     if (!open && (rc = vo_set_calibration(ctx, 0, 2 * n, P_l, P_r, n))) return rc;
     ctx->seq_slot = 0;
@@ -438,6 +448,9 @@ static int seq_begin(vo_ctx* ctx, const char* who, bool multi, int n, int flags,
     ctx->seq_pose.assign(16 * (size_t)n, 0.0);
     for (int q = 0; q < n; q++)
         for (int i = 0; i < 4; i++) ctx->seq_pose[16 * q + 5 * i] = 1.0;
+    // (a pageable copy: the host vector may go once the call returns, which the synchronise below covers anyway)
+    if (ctx->seq_dres)
+        VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_seq_pose, ctx->seq_pose.data(), 16 * (size_t)n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     ctx->seq_retired.assign(n, open ? 1 : 0);
     ctx->seq_live.assign(2 * (size_t)n, open ? 0 : 1);
     ctx->seq_cal_next.assign(2 * (size_t)n, CamCalib{});
@@ -567,6 +580,11 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
     if (!ctx) return VO_E_INVALID;
     int rc;
     if ((rc = seq_frame_check(ctx, who, multi, SEQ_SUBMIT))) return rc;
+    if (ctx->seq_dres && !in.device) {
+        vo_set_error(ctx, "%s: the sequences were begun with VO_MSEQ_DEVICE_RESULTS, which takes frames through "
+                          "vo_mseq_submit_device only (a wait that does not block cannot release host images)", who);
+        return VO_E_INVALID;
+    }
     const int n = ctx->seq_n;
     // a submission without starts checks its pairs against the running sizes, with no per-slot copies
     std::vector<char> starting;
@@ -683,13 +701,16 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
         VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_tprev + 3 * (size_t)((1 - p) * n + starts[i].slot), 0, 3 * sizeof(double), sb));
     const int u0 = p * n;
     const SeqPinned pin = seq_pinned(ctx, n);
-    VO_CUDA_CHECK(cudaMemcpyAsync(pin.rec + u0, ctx->d_results + u0, n * sizeof(vo_unit_result_dev), cudaMemcpyDeviceToHost, sb));
-    VO_CUDA_CHECK(cudaMemcpyAsync(pin.err + u0, ctx->d_seq_err + 1 + u0, n * sizeof(int), cudaMemcpyDeviceToHost, sb));
-    if (ctx->seq_mono) {                // the n results, one per scratch block, into n consecutive records: one strided copy
-        EssArgs e;
-        seq_ess_args(ctx, u0, n, e);
-        VO_CUDA_CHECK(cudaMemcpy2DAsync(pin.ess + u0, sizeof(EssResult), e.result, e.result_stride, sizeof(EssResult), n,
-                                        cudaMemcpyDeviceToHost, sb));
+    // (vo_mseq_wait_device reads the records, error words and essential results on the device: no copies)
+    if (!ctx->seq_dres) {
+        VO_CUDA_CHECK(cudaMemcpyAsync(pin.rec + u0, ctx->d_results + u0, n * sizeof(vo_unit_result_dev), cudaMemcpyDeviceToHost, sb));
+        VO_CUDA_CHECK(cudaMemcpyAsync(pin.err + u0, ctx->d_seq_err + 1 + u0, n * sizeof(int), cudaMemcpyDeviceToHost, sb));
+        if (ctx->seq_mono) {            // the n results, one per scratch block, into n consecutive records: one strided copy
+            EssArgs e;
+            seq_ess_args(ctx, u0, n, e);
+            VO_CUDA_CHECK(cudaMemcpy2DAsync(pin.ess + u0, sizeof(EssResult), e.result, e.result_stride, sizeof(EssResult), n,
+                                            cudaMemcpyDeviceToHost, sb));
+        }
     }
     VO_CUDA_CHECK(cudaEventRecord(ctx->seq_back_ev[p], sb));
     ctx->seq_slot = s1;                 // imageLeft_t0 = imageLeft_t1 (main.cpp:157-158)
@@ -709,6 +730,10 @@ static int seq_wait(vo_ctx* ctx, const char* who, bool multi, bool want_mono, vo
     if (!ctx) return VO_E_INVALID;
     int rc;
     if ((rc = seq_frame_check(ctx, who, multi, SEQ_WAIT))) return rc;
+    if (ctx->seq_dres) {
+        vo_set_error(ctx, "%s: the sequences were begun with VO_MSEQ_DEVICE_RESULTS: use vo_mseq_wait_device", who);
+        return VO_E_INVALID;
+    }
     if (!out || (multi && !status) || (want_mono && !mono)) { vo_set_error(ctx, "%s: null result", who); return VO_E_INVALID; }
     if (want_mono && !ctx->seq_mono) {
         vo_set_error(ctx, multi ? "%s: the sequences were begun without the flag VO_MSEQ_MONO_ROTATION"
@@ -784,6 +809,79 @@ static int seq_wait(vo_ctx* ctx, const char* who, bool multi, bool want_mono, vo
     }
     if (copies) VO_CUDA_CHECK(cudaStreamSynchronize(sb));
     return rc;
+}
+
+static_assert(sizeof(vo_unit_result) == sizeof(vo_unit_result_dev), "k_seq_collect writes vo_unit_result records");
+
+// VO_E_INVALID + message unless p is NULL or device (managed) memory of the context's GPU
+static int seq_check_dptr(vo_ctx* ctx, const char* who, const char* name, const void* p)
+{
+    if (!p) return VO_OK;
+    cudaPointerAttributes a;
+    const cudaError_t e = cudaPointerGetAttributes(&a, p);
+    if (e != cudaSuccess) { cudaGetLastError(); vo_set_error(ctx, "%s: %s: not a CUDA pointer (%s)", who, name, cudaGetErrorString(e)); return VO_E_INVALID; }
+    if (a.type == cudaMemoryTypeManaged) return VO_OK;
+    if (a.type != cudaMemoryTypeDevice || a.device != ctx->device) {
+        vo_set_error(ctx, "%s: %s is not device memory of GPU %d", who, name, ctx->device);
+        return VO_E_INVALID;
+    }
+    return VO_OK;
+}
+
+// vo_mseq_wait_device: the oldest submission retired by ONE k_seq_collect launch on the context's stream, after the
+// caller's work there and after that submission's back stage (seq_back_ev of its parity; the next submission's back stage
+// on the side stream is not waited for).  The stream order also covers the unit buffers: the next submission of the same
+// parity, which overwrites them, queues its front stage on the context's stream after this launch, and its back stage
+// after that front stage.  The host only moves its bookkeeping on.
+static int seq_wait_device(vo_ctx* ctx, const char* who, const vo_mseq_dresults* r)
+{
+    if (!ctx) return VO_E_INVALID;
+    int rc;
+    if ((rc = seq_frame_check(ctx, who, true, SEQ_WAIT))) return rc;
+    if (!ctx->seq_dres) {
+        vo_set_error(ctx, "%s: the sequences were begun without the flag VO_MSEQ_DEVICE_RESULTS (use vo_mseq_wait)", who);
+        return VO_E_INVALID;
+    }
+    if (!r) { vo_set_error(ctx, "%s: null result table", who); return VO_E_INVALID; }
+    const bool lists = r->pts4 || r->points3d || r->inliers || r->ess_mask;
+    if (r->pts_cap < 0 || (lists && r->pts_cap == 0)) {
+        vo_set_error(ctx, "%s: pts_cap = %d with point arrays", who, r->pts_cap);
+        return VO_E_INVALID;
+    }
+    if ((r->mono || r->ess_mask) && !ctx->seq_mono) {
+        vo_set_error(ctx, "%s: mono / ess_mask: the sequences were begun without the flag VO_MSEQ_MONO_ROTATION", who);
+        return VO_E_INVALID;
+    }
+    VO_CUDA_CHECK(cudaSetDevice(ctx->device));
+    const struct { const char* name; const void* p; } ptrs[] = {
+        {"status", r->status}, {"records", r->records}, {"frame_pose", r->frame_pose}, {"pts4", r->pts4},
+        {"points3d", r->points3d}, {"inliers", r->inliers}, {"mono", r->mono}, {"ess_mask", r->ess_mask}};
+    for (const auto& x : ptrs)
+        if ((rc = seq_check_dptr(ctx, who, x.name, x.p))) return rc;
+    const int n = ctx->seq_n;
+    const int p = (int)((ctx->seq_submitted - ctx->seq_inflight) & 1);      // the parity of the oldest frame in flight
+    const int u0 = p * n;
+    const size_t cs = (size_t)ctx->units * ctx->cap, uo = (size_t)u0 * ctx->cap;
+    CollectArgs a;
+    memset(&a, 0, sizeof(a));
+    a.res = ctx->d_results + u0; a.err = ctx->d_seq_err + 1 + u0; a.cap = ctx->cap;
+    a.valid4 = ctx->d_valid4 + uo; a.plane_stride = cs;
+    a.X = ctx->d_X + uo; a.inliers = ctx->d_inliers + uo;
+    if (ctx->seq_mono) {
+        EssArgs e;
+        seq_ess_args(ctx, u0, n, e);
+        a.ess = e.result; a.ess_mask = e.mask; a.ess_stride = ctx->seq_ess_bytes;
+    }
+    a.pose = ctx->d_seq_pose;
+    a.status = r->status; a.records = (vo_unit_result_dev*)r->records; a.pose_out = r->frame_pose; a.pts_cap = r->pts_cap;
+    a.pts4 = (float2*)r->pts4; a.points3d = (float3*)r->points3d; a.inliers_out = r->inliers; a.mono = r->mono;
+    a.mask_out = r->ess_mask;
+    for (int q = 0; q < n; q++) a.mode[q] = (unsigned char)ctx->seq_live[u0 + q];
+    VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->seq_back_ev[p], 0));
+    ctx->launches += vo_launch_seq_collect(a, n, ctx->stream);
+    VO_CUDA_CHECK(cudaGetLastError());
+    ctx->seq_inflight--;
+    return VO_OK;
 }
 
 // currentVOFeatures and the carried translation of sequence q (after the frames in flight)
@@ -968,12 +1066,24 @@ extern "C" int vo_mseq_wait_mono(vo_ctx* ctx, vo_unit_result* out, int* status, 
     return seq_wait(ctx, "vo_mseq_wait_mono", true, true, out, status, mono, ess_mask, mask_cap, pts4, pts_cap);
 }
 
+extern "C" int vo_mseq_wait_device(vo_ctx* ctx, const vo_mseq_dresults* r)
+{
+    return seq_wait_device(ctx, "vo_mseq_wait_device", r);
+}
+
 extern "C" int vo_mseq_pose(vo_ctx* ctx, int q, double frame_pose[16])
 {
     if (!ctx) return VO_E_INVALID;
     int rc;
     if ((rc = seq_frame_check(ctx, "vo_mseq_pose", true, SEQ_QUERY))) return rc;
     if (q < 0 || q >= ctx->seq_n || !frame_pose) { vo_set_error(ctx, "vo_mseq_pose: bad argument"); return VO_E_INVALID; }
+    if (ctx->seq_dres) {            // after the last vo_mseq_wait_device's k_seq_collect (the context's stream)
+        VO_CUDA_CHECK(cudaSetDevice(ctx->device));
+        if ((rc = seq_drain(ctx))) return rc;
+        VO_CUDA_CHECK(cudaMemcpyAsync(frame_pose, ctx->d_seq_pose + 16 * (size_t)q, 16 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+        VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+        return VO_OK;
+    }
     memcpy(frame_pose, ctx->seq_pose.data() + 16 * (size_t)q, 16 * sizeof(double));
     return VO_OK;
 }
