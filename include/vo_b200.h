@@ -49,7 +49,9 @@ typedef struct vo_point2f { float x, y; } vo_point2f;
 typedef struct vo_point3f { float x, y, z; } vo_point3f;
 
 /* All literals the reference hard-codes, as run-time parameters (SURVEY.md section 5, "Config").  Away from the
- * reference's values each one does what OpenCV does with it: clamped where OpenCV clamps, refused where it asserts. */
+ * reference's values each one does what OpenCV does with it: clamped where OpenCV clamps, refused where it asserts.
+ * vo_create sets the context's values.  Every field but lk_win, lk_max_level, fast_nonmax, max_features and max_units
+ * can also differ per multi-sequence slot (vo_mseq_params) and per batched unit (vo_batch_params). */
 typedef struct vo_params {
     int fast_threshold;      /* 20      reference src/feature.cpp:43; vo_create refuses values
                                         outside [0, 255] (VO_E_INVALID)                           */
@@ -80,7 +82,7 @@ typedef struct vo_params {
     int max_units;           /* work units the batched path can hold at once (default 1)      */
     /* matchingFeatures()' feature bookkeeping (reference src/visualOdometry.cpp:95-107, src/bucket.cpp:16).  Only the
      * sequence modes (vo_seq_*, vo_mseq_*) use them; the batched path (vo_frame_batch, vo_batch_*) selects features by
-     * stride and never buckets, so it ignores them.  They are context-wide, fixed at vo_create.  A sequence mode reads
+     * stride and never buckets, so it ignores them.  A multi-sequence slot can have its own (vo_mseq_params).  A sequence mode reads
      * back at most (rows/bs + 1) * (cols/bs + 1) * features_per_bucket points per frame, bs = rows / bucket_rows_divisor
      * (the bucket bound); a begin, open or start whose largest bound exceeds max_features is refused with
      * VO_E_CAPACITY.  These four fields were appended in this order after max_units: callers compiled against a header
@@ -228,6 +230,15 @@ VO_API int vo_batch_configure(vo_ctx* ctx, int w, int h, int n_units, const floa
  * (VO_E_INVALID): a range outside the configured units, NULL matrices, or a call while submissions are in flight
  * (vo_batch_wait them first); like vo_batch_configure it ends an idle sequence-mode run. */
 VO_API int vo_batch_calibrate(vo_ctx* ctx, int first_unit, int n_units, const float* P_l, const float* P_r);
+/* Units [first_unit, first_unit + n_units) get their own tracking parameters: unit first_unit + i runs with p[i] (NULL p:
+ * the context's).  The batched path reads fast_threshold, the LK criteria, circ_threshold and the three PnP fields; the
+ * four bookkeeping fields are ignored, as for the context.  A unit keeps its parameters until they are set again
+ * (vo_batch_configure resets every unit to the context's); each unit's results are those of vo_frame_batch in a context
+ * created with its parameters, bit for bit.  Refused, changing nothing: the range and in-flight rules of
+ * vo_batch_calibrate (VO_E_INVALID); an entry that vo_create would refuse (its code and message); lk_win, lk_max_level
+ * or fast_nonmax other than the context's (VO_E_UNSUPPORTED); pnp_iterations above the context's (VO_E_CAPACITY: the
+ * RANSAC scratch is sized for it).  Like vo_batch_calibrate it ends an idle sequence-mode run. */
+VO_API int vo_batch_params(vo_ctx* ctx, int first_unit, int n_units, const vo_params* p);
 /* async: copy the units' images (and features) host->device on the context's stream. */
 VO_API int vo_batch_upload(vo_ctx* ctx, const vo_unit* units, int n_units, size_t pitch);
 /* async: run the whole path for the uploaded units. */
@@ -445,6 +456,17 @@ VO_API int vo_mseq_begin_calib(vo_ctx* ctx, int n_seq, int w, int h, const float
 VO_API int vo_mseq_begin_sized(vo_ctx* ctx, int n_seq, const int* w, const int* h, const float* P_l, const float* P_r,
                                const uint8_t* const* left0, const uint8_t* const* right0, const size_t* pitch,
                                int channels, int flags);
+/* Slots [first_slot, first_slot + n) get their own tracking parameters: slot first_slot + i gets p[i] (NULL p: the
+ * context's again).  A slot keeps its setting until it is set again.  Every begin call (vo_mseq_begin*,
+ * vo_mseq_begin_device), vo_mseq_open and every start reads the setting of each slot it begins, opens or starts; a
+ * running sequence keeps the values it began with.  The call changes host state only, so it may be made while frames
+ * are in flight.  Each sequence's results are those of a context created with its slot's parameters running it alone,
+ * bit for bit, and a submission costs the same launches.  The begin, open and start checks of the bucket bound (rows /
+ * bucket_rows_divisor == 0: VO_E_UNSUPPORTED; a bound above max_features: VO_E_CAPACITY) use each slot's own fields.
+ * Refused, changing nothing: a range outside 0 .. VO_MSEQ_MAX (VO_E_INVALID); an entry that vo_create would refuse (its
+ * code and message); lk_win, lk_max_level or fast_nonmax other than the context's (VO_E_UNSUPPORTED); pnp_iterations
+ * above the context's (VO_E_CAPACITY: the RANSAC scratch is sized for it).  max_features and max_units are not read. */
+VO_API int vo_mseq_params(vo_ctx* ctx, int first_slot, int n, const vo_params* p);
 /* vo_mseq_submit with one row pitch per sequence (pitch[q] is not read for a retiring sequence); vo_mseq_submit is this
  * call with its pitch repeated, so with several sizes it needs a pitch that covers every live sequence's width. */
 VO_API int vo_mseq_submit(vo_ctx* ctx, const uint8_t* const* left1, const uint8_t* const* right1, size_t pitch, int channels);

@@ -2,7 +2,7 @@
 """Scaling of the multi-sequence streaming mode (vo_mseq_*) with the number of sequences, measured on the GPU.
 
     python tools/mseq_timing.py [--frames 40] [--rounds 5] [--counts 1,2,4,8,16,32] [--mono-rotation] [--mixed-calibration]
-                                [--mixed-sizes] [--device-input] [--device-results] [--json out.json]
+                                [--mixed-sizes] [--device-input] [--device-results] [--mixed-params] [--json out.json]
 
 Synthetic 1241x376 drives (synth.stereo_unit; eight seeds, each with its own motion) of `--frames` frames each;
 sequence q replays drive q % 8, forwards for even q // 8 and backwards for odd, so up to 16 sequences are distinct and
@@ -29,7 +29,11 @@ vo_mseq_* count two ways in the same rounds, alternated, both with resident gray
 vo_mseq_submit_device: host waits that return the point lists (vo_mseq_wait with pts4), and a run begun with
 VO_MSEQ_DEVICE_RESULTS whose waits are vo_mseq_wait_device into one reused set of CUDA tensors, each followed by a trivial
 torch consumer of them on the same stream (the loop ends with a synchronise, inside the timed window).  It adds the host
-time per step spent inside the submit and wait calls, and the kernel launches per submission and per wait.  The card's name, power limit and max SM clock, read in the same run, are printed with the numbers;
+time per step spent inside the submit and wait calls, and the kernel launches per submission and per wait.
+`--mixed-params` (counts 1, 8 and 32 unless --counts is given) also runs every vo_mseq_* count with one set of tracking
+parameters per sequence (vo_mseq_params: sequence q takes set q mod 8 of PARAM_SETS, FAST thresholds, LK criteria, PnP
+settings, bucket grids and densities), timed against the same count at the context's one set in the same rounds,
+alternated.  The card's name, power limit and max SM clock, read in the same run, are printed with the numbers;
 they are part of them."""
 import argparse
 import json
@@ -44,6 +48,13 @@ import numpy as np
 
 W, H, DRIVES = 1241, 376, 8
 KITTI_SIZES = [(1241, 376)] * 3 + [(1242, 375)] + [(1226, 370)] * 7      # training sequences 00 .. 10
+
+
+# --mixed-params: sequence q runs with PARAM_SETS[q % 8] (every bound within max_features = 4096 at 1241x376)
+PARAM_SETS = [dict(), dict(fast_threshold=12), dict(features_per_bucket=3, bucket_rows_divisor=6),
+              dict(lk_max_iters=7, lk_epsilon=0.05, lk_min_eig=1e-2), dict(pnp_iterations=40, pnp_reproj_error=1.5, pnp_confidence=0.99),
+              dict(refill_threshold=500, bucket_age_threshold=3, circ_threshold=1), dict(fast_threshold=30, lk_max_iters=15),
+              dict(features_per_bucket=2, bucket_rows_divisor=12)]
 
 
 def card():
@@ -214,13 +225,15 @@ def main():
                     help="also time every vo_mseq_* count with frames resident in GPU memory (gray and BGR tensors)")
     ap.add_argument("--device-results", action="store_true",
                     help="also time device input with host waits against vo_mseq_wait_device (VO_MSEQ_DEVICE_RESULTS)")
+    ap.add_argument("--mixed-params", action="store_true",
+                    help="also time every vo_mseq_* count with one set of tracking parameters per sequence")
     ap.add_argument("--json", help="also write the result here")
     a = ap.parse_args()
     if a.mixed_sizes and a.counts == ap.get_default("counts"):
         a.counts = "3,11,32"
     if a.device_input and a.counts == ap.get_default("counts"):
         a.counts = "1,8,16,32"
-    if a.device_results and a.counts == ap.get_default("counts"):
+    if (a.device_results or a.mixed_params) and a.counts == ap.get_default("counts"):
         a.counts = "1,8,32"
     counts = [int(c) for c in a.counts.split(",")]
     from visual_odom_b200 import capi, synth
@@ -237,6 +250,8 @@ def main():
         modes += [(m, False, kind) for m in counts for kind in ("dev-gray", "dev-bgr")]
     if a.device_results:
         modes += [(m, False, kind) for m in counts for kind in ("dres-host", "dres-dev")]
+    if a.mixed_params:
+        modes += [(m, False, "params") for m in counts]
     seqs = {n: [sequence(dr, q) for q in range(n)] for n in counts}
     mixed = {}
     if a.mixed_calibration:              # per count n: sequence q rendered with calibration(q, n), played like sequence(dr, q)
@@ -277,6 +292,12 @@ def main():
         if mix in ("dev-gray", "dev-bgr"):
             s = dev[mix][m] if fr_cut is None else [x[:fr_cut] for x in dev[mix][m]]
             return run_mseq_device(ctx, P_l, P_r, s, "bgr" if mix == "dev-bgr" else None)
+        if mix == "params":
+            ctx.mseq_params(0, [PARAM_SETS[q % len(PARAM_SETS)] for q in range(m)])
+            try:
+                return run_mseq(ctx, P_l, P_r, seqs[m] if fr_cut is None else [x[:fr_cut] for x in seqs[m]], mono)
+            finally:
+                ctx.mseq_params(0, [None] * m)
         s, Pl, Pr = (sized[m], P_l, P_r) if mix == "sizes" else (mixed[m] if mix else (seqs[m], P_l, P_r))
         s = s if fr_cut is None else [x[:fr_cut] for x in s]
         return run_mseq(ctx, Pl, Pr, s, mono)
@@ -303,11 +324,12 @@ def main():
         if r["host"]:
             o.update(host_ms_per_step=1e3 * float(np.median(r["host"])), launches_per_wait=float(np.median(r["wait_launches"])))
         m, mono, mix = mode
-        out["modes"][str(m) + ("+mono" if mono else "") + ("+sizes" if mix == "sizes" else f"+{mix}" if mix in ("dev-gray", "dev-bgr", "dres-host", "dres-dev")
+        out["modes"][str(m) + ("+mono" if mono else "") + ("+sizes" if mix == "sizes" else f"+{mix}" if mix in ("dev-gray", "dev-bgr", "dres-host", "dres-dev", "params")
                                else "+mixed" if mix else "")] = o
         name = ("vo_seq (1 sequence)" if m == "seq" else f"vo_mseq n_seq = {m:2d}") + (", mono" if mono else "") + \
             (", KITTI sizes" if mix == "sizes" else ", device gray" if mix == "dev-gray" else ", device BGR" if mix == "dev-bgr"
              else ", dev in, host wait" if mix == "dres-host" else ", dev in, dev results" if mix == "dres-dev"
+             else ", params per sequence" if mix == "params"
              else ", mixed cal." if mix else "")
         print(f"{name:40s}: {o['aggregate_fps']:8.0f} frames/s [{o['aggregate_fps_min']:.0f}, {o['aggregate_fps_max']:.0f}], "
               f"step {o['step_latency_ms']:.3f} ms, {o['launches_per_submission']:.1f} launches / submission"

@@ -19,7 +19,12 @@ the translation from the PnP; frames where that branch would abort are reported 
 the datasets as a queue through N slots (vo_mseq_open + vo_mseq_submit_start): the first N start together, and each
 next one starts in the first slot that frees (the lowest slot on a tie), in the order given, so any number of datasets
 runs through one context; their sizes may differ (one pyramid depth, the envelope of all of them), and every pose file
-is the same for every N.  `--check` only validates the inputs and prints the schedule of --slots (no GPU needed)."""
+is the same for every N.  `--params-for NAME=FIELD=V[,FIELD=V...]` gives the dataset NAME its own tracking parameters
+(vo_params fields such as fast_threshold, lk_max_iters, circ_threshold, pnp_reproj_error or features_per_bucket; the
+context-wide lk_win, lk_max_level, fast_nonmax, max_features and max_units are refused); each sequence runs in its own
+slot as a context created with its parameters would run it alone (vo_mseq_params).  `--sweep FIELD=V1,V2,...` runs the
+first dataset once per value, each in its own slot of one context, with pose files OUTDIR/<name>_<FIELD>=<V>.txt.
+`--check` only validates the inputs and prints each sequence's parameters and the schedule of --slots (no GPU needed)."""
 import argparse
 import os
 import sys
@@ -47,6 +52,33 @@ def pyramid_depth(w, h):
             break
         n += 1
     return n
+
+
+# vo_params fields a slot may set (vo_mseq_params); the others are the context's
+SEQ_FIELDS = ("fast_threshold", "lk_max_iters", "lk_epsilon", "lk_min_eig", "circ_threshold", "pnp_iterations",
+              "pnp_reproj_error", "pnp_confidence", "refill_threshold", "bucket_rows_divisor", "features_per_bucket",
+              "bucket_age_threshold")
+
+
+def parse_fields(spec, what):
+    """FIELD=V[,FIELD=V...] -> {field: value} typed as vo_params declares the field"""
+    import ctypes as C
+    from visual_odom_b200 import capi
+    types = dict(capi.VoParams._fields_)
+    out = {}
+    for item in spec.split(","):
+        field, sep, v = item.partition("=")
+        if not sep or not field or not v:
+            raise SystemExit(f"{what} {spec}: expected FIELD=VALUE[,FIELD=VALUE...]")
+        if field not in types:
+            raise SystemExit(f"{what} {spec}: vo_params has no field {field}")
+        if field not in SEQ_FIELDS:
+            raise SystemExit(f"{what} {spec}: {field} is context-wide (one value for every sequence of a context)")
+        try:
+            out[field] = int(v) if types[field] is C.c_int else float(v)
+        except ValueError:
+            raise SystemExit(f"{what} {spec}: {field} takes {'an integer' if types[field] is C.c_int else 'a number'}, not {v}")
+    return out
 
 
 def queue_schedule(lengths, n_slots):
@@ -79,6 +111,10 @@ def main():
     ap.add_argument("--slots", type=int, metavar="N",
                     help="run the datasets as a queue through N slots, each starting in the first slot that frees")
     add_bucket_args(ap)
+    ap.add_argument("--params-for", action="append", default=[], metavar="NAME=FIELD=V[,FIELD=V...]",
+                    help="tracking parameters of the dataset named NAME (repeatable; the others use the flags' values)")
+    ap.add_argument("--sweep", metavar="FIELD=V1,V2,...",
+                    help="run the first dataset once per value of FIELD, each in its own slot of one context")
     ap.add_argument("--check", action="store_true")
     a = ap.parse_args()
     from visual_odom_b200 import capi, synth
@@ -91,6 +127,24 @@ def main():
     names = [os.path.basename(os.path.normpath(d)) for d in a.datasets]
     if len(set(names)) != len(names):
         raise SystemExit(f"two datasets share a directory name ({names}): their pose files would collide")
+    params_for = {}
+    for spec in a.params_for:
+        name, sep, rest = spec.partition("=")
+        if not sep or not name:
+            raise SystemExit(f"--params-for {spec}: expected NAME=FIELD=VALUE[,FIELD=VALUE...]")
+        if name not in names:
+            raise SystemExit(f"--params-for {spec}: no dataset is named {name} (names: {', '.join(names)})")
+        if name in params_for:
+            raise SystemExit(f"--params-for: {name} is given twice")
+        params_for[name] = parse_fields(rest, "--params-for")
+    sweep = None
+    if a.sweep:
+        field, sep, values = a.sweep.partition("=")
+        if a.slots is not None:
+            raise SystemExit("--sweep runs every value in a slot of its own: it does not combine with --slots")
+        sweep = [(v, parse_fields(f"{field}={v}", "--sweep")) for v in values.split(",")] if sep else None
+        if not sweep or len(sweep) > capi.VO_MSEQ_MAX or len({v for v, _ in sweep}) != len(sweep):
+            raise SystemExit(f"--sweep {a.sweep}: expected FIELD=V1,V2,... with 1 to {capi.VO_MSEQ_MAX} distinct values")
     cal_for = {}
     for spec in a.calibration_for:
         name, sep, path = spec.partition("=")
@@ -124,9 +178,34 @@ def main():
             raise SystemExit(f"{gt}: no ground truth for sequence {name}")
         cal_path, cal = cal_for.get(name, (a.calibration, default_cal))
         P_l, P_r = synth.proj_matrices(cal)
-        seqs.append(dict(dir=d, name=name, n=n, w=w, h=h, gray=ctype == 0, gt=gt, P_l=P_l, P_r=P_r))
+        seqs.append(dict(dir=d, name=name, n=n, w=w, h=h, gray=ctype == 0, gt=gt, P_l=P_l, P_r=P_r, own=params_for.get(name, {})))
         print(f"{name}: {n} stereo pairs of {w}x{h} (PNG colour type {ctype}, {depth} bit), calibration {cal_path}")
         print(f"  P_left =\n{P_l}\n  P_right =\n{P_r}")
+        if sweep:
+            break                            # the sweep runs the first dataset only
+    if sweep:
+        first = seqs.pop()
+        field = a.sweep.partition("=")[0]
+        for v, own in sweep:
+            seqs.append(dict(first, name=f"{first['name']}_{field}={v}", own=dict(first["own"], **own)))
+    # each sequence's parameters: the flags' values (the library's defaults elsewhere), then its own
+    import ctypes as C
+    base = capi.VoParams()
+    capi.load_library().vo_default_params(C.byref(base))
+    flags = dict(refill_threshold=a.refill_threshold, bucket_rows_divisor=a.bucket_divisor,
+                 features_per_bucket=a.features_per_bucket, bucket_age_threshold=a.age_threshold)
+    for s in seqs:
+        s["params"] = {f: flags.get(f, getattr(base, f)) for f in SEQ_FIELDS}
+        s["params"].update(s["own"])
+        p = s["params"]
+        if p["features_per_bucket"] < 1 or p["bucket_rows_divisor"] < 1:
+            raise SystemExit(f"{s['name']}: features_per_bucket and bucket_rows_divisor must be positive")
+        if s["h"] // p["bucket_rows_divisor"] == 0:
+            raise SystemExit(f"{s['name']}: {s['w']}x{s['h']} images are too small for the rows/{p['bucket_rows_divisor']} bucket size")
+        s["grid"] = bucket_grid(s["w"], s["h"], p["bucket_rows_divisor"], p["features_per_bucket"])
+    if sweep or params_for:
+        for s in seqs:
+            print(f"{s['name']}: " + " ".join(f"{f}={s['params'][f]:g}" for f in SEQ_FIELDS))
     if sized:
         print("image sizes: " + ", ".join(f"{s['name']} {s['w']}x{s['h']}" for s in seqs))
     if a.slots is not None:
@@ -134,11 +213,14 @@ def main():
         if pyramid_depth(W, H) != pyramid_depth(seqs[0]["w"], seqs[0]["h"]):
             raise SystemExit(f"the envelope {W}x{H} of the sizes has {pyramid_depth(W, H)} pyramid levels, the sizes "
                              f"{pyramid_depth(seqs[0]['w'], seqs[0]['h'])}: one context runs one pyramid depth")
+        # every slot opens at the densest sequence's parameters, which size the mono scratch for the envelope
+        densest = max(seqs, key=lambda s: bucket_grid(W, H, s["params"]["bucket_rows_divisor"], s["params"]["features_per_bucket"]))
+        a.open_params = densest["params"]
+        env = bucket_grid(W, H, a.open_params["bucket_rows_divisor"], a.open_params["features_per_bucket"])
         for s in seqs:
-            grid = lambda w, h: bucket_grid(w, h, a.bucket_divisor, a.features_per_bucket)
-            if a.mono_rotation and grid(s["w"], s["h"]) > grid(W, H):
-                raise SystemExit(f"{s['dir']}: {s['w']}x{s['h']} reads back {grid(s['w'], s['h'])} points, more than "
-                                 f"the {grid(W, H)} of the envelope {W}x{H} the mono scratch is sized for")
+            if a.mono_rotation and s["grid"] > env:
+                raise SystemExit(f"{s['dir']}: {s['w']}x{s['h']} reads back {s['grid']} points, more than "
+                                 f"the {env} of the envelope {W}x{H} the mono scratch is sized for")
         sched = queue_schedule([s["n"] for s in seqs], a.slots)
         steps = max(k0 + s["n"] - 1 for s, (_, k0) in zip(seqs, sched))
         print(f"schedule: {len(seqs)} sequences through {a.slots} slots of {W}x{H}, {steps} submissions")
@@ -148,6 +230,11 @@ def main():
     print("rotation: " + ("findEssentialMat + recoverPose (mono_rotation = true)" if a.mono_rotation else
                           "Rodrigues of the PnP rvec (mono_rotation = false)"))
     prm = bucket_params(a, [(s["w"], s["h"]) for s in seqs] + ([(W, H)] if a.slots is not None else []))
+    # max_features covers every sequence's own bound, and pnp_iterations (the RANSAC scratch) every sequence's count;
+    # each sequence then runs with its own parameters
+    prm["max_features"] = max([prm["max_features"]] + [s["grid"] for s in seqs] +
+                              ([env] if a.slots is not None else []))
+    prm["pnp_iterations"] = max(max(s["params"]["pnp_iterations"] for s in seqs), base.pnp_iterations)
     print(f"bucketing: {a.features_per_bucket} feature(s) per bucket of rows/{a.bucket_divisor}, ages < {a.age_threshold}, "
           f"refill below {a.refill_threshold} features; max_features {prm['max_features']}")
     if a.check:
@@ -159,6 +246,7 @@ def main():
     # sequences mix gray and colour files, then all are converted to gray while decoding
     force = 0 if len({s["gray"] for s in seqs}) == 1 else 1
     ctx = capi.Context(a.device, **a.context_params)
+    ctx.mseq_params(0, [s["params"] for s in seqs])
     rds = [capi.SequenceReader(s["dir"], 0, s["n"], threads=a.threads, depth=a.threads + 3, force_channels=force) for s in seqs]
 
     def pairs(k):
@@ -229,6 +317,7 @@ def run_queue(a, capi, seqs, sched, W, H):
     """--slots: every dataset starts in its scheduled slot (vo_mseq_submit_start) and retires after its last frame."""
     force = 0 if len({s["gray"] for s in seqs}) == 1 else 1
     ctx = capi.Context(a.device, **a.context_params)
+    ctx.mseq_params(0, [a.open_params] * a.slots)
     ctx.mseq_open(a.slots, W, H, mono_rotation=a.mono_rotation)
     steps = max(s["k0"] + s["n"] - 1 for s in seqs)
     rds = {}                   # dataset index -> its reader, opened at its first pair, closed after its last wait
@@ -244,6 +333,7 @@ def run_queue(a, capi, seqs, sched, W, H):
             if k == s["k0"]:
                 rds[i] = capi.SequenceReader(s["dir"], 0, s["n"], threads=a.threads, depth=a.threads + 3, force_channels=force)
                 start[s["slot"]] = (s["w"], s["h"], s["P_l"], s["P_r"])
+                ctx.mseq_params(s["slot"], [s["params"]])         # read by the start (host state: the slot may be in flight)
             l, r, _, _, pitch, ch, _ = rds[i].next_ptr()
             lp[s["slot"]], rp[s["slot"]], pitches[s["slot"]] = l, r, pitch
             chs.add(ch)

@@ -199,6 +199,8 @@ SIGNATURES = {
     "vo_mseq_begin_calib": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_size_t, C.c_int, C.c_int]),
     "vo_batch_calibrate": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vo_batch_params": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(VoParams)]),
+    "vo_mseq_params": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(VoParams)]),
     "vo_mseq_begin_sized": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     "vo_mseq_submit": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
@@ -418,6 +420,30 @@ class Context:
         if P_l.ndim != 3 or P_l.shape[1:] != (3, 4) or P_r.shape != P_l.shape:
             raise ValueError(f"P_l / P_r must be (n, 3, 4), got {P_l.shape} / {P_r.shape}")
         self._check(self.lib.vo_batch_calibrate(self.h, first_unit, len(P_l), _p(P_l), _p(P_r)))
+
+    def params_with(self, override=None):
+        """A VoParams: the context's own (self.params) with the fields of the dict `override` (None: none) changed."""
+        p = VoParams()
+        C.memmove(C.byref(p), C.byref(self.params), C.sizeof(VoParams))
+        for k, v in (override or {}).items():
+            if not hasattr(p, k):
+                raise TypeError(f"unknown vo_params field {k}")
+            setattr(p, k, v)
+        return p
+
+    def _params_array(self, overrides):
+        arr = (VoParams * len(overrides))()
+        for i, o in enumerate(overrides):
+            arr[i] = self.params_with(o)
+        return arr
+
+    def batch_params(self, first_unit, overrides):
+        """Units [first_unit, first_unit + len(overrides)) get their own tracking parameters (vo_batch_params): each entry
+        of `overrides` is a dict of the vo_params fields that differ from the context's, or None for the context's own.
+        Refused while submissions are in flight."""
+        if not overrides:
+            raise ValueError("batch_params: no units")
+        self._check(self.lib.vo_batch_params(self.h, first_unit, len(overrides), self._params_array(overrides)))
 
     def make_units(self, units):
         """units: list of dicts(l0,r0,l1,r1 uint8 HxW [, pts (n,2) f32 | n_select int] [, t_prev]).
@@ -815,6 +841,14 @@ class Context:
         n = len(left_ptrs)
         lp, rp = (C.c_void_p * n)(*left_ptrs), (C.c_void_p * n)(*right_ptrs)
         self._mseq_begin(n, w, h, lp, rp, pitch, channels, P_l, P_r, mono_rotation)
+
+    def mseq_params(self, first_slot, overrides):
+        """Slots [first_slot, first_slot + len(overrides)) get their own tracking parameters (vo_mseq_params), read by the
+        next begin, open or start of each slot: each entry of `overrides` is a dict of the vo_params fields that differ
+        from the context's, or None for the context's own.  Host state only: allowed while frames are in flight."""
+        if not overrides:
+            raise ValueError("mseq_params: no slots")
+        self._check(self.lib.vo_mseq_params(self.h, first_slot, len(overrides), self._params_array(overrides)))
 
     def mseq_open(self, n_slots, max_w, max_h, mono_rotation=False, device_results=False):
         """n_slots empty slots for sequences of any size inside max_w x max_h with that size's pyramid depth

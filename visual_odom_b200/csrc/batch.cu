@@ -116,6 +116,8 @@ extern "C" int vo_batch_configure(vo_ctx* ctx, int w, int h, int n_units, const 
     if (rc) return rc;
     if ((rc = vo_ensure_state(ctx, w, h, n_units))) return rc;
     if ((rc = vo_set_calibration(ctx, 0, ctx->units, P_l, P_r, 1))) return rc;        // every unit, as the resident state holds them
+    const std::vector<UnitParams> e(ctx->units, vo_unit_params(ctx->p));              // and the context's parameters
+    if ((rc = vo_write_params(ctx, 0, ctx->units, e.data()))) return rc;
     ctx->batch_units = n_units;
     ctx->batch_uploaded = 0;
     ctx->slot_pts.assign(n_units, 0);
@@ -136,6 +138,27 @@ extern "C" int vo_batch_calibrate(vo_ctx* ctx, int first_unit, int n_units, cons
     int rc = vo_claim_buffers(ctx, "vo_batch_calibrate");
     if (rc) return rc;
     return vo_set_calibration(ctx, first_unit, n_units, P_l, P_r, n_units);
+}
+
+// the same rules as vo_batch_calibrate; each entry checked before anything changes
+extern "C" int vo_batch_params(vo_ctx* ctx, int first_unit, int n_units, const vo_params* p)
+{
+    if (!ctx) return VO_E_INVALID;
+    if (first_unit < 0 || n_units <= 0 || first_unit + n_units > ctx->batch_units) {
+        vo_set_error(ctx, "vo_batch_params: units [%d, %d) outside the configured batch (%d)", first_unit, first_unit + n_units, ctx->batch_units);
+        return VO_E_INVALID;
+    }
+    int rc;
+    std::vector<UnitParams> e(n_units, vo_unit_params(ctx->p));
+    for (int i = 0; p && i < n_units; i++) {
+        char what[32];
+        snprintf(what, sizeof(what), "unit %d", first_unit + i);
+        if ((rc = vo_check_unit_params(ctx, "vo_batch_params", what, p[i]))) return rc;
+        e[i] = vo_unit_params(p[i]);
+    }
+    VO_CUDA_CHECK(cudaSetDevice(ctx->device));
+    if ((rc = vo_claim_buffers(ctx, "vo_batch_params"))) return rc;
+    return vo_write_params(ctx, first_unit, n_units, e.data());
 }
 
 // Pinned staging of the batched path, disjoint per unit: t_prev [batch_units][3] | counts [batch_units] | result records
@@ -288,18 +311,18 @@ static int run_range_launch(vo_ctx* ctx, const View& v)
     };
     if ((rc = hand_over(0, v.s, pre.s))) return rc;
     if (ctx->batch_detect) {
-        if ((rc = vo_run_fast(ctx, pre, 0, false))) return rc;
+        if ((rc = vo_run_fast(ctx, pre, 0, false, ctx->d_par))) return rc;
         if ((rc = vo_run_select(ctx, pre))) return rc;
     }
     if ((rc = vo_run_pyramid(ctx, v.u0 * v.imgs, v.n * v.imgs, pre.s))) return rc;
     if ((rc = hand_over(1, pre.s, lk.s))) return rc;
     const int ip[4] = {0, 1, 3, 2}, in[4] = {1, 3, 2, 0};      // ring L0->R0->R1->L1->L0 (planes L0,R0,L1,R1)
-    if ((rc = vo_run_lk_ring(ctx, lk, 4, ip, in, false))) return rc;
+    if ((rc = vo_run_lk_ring(ctx, lk, 4, ip, in, false, ctx->d_par))) return rc;
     if ((rc = hand_over(2, lk.s, post.s))) return rc;
-    if ((rc = vo_run_filter(ctx, post, false))) return rc;
+    if ((rc = vo_run_filter(ctx, post, false, ctx->d_par))) return rc;
     const size_t cs = (size_t)ctx->units * ctx->cap;
     if ((rc = vo_run_triangulate(ctx, post, ctx->d_valid4, ctx->d_valid4 + cs, ctx->d_n5, ctx->d_cal))) return rc;
-    if ((rc = vo_run_pnp(ctx, post, ctx->d_valid4 + 2 * cs, ctx->d_n5, ctx->d_cal))) return rc;
+    if ((rc = vo_run_pnp(ctx, post, ctx->d_valid4 + 2 * cs, ctx->d_n5, ctx->d_cal, ctx->d_par))) return rc;
     k_pack_counts<<<(v.n + 63) / 64, 64, 0, post.s>>>(ctx->d_results + v.u0, ctx->d_npts + v.u0, ctx->d_ndet + v.u0, ctx->d_n3 + v.u0,
                                                      ctx->d_n5 + v.u0, v.n, ctx->batch_detect ? 1 : 0);
     ctx->launches += 1;

@@ -32,7 +32,7 @@ extern "C" int vo_lk_track(vo_ctx* ctx, const uint8_t* prev, const uint8_t* next
     VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_pts_in, prev_pts, (size_t)n * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
     VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_npts, &n, sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
     const int ip[1] = {0}, in[1] = {1};
-    if ((rc = vo_run_lk(ctx, View{0, 1, ctx->stream, -1, 2, n}, 1, ip, in, err != nullptr))) return rc;
+    if ((rc = vo_run_lk(ctx, View{0, 1, ctx->stream, -1, 2, n}, 1, ip, in, err != nullptr, ctx->d_par_tab))) return rc;
     VO_CUDA_CHECK(cudaMemcpyAsync(next_pts, ctx->d_pts_out, (size_t)n * sizeof(float2), cudaMemcpyDeviceToHost, ctx->stream));
     VO_CUDA_CHECK(cudaMemcpyAsync(status, ctx->d_status, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
     if (err) VO_CUDA_CHECK(cudaMemcpyAsync(err, ctx->d_err, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
@@ -64,8 +64,8 @@ extern "C" int vo_circular_match(vo_ctx* ctx, const uint8_t* l0, const uint8_t* 
         VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_ages_in, ages_io, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
     // ring order: L0->R0, R0->R1, R1->L1, L1->L0   (planes: L0=0, R0=1, L1=2, R1=3)
     const int ip[4] = {0, 1, 3, 2}, in[4] = {1, 3, 2, 0};
-    if ((rc = vo_run_lk(ctx, View{0, 1, ctx->stream, -1, 4, n}, 4, ip, in, false))) return rc;
-    if ((rc = vo_run_filter(ctx, View{0, 1, ctx->stream}, ages_io != nullptr))) return rc;
+    if ((rc = vo_run_lk(ctx, View{0, 1, ctx->stream, -1, 4, n}, 4, ip, in, false, ctx->d_par_tab))) return rc;
+    if ((rc = vo_run_filter(ctx, View{0, 1, ctx->stream}, ages_io != nullptr, ctx->d_par_tab))) return rc;
     int n3 = 0;
     VO_CUDA_CHECK(cudaMemcpyAsync(&n3, ctx->d_n3, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     const size_t cs = (size_t)ctx->units * ctx->cap;
@@ -106,7 +106,7 @@ extern "C" int vo_fast_detect(vo_ctx* ctx, const uint8_t* img, int w, int h, siz
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
     if ((rc = vo_ensure_state(ctx, w, h, 1))) return rc;
     if ((rc = upload_image(ctx, 0, img, w, h, pitch))) return rc;
-    if ((rc = vo_run_fast(ctx, View{0, 1, ctx->stream}, 0, response != nullptr))) return rc;
+    if ((rc = vo_run_fast(ctx, View{0, 1, ctx->stream}, 0, response != nullptr, ctx->d_par_tab))) return rc;
     int n = 0;
     VO_CUDA_CHECK(cudaMemcpyAsync(&n, ctx->d_ndet, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
@@ -188,7 +188,7 @@ extern "C" int vo_pnp_ransac(vo_ctx* ctx, const vo_point3f* X, const vo_point2f*
     CamCalib c = ctx->cal[0];           // the stage calls' entry
     vo_calib_set_pnp(c, K);
     if ((rc = vo_write_calib(ctx, -1, 1, &c))) return rc;
-    if ((rc = vo_run_pnp(ctx, View{0, 1, ctx->stream}, ctx->d_valid4 + 2 * cs, ctx->d_n5, ctx->d_cal_tab))) return rc;
+    if ((rc = vo_run_pnp(ctx, View{0, 1, ctx->stream}, ctx->d_valid4 + 2 * cs, ctx->d_n5, ctx->d_cal_tab, ctx->d_par_tab))) return rc;
     vo_unit_result_dev r;
     VO_CUDA_CHECK(cudaMemcpyAsync(&r, ctx->d_results, sizeof(r), cudaMemcpyDeviceToHost, ctx->stream));
     VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));

@@ -70,6 +70,21 @@ struct CamCalib {
     int pad_;
 };
 
+// One unit's tracking parameters as the kernels read them: one entry per buffer unit in the context's parameter table
+// (ctx.h vo_ctx::d_par), beside the unit's calibration entry.  vo_unit_params (ctx.h) computes every value on the host
+// with the expressions the launch sites used when the values were launch-wide, so a unit at the context's vo_params sees
+// the same bits.
+struct UnitParams {
+    double eps2;                  // LK: epsilon^2 of the epsilon clamped to [0, 10]
+    double confidence;            // PnP: pnp_confidence
+    float min_eig;                // LK: lk_min_eig as a float (cv::LKTrackerInvoker keeps minEigThreshold as one)
+    float thr2;                   // PnP: (float)((double)pnp_reproj_error^2)
+    int max_iters;                // LK: lk_max_iters clamped to [0, 100]
+    int pnp_iterations;           // PnP: max(pnp_iterations, 1), at most the context's (the RANSAC scratch)
+    int fast_threshold, circ_threshold;
+    int refill_threshold, bucket_rows_divisor, features_per_bucket, bucket_age_threshold;   // sequence modes only
+};
+
 // the five-point branch's camera values (also vo_mono_rotation's, which takes focal / pp directly)
 static inline void vo_calib_set_ess(CamCalib& c, double focal, double ppx, double ppy)
 {

@@ -33,6 +33,88 @@ extern "C" void vo_default_params(vo_params* p)
     p->bucket_age_threshold = 10;         // bucket.cpp:16
 }
 
+int vo_check_params(vo_ctx* ctx, const vo_params& p)
+{
+    if (p.fast_threshold < 0 || p.fast_threshold > 255) {
+        // a pixel difference lies in [-255, 255]: other thresholds have no meaning (cv::FAST gives arbitrary lists for them)
+        vo_set_error(ctx, "fast_threshold=%d outside [0,255]", p.fast_threshold);
+        return VO_E_INVALID;
+    }
+    if (!(p.pnp_confidence > 0.0 && p.pnp_confidence < 1.0)) {
+        // cv::solvePnPRansac asserts 0 < confidence < 1 (NaN included); outside it the iteration bound has no meaning
+        vo_set_error(ctx, "pnp_confidence=%g outside (0,1)", p.pnp_confidence);
+        return VO_E_INVALID;
+    }
+    if (p.bucket_rows_divisor <= 0) {
+        vo_set_error(ctx, "bucket_rows_divisor=%d: bucket_size = rows / divisor needs a positive divisor", p.bucket_rows_divisor);
+        return VO_E_INVALID;
+    }
+    if (p.features_per_bucket <= 0) {
+        // Bucket::add_feature on a full bucket of max_size 0 reads ages[0] of an empty vector
+        vo_set_error(ctx, "features_per_bucket=%d: a bucket holds at least one feature", p.features_per_bucket);
+        return VO_E_INVALID;
+    }
+    if (p.lk_win != VO_WIN) {
+        vo_set_error(ctx, "lk_win=%d unsupported: the LK kernel is built for the reference's 21x21 window", p.lk_win);
+        return VO_E_UNSUPPORTED;
+    }
+    if (p.lk_max_level < 0 || p.lk_max_level >= VO_MAX_LEVELS) {
+        vo_set_error(ctx, "lk_max_level=%d outside [0,%d]", p.lk_max_level, VO_MAX_LEVELS - 1);
+        return VO_E_UNSUPPORTED;
+    }
+    return VO_OK;
+}
+
+int vo_check_unit_params(vo_ctx* ctx, const char* who, const char* what, const vo_params& p)
+{
+    int rc = vo_check_params(ctx, p);
+    if (rc) {
+        char msg[sizeof(ctx->err)];
+        snprintf(msg, sizeof(msg), "%s", ctx->err);
+        vo_set_error(ctx, "%s: %s: %s", who, what, msg);
+        return rc;
+    }
+    // the pyramid depth, the window and the corner capacity are the context's
+    const struct { const char* name; int v, c; } common[] = {
+        {"lk_win", p.lk_win, ctx->p.lk_win}, {"lk_max_level", p.lk_max_level, ctx->p.lk_max_level},
+        {"fast_nonmax", p.fast_nonmax, ctx->p.fast_nonmax}};
+    for (const auto& f : common)
+        if (f.v != f.c) {
+            vo_set_error(ctx, "%s: %s: %s=%d differs from the context's %d (it is context-wide)", who, what, f.name, f.v, f.c);
+            return VO_E_UNSUPPORTED;
+        }
+    // the RANSAC scratch holds the context's iteration count
+    if (p.pnp_iterations > vo_pnp_iterations(ctx)) {
+        vo_set_error(ctx, "%s: %s: pnp_iterations=%d above the context's %d (the RANSAC scratch is sized for it)", who, what,
+                     p.pnp_iterations, vo_pnp_iterations(ctx));
+        return VO_E_CAPACITY;
+    }
+    return VO_OK;
+}
+
+UnitParams vo_unit_params(const vo_params& p)
+{
+    UnitParams e;
+    memset(&e, 0, sizeof(e));
+    // calcOpticalFlowPyrLK clamps the criteria: maxCount to [0, 100], epsilon to [0, 10]
+    e.max_iters = p.lk_max_iters < 0 ? 0 : p.lk_max_iters > 100 ? 100 : p.lk_max_iters;
+    double eps = p.lk_epsilon;
+    if (eps < 0.) eps = 0.; if (eps > 10.) eps = 10.;
+    e.eps2 = eps * eps;
+    e.min_eig = (float)p.lk_min_eig;
+    const double thr = (double)p.pnp_reproj_error;      // float -> double, squared in double, stored float
+    e.thr2 = (float)(thr * thr);
+    e.confidence = p.pnp_confidence;
+    e.pnp_iterations = p.pnp_iterations > 1 ? p.pnp_iterations : 1;   // cv::RANSACPointSetRegistrator runs at least one
+    e.fast_threshold = p.fast_threshold;
+    e.circ_threshold = p.circ_threshold;
+    e.refill_threshold = p.refill_threshold;
+    e.bucket_rows_divisor = p.bucket_rows_divisor;
+    e.features_per_bucket = p.features_per_bucket;
+    e.bucket_age_threshold = p.bucket_age_threshold;
+    return e;
+}
+
 extern "C" int vo_create(int device, const vo_params* params, vo_ctx** out)
 {
     if (!out) return VO_E_INVALID;
@@ -41,37 +123,13 @@ extern "C" int vo_create(int device, const vo_params* params, vo_ctx** out)
     if (params) ctx->p = *params; else vo_default_params(&ctx->p);
     ctx->device = device;
     *out = ctx;      // returned even on failure so the caller can read vo_last_error()
-    if (ctx->p.fast_threshold < 0 || ctx->p.fast_threshold > 255) {
-        // a pixel difference lies in [-255, 255]: other thresholds have no meaning (cv::FAST gives arbitrary lists for them)
-        vo_set_error(ctx, "fast_threshold=%d outside [0,255]", ctx->p.fast_threshold);
-        return VO_E_INVALID;
-    }
-    if (!(ctx->p.pnp_confidence > 0.0 && ctx->p.pnp_confidence < 1.0)) {
-        // cv::solvePnPRansac asserts 0 < confidence < 1 (NaN included); outside it the iteration bound has no meaning
-        vo_set_error(ctx, "pnp_confidence=%g outside (0,1)", ctx->p.pnp_confidence);
-        return VO_E_INVALID;
-    }
     if (ctx->p.max_features <= 0) {
         vo_set_error(ctx, "max_features=%d: the per-unit feature capacity must be positive", ctx->p.max_features);
         return VO_E_INVALID;
     }
-    if (ctx->p.bucket_rows_divisor <= 0) {
-        vo_set_error(ctx, "bucket_rows_divisor=%d: bucket_size = rows / divisor needs a positive divisor", ctx->p.bucket_rows_divisor);
-        return VO_E_INVALID;
-    }
-    if (ctx->p.features_per_bucket <= 0) {
-        // Bucket::add_feature on a full bucket of max_size 0 reads ages[0] of an empty vector
-        vo_set_error(ctx, "features_per_bucket=%d: a bucket holds at least one feature", ctx->p.features_per_bucket);
-        return VO_E_INVALID;
-    }
-    if (ctx->p.lk_win != VO_WIN) {
-        vo_set_error(ctx, "lk_win=%d unsupported: the LK kernel is built for the reference's 21x21 window", ctx->p.lk_win);
-        return VO_E_UNSUPPORTED;
-    }
-    if (ctx->p.lk_max_level < 0 || ctx->p.lk_max_level >= VO_MAX_LEVELS) {
-        vo_set_error(ctx, "lk_max_level=%d outside [0,%d]", ctx->p.lk_max_level, VO_MAX_LEVELS - 1);
-        return VO_E_UNSUPPORTED;
-    }
+    int rc = vo_check_params(ctx, ctx->p);
+    if (rc) return rc;
+    ctx->slot_par.assign(VO_MSEQ_MAX, ctx->p);
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
     if (e != cudaSuccess || ndev <= 0) {
@@ -90,7 +148,7 @@ extern "C" int vo_create(int device, const vo_params* params, vo_ctx** out)
     ctx->stream = ctx->own_stream;
     VO_CUDA_CHECK(vo_lk_prepare());
     ctx->cap = ctx->p.max_features;
-    ctx->bucket_cap = (size_t)(ctx->cap / ctx->p.features_per_bucket) * ((size_t)ctx->p.features_per_bucket + 1);
+    ctx->bucket_cap = 2 * (size_t)ctx->cap;
     VO_CUDA_CHECK(cudaMalloc(&ctx->d_lk_queue, LK_QUEUES * 2 * sizeof(int)));
     VO_CUDA_CHECK(cudaMemset(ctx->d_lk_queue, 0, LK_QUEUES * 2 * sizeof(int)));
     {   // VO_LK_STAGING=ldg switches the LK window staging from TMA to plain loads (debug / A-B runs)
@@ -384,16 +442,22 @@ int vo_ensure_lanes(vo_ctx* ctx)
     return VO_OK;
 }
 
-int vo_write_calib(vo_ctx* ctx, int u0, int n, const CamCalib* c)
+// entries [1 + u0, 1 + u0 + n) of a per-unit table (host copy `host`, device table `dev`)
+template <typename T>
+static int write_table(vo_ctx* ctx, std::vector<T>& host, T* dev, int u0, int n, const T* e)
 {
     const size_t e0 = (size_t)(1 + u0);
-    if (memcmp(ctx->cal.data() + e0, c, n * sizeof(CamCalib)) == 0) return VO_OK;
-    memcpy(ctx->cal.data() + e0, c, n * sizeof(CamCalib));
+    if (memcmp(host.data() + e0, e, n * sizeof(T)) == 0) return VO_OK;
+    memcpy(host.data() + e0, e, n * sizeof(T));
     for (auto& p : ctx->pending)
         if (p.active) VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, p.done, 0));
-    VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_cal_tab + e0, ctx->cal.data() + e0, n * sizeof(CamCalib), cudaMemcpyHostToDevice, ctx->stream));
+    VO_CUDA_CHECK(cudaMemcpyAsync(dev + e0, host.data() + e0, n * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
     return VO_OK;
 }
+
+int vo_write_calib(vo_ctx* ctx, int u0, int n, const CamCalib* c) { return write_table(ctx, ctx->cal, ctx->d_cal_tab, u0, n, c); }
+
+int vo_write_params(vo_ctx* ctx, int u0, int n, const UnitParams* e) { return write_table(ctx, ctx->par, ctx->d_par_tab, u0, n, e); }
 
 int vo_set_calibration(vo_ctx* ctx, int u0, int n, const float* P_l, const float* P_r, int n_mat)
 {
@@ -412,6 +476,7 @@ void vo_free_state(vo_ctx* ctx)
     ctx->d_feat_pts = nullptr; ctx->d_feat_ages = nullptr; ctx->d_feat_cnt = ctx->d_bucket = ctx->d_seq_err = ctx->d_seq_live = nullptr;
     ctx->d_out = nullptr; ctx->out_stride = 0; ctx->out_per = 0;
     ctx->d_cal_tab = ctx->d_cal = nullptr;
+    ctx->d_par_tab = ctx->d_par = nullptr;
     ctx->d_geo = nullptr;
     ctx->w = ctx->h = ctx->units = 0;
 }
@@ -557,6 +622,11 @@ int vo_ensure_state(vo_ctx* ctx, int w, int h, int units, int levels)
     ctx->d_cal = ctx->d_cal_tab + 1;
     ctx->cal.resize(1 + (size_t)units, CamCalib{});
     VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_cal_tab, ctx->cal.data(), (1 + (size_t)units) * sizeof(CamCalib), cudaMemcpyHostToDevice, ctx->stream));
+    // parameter table: likewise; new entries (and entry 0, always) hold the context's vo_params
+    VO_CUDA_CHECK(dalloc(ctx, &ctx->d_par_tab, 1 + (size_t)units));
+    ctx->d_par = ctx->d_par_tab + 1;
+    ctx->par.resize(1 + (size_t)units, vo_unit_params(ctx->p));
+    VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_par_tab, ctx->par.data(), (1 + (size_t)units) * sizeof(UnitParams), cudaMemcpyHostToDevice, ctx->stream));
     // sequence mode state: sized per sequence at vo_seq_begin / vo_mseq_begin (seq_api.cu)
     ctx->feat_cap = ctx->corner_cap + cap;
     ctx->seq_active = false;
@@ -609,15 +679,16 @@ int vo_run_pyramid(vo_ctx* ctx, int plane0, int nplanes, cudaStream_t s, bool si
     return VO_OK;
 }
 
-int vo_run_lk(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, const int* img_next, bool want_err)
+int vo_run_lk(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, const int* img_next, bool want_err, const UnitParams* par)
 {
     int rc = vo_run_pyramid(ctx, v.u0 * v.imgs, v.n * v.imgs, v.s);
     if (rc) return rc;
-    return vo_run_lk_ring(ctx, v, ncalls, img_prev, img_next, want_err);
+    return vo_run_lk_ring(ctx, v, ncalls, img_prev, img_next, want_err, par);
 }
 
 // the ring kernel alone (pyramids of every plane it touches must be up to date)
-int vo_run_lk_ring(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, const int* img_next, bool want_err)
+int vo_run_lk_ring(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, const int* img_next, bool want_err,
+                   const UnitParams* par)
 {
     const size_t uo = (size_t)v.u0 * ctx->cap;
     const PyrGeom& pg = ctx->pg;
@@ -634,12 +705,7 @@ int vo_run_lk_ring(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, 
     a.nlevels = pg.nlevels;
     for (int l = 0; l < pg.nlevels; l++) { a.lw[l] = pg.lv[l].w; a.lh[l] = pg.lv[l].h; }
     a.geo = v.sized ? ctx->d_geo : nullptr;
-    // calcOpticalFlowPyrLK clamps the criteria: maxCount to [0, 100], epsilon to [0, 10]
-    a.max_iters = ctx->p.lk_max_iters < 0 ? 0 : ctx->p.lk_max_iters > 100 ? 100 : ctx->p.lk_max_iters;
-    double eps = ctx->p.lk_epsilon;
-    if (eps < 0.) eps = 0.; if (eps > 10.) eps = 10.;
-    a.eps2 = eps * eps;
-    a.min_eig = (float)ctx->p.lk_min_eig;          // LKTrackerInvoker keeps minEigThreshold as a float
+    a.par = par + v.u0;
     a.pts_in = ctx->d_pts_in + uo;
     a.pts_out = ctx->d_pts_out + uo;
     a.status_out = ctx->d_status + uo;
@@ -686,14 +752,14 @@ int vo_run_lk_ring(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, 
     return VO_OK;
 }
 
-int vo_run_filter(vo_ctx* ctx, const View& v, bool with_ages)
+int vo_run_filter(vo_ctx* ctx, const View& v, bool with_ages, const UnitParams* par)
 {
     const size_t uo = (size_t)v.u0 * ctx->cap;
     FilterArgs f;
     memset(&f, 0, sizeof(f));
     f.cap = ctx->cap;
     f.call_stride = (size_t)ctx->units * ctx->cap;
-    f.circ_threshold = ctx->p.circ_threshold;
+    f.par = par + v.u0;
     f.n_pts = ctx->d_npts + v.u0;
     f.pts_in = ctx->d_pts_in + uo;
     f.pts_out = ctx->d_pts_out + uo;
@@ -711,7 +777,7 @@ int vo_run_filter(vo_ctx* ctx, const View& v, bool with_ages)
     return VO_OK;
 }
 
-int vo_run_fast(vo_ctx* ctx, const View& v, int plane_in_unit, bool want_resp)
+int vo_run_fast(vo_ctx* ctx, const View& v, int plane_in_unit, bool want_resp, const UnitParams* par)
 {
     FastArgs a;
     memset(&a, 0, sizeof(a));
@@ -720,7 +786,7 @@ int vo_run_fast(vo_ctx* ctx, const View& v, int plane_in_unit, bool want_resp)
     a.img_tab = ctx->d_raw_tab + (size_t)(v.plane0 >= 0 ? v.plane0 : v.u0 * v.imgs) + plane_in_unit;
     a.img_stride_idx = v.imgs;
     a.w = ctx->w; a.h = ctx->h; a.pitch = ctx->w;
-    a.threshold = ctx->p.fast_threshold; a.nonmax = ctx->p.fast_nonmax;
+    a.par = par + v.u0; a.nonmax = ctx->p.fast_nonmax;
     a.score = ctx->d_score + v.u0 * plane; a.score_plane = plane;
     a.rowbuf = ctx->d_rowbuf + v.u0 * plane; a.rowcap = ctx->w;
     a.rowcount = ctx->d_rowcount + (size_t)v.u0 * ctx->h; a.rowoff = ctx->d_rowoff + (size_t)v.u0 * ctx->h;
@@ -756,18 +822,16 @@ int vo_run_triangulate(vo_ctx* ctx, const View& v, const float2* pts_l, const fl
     return VO_OK;
 }
 
-int vo_run_pnp(vo_ctx* ctx, const View& v, const float2* pts2d, const int* n, const CamCalib* cal)
+int vo_run_pnp(vo_ctx* ctx, const View& v, const float2* pts2d, const int* n, const CamCalib* cal, const UnitParams* par)
 {
-    const int iterations = vo_pnp_iterations(ctx);
+    const int iterations = vo_pnp_iterations(ctx);      // the stride of the RANSAC scratch; each unit runs its own count
     const size_t uo = (size_t)v.u0 * ctx->cap, its = (size_t)iterations;
     PnpArgs a;
     memset(&a, 0, sizeof(a));
     a.n_units = v.n; a.cap = ctx->cap; a.iterations = iterations;
     a.n_pts = n + v.u0; a.X = ctx->d_X + uo; a.x = pts2d + uo;
     a.cal = cal + v.u0;
-    const double thr = (double)ctx->p.pnp_reproj_error;      // float -> double, squared in double, stored float
-    a.thr2 = (float)(thr * thr);
-    a.confidence = ctx->p.pnp_confidence;
+    a.par = par + v.u0;
     a.t_prev = ctx->d_tprev + (size_t)v.u0 * 3;
     a.state = ctx->d_pnp_state + v.u0; a.subsets = ctx->d_subsets + v.u0 * its * 5; a.models = ctx->d_models + v.u0 * its * 12;
     a.counts = ctx->d_counts + v.u0 * its;

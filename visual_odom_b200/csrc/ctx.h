@@ -47,6 +47,14 @@ struct vo_ctx {
     CamCalib* d_cal_tab = nullptr;      // [1 + units]
     CamCalib* d_cal = nullptr;          // d_cal_tab + 1: indexed by buffer unit
     std::vector<CamCalib> cal;          // [1 + units] host copy (kept across re-allocations of the batch state)
+    // parameter table (the same layout and life as the calibration table): entry 0 the stage calls' (always the context's
+    // vo_params), entry 1 + u buffer unit u's tracking parameters (vo_mseq_params, vo_batch_params).  par mirrors it.
+    UnitParams* d_par_tab = nullptr;    // [1 + units]
+    UnitParams* d_par = nullptr;        // d_par_tab + 1: indexed by buffer unit
+    std::vector<UnitParams> par;        // [1 + units] host copy (kept across re-allocations of the batch state)
+    // vo_mseq_params: each slot's setting, which the begin and start calls of the slot read ([VO_MSEQ_MAX], the context's
+    // vo_params until set)
+    std::vector<vo_params> slot_par;
     // geometry table (the same life as d_cal_tab): one entry per raw image plane, its own size per level and raw pitch.
     // w / h above are then the envelope of the sizes; only runs of several sizes (vo_mseq_begin_sized) point kernels at
     // it, every other path uses the launch-wide sizes.  Entries start out as w x h.  geo mirrors it.
@@ -100,14 +108,16 @@ struct vo_ctx {
     void* d_seq_state = nullptr;        // the one allocation behind the six arrays above (freed with the batch state)
     int seq_n_cap = 0;                  // sequences those arrays hold
     int feat_cap = 0;
-    // ints of bucketing scratch per sequence: a grid of nb cells takes nb * (features_per_bucket + 1), and every run the
-    // begin and start calls accept has nb * features_per_bucket <= max_features (vo_create)
+    // ints of bucketing scratch per sequence: a grid of nb cells takes nb * (k + 1) at features_per_bucket k, and every
+    // run the begin and start calls accept has nb * k <= max_features, so nb <= max_features and nb * (k + 1) <=
+    // 2 * max_features whatever each sequence's k (vo_create)
     size_t bucket_cap = 0;
     bool seq_active = false;
     bool seq_multi = false;             // begun with vo_mseq_begin (the vo_seq_* frame calls are refused, and vice versa)
     int seq_n = 1;                      // sequences of the running sequence mode
     bool seq_sized = false;             // the sequences' image sizes differ (planes are envelope-sized, kernels read d_geo)
     std::vector<int> seq_w, seq_h;      // [seq_n] each sequence's image size
+    std::vector<vo_params> seq_par;     // [seq_n] each sequence's parameters (its slot's setting when it began or started)
     int seq_slot = 0;                   // image slot holding the previous stereo pairs: raw/pyramid planes
                                         // 2 * seq_n * slot + 2q (left), + 1 (right) of sequence q
     int seq_inflight = 0;               // frames submitted and not yet waited for (<= 2)
@@ -126,8 +136,9 @@ struct vo_ctx {
     double* d_seq_pose = nullptr;
     cudaEvent_t seq_tab_ev[3] = {nullptr, nullptr, nullptr};
     int seq_lk_bound = 0;               // the LK launch bound: the largest bucket grid of the run's sizes (raised by starts)
-    std::vector<CamCalib> seq_cal_next; // [2 * seq_n] calibration entries of started sequences that the frame in flight
-    std::vector<char> seq_cal_due;      // still reads: written by the next submission of that buffer parity
+    std::vector<CamCalib> seq_cal_next; // [2 * seq_n] calibration and parameter entries of started sequences that the
+    std::vector<UnitParams> seq_par_next;   // frame in flight still reads: written by the next submission of that buffer
+    std::vector<char> seq_cal_due;      // parity
     std::vector<char> seq_geo_due;      // [seq_n] image slots whose geometry entries still hold the slot's previous size
     uint8_t* d_bgr = nullptr;           // staging of colour (BGR) inputs, converted by k_bgr_to_gray (ingest.cu)
     size_t bgr_bytes = 0;
@@ -245,6 +256,17 @@ int vo_ensure_lanes(vo_ctx* ctx);
 int vo_write_calib(vo_ctx* ctx, int u0, int n, const CamCalib* c);
 // buffer units [u0, u0 + n): unit u0 + i from the matrices P_l + 12 * (i % n_mat), P_r + 12 * (i % n_mat)
 int vo_set_calibration(vo_ctx* ctx, int u0, int n, const float* P_l, const float* P_r, int n_mat);
+// Parameter table entries [1 + u0, 1 + u0 + n) = e[0 .. n), written as vo_write_calib writes its table
+int vo_write_params(vo_ctx* ctx, int u0, int n, const UnitParams* e);
+// the kernels' entry of a vo_params
+UnitParams vo_unit_params(const vo_params& p);
+// The field rules vo_create applies to a vo_params (every field but max_features and max_units): VO_E_INVALID or
+// VO_E_UNSUPPORTED with vo_create's message
+int vo_check_params(vo_ctx* ctx, const vo_params& p);
+// vo_check_params, then the rules of a unit's or slot's own vo_params against the context's (who / what: "vo_mseq_params",
+// "slot 3"): lk_win, lk_max_level and fast_nonmax equal (VO_E_UNSUPPORTED), pnp_iterations within the RANSAC scratch
+// (VO_E_CAPACITY)
+int vo_check_unit_params(vo_ctx* ctx, const char* who, const char* what, const vo_params& p);
 int vo_drain_pending(vo_ctx* ctx);
 // Entry points that overwrite the shared image planes / unit-0 buffers call this first: refused (VO_E_INVALID) while
 // sequence frames or batch submissions are in flight; an idle sequence is ended (its planes are about to be reused).
@@ -279,19 +301,22 @@ int vo_ingest_device(vo_ctx* ctx, const vo_dimage* h_tab, int n, int plane0, cud
 // (0 = cap), which sizes the LK launch.
 // sized: the image planes hold images of several sizes; FAST and the LK ring read each one's from the geometry table.
 struct View { int u0, n; cudaStream_t s; int plane0 = -1; int imgs = 4; int max_pts = 0; bool sized = false; };
+// The stage runners below read unit u's parameters from par[u] (ctx->d_par, or the stage calls' entry ctx->d_par_tab
+// with v.u0 = 0) and its camera from cal[u] alike.
 // run pyramids + LK (ncalls chained) for the units of `v`; images must already be in d_raw/d_raw_tab
-int vo_run_lk(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, const int* img_next, bool want_err);
+int vo_run_lk(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, const int* img_next, bool want_err, const UnitParams* par);
 // sized: the planes hold images of several sizes, read from the geometry table (vo_mseq_begin_sized)
 int vo_run_pyramid(vo_ctx* ctx, int plane0, int nplanes, cudaStream_t s, bool sized = false);
-int vo_run_lk_ring(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, const int* img_next, bool want_err);
-int vo_run_filter(vo_ctx* ctx, const View& v, bool with_ages);
+int vo_run_lk_ring(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, const int* img_next, bool want_err,
+                   const UnitParams* par);
+int vo_run_filter(vo_ctx* ctx, const View& v, bool with_ages, const UnitParams* par);
 // FAST on raw plane `plane_in_unit` of each unit -> d_corners / d_ndet ; stride selection -> d_pts_in / d_npts
-int vo_run_fast(vo_ctx* ctx, const View& v, int plane_in_unit, bool want_resp);
+int vo_run_fast(vo_ctx* ctx, const View& v, int plane_in_unit, bool want_resp, const UnitParams* par);
 int vo_run_select(vo_ctx* ctx, const View& v);
 // triangulate pts_l/pts_r ([units][cap], counts n) -> d_X ; PnP on (d_X, pts2d) -> d_results / d_inliers.  Unit u reads
 // the camera cal[u] (ctx->d_cal, or the stage calls' single entry with v.u0 = 0).
 int vo_run_triangulate(vo_ctx* ctx, const View& v, const float2* pts_l, const float2* pts_r, const int* n, const CamCalib* cal,
                        float4* X4 = nullptr);
-int vo_run_pnp(vo_ctx* ctx, const View& v, const float2* pts2d, const int* n, const CamCalib* cal);
+int vo_run_pnp(vo_ctx* ctx, const View& v, const float2* pts2d, const int* n, const CamCalib* cal, const UnitParams* par);
 // RANSAC iterations the PnP stage sizes and runs: cv::RANSACPointSetRegistrator runs at least one (max(maxIters, 1))
 inline int vo_pnp_iterations(const vo_ctx* ctx) { return ctx->p.pnp_iterations > 1 ? ctx->p.pnp_iterations : 1; }

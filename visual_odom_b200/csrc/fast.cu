@@ -23,7 +23,7 @@
 // With a geometry table (geo[unit * img_stride_idx]: images of several sizes) every kernel takes the image's own size for
 // its border, raster and score map; w / h are then the envelope and only lay out the per-row buffers.
 __global__ void __launch_bounds__(256) k_fast_score(const uint8_t* const* __restrict__ img_tab, int img_stride_idx,
-                                                    int w, int h, int pitch, int threshold, int nonmax,
+                                                    int w, int h, int pitch, const UnitParams* __restrict__ par, int nonmax,
                                                     uint8_t* __restrict__ score, size_t score_plane,
                                                     const PlaneGeom* __restrict__ geo)
 {
@@ -31,6 +31,7 @@ __global__ void __launch_bounds__(256) k_fast_score(const uint8_t* const* __rest
     constexpr int ring_dx[16] = {0, 1, 2, 3, 3, 3, 2, 1, 0, -1, -2, -3, -3, -3, -2, -1};
     constexpr int ring_dy[16] = {3, 3, 2, 1, 0, -1, -2, -3, -3, -3, -2, -1, 0, 1, 2, 3};
     const int unit = blockIdx.z;
+    const int threshold = par[unit].fast_threshold;
     const uint8_t* __restrict__ img = img_tab[unit * img_stride_idx];
     uint8_t* __restrict__ sc = score + (size_t)unit * score_plane;
     if (geo) { const PlaneGeom& g = geo[unit * img_stride_idx]; w = g.w[0]; h = g.h[0]; pitch = g.pitch; }
@@ -243,7 +244,7 @@ __global__ void k_select_stride(const float2* __restrict__ corners, int corner_c
 int vo_launch_fast(const FastArgs& a, cudaStream_t stream)
 {
     dim3 g1((a.w + 31) / 32, (a.h + 7) / 8, a.n_units);
-    k_fast_score<<<g1, 256, 0, stream>>>(a.img_tab, a.img_stride_idx, a.w, a.h, a.pitch, a.threshold, a.nonmax, a.score,
+    k_fast_score<<<g1, 256, 0, stream>>>(a.img_tab, a.img_stride_idx, a.w, a.h, a.pitch, a.par, a.nonmax, a.score,
                                           a.score_plane, a.geo);
     dim3 g2(a.h, a.n_units);
     k_fast_nms_row<<<g2, NMS_T, 0, stream>>>(a.score, a.score_plane, a.w, a.h, a.nonmax, a.rowbuf, a.rowcap, a.rowcount, a.geo,

@@ -7,7 +7,8 @@ struct FastArgs {
     const uint8_t* const* img_tab;   // device table of raw image pointers
     int img_stride_idx;              // table entries per unit (4); the detector reads entry unit*stride
     int w, h, pitch;                 // raw image geometry
-    int threshold, nonmax;
+    const UnitParams* par;           // [n_units] fast_threshold
+    int nonmax;
     uint8_t* score;                  // [units][h*w]
     size_t score_plane;
     uint16_t* rowbuf;                // [units][h][rowcap] x coordinates per row

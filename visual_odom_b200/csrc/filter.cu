@@ -18,6 +18,7 @@ __global__ void __launch_bounds__(FT) k_ring_filter(const FilterArgs a)
 {
     const int unit = blockIdx.x;
     const int n = a.n_pts[unit];
+    const int circ_threshold = a.par[unit].circ_threshold;
     const size_t ub = (size_t)unit * a.cap;
     const float2* p0 = a.pts_in + ub;                        // L0
     const float2* p1 = a.pts_out + 0 * a.call_stride + ub;   // R0
@@ -47,7 +48,7 @@ __global__ void __launch_bounds__(FT) k_ring_filter(const FilterArgs a)
             if (keep3) {
                 const float m = fmaxf(fabsf(q0.x - qr.x), fabsf(q0.y - qr.y));
                 const int offset = (int)m;            // float -> int truncation, as the reference's `int offset`
-                keep5 = !(offset > a.circ_threshold);
+                keep5 = !(offset > circ_threshold);
             }
         }
         const unsigned b3 = __ballot_sync(0xffffffffu, keep3);

@@ -5,7 +5,7 @@
 struct FilterArgs {
     int cap;
     size_t call_stride;       // n_units * cap
-    int circ_threshold;
+    const UnitParams* par;    // [units] circ_threshold
     const int* n_pts;         // [units]
     const float2* pts_in;     // [units][cap]           L0
     const float2* pts_out;    // [4][units][cap]        R0, R1, L1, L0_return (ring order)

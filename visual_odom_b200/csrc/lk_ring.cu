@@ -131,7 +131,12 @@ struct __align__(128) WarpSmem {
     uint32_t dwin[DW * I_ROWS + 24];        // derivative window; then A22 chain slots; then residuals    2560
     float chain[2 * QSTRIDE];               // chain-ordered float addends of two quantities              3616
     uint64_t bar;                           // mbarrier for TMA completion
-    uint64_t pad_[11];
+    // the work item's unit criteria, staged at item start (registers have no room for them across the item, and a load
+    // from the parameter table at each use would put its latency on every level-solve)
+    double eps2;
+    float eps2_lo, eps2_hi, min_eig;
+    int max_iters;
+    uint64_t pad_[8];
 };
 static_assert(sizeof(WarpSmem) == 8960, "WarpSmem layout");
 static_assert(A22_OFF + QSTRIDE <= DW * I_ROWS + 24, "A22 slots must fit the derivative window");
@@ -264,9 +269,6 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
 
     const float half_win = (VO_WIN - 1) * 0.5f;
     const float FLT_SCALE = 1.f / (1 << 20);
-    // delta.ddot(delta) <= eps^2 is a double test in OpenCV; dx*dx + dy*dy in float is within 2e-7 of it, so the double
-    // form is only evaluated inside this band
-    const float eps2_lo = (float)(args.eps2 * 0.999999), eps2_hi = (float)(args.eps2 * 1.000001);
     const int max_level = args.nlevels - 1;
     // Work items.  A feature-ring is ncalls x nlevels PHASES (one level-solve each).  An item is `span`
     // consecutive phases of one feature; items are queued phase-major, so every feature's phase p is handed out
@@ -293,6 +295,16 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
         if (f >= npts) continue;
 
         const size_t pbase = (size_t)unit * args.cap + f;
+        // the unit's criteria (warp-uniform) into the warp's shared memory.  delta.ddot(delta) <= eps^2 is a double test in
+        // OpenCV; dx*dx + dy*dy in float is within 2e-7 of it, so the double form is only evaluated inside this band.
+        __syncwarp();                           // every lane is done with the previous item's values
+        if (lane == 0) {
+            const UnitParams& par = args.par[unit];
+            const double eps2 = par.eps2;
+            sm.eps2 = eps2; sm.eps2_lo = (float)(eps2 * 0.999999); sm.eps2_hi = (float)(eps2 * 1.000001);
+            sm.min_eig = par.min_eig; sm.max_iters = par.max_iters;
+        }
+        __syncwarp();
         const int p0 = grp * span, p1 = min(p0 + span, nphases);
         if (p0 > 0) {                           // the predecessor item has published its state
             if (lane == 0)
@@ -415,7 +427,7 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                     float dd = __fsub_rn(A11, A22);
                     float rad = __fadd_rn(__fmul_rn(dd, dd), __fmul_rn(__fmul_rn(4.f, A12), A12));
                     float minEig = __fdiv_rn(__fsub_rn(__fadd_rn(A22, A11), __fsqrt_rn(rad)), (float)(2 * VO_WIN * VO_WIN));
-                    if (minEig < args.min_eig || D < 1.1920928955078125e-07f) {
+                    if (minEig < sm.min_eig || D < 1.1920928955078125e-07f) {
                         if (level == 0) status = 0;
                         break;
                     }
@@ -426,7 +438,10 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                 float pdx = 0.f, pdy = 0.f;
                 bool tile_valid = j_ok0;
                 bool force_replay = false;          // set by the first faithful replay of this level-solve
-                for (int j = 0; j < args.max_iters; j++) {
+                // in registers for the Newton loop, whose shared-memory stores would otherwise make every iteration reload them
+                const int max_iters = sm.max_iters;
+                const float eps2_lo = sm.eps2_lo, eps2_hi = sm.eps2_hi;
+                for (int j = 0; j < max_iters; j++) {
                     inx = __float2int_rd(npx); iny = __float2int_rd(npy);
                     if (inx < -VO_WIN || inx >= lw || iny < -VO_WIN || iny >= lh) {
                         if (level == 0) status = 0;
@@ -547,7 +562,7 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                     {
                         const float d2 = __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy));
                         if (d2 < eps2_lo) break;
-                        if (d2 <= eps2_hi && (double)dx * (double)dx + (double)dy * (double)dy <= args.eps2) break;
+                        if (d2 <= eps2_hi && (double)dx * (double)dx + (double)dy * (double)dy <= sm.eps2) break;
                     }
                     // std::abs(double(x)) < 0.01 for a float x  <=>  |x| <= 0.01f (0.01f is the largest float below 0.01)
                     if (j > 0 && fabsf(__fadd_rn(dx, pdx)) <= 0.01f && fabsf(__fadd_rn(dy, pdy)) <= 0.01f) {

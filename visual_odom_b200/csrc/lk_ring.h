@@ -24,9 +24,7 @@ struct LkArgs {
     int nlevels;            // pyramid images (effective maxLevel + 1)
     int lw[VO_MAX_LEVELS], lh[VO_MAX_LEVELS];
     const PlaneGeom* geo;   // geometry table indexed by absolute plane (images of several sizes), or nullptr = lw / lh
-    int max_iters;          // 30 (clamped to [0, 100] as calcOpticalFlowPyrLK does)
-    double eps2;            // epsilon^2 (0.01^2)
-    float min_eig;          // 1e-3, as a float: cv::LKTrackerInvoker compares minEig with a float threshold
+    const UnitParams* par;  // [n_units] each unit's criteria: max_iters, eps2, min_eig
     const float2* pts_in;   // [n_units][cap]
     float2* pts_out;        // [ncalls][n_units][cap]   (call_stride = n_units*cap)
     uint8_t* status_out;    // [ncalls][n_units][cap]

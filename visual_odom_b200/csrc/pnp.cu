@@ -73,7 +73,7 @@ __global__ void k_pnp_init(const PnpArgs a)
     if (unit >= a.n_units) return;
     PnpState& s = a.state[unit];
     s.rng_state = 0xffffffffffffffffULL;
-    s.niters = a.iterations;
+    s.niters = a.par[unit].pnp_iterations;        // the unit's own bound (a.iterations is the scratch stride)
     s.max_good = 0;
     s.best_it = -1;
     s.iters_run = 0;
@@ -302,6 +302,7 @@ __global__ void __launch_bounds__(128) k_pnp_count(const PnpArgs a, int it0, int
     if (s.done || it >= it1 || it >= s.niters) return;
     __shared__ double m[12], cam[4];         // the model; the unit's fu, fv, uc, vc
     __shared__ int total;
+    const float thr2 = a.par[unit].thr2;
     if (threadIdx.x < 12) m[threadIdx.x] = a.models[((size_t)unit * a.iterations + it) * 12 + threadIdx.x];
     else if (threadIdx.x < 16) cam[threadIdx.x - 12] = (&a.cal[unit].fu)[threadIdx.x - 12];
     if (threadIdx.x == 0) total = 0;
@@ -310,7 +311,7 @@ __global__ void __launch_bounds__(128) k_pnp_count(const PnpArgs a, int it0, int
     int c = 0;
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
         const float e = reproj_err(m, a.X[(size_t)unit * a.cap + i], a.x[(size_t)unit * a.cap + i], cam[0], cam[1], cam[2], cam[3]);
-        c += (e <= a.thr2) ? 1 : 0;
+        c += (e <= thr2) ? 1 : 0;
     }
 #pragma unroll
     for (int d = 16; d > 0; d >>= 1) c += __shfl_xor_sync(0xffffffffu, c, d);
@@ -333,11 +334,11 @@ __global__ void k_pnp_replay(const PnpArgs a, int it0, int it1)
         if (good > max(s.max_good, 4)) {
             s.best_it = it;
             s.max_good = good;
-            s.niters = ransac_update_num_iters(a.confidence, (double)(n - good) / n, 5, s.niters);
+            s.niters = ransac_update_num_iters(a.par[unit].confidence, (double)(n - good) / n, 5, s.niters);
         }
     }
     s.iters_run = it;
-    if (it >= s.niters || it1 >= a.iterations) s.done = 1;
+    if (it >= s.niters || it1 >= a.par[unit].pnp_iterations) s.done = 1;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -458,12 +459,13 @@ __global__ void __launch_bounds__(FIN_T, 1) k_pnp_finalize(const PnpArgs a)
     if (threadIdx.x == 0) base = 0;
     __syncthreads();
     const double fu = cam[0], fv = cam[1], uc = cam[2], vc = cam[3];
+    const float thr2 = a.par[unit].thr2;
     // ---- inlier mask of the best model, ordered compaction -----------------------------------
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int c0 = 0; c0 < n; c0 += FIN_T) {
         const int i = c0 + threadIdx.x;
         bool keep = false;
-        if (i < n) keep = reproj_err(sm_model, X[i], x[i], fu, fv, uc, vc) <= a.thr2;
+        if (i < n) keep = reproj_err(sm_model, X[i], x[i], fu, fv, uc, vc) <= thr2;
         const unsigned b = __ballot_sync(0xffffffffu, keep);
         if (lane == 0) wcnt[warp] = __popc(b);
         __syncthreads();

@@ -31,13 +31,13 @@ struct TriArgs {
 };
 
 struct PnpArgs {
-    int n_units, cap, iterations;
+    int n_units, cap;
+    int iterations;          // the stride of subsets / models / counts (the largest count); unit u runs par[u].pnp_iterations
     const int* n_pts;        // [units]
     const float3* X;         // [units][cap]
     const float2* x;         // [units][cap]   image points (pointsLeft_t1)
     const CamCalib* cal;     // [units]: fu, fv, uc, vc of each unit
-    float thr2;              // (float)(reprojectionError^2)
-    double confidence;
+    const UnitParams* par;   // [units]: pnp_iterations, thr2, confidence of each unit
     const double* t_prev;    // [units][3]
     PnpState* state;         // [units]
     int* subsets;            // [units][iterations][5]

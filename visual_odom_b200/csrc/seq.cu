@@ -23,7 +23,7 @@
 
 __global__ void __launch_bounds__(1024) k_seq_append(const float2* __restrict__ corners, const int* __restrict__ n_det,
                                                      int corner_cap, float2* feat_pts, int* feat_ages, int* cnt, int feat_cap,
-                                                     int refill_below, int* err, const int* __restrict__ live)
+                                                     const UnitParams* __restrict__ par, int* err, const int* __restrict__ live)
 {
     const int q = blockIdx.y;
     corners += (size_t)q * corner_cap; n_det += q; feat_pts += (size_t)q * feat_cap; feat_ages += (size_t)q * feat_cap;
@@ -34,7 +34,7 @@ __global__ void __launch_bounds__(1024) k_seq_append(const float2* __restrict__ 
     if (!live[q]) return;                              // retired: the state stays as it is
     const int n_pts = cnt[0], n_ages = cnt[1];
     // `if (currentVOFeatures.size() < 2000)`: no refill leaves the FeatureSet as it is (n_det still counts the corners)
-    if (n_pts >= refill_below) return;
+    if (n_pts >= par[q].refill_threshold) return;
     int m = *n_det;
     if (m > corner_cap) { m = corner_cap; if (threadIdx.x == 0) atomicOr(err, 1); }
     if (n_pts + m > feat_cap || n_ages + m > feat_cap) { m = min(feat_cap - n_pts, feat_cap - n_ages); if (m < 0) m = 0; if (threadIdx.x == 0) atomicOr(err, 2); }
@@ -55,9 +55,11 @@ __global__ void __launch_bounds__(1024) k_seq_append(const float2* __restrict__ 
 // larger one on, so slot s ends up with the (s + 1)-th smallest index whatever order the threads run in).  The number of
 // filled slots is min(c, k), and c > k exactly when the cell is full and its largest index is not its k-th smallest.
 // Scratch per sequence: last[nb] | first[nb][k].  At k = 1 every non-empty cell reads back its last admitted feature.
-__global__ void __launch_bounds__(1024) k_seq_bucket(const float2* __restrict__ feat_pts, const int* __restrict__ feat_ages,
-                                                     int feat_cap, const int* __restrict__ cnt, int rows, int cols, int divisor,
-                                                     int k, int age_threshold, int* bucket /* scratch */, size_t nb_cap,
+// (One block per SM: with k, the gate and the divisor read from the sequence's parameter entry, the default bound of two
+// blocks per SM leaves 32 registers and spills; a launch has one block per sequence, far fewer than the SMs.)
+__global__ void __launch_bounds__(1024, 1) k_seq_bucket(const float2* __restrict__ feat_pts, const int* __restrict__ feat_ages,
+                                                     int feat_cap, const int* __restrict__ cnt, int rows, int cols,
+                                                     const UnitParams* __restrict__ par, int* bucket /* scratch */, size_t nb_cap,
                                                      float2* out_pts, int* out_ages, int* out_n, int out_cap, int* err,
                                                      const int* __restrict__ live, const PlaneGeom* __restrict__ geo, int geo_stride)
 {
@@ -65,6 +67,7 @@ __global__ void __launch_bounds__(1024) k_seq_bucket(const float2* __restrict__ 
     if (geo) {             // the sequence's own grid: the stride-nw aliasing below depends on nw
         rows = geo[q * geo_stride].h[0]; cols = geo[q * geo_stride].w[0];
     }
+    const int divisor = par[q].bucket_rows_divisor, k = par[q].features_per_bucket, age_threshold = par[q].bucket_age_threshold;
     const int bucket_size = rows / divisor;
     feat_pts += (size_t)q * feat_cap; feat_ages += (size_t)q * feat_cap; cnt += 2 * q; bucket += (size_t)q * nb_cap;
     out_pts += (size_t)q * out_cap; out_ages += (size_t)q * out_cap; out_n += q; err += q;
@@ -255,13 +258,12 @@ int vo_launch_seq_collect(const CollectArgs& a, int n_seq, cudaStream_t s)
 int vo_launch_seq_append(const SeqArgs& a, int n_seq, cudaStream_t s)
 {
     k_seq_append<<<dim3(1, n_seq), 1024, 0, s>>>(a.corners, a.n_det, a.corner_cap, a.feat_pts, a.feat_ages, a.cnt, a.feat_cap,
-                                                 a.refill_below, a.err, a.live);
+                                                 a.par, a.err, a.live);
     return 1;
 }
 int vo_launch_seq_bucket(const SeqArgs& a, int n_seq, cudaStream_t s)
 {
-    k_seq_bucket<<<dim3(1, n_seq), 1024, 0, s>>>(a.feat_pts, a.feat_ages, a.feat_cap, a.cnt, a.rows, a.cols, a.bucket_divisor,
-                                                 a.per_bucket, a.age_threshold, a.bucket, a.bucket_cap, a.out_pts, a.out_ages, a.out_n, a.out_cap, a.err, a.live,
+    k_seq_bucket<<<dim3(1, n_seq), 1024, 0, s>>>(a.feat_pts, a.feat_ages, a.feat_cap, a.cnt, a.rows, a.cols, a.par, a.bucket, a.bucket_cap, a.out_pts, a.out_ages, a.out_n, a.out_cap, a.err, a.live,
                                                  a.geo, a.geo_stride);
     return 1;
 }

@@ -13,10 +13,11 @@ struct SeqArgs {
     // append
     const float2* corners; const int* n_det; int corner_cap;
     float2* feat_pts; int* feat_ages; int* cnt /* [2]: points, ages */; int feat_cap;
-    int refill_below;                   // vo_params.refill_threshold
-    // bucketing: bucket_size = rows / bucket_divisor, per_bucket slots per cell, ages >= age_threshold refused (vo_params
-    // bucket_rows_divisor, features_per_bucket, bucket_age_threshold); bucket: last[nb] | first[nb][per_bucket] scratch
-    int rows, cols, bucket_divisor, per_bucket, age_threshold; int* bucket; size_t bucket_cap;
+    // each sequence's parameter entry (stride 1): the refill threshold (append), and the bucketing's bucket_size = rows /
+    // bucket_rows_divisor, features_per_bucket slots per cell, ages >= bucket_age_threshold refused
+    const UnitParams* par;
+    // bucketing: bucket: last[nb] | first[nb][features_per_bucket] scratch
+    int rows, cols; int* bucket; size_t bucket_cap;
     // images of several sizes: sequence q's rows / cols (and so its bucket_size) are those of geo[q * geo_stride]
     const PlaneGeom* geo; int geo_stride;
     float2* out_pts; int* out_ages; int* out_n; int out_cap;
