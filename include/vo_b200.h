@@ -391,6 +391,38 @@ typedef struct vo_mono_result {
 } vo_mono_result;
 VO_API int vo_seq_wait_mono(vo_ctx* ctx, vo_unit_result* out, vo_mono_result* mono, uint8_t* ess_mask, int mask_cap,
                             vo_point2f* pts4, int pts_cap);
+
+/* trackingFrame2Frame(..., mono_rotation = true) (reference src/visualOdometry.h:42, src/visualOdometry.cpp:146-157,186-189)
+ * per unit of the batched mode.  Unit first_unit + i runs the branch when on[i] != 0 (on == NULL: the range off); a unit
+ * keeps its setting until it is set again, and vo_batch_configure switches every unit off.  The context option
+ * "mono_rotation" is a vo_seq_begin* switch only; the batched mode ignores it.  Refused, changing nothing (VO_E_INVALID):
+ * the range and in-flight rules of vo_batch_calibrate; like it, the call ends an idle sequence-mode run.  The call
+ * allocates the five-point scratch (one block per configured unit, for max_features points), so a submission never does.
+ * A unit with the branch on, in every entry path (vo_frame_batch, vo_batch_run, vo_batch_submit[_device]), runs
+ *     E = cv::findEssentialMat(pointsLeft_t0, pointsLeft_t1, focal, pp, cv::RANSAC, 0.999, 1.0, mask);
+ *     cv::recoverPose(E, pointsLeft_t0, pointsLeft_t1, rotation, translation_mono, focal, pp, mask);
+ * on its n_valid filtered L0 / L1 points (vo_batch_fetch's pts4 planes 0 and 2), with focal / pp the float entries of its
+ * own P_l (vo_batch_calibrate).  Its record's R becomes recoverPose's rotation; rvec, tvec, n_inliers, ransac_iters,
+ * pnp_status, every count, the point lists, kept_idx, X and the inliers stay the PnP path's, the same bits as with the
+ * branch off.  Where the reference would throw (n_valid < 5, no E with more than 4 inliers, exactly 5 points with other
+ * than one five-point candidate) mono.status = VO_E_TOO_FEW_POINTS and R = I, as vo_seq_wait_mono reports it.  A range
+ * with no unit switched on launches exactly what it launches without the branch; one with any adds a fixed number of
+ * launches, however many of its units are on.  vo_dist_gather_* gathers the records as they are, so a unit with the
+ * branch on sends the mono R (its vo_mono_result is not gathered). */
+VO_API int vo_batch_mono_rotation(vo_ctx* ctx, int first_unit, int n_units, const uint8_t* on);
+/* vo_batch_wait plus mono[i] for unit first_unit + i, staged in pinned memory by the submission itself (no extra device
+ * sync); mono[i] is zeroed for a unit that ran with the branch off.  vo_batch_wait works on such submissions too (R =
+ * the mono rotation). */
+VO_API int vo_batch_wait_mono(vo_ctx* ctx, int first_unit, int n_units, vo_unit_result* results, vo_mono_result* mono);
+/* The synchronous read matching vo_batch_fetch, valid after every entry path: the branch's result of the unit's last run
+ * and, optionally, its essential inlier mask (capacity max_features; the first n_valid bytes are meaningful, aligned with
+ * the unit's point lists).  A unit that ran with the branch off: mono zeroed, ess_mask untouched.  Refused
+ * (VO_E_INVALID): a unit outside the resident batch or of a submission that has not been waited for. */
+VO_API int vo_batch_fetch_mono(vo_ctx* ctx, int unit, vo_mono_result* mono, uint8_t* ess_mask);
+/* With "batch_outputs" = 1 the mask of a unit with the branch on travels in the submission's one packed copy (from the
+ * first vo_batch_mono_rotation that switches a unit on, each unit's block grows by one byte per point slot, which
+ * *d2h_bytes_per_unit reports); this reads it and the staged result of a waited unit, under vo_batch_outputs' rules. */
+VO_API int vo_batch_outputs_mono(vo_ctx* ctx, int unit, vo_mono_result* mono, uint8_t* ess_mask);
 /* currentVOFeatures (points / ages may differ in length) and the carried translation (waits for frames in flight) */
 VO_API int vo_seq_state(vo_ctx* ctx, vo_point2f* points, int32_t* ages, int cap, int* n_points, int* n_ages, double t_out[3]);
 

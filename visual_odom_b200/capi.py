@@ -200,6 +200,10 @@ SIGNATURES = {
                                       C.c_size_t, C.c_int, C.c_int]),
     "vo_batch_calibrate": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "vo_batch_params": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(VoParams)]),
+    "vo_batch_mono_rotation": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "vo_batch_wait_mono": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(VoUnitResult), C.POINTER(VoMonoResult)]),
+    "vo_batch_fetch_mono": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(VoMonoResult), C.c_void_p]),
+    "vo_batch_outputs_mono": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(VoMonoResult), C.c_void_p]),
     "vo_mseq_params": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(VoParams)]),
     "vo_mseq_begin_sized": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
@@ -444,6 +448,42 @@ class Context:
         if not overrides:
             raise ValueError("batch_params: no units")
         self._check(self.lib.vo_batch_params(self.h, first_unit, len(overrides), self._params_array(overrides)))
+
+    def batch_mono_rotation(self, first_unit, on):
+        """Units [first_unit, first_unit + len(on)) run trackingFrame2Frame(mono_rotation = bool(on[i])) in every batched
+        entry path (vo_batch_mono_rotation); on=None is refused here (pass zeros to switch a range off).  Refused while
+        submissions are in flight."""
+        flags = np.ascontiguousarray(np.asarray(on, dtype=bool), np.uint8).reshape(-1)
+        if flags.size == 0:
+            raise ValueError("batch_mono_rotation: no units")
+        self._check(self.lib.vo_batch_mono_rotation(self.h, first_unit, int(flags.size), _p(flags)))
+
+    @staticmethod
+    def _mono_dict(m):
+        return dict(status=m.status, n_inliers=m.n_inliers, ransac_iters=m.ransac_iters, n_good=m.n_good,
+                    R=np.array(m.R[:]).reshape(3, 3), t=np.array(m.t[:]))
+
+    def batch_wait_mono(self, first_unit, n_units):
+        """vo_batch_wait_mono: (records as batch_wait returns them, mono dicts: status, n_inliers, ransac_iters, n_good, R
+        3x3, t; all zero for a unit that ran with the branch off)."""
+        res = (VoUnitResult * n_units)()
+        ms = (VoMonoResult * n_units)()
+        self._check(self.lib.vo_batch_wait_mono(self.h, first_unit, n_units, res, ms))
+        return [self._result_dict(r) for r in res], [self._mono_dict(m) for m in ms]
+
+    def batch_fetch_mono(self, unit, res):
+        """vo_batch_fetch_mono: dict(mono=..., ess_mask=bool array of res["n_valid"] entries) of the unit's last run."""
+        mask = np.zeros(max(self.params.max_features, 1), np.uint8)
+        m = VoMonoResult()
+        self._check(self.lib.vo_batch_fetch_mono(self.h, unit, C.byref(m), _p(mask)))
+        return dict(mono=self._mono_dict(m), ess_mask=mask[:res["n_valid"]].astype(bool))
+
+    def batch_outputs_mono(self, unit, res):
+        """vo_batch_outputs_mono: as batch_fetch_mono, from the waited submission's staging (option batch_outputs = 1)."""
+        mask = np.zeros(max(self.params.max_features, 1), np.uint8)
+        m = VoMonoResult()
+        self._check(self.lib.vo_batch_outputs_mono(self.h, unit, C.byref(m), _p(mask)))
+        return dict(mono=self._mono_dict(m), ess_mask=mask[:res["n_valid"]].astype(bool))
 
     def make_units(self, units):
         """units: list of dicts(l0,r0,l1,r1 uint8 HxW [, pts (n,2) f32 | n_select int] [, t_prev]).

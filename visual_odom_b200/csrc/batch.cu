@@ -21,11 +21,14 @@ __global__ void k_pack_counts(vo_unit_result_dev* res, const int* n_pts, const i
 }
 
 // Packed outputs of one unit: float2 pts4[4][per] (L0, R0, L1, R1 of the valid tracks) | int kept_idx[per] |
-// float3 X[per] | int inliers[per], `per` point slots each (only the first n_valid / n_inliers are written).
+// float3 X[per] | int inliers[per] [| uint8 ess_mask[per]], `per` point slots each (only the first n_valid / n_inliers are
+// written).  The mask section exists once a unit of the context ran the mono_rotation branch (ctx->out_mask); it is
+// written for the units whose switch on[u] is set, from their five-point scratch blocks mask_stride bytes apart.
 #define VO_OUT_BYTES_PER_SLOT (4 * sizeof(float2) + sizeof(int) + sizeof(float3) + sizeof(int))
 __global__ void k_pack_outputs(uint8_t* __restrict__ out, size_t stride, int per, const float2* __restrict__ valid4, size_t cs,
                                const int* __restrict__ idx5, const float3* __restrict__ X, const int* __restrict__ inliers,
-                               const int* __restrict__ n5, const vo_unit_result_dev* __restrict__ res, int cap)
+                               const int* __restrict__ n5, const vo_unit_result_dev* __restrict__ res, int cap,
+                               const uint8_t* __restrict__ mask, size_t mask_stride, const int* __restrict__ on)
 {
     const int u = blockIdx.x;
     const int nv = min(n5[u], per), ni = min(res[u].n_inliers, per);
@@ -42,10 +45,21 @@ __global__ void k_pack_outputs(uint8_t* __restrict__ out, size_t stride, int per
         oX[3 * i] = x.x; oX[3 * i + 1] = x.y; oX[3 * i + 2] = x.z;
     }
     for (int i = threadIdx.x; i < ni; i += blockDim.x) oi[i] = inliers[ub + i];
+    if (mask && on[u]) {
+        uint8_t* om = reinterpret_cast<uint8_t*>(oi + per);
+        for (int i = threadIdx.x; i < nv; i += blockDim.x) om[i] = mask[(size_t)u * mask_stride + i];
+    }
+}
+
+// the point count of each unit's mono_rotation problem: its n_valid when its switch is on, else 0 (no RANSAC work)
+__global__ void k_batch_mono_n(int* __restrict__ n_out, const int* __restrict__ on, const int* __restrict__ n5, int n_units)
+{
+    const int u = blockIdx.x * blockDim.x + threadIdx.x;
+    if (u < n_units) n_out[u] = on[u] ? n5[u] : 0;
 }
 
 // the four parts of one unit's packed block with `per` point slots (layout of k_pack_outputs)
-struct PackedUnit { float2* o4; int* ok; float* oX; int* oi; };
+struct PackedUnit { float2* o4; int* ok; float* oX; int* oi; uint8_t* om; };
 static PackedUnit packed_unit(uint8_t* base, int per)
 {
     PackedUnit p;
@@ -53,7 +67,32 @@ static PackedUnit packed_unit(uint8_t* base, int per)
     p.ok = (int*)(p.o4 + 4 * (size_t)per);
     p.oX = (float*)(p.ok + per);
     p.oi = (int*)(p.oX + 3 * (size_t)per);
+    p.om = (uint8_t*)(p.oi + per);
     return p;
+}
+
+// whether a unit of [u0, u0 + n) has the mono_rotation branch switched on
+static bool range_mono(const vo_ctx* ctx, int u0, int n)
+{
+    for (int u = u0; u < u0 + n && u < (int)ctx->batch_mono.size(); u++)
+        if (ctx->batch_mono[u]) return true;
+    return false;
+}
+
+// the mono_rotation problems of units [u0, u0 + n) (one each): pointsLeft_t0 / pointsLeft_t1 = the filtered L0 / L1 lists
+// (d_valid4 planes 0, 2), scratch block u for unit u (laid out for max_features points), the count of d_batch_mono, the
+// camera of the unit's own P_l.  bound (the range's feature bound) sizes the per-point grids.
+static void batch_ess_args(const vo_ctx* ctx, int u0, int n, int bound, EssArgs& a)
+{
+    memset(&a, 0, sizeof(a));
+    const size_t uo = (size_t)u0 * ctx->cap, cs = (size_t)ctx->units * ctx->cap;
+    vo_ess_bind(a, (uint8_t*)ctx->d_batch_ess + (size_t)u0 * ctx->batch_ess_bytes, ctx->cap, VO_ESS_ITERS);
+    a.n_max = bound;
+    a.n = ctx->d_batch_mono + ctx->batch_ess_units + u0;
+    a.cal = ctx->d_cal + u0;
+    a.pts0 = ctx->d_valid4 + uo; a.pts1 = ctx->d_valid4 + 2 * cs + uo;
+    a.n_prob = n;
+    a.scratch_stride = a.result_stride = ctx->batch_ess_bytes; a.pts_stride = ctx->cap; a.n_stride = 1; a.cal_stride = 1;
 }
 
 // largest feature bound of the slots [u0, u0 + n): the LK launch of that range has no unit with more live features
@@ -75,8 +114,9 @@ static int ensure_outputs(vo_ctx* ctx, int u0, int n, int bound)
         if ((u < u0 || u >= u0 + n) && ctx->slot_pts[u] > per) per = ctx->slot_pts[u];
     per = ((per > 1 ? per : 1) + 63) / 64 * 64;
     if (per > ctx->cap) per = ctx->cap;
-    if (ctx->d_out && ctx->h_out && ctx->out_per == per && ctx->out_units >= ctx->units) return VO_OK;
-    const size_t stride = ((size_t)per * VO_OUT_BYTES_PER_SLOT + 255) / 256 * 256;
+    const bool mask = ctx->batch_mono_used;
+    if (ctx->d_out && ctx->h_out && ctx->out_per == per && ctx->out_mask == mask && ctx->out_units >= ctx->units) return VO_OK;
+    const size_t stride = ((size_t)per * (VO_OUT_BYTES_PER_SLOT + (mask ? 1 : 0)) + 255) / 256 * 256;
     for (auto& p : ctx->pending)                // their copies land in the old blocks
         if (p.active) VO_CUDA_CHECK(cudaEventSynchronize(p.done));
     void* q = nullptr;                          // both new blocks first: a failed allocation leaves the old ones in use
@@ -93,6 +133,7 @@ static int ensure_outputs(vo_ctx* ctx, int u0, int n, int bound)
             memcpy(b.ok, a.ok, (size_t)m * sizeof(int));
             memcpy(b.oX, a.oX, (size_t)m * 3 * sizeof(float));
             memcpy(b.oi, a.oi, (size_t)m * sizeof(int));
+            if (mask && ctx->out_mask) memcpy(b.om, a.om, (size_t)m);
         }
         cudaFreeHost(ctx->h_out);
     }
@@ -103,7 +144,7 @@ static int ensure_outputs(vo_ctx* ctx, int u0, int n, int bound)
     }
     ctx->allocs.push_back(q);                   // freed with the batch state
     ctx->d_out = (uint8_t*)q;
-    ctx->out_units = ctx->units; ctx->out_per = per; ctx->out_stride = stride;
+    ctx->out_units = ctx->units; ctx->out_per = per; ctx->out_stride = stride; ctx->out_mask = mask;
     return VO_OK;
 }
 
@@ -121,6 +162,9 @@ extern "C" int vo_batch_configure(vo_ctx* ctx, int w, int h, int n_units, const 
     ctx->batch_units = n_units;
     ctx->batch_uploaded = 0;
     ctx->slot_pts.assign(n_units, 0);
+    ctx->batch_mono.assign(n_units, 0);         // every unit off (the device switch table is rewritten when one is set)
+    ctx->batch_mono_ran.assign(n_units, 0);
+    ctx->batch_mono_used = false;
     return VO_OK;
 }
 
@@ -161,11 +205,46 @@ extern "C" int vo_batch_params(vo_ctx* ctx, int first_unit, int n_units, const v
     return vo_write_params(ctx, first_unit, n_units, e.data());
 }
 
+// the same rules as vo_batch_calibrate.  The scratch (one block per configured unit) is allocated here, never by a
+// submission; the whole switch table is then written on the context's stream, ahead of every later submission.
+extern "C" int vo_batch_mono_rotation(vo_ctx* ctx, int first_unit, int n_units, const uint8_t* on)
+{
+    if (!ctx) return VO_E_INVALID;
+    if (first_unit < 0 || n_units <= 0 || first_unit + n_units > ctx->batch_units) {
+        vo_set_error(ctx, "vo_batch_mono_rotation: units [%d, %d) outside the configured batch (%d)", first_unit, first_unit + n_units, ctx->batch_units);
+        return VO_E_INVALID;
+    }
+    VO_CUDA_CHECK(cudaSetDevice(ctx->device));
+    int rc = vo_claim_buffers(ctx, "vo_batch_mono_rotation");
+    if (rc) return rc;
+    if (!ctx->batch_mono_stream) {
+        VO_CUDA_CHECK(cudaStreamCreateWithFlags(&ctx->batch_mono_stream, cudaStreamNonBlocking));
+        for (int k = 0; k < 2; k++) VO_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->batch_mono_ev[k], cudaEventDisableTiming));
+    }
+    if (!ctx->d_batch_ess || ctx->batch_ess_units < ctx->batch_units) {
+        const size_t bytes = (vo_ess_scratch_bytes(ctx->cap, VO_ESS_ITERS) + 255) / 256 * 256;
+        const size_t table = ((size_t)2 * ctx->batch_units * sizeof(int) + 255) / 256 * 256;
+        void* q = nullptr;
+        VO_CUDA_CHECK(cudaMalloc(&q, table + (size_t)ctx->batch_units * bytes));
+        vo_drop_graphs(ctx);                    // captured graphs hold the old blocks
+        if (ctx->d_batch_mono) { VO_CUDA_CHECK(cudaDeviceSynchronize()); cudaFree(ctx->d_batch_mono); }      // the allocation's base
+        ctx->d_batch_ess = (uint8_t*)q + table; ctx->d_batch_mono = (int*)q;
+        ctx->batch_ess_bytes = bytes; ctx->batch_ess_units = ctx->batch_units;
+    }
+    for (int i = 0; i < n_units; i++) ctx->batch_mono[first_unit + i] = on && on[i] ? 1 : 0;
+    if (range_mono(ctx, 0, ctx->batch_units)) ctx->batch_mono_used = true;
+    VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_batch_mono, ctx->batch_mono.data(), (size_t)ctx->batch_units * sizeof(int),
+                                  cudaMemcpyHostToDevice, ctx->stream));
+    return VO_OK;
+}
+
 // Pinned staging of the batched path, disjoint per unit: t_prev [batch_units][3] | counts [batch_units] | result records
-// [batch_units] (64-byte aligned) | descriptors of caller device images [batch_units][4]
+// [batch_units] (64-byte aligned) | descriptors of caller device images [batch_units][4] | mono_rotation results
+// [batch_units]
 static size_t batch_pinned_bytes(const vo_ctx* ctx)
 {
-    return (size_t)ctx->batch_units * (3 * sizeof(double) + sizeof(int) + sizeof(vo_unit_result_dev) + 4 * sizeof(vo_dimage)) + 256;
+    return (size_t)ctx->batch_units * (3 * sizeof(double) + sizeof(int) + sizeof(vo_unit_result_dev) + 4 * sizeof(vo_dimage) +
+                                       sizeof(EssResult)) + 256;
 }
 
 static vo_unit_result_dev* pinned_results(vo_ctx* ctx)
@@ -176,6 +255,8 @@ static vo_unit_result_dev* pinned_results(vo_ctx* ctx)
 }
 
 static vo_dimage* pinned_ingest_tab(vo_ctx* ctx) { return (vo_dimage*)(pinned_results(ctx) + ctx->batch_units); }
+
+static EssResult* pinned_ess(vo_ctx* ctx) { return (EssResult*)(pinned_ingest_tab(ctx) + 4 * (size_t)ctx->batch_units); }
 
 // features and scalars of units [u0, u0+n) on stream `st`, through the pinned staging block; units[src0 + i] fills slot u0 + i
 template <typename Unit>
@@ -284,6 +365,7 @@ static int ensure_helpers(vo_ctx* ctx)
     VO_CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&lo, &hi));      // hi is the numerically smallest value
     for (auto& L : ctx->lane) {
         VO_CUDA_CHECK(cudaStreamCreateWithPriority(&L.pre, cudaStreamNonBlocking, hi));
+        VO_CUDA_CHECK(cudaStreamCreateWithPriority(&L.mono, cudaStreamNonBlocking, hi));
         L.post = L.pre;
         L.lk = L.side;
     }
@@ -297,11 +379,16 @@ static int run_range_launch(vo_ctx* ctx, const View& v)
     int rc;
     View pre = v, lk = v, post = v;              // FAST + pyramids / the LK ring / the kernels after the ring
     cudaEvent_t* ev = nullptr;
+    // the five-point kernels of the mono_rotation branch, forked from post after the filters and joined before the fold
+    cudaStream_t mono_s = ctx->batch_mono_stream;
+    cudaEvent_t mono_ev[2] = {ctx->batch_mono_ev[0], ctx->batch_mono_ev[1]};
     for (auto& L : ctx->lane)
         if (L.side && v.s == L.side) {
             if ((rc = ensure_helpers(ctx))) return rc;
             pre.s = L.pre; lk.s = L.lk; post.s = L.post; ev = L.ev;
+            mono_s = L.mono; mono_ev[0] = L.ev[4]; mono_ev[1] = L.ev[5];
         }
+    const bool mono = range_mono(ctx, v.u0, v.n);
     // work on `to` after the work enqueued so far on `from`
     auto hand_over = [&](int k, cudaStream_t from, cudaStream_t to) -> int {
         if (from == to) return VO_OK;
@@ -320,12 +407,27 @@ static int run_range_launch(vo_ctx* ctx, const View& v)
     if ((rc = vo_run_lk_ring(ctx, lk, 4, ip, in, false, ctx->d_par))) return rc;
     if ((rc = hand_over(2, lk.s, post.s))) return rc;
     if ((rc = vo_run_filter(ctx, post, false, ctx->d_par))) return rc;
+    EssArgs e;
+    if (mono) {     // findEssentialMat + recoverPose on (L0, L1) of the units switched on, beside triangulation and PnP
+        batch_ess_args(ctx, v.u0, v.n, v.max_pts, e);
+        VO_CUDA_CHECK(cudaEventRecord(mono_ev[0], post.s));
+        VO_CUDA_CHECK(cudaStreamWaitEvent(mono_s, mono_ev[0], 0));
+        int* count = ctx->d_batch_mono + ctx->batch_ess_units + v.u0;
+        k_batch_mono_n<<<(v.n + 63) / 64, 64, 0, mono_s>>>(count, ctx->d_batch_mono + v.u0, ctx->d_n5 + v.u0, v.n);
+        ctx->launches += 1 + vo_launch_essential(e, mono_s);
+        VO_CUDA_CHECK(cudaGetLastError());
+        VO_CUDA_CHECK(cudaEventRecord(mono_ev[1], mono_s));
+    }
     const size_t cs = (size_t)ctx->units * ctx->cap;
     if ((rc = vo_run_triangulate(ctx, post, ctx->d_valid4, ctx->d_valid4 + cs, ctx->d_n5, ctx->d_cal))) return rc;
     if ((rc = vo_run_pnp(ctx, post, ctx->d_valid4 + 2 * cs, ctx->d_n5, ctx->d_cal, ctx->d_par))) return rc;
     k_pack_counts<<<(v.n + 63) / 64, 64, 0, post.s>>>(ctx->d_results + v.u0, ctx->d_npts + v.u0, ctx->d_ndet + v.u0, ctx->d_n3 + v.u0,
                                                      ctx->d_n5 + v.u0, v.n, ctx->batch_detect ? 1 : 0);
     ctx->launches += 1;
+    if (mono) {     // the record's R becomes recoverPose's rotation (I where the branch aborted) for the units switched on
+        VO_CUDA_CHECK(cudaStreamWaitEvent(post.s, mono_ev[1], 0));
+        ctx->launches += vo_launch_mono_fold(ctx->d_results + v.u0, e.result, e.result_stride, ctx->d_batch_mono + v.u0, v.n, post.s);
+    }
     VO_CUDA_CHECK(cudaGetLastError());
     return hand_over(3, post.s, v.s);            // join: later work on v.s (result copy, the next submission) sees everything
 }
@@ -339,12 +441,13 @@ static int run_range(vo_ctx* ctx, int u0, int n, cudaStream_t s)
 {
     View v{u0, n, s};
     v.max_pts = range_bound(ctx, u0, n);         // the LK launch geometry depends on it
+    for (int u = u0; u < u0 + n; u++) ctx->batch_mono_ran[u] = ctx->batch_mono[u];
     bool on_side = false;
     for (const auto& L : ctx->lane) on_side = on_side || (L.side && s == L.side);
     if (on_side) return run_range_launch(ctx, v);
     GraphKey key{};
     key.kind = GraphKey::BATCH_RANGE; key.s = s; key.tma = ctx->lk_use_tma;
-    key.u0 = u0; key.n = n; key.max_pts = v.max_pts; key.detect = ctx->batch_detect;
+    key.u0 = u0; key.n = n; key.max_pts = v.max_pts; key.detect = ctx->batch_detect; key.mono = range_mono(ctx, u0, n);
     return vo_run_graph(ctx, key, [&] { return run_range_launch(ctx, v); });
 }
 
@@ -508,11 +611,19 @@ static int batch_submit(vo_ctx* ctx, const char* who, const Unit* units, int fir
     if ((rc = run_range(ctx, first_unit, n_units, st))) return rc;
     vo_unit_result_dev* h_res = pinned_results(ctx);
     VO_CUDA_CHECK(cudaMemcpyAsync(h_res + first_unit, ctx->d_results + first_unit, (size_t)n_units * sizeof(vo_unit_result_dev), cudaMemcpyDeviceToHost, st));
+    const bool mono = range_mono(ctx, first_unit, n_units);
+    EssArgs e;
+    if (mono) {                                  // the branch's results for vo_batch_wait_mono: one strided copy
+        batch_ess_args(ctx, first_unit, n_units, max_pts, e);
+        VO_CUDA_CHECK(cudaMemcpy2DAsync(pinned_ess(ctx) + first_unit, sizeof(EssResult), e.result, e.result_stride, sizeof(EssResult),
+                                        n_units, cudaMemcpyDeviceToHost, st));
+    }
     if (ctx->batch_outputs) {                    // the point lists of the submission: one packed block, one copy
         const size_t cs = (size_t)ctx->units * ctx->cap, ub = (size_t)first_unit * ctx->cap;
         k_pack_outputs<<<n_units, 256, 0, st>>>(ctx->d_out + (size_t)first_unit * ctx->out_stride, ctx->out_stride, ctx->out_per,
                                                ctx->d_valid4 + ub, cs, ctx->d_idx5 + ub, ctx->d_X + ub, ctx->d_inliers + ub,
-                                               ctx->d_n5 + first_unit, ctx->d_results + first_unit, ctx->cap);
+                                               ctx->d_n5 + first_unit, ctx->d_results + first_unit, ctx->cap,
+                                               mono ? e.mask : nullptr, ctx->batch_ess_bytes, ctx->d_batch_mono + first_unit);
         ctx->launches += 1;
         VO_CUDA_CHECK(cudaGetLastError());
         VO_CUDA_CHECK(cudaMemcpyAsync(ctx->h_out + (size_t)first_unit * ctx->out_stride, ctx->d_out + (size_t)first_unit * ctx->out_stride,
@@ -533,7 +644,18 @@ extern "C" int vo_batch_submit_device(vo_ctx* ctx, const vo_dunit* units, int fi
     return batch_submit(ctx, "vo_batch_submit_device", units, first_unit, n_units, 0);
 }
 
-extern "C" int vo_batch_wait(vo_ctx* ctx, int first_unit, int n_units, vo_unit_result* results)
+// vo_mono_result of a unit whose last run had the branch on (status as vo_seq_wait_mono reports it), zeroed otherwise
+static void mono_result(const vo_ctx* ctx, int unit, const EssResult& ess, vo_mono_result* m)
+{
+    memset(m, 0, sizeof(*m));
+    if (!ctx->batch_mono_ran[unit]) return;
+    m->status = ess.status == ESS_OK ? VO_OK : VO_E_TOO_FEW_POINTS;
+    m->n_inliers = ess.n_inliers; m->ransac_iters = ess.iters; m->n_good = ess.n_good;
+    for (int k = 0; k < 9; k++) m->R[k] = ess.R[k];
+    for (int k = 0; k < 3; k++) m->t[k] = ess.t[k];
+}
+
+static int batch_wait(vo_ctx* ctx, const char* who, int first_unit, int n_units, vo_unit_result* results, vo_mono_result* mono)
 {
     if (!ctx) return VO_E_INVALID;
     for (auto& p : ctx->pending)
@@ -543,10 +665,57 @@ extern "C" int vo_batch_wait(vo_ctx* ctx, int first_unit, int n_units, vo_unit_r
             VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, p.done, 0));     // later work on the caller's stream sees the results
             p.active = false;
             if (results) memcpy(results, pinned_results(ctx) + first_unit, (size_t)n_units * sizeof(vo_unit_result));
+            for (int i = 0; mono && i < n_units; i++) mono_result(ctx, first_unit + i, pinned_ess(ctx)[first_unit + i], &mono[i]);
             return VO_OK;
         }
-    vo_set_error(ctx, "vo_batch_wait: no pending submission for slots [%d, %d)", first_unit, first_unit + n_units);
+    vo_set_error(ctx, "%s: no pending submission for slots [%d, %d)", who, first_unit, first_unit + n_units);
     return VO_E_INVALID;
+}
+
+extern "C" int vo_batch_wait(vo_ctx* ctx, int first_unit, int n_units, vo_unit_result* results)
+{
+    return batch_wait(ctx, "vo_batch_wait", first_unit, n_units, results, nullptr);
+}
+
+extern "C" int vo_batch_wait_mono(vo_ctx* ctx, int first_unit, int n_units, vo_unit_result* results, vo_mono_result* mono)
+{
+    if (ctx && !mono) { vo_set_error(ctx, "vo_batch_wait_mono: null mono"); return VO_E_INVALID; }
+    return batch_wait(ctx, "vo_batch_wait_mono", first_unit, n_units, results, mono);
+}
+
+// VO_E_INVALID + message unless `unit` is resident and not part of a submission that has not been waited for
+static int check_waited(vo_ctx* ctx, const char* who, int unit)
+{
+    if (unit < 0 || unit >= ctx->batch_uploaded) { vo_set_error(ctx, "%s: unit %d outside the resident batch", who, unit); return VO_E_INVALID; }
+    for (auto& p : ctx->pending)
+        if (p.active && unit >= p.u0 && unit < p.u0 + p.n) { vo_set_error(ctx, "%s: unit %d has not been waited for", who, unit); return VO_E_INVALID; }
+    return VO_OK;
+}
+
+// The branch's result of the unit's last run and its mask (n_valid bytes, aligned with vo_batch_fetch's lists), read
+// synchronously from the unit's scratch block.  A unit that ran with the branch off: mono zeroed, ess_mask untouched.
+extern "C" int vo_batch_fetch_mono(vo_ctx* ctx, int unit, vo_mono_result* mono, uint8_t* ess_mask)
+{
+    if (!ctx) return VO_E_INVALID;
+    if (!mono) { vo_set_error(ctx, "vo_batch_fetch_mono: null mono"); return VO_E_INVALID; }
+    int rc = check_waited(ctx, "vo_batch_fetch_mono", unit);
+    if (rc) return rc;
+    EssResult ess;
+    memset(&ess, 0, sizeof(ess));
+    if (!ctx->batch_mono_ran[unit]) { mono_result(ctx, unit, ess, mono); return VO_OK; }
+    VO_CUDA_CHECK(cudaSetDevice(ctx->device));
+    EssArgs e;
+    batch_ess_args(ctx, unit, 1, ctx->cap, e);
+    vo_unit_result_dev r;
+    VO_CUDA_CHECK(cudaMemcpyAsync(&r, ctx->d_results + unit, sizeof(r), cudaMemcpyDeviceToHost, ctx->stream));
+    VO_CUDA_CHECK(cudaMemcpyAsync(&ess, e.result, sizeof(ess), cudaMemcpyDeviceToHost, ctx->stream));
+    VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+    if (ess_mask && r.n_valid > 0) {
+        VO_CUDA_CHECK(cudaMemcpyAsync(ess_mask, e.mask, (size_t)std::min(r.n_valid, ctx->cap), cudaMemcpyDeviceToHost, ctx->stream));
+        VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+    }
+    mono_result(ctx, unit, ess, mono);
+    return VO_OK;
 }
 
 // The point lists of a waited submission, from the pinned block its single D2H copy filled ("batch_outputs" = 1):
@@ -568,6 +737,23 @@ extern "C" int vo_batch_outputs(vo_ctx* ctx, int unit, vo_point2f* pts4, int32_t
     if (X) memcpy(X, o.oX, (size_t)nv * 3 * sizeof(float));
     if (inliers) memcpy(inliers, o.oi, (size_t)ni * sizeof(int));
     if (d2h_bytes_per_unit) *d2h_bytes_per_unit = ctx->out_stride;
+    return VO_OK;
+}
+
+// vo_batch_outputs' counterpart for the branch: the result staged by the submission and the mask its packed copy carried
+extern "C" int vo_batch_outputs_mono(vo_ctx* ctx, int unit, vo_mono_result* mono, uint8_t* ess_mask)
+{
+    if (!ctx) return VO_E_INVALID;
+    if (!mono) { vo_set_error(ctx, "vo_batch_outputs_mono: null mono"); return VO_E_INVALID; }
+    if (!ctx->batch_outputs || !ctx->h_out) { vo_set_error(ctx, "vo_batch_outputs_mono: option batch_outputs is off"); return VO_E_INVALID; }
+    if (unit >= ctx->out_units) { vo_set_error(ctx, "vo_batch_outputs_mono: unit %d outside the resident batch", unit); return VO_E_INVALID; }
+    int rc = check_waited(ctx, "vo_batch_outputs_mono", unit);
+    if (rc) return rc;
+    mono_result(ctx, unit, pinned_ess(ctx)[unit], mono);
+    if (ess_mask && ctx->batch_mono_ran[unit] && ctx->out_mask) {
+        const int per = ctx->out_per, nv = std::min(pinned_results(ctx)[unit].n_valid, per);
+        if (nv > 0) memcpy(ess_mask, packed_unit(ctx->h_out + (size_t)unit * ctx->out_stride, per).om, (size_t)nv);
+    }
     return VO_OK;
 }
 

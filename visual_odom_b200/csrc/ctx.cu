@@ -186,6 +186,9 @@ extern "C" void vo_destroy(vo_ctx* ctx)
     if (ctx->d_lk_queue) cudaFree(ctx->d_lk_queue);
     if (ctx->d_ess) cudaFree(ctx->d_ess);
     if (ctx->d_seq_ess) cudaFree(ctx->d_seq_ess);
+    if (ctx->d_batch_mono) cudaFree(ctx->d_batch_mono);           // the base of d_batch_ess's allocation
+    for (int k = 0; k < 2; k++) if (ctx->batch_mono_ev[k]) cudaEventDestroy(ctx->batch_mono_ev[k]);
+    if (ctx->batch_mono_stream) cudaStreamDestroy(ctx->batch_mono_stream);
     if (ctx->d_seq_pose) cudaFree(ctx->d_seq_pose);
     for (cudaEvent_t e : ctx->seq_tab_ev) if (e) cudaEventDestroy(e);
     for (int k = 0; k < 2; k++) if (ctx->seq_mono_ev[k]) cudaEventDestroy(ctx->seq_mono_ev[k]);
@@ -313,7 +316,8 @@ void vo_partition_destroy(vo_ctx* ctx)
     for (auto& L : ctx->lane) {
         if (L.pre) cudaStreamDestroy(L.pre);                            // partition: pre = lk; helpers: pre = post, lk = side
         if (L.post && L.post != L.pre) cudaStreamDestroy(L.post);
-        L.pre = L.lk = L.post = nullptr;
+        if (L.mono) cudaStreamDestroy(L.mono);
+        L.pre = L.lk = L.post = L.mono = nullptr;
     }
     PFN_cuGreenCtxDestroy destroy = nullptr;
     if (drv("cuGreenCtxDestroy", &destroy))
@@ -360,9 +364,10 @@ int vo_partition_enable(vo_ctx* ctx, int helper_sms)
     }
     ctx->part_helper_sms = (int)part[0].sm.smCount; ctx->part_lk_sms = (int)rest.sm.smCount;
     for (int c = 0; c < VO_LANES; c++) {
-        CUstream a, b;
+        CUstream a, b, m;
         if ((r = screate(&a, (CUgreenCtx)ctx->part_gctx[0], CU_STREAM_NON_BLOCKING, 0)) != CUDA_SUCCESS ||
-            (r = screate(&b, (CUgreenCtx)ctx->part_gctx[1], CU_STREAM_NON_BLOCKING, 0)) != CUDA_SUCCESS) {
+            (r = screate(&b, (CUgreenCtx)ctx->part_gctx[1], CU_STREAM_NON_BLOCKING, 0)) != CUDA_SUCCESS ||
+            (r = screate(&m, (CUgreenCtx)ctx->part_gctx[0], CU_STREAM_NON_BLOCKING, 0)) != CUDA_SUCCESS) {
             vo_set_error(ctx, "sm_partition: cuGreenCtxStreamCreate failed (driver error %d)", (int)r);
             vo_partition_destroy(ctx);
             return VO_E_UNSUPPORTED;
@@ -370,6 +375,7 @@ int vo_partition_enable(vo_ctx* ctx, int helper_sms)
         vo_ctx::Lane& L = ctx->lane[c];
         L.pre = L.lk = (cudaStream_t)b;
         L.post = (cudaStream_t)a;
+        L.mono = (cudaStream_t)m;                                       // the five-point kernels beside post, on the same SMs
     }
     ctx->part_on = true;
     return VO_OK;
@@ -398,7 +404,7 @@ void vo_drop_graphs(vo_ctx* ctx)
 static bool same_key(const GraphKey& a, const GraphKey& b)
 {
     return a.kind == b.kind && a.s == b.s && a.tma == b.tma && a.u0 == b.u0 && a.n == b.n && a.max_pts == b.max_pts &&
-           a.detect == b.detect && a.slot == b.slot && a.parity == b.parity && a.bgr == b.bgr;
+           a.detect == b.detect && a.mono == b.mono && a.slot == b.slot && a.parity == b.parity && a.bgr == b.bgr;
 }
 
 int vo_run_graph(vo_ctx* ctx, const GraphKey& key, const std::function<int()>& launch)

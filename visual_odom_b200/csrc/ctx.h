@@ -24,6 +24,7 @@ struct GraphKey {
     bool tma;
     int u0, n, max_pts; bool detect;        // BATCH_RANGE: the unit range, its feature bound, on-GPU detection
                                             // (SEQ_FRONT: max_pts = the LK launch bound, the sequences' largest bucket grid)
+    bool mono;                              // BATCH_RANGE: a unit of the range runs the mono_rotation branch
     int slot, parity; bool bgr;             // SEQ_FRONT / SEQ_BACK: image slot of the previous pairs, buffer parity, colour input
 };
 
@@ -215,10 +216,12 @@ struct vo_ctx {
     // after the ring on `post`, ordered by ev[0..3].  With the SM partition on, pre = lk = the LK partition's stream and
     // post = the helper partition's (vo_partition_enable); otherwise pre = post = a high-priority helper stream and lk =
     // side (created on first use), so the helpers' few CTAs never queue behind the other range's LK launch.
+    // A range with a unit that runs the mono_rotation branch forks the five-point kernels from `post` to `mono` (a stream
+    // of the same kind: the helper partition's, or high priority) by ev[4] and joins them back by ev[5].
     struct Lane {
         cudaStream_t side = nullptr;                    // forked from / joined into ctx->stream
-        cudaStream_t pre = nullptr, lk = nullptr, post = nullptr;
-        cudaEvent_t join = nullptr, ev[4] = {};
+        cudaStream_t pre = nullptr, lk = nullptr, post = nullptr, mono = nullptr;
+        cudaEvent_t join = nullptr, ev[6] = {};
     };
     Lane lane[VO_LANES];
     cudaEvent_t fork_ev = nullptr;
@@ -231,7 +234,22 @@ struct vo_ctx {
     uint8_t* h_out = nullptr;       // pinned, [out_units][out_stride]
     size_t out_stride = 0;
     int out_per = 0, out_units = 0; // point slots per unit in a packed block (>= every resident slot's bound); units the pinned block holds
+    bool out_mask = false;          // the packed blocks end with the essential mask (per bytes): batch_mono_used when laid out
     unsigned submit_count = 0;
+    // trackingFrame2Frame's mono_rotation branch per batched unit (vo_batch_mono_rotation): batch_mono[u] is unit u's switch,
+    // mirrored in the device table d_batch_mono[u] that the kernels read (so a toggle never recaptures a graph);
+    // batch_mono_ran[u] what the unit's last run did.  A range with no unit switched on launches what it did without the
+    // branch.  d_batch_ess: one five-point scratch block per configured unit, sized for max_features, allocated by
+    // vo_batch_mono_rotation (outside any capture); d_batch_mono[batch_ess_units + u] is unit u's count for the branch
+    // (its n_valid, 0 when it is off, which ends its problem at k_ess_init).
+    std::vector<int> batch_mono, batch_mono_ran;
+    bool batch_mono_used = false;   // a unit was switched on since vo_batch_configure (the packed outputs carry masks)
+    void* d_batch_ess = nullptr;    // [batch_ess_units][batch_ess_bytes]
+    int* d_batch_mono = nullptr;    // [2][batch_ess_units]: switch | count (the allocation's base, d_batch_ess after it)
+    size_t batch_ess_bytes = 0;
+    int batch_ess_units = 0;
+    cudaStream_t batch_mono_stream = nullptr;       // the fork of a range on ctx->stream (lanes use Lane::mono)
+    cudaEvent_t batch_mono_ev[2] = {nullptr, nullptr};
 };
 
 void vo_set_error(vo_ctx* ctx, const char* fmt, ...);

@@ -187,7 +187,8 @@ __global__ void k_seq_finish(vo_unit_result_dev* res, double* tprev_next, const 
 
 // trackingFrame2Frame(mono_rotation = true) (src/visualOdometry.cpp:146-157,186-189): `rotation` comes from recoverPose,
 // the PnP supplies only `translation`.  Runs after k_seq_finish, so the translation carry is the PnP's as without the branch.
-// Sequence q's result is ess_stride bytes after sequence q - 1's.
+// Sequence q's result is ess_stride bytes after sequence q - 1's.  The batched mode folds its units with the same kernel
+// (vo_launch_mono_fold), `live` then being the per-unit switch.
 __global__ void k_seq_mono(vo_unit_result_dev* res, const EssResult* __restrict__ ess, size_t ess_stride, const int* __restrict__ live)
 {
     const int q = blockIdx.y;
@@ -280,6 +281,10 @@ int vo_launch_seq_finish(const SeqArgs& a, int n_seq, cudaStream_t s)
 }
 int vo_launch_seq_mono(const SeqArgs& a, const EssResult* ess, size_t ess_stride, int n_seq, cudaStream_t s)
 {
-    k_seq_mono<<<dim3(1, n_seq), 32, 0, s>>>(a.res, ess, ess_stride, a.live);
+    return vo_launch_mono_fold(a.res, ess, ess_stride, a.live, n_seq, s);
+}
+int vo_launch_mono_fold(vo_unit_result_dev* res, const EssResult* ess, size_t ess_stride, const int* on, int n, cudaStream_t s)
+{
+    k_seq_mono<<<dim3(1, n), 32, 0, s>>>(res, ess, ess_stride, on);
     return 1;
 }

@@ -36,6 +36,9 @@ int vo_launch_seq_finish(const SeqArgs& a, int n_seq, cudaStream_t s);
 // mono_rotation = true: each live sequence's record R becomes recoverPose's rotation (I where the branch aborted);
 // everything else in the record stays the PnP's.  ess: sequence 0's result, sequence q's ess_stride bytes further on.
 int vo_launch_seq_mono(const SeqArgs& a, const EssResult* ess, size_t ess_stride, int n_seq, cudaStream_t s);
+// the same fold for n records res[0 .. n) and their results (ess_stride bytes apart): record q takes ess q's rotation
+// when on[q] != 0 (the batched mode's per-unit switch, vo_batch_mono_rotation)
+int vo_launch_mono_fold(vo_unit_result_dev* res, const EssResult* ess, size_t ess_stride, const int* on, int n, cudaStream_t s);
 
 // vo_mseq_wait_device: the oldest submission's results (buffer units u0 .. u0 + n_seq - 1) into caller device buffers.
 // mode[q]: 1 the sequence ran in that submission, 0 retired or empty, SEQ_STARTED started by it.  Sources are
