@@ -310,7 +310,8 @@ typedef struct vo_dunit {
  *                                                (a push is submit + wait).  The conversion runs on the sequence's copy
  *                                                stream, straight into the image ring, under the previous frame.
  *   vo_batch_submit_device                       vo_batch_submit; results through vo_batch_wait / vo_batch_outputs /
- *                                                vo_batch_fetch.  units == NULL re-runs what is resident, as there. */
+ *                                                vo_batch_fetch, or into device memory through vo_batch_wait_device.
+ *                                                units == NULL re-runs what is resident, as there. */
 VO_API int vo_seq_begin_device(vo_ctx* ctx, int w, int h, const float P_l[12], const float P_r[12], const vo_dimage* left0,
                                const vo_dimage* right0);
 VO_API int vo_seq_submit_device(vo_ctx* ctx, const vo_dimage* left1, const vo_dimage* right1);
@@ -423,6 +424,42 @@ VO_API int vo_batch_fetch_mono(vo_ctx* ctx, int unit, vo_mono_result* mono, uint
  * first vo_batch_mono_rotation that switches a unit on, each unit's block grows by one byte per point slot, which
  * *d2h_bytes_per_unit reports); this reads it and the staged result of a waited unit, under vo_batch_outputs' rules. */
 VO_API int vo_batch_outputs_mono(vo_ctx* ctx, int unit, vo_mono_result* mono, uint8_t* ess_mask);
+/* Batched results into GPU memory, without a host wait (a GPU consumer: a torch pose graph or learning pipeline, a
+ * device-side filter of bad pairs).  vo_batch_wait_device retires the pending submission of [first_unit, first_unit +
+ * n_units), found as vo_batch_wait finds it (in any order among the pending ones), with ONE kernel launch on the context's
+ * stream, ordered after the work already enqueued there and after that submission; the host never blocks.  Work enqueued
+ * on the context's stream after the call sees the results (the stream contract above).  Unit first_unit + i is written
+ * at index i of every array; every pointer may be NULL (skipped) and must otherwise be device (or managed) memory of the
+ * context's GPU; nothing else in the arrays is written:
+ *   records    vo_batch_wait's record, byte for byte (with the mono_rotation branch on, R is recoverPose's)
+ *   pts4       [n_units][4][pts_cap]  L0, R0, L1, R1 (vo_batch_fetch's pts4)  \
+ *   kept_idx   [n_units][pts_cap]                                              > the first min(n_valid, pts_cap) entries
+ *   points3d   [n_units][pts_cap]     points3D_t0                             /
+ *   inliers    [n_units][pts_cap]     the first min(n_inliers, pts_cap): indices into the unit's n_valid list
+ *   mono       [n_units]              vo_batch_wait_mono's: zeroed for a unit that ran with the branch off
+ *   ess_mask   [n_units][pts_cap]     the first min(n_valid, pts_cap) bytes for units with the branch on, untouched for
+ *                                     the others (vo_batch_fetch_mono)
+ * Only submissions made by vo_batch_submit_device or vo_batch_submit(units == NULL) are accepted: a submission from host
+ * images is refused and stays pending for vo_batch_wait, because a wait that does not block gives no point after which a
+ * pinned host image is free again.  Refused with VO_E_INVALID, changing nothing: no pending submission for the range, a
+ * host-image submission, r == NULL, pts_cap < 0, a point array with pts_cap == 0, a pointer that is not device memory of
+ * the context's GPU.  The submission still stages its records (and, with "batch_outputs" = 1, its packed lists) in pinned
+ * memory as ever: after a device wait vo_batch_fetch[_mono] and vo_batch_outputs[_mono] of its units BLOCK until the
+ * submission has finished, then read what they read after vo_batch_wait.  Every call that refuses pending submissions
+ * (vo_batch_configure, _calibrate, _params, _mono_rotation, _upload, _run, vo_frame_batch, the stage calls,
+ * vo_bgr_to_gray, the vo_seq_* / vo_mseq_* begins) and vo_destroy first wait on the host for device-waited submissions
+ * still running.  A range may be resubmitted right after its device wait. */
+typedef struct vo_batch_dresults {
+    vo_unit_result* records;     /* [n_units] */
+    int pts_cap;                 /* entries per unit of each list below */
+    vo_point2f* pts4;            /* [n_units][4][pts_cap]  L0, R0, L1, R1 (vo_batch_fetch's pts4) */
+    int32_t* kept_idx;           /* [n_units][pts_cap] */
+    vo_point3f* points3d;        /* [n_units][pts_cap]  points3D_t0 */
+    int32_t* inliers;            /* [n_units][pts_cap]  indices into the unit's n_valid list */
+    vo_mono_result* mono;        /* [n_units]  as vo_batch_wait_mono: zeroed for a unit with the branch off */
+    uint8_t* ess_mask;           /* [n_units][pts_cap]  written for units with the branch on, untouched otherwise */
+} vo_batch_dresults;
+VO_API int vo_batch_wait_device(vo_ctx* ctx, int first_unit, int n_units, const vo_batch_dresults* r);
 /* currentVOFeatures (points / ages may differ in length) and the carried translation (waits for frames in flight) */
 VO_API int vo_seq_state(vo_ctx* ctx, vo_point2f* points, int32_t* ages, int cap, int* n_points, int* n_ages, double t_out[3]);
 

@@ -117,6 +117,12 @@ class VoMseqDResults(C.Structure):
                 ("ess_mask", C.c_void_p)]
 
 
+class VoBatchDResults(C.Structure):
+    """vo_batch_dresults: the caller's device buffers vo_batch_wait_device writes (any pointer may be NULL)."""
+    _fields_ = [("records", C.c_void_p), ("pts_cap", C.c_int), ("pts4", C.c_void_p), ("kept_idx", C.c_void_p),
+                ("points3d", C.c_void_p), ("inliers", C.c_void_p), ("mono", C.c_void_p), ("ess_mask", C.c_void_p)]
+
+
 # the same record as a numpy structured dtype (C layout, 152 bytes): arrays of records can be handed out without building
 # one Python dict per record (a gathered table of a multi-GPU step has world x units of them)
 RESULT_DTYPE = np.dtype([("n_features", "<i4"), ("n_detected", "<i4"), ("n_tracked", "<i4"), ("n_valid", "<i4"), ("n_inliers", "<i4"),
@@ -204,6 +210,7 @@ SIGNATURES = {
     "vo_batch_wait_mono": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(VoUnitResult), C.POINTER(VoMonoResult)]),
     "vo_batch_fetch_mono": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(VoMonoResult), C.c_void_p]),
     "vo_batch_outputs_mono": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(VoMonoResult), C.c_void_p]),
+    "vo_batch_wait_device": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(VoBatchDResults)]),
     "vo_mseq_params": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(VoParams)]),
     "vo_mseq_begin_sized": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
@@ -1052,15 +1059,25 @@ class Context:
         and "ess_mask" (n, pts_cap) uint8."""
         import torch
         n, dev = self._mseq_n, torch.device("cuda", self.device)
-        lists = points or points3d or inliers or mono
+        out = self._dresults_tensors(n, pts_cap, points, False, points3d, inliers, mono)
+        out.update(status=torch.zeros(n, dtype=torch.int32, device=dev), frame_pose=torch.zeros((n, 4, 4), dtype=torch.float64, device=dev))
+        return out
+
+    def _dresults_tensors(self, n, pts_cap, points, kept_idx, points3d, inliers, mono):
+        """The tensors the two device waits share for n sequences or units: the records and their views, the lists asked
+        for, the mono results and mask (see mseq_dresults_alloc)."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        lists = points or kept_idx or points3d or inliers or mono
         if lists and (not isinstance(pts_cap, (int, np.integer)) or pts_cap <= 0):
             raise ValueError(f"pts_cap = {pts_cap!r}: point outputs need pts_cap > 0")
         rec = torch.zeros((n, 19), dtype=torch.float64, device=dev)
         out = dict(records=rec, counts=rec[:, :4].view(torch.int32)[:, :7], rvec=rec[:, 4:7], tvec=rec[:, 7:10],
-                   R=rec[:, 10:19].view(n, 3, 3), status=torch.zeros(n, dtype=torch.int32, device=dev),
-                   frame_pose=torch.zeros((n, 4, 4), dtype=torch.float64, device=dev), pts_cap=int(pts_cap) if lists else 0)
+                   R=rec[:, 10:19].view(n, 3, 3), pts_cap=int(pts_cap) if lists else 0)
         if points:
             out["pts4"] = torch.zeros((n, 4, pts_cap, 2), dtype=torch.float32, device=dev)
+        if kept_idx:
+            out["kept_idx"] = torch.zeros((n, pts_cap), dtype=torch.int32, device=dev)
         if points3d:
             out["points3d"] = torch.zeros((n, pts_cap, 3), dtype=torch.float32, device=dev)
         if inliers:
@@ -1071,9 +1088,11 @@ class Context:
                        ess_mask=torch.zeros((n, pts_cap), dtype=torch.uint8, device=dev))
         return out
 
+    # out= tensors of the device waits: dtype and the shape after the leading count (None: pts_cap)
     _DRES_SHAPES = {"records": ("float64", (19,)), "status": ("int32", ()), "frame_pose": ("float64", (4, 4)),
-                    "pts4": ("float32", (4, None, 2)), "points3d": ("float32", (None, 3)), "inliers": ("int32", (None,)),
-                    "mono_raw": ("float64", (14,)), "ess_mask": ("uint8", (None,))}
+                    "pts4": ("float32", (4, None, 2)), "kept_idx": ("int32", (None,)), "points3d": ("float32", (None, 3)),
+                    "inliers": ("int32", (None,)), "mono_raw": ("float64", (14,)), "ess_mask": ("uint8", (None,))}
+    _DRES_LISTS = ("pts4", "kept_idx", "points3d", "inliers", "ess_mask")
 
     def mseq_wait_device(self, pts_cap=4096, points=True, points3d=True, inliers=True, out=None):
         """Retire the oldest submission of a run begun with device_results=True without blocking the host
@@ -1086,7 +1105,7 @@ class Context:
         if out is None:
             out = self.mseq_dresults_alloc(pts_cap, points, points3d, inliers, mono)
         else:
-            self._check_dresults(out)
+            self._check_dresults(out, self._mseq_n)
         r = VoMseqDResults()
         r.pts_cap = int(out.get("pts_cap", 0))
         for f, k in (("status", "status"), ("records", "records"), ("frame_pose", "frame_pose"), ("pts4", "pts4"),
@@ -1096,12 +1115,41 @@ class Context:
         self._device_call(self.lib.vo_mseq_wait_device, C.byref(r))
         return out
 
-    def _check_dresults(self, out):
-        """out= of mseq_wait_device: CUDA tensors on the context's GPU, contiguous, of the run's sequence count, the
-        dtypes mseq_dresults_alloc gives and one pts_cap."""
+    def batch_dresults_alloc(self, n_units, pts_cap=4096, points=True, kept_idx=True, points3d=True, inliers=True, mono=False):
+        """The CUDA tensors batch_wait_device writes for a submission of n_units units (pass them back as out= to reuse
+        them): "records" (n, 19) float64 with the views "counts", "rvec", "tvec" and "R", "pts4" (n, 4, pts_cap, 2),
+        "kept_idx" (n, pts_cap) int32, "points3d" (n, pts_cap, 3), "inliers" (n, pts_cap), and with mono "mono_raw" and
+        its views and "ess_mask", all as mseq_dresults_alloc lays them out."""
+        return self._dresults_tensors(int(n_units), pts_cap, points, kept_idx, points3d, inliers, mono)
+
+    def batch_wait_device(self, first_unit, n_units, pts_cap=4096, points=True, kept_idx=True, points3d=True, inliers=True,
+                          mono=False, out=None):
+        """Retire the pending submission of [first_unit, first_unit + n_units) without blocking the host
+        (vo_batch_wait_device; the submission must come from batch_submit_device or a units=None re-run): one kernel on
+        torch.cuda.current_stream() writes every unit's results into CUDA tensors, which work queued on that stream
+        afterwards may read at once.  Returns the dict of batch_dresults_alloc; out= such a dict, filled in place, so a loop
+        allocates nothing.  Only the first n_valid entries of a unit's lists (inliers: n_inliers) are written; "ess_mask"
+        only for units with the mono_rotation branch on."""
+        if out is None:
+            out = self.batch_dresults_alloc(n_units, pts_cap, points, kept_idx, points3d, inliers, mono)
+        else:
+            self._check_dresults(out, int(n_units))
+        r = VoBatchDResults()
+        r.pts_cap = int(out.get("pts_cap", 0))
+        for f, k in (("records", "records"), ("pts4", "pts4"), ("kept_idx", "kept_idx"), ("points3d", "points3d"),
+                     ("inliers", "inliers"), ("mono", "mono_raw"), ("ess_mask", "ess_mask")):
+            t = out.get(k)
+            setattr(r, f, None if t is None else t.data_ptr())
+        self._device_call(self.lib.vo_batch_wait_device, int(first_unit), int(n_units), C.byref(r))
+        return out
+
+    def _check_dresults(self, out, n):
+        """out= of a device wait: CUDA tensors on the context's GPU, contiguous, of n sequences or units, the dtypes the
+        alloc calls give and one pts_cap (a positive one when there are lists)."""
         import torch
-        n = self._mseq_n
         cap = out.get("pts_cap", 0)
+        if any(out.get(k) is not None for k in self._DRES_LISTS) and (not isinstance(cap, (int, np.integer)) or cap <= 0):
+            raise ValueError(f"out['pts_cap'] = {cap!r}: point outputs need pts_cap > 0")
         for k, (dt, tail) in self._DRES_SHAPES.items():
             t = out.get(k)
             if t is None:

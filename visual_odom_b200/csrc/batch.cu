@@ -8,6 +8,7 @@
 #include "ctx.h"
 #include <string.h>
 #include <algorithm>
+#include <type_traits>
 
 __global__ void k_pack_counts(vo_unit_result_dev* res, const int* n_pts, const int* n_det, const int* n3, const int* n5,
                               int n_units, int detect)
@@ -119,7 +120,9 @@ static int ensure_outputs(vo_ctx* ctx, int u0, int n, int bound)
     const size_t stride = ((size_t)per * (VO_OUT_BYTES_PER_SLOT + (mask ? 1 : 0)) + 255) / 256 * 256;
     for (auto& p : ctx->pending)                // their copies land in the old blocks
         if (p.active) VO_CUDA_CHECK(cudaEventSynchronize(p.done));
-    void* q = nullptr;                          // both new blocks first: a failed allocation leaves the old ones in use
+    int rc = vo_sync_device_retired(ctx);       // so do those of device-waited submissions still running
+    if (rc) return rc;
+    void* q = nullptr;                         // both new blocks first: a failed allocation leaves the old ones in use
     VO_CUDA_CHECK(cudaMalloc(&q, stride * ctx->units + 256));
     uint8_t* h = nullptr;
     const cudaError_t e = cudaMallocHost(&h, stride * ctx->units + 256);
@@ -591,15 +594,32 @@ static int batch_submit(vo_ctx* ctx, const char* who, const Unit* units, int fir
         if (vo_partition_enable(ctx, 8) != VO_OK) ctx->err[0] = 0;      // no green contexts on this driver: run unpartitioned
     }
     if (ctx->batch_outputs && (rc = ensure_outputs(ctx, first_unit, n_units, max_pts))) return rc;
+    // A device-waited submission of these units may not have copied its pinned staging to the device yet: the host
+    // rewrites that staging below only after those copies (never after its pose solve).
+    for (auto& p : ctx->pending)
+        if (units && p.device_retired && first_unit < p.u0 + p.n && p.u0 < first_unit + n_units)
+            VO_CUDA_CHECK(cudaEventSynchronize(p.staged));
+    // a free record: neither in flight nor possibly still running after a device wait
     vo_ctx::Pending* slot = nullptr;
-    for (auto& p : ctx->pending) if (!p.active) { slot = &p; break; }
+    for (auto& p : ctx->pending) {
+        if (p.active) continue;
+        if (p.device_retired) {
+            const cudaError_t e = cudaEventQuery(p.done);
+            if (e == cudaSuccess) p.device_retired = false;
+            else if (e != cudaErrorNotReady) VO_CUDA_CHECK(e);
+        }
+        if (!p.device_retired) { slot = &p; break; }
+    }
     if (!slot) {
         ctx->pending.emplace_back();
         slot = &ctx->pending.back();
         VO_CUDA_CHECK(cudaEventCreateWithFlags(&slot->done, cudaEventDisableTiming));
+        VO_CUDA_CHECK(cudaEventCreateWithFlags(&slot->staged, cudaEventDisableTiming));
     }
     const int c = (int)((ctx->submit_count++) % VO_LANES);     // up to VO_LANES submissions in flight, each on its own lane
     cudaStream_t st = ctx->lane[c].side;
+    // The lane follows everything on ctx->stream, including the k_seq_collect launch of a vo_batch_wait_device of these
+    // slots: a range resubmitted right after a device wait overwrites its unit buffers only once they have been read.
     VO_CUDA_CHECK(cudaEventRecord(ctx->fork_ev, ctx->stream));
     VO_CUDA_CHECK(cudaStreamWaitEvent(st, ctx->fork_ev, 0));
     if ((rc = vo_dist_order_after_gathers(ctx, st))) return rc;
@@ -608,6 +628,8 @@ static int batch_submit(vo_ctx* ctx, const char* who, const Unit* units, int fir
         if ((rc = upload_units(ctx, units, first_unit, n_units, pitch, st, c, detect))) return rc;
         if (ctx->batch_uploaded < first_unit + n_units) ctx->batch_uploaded = first_unit + n_units;
     }
+    const bool device_in = !units || std::is_same<Unit, vo_dunit>::value;
+    if (device_in) VO_CUDA_CHECK(cudaEventRecord(slot->staged, st));
     if ((rc = run_range(ctx, first_unit, n_units, st))) return rc;
     vo_unit_result_dev* h_res = pinned_results(ctx);
     VO_CUDA_CHECK(cudaMemcpyAsync(h_res + first_unit, ctx->d_results + first_unit, (size_t)n_units * sizeof(vo_unit_result_dev), cudaMemcpyDeviceToHost, st));
@@ -630,7 +652,7 @@ static int batch_submit(vo_ctx* ctx, const char* who, const Unit* units, int fir
                                       (size_t)n_units * ctx->out_stride, cudaMemcpyDeviceToHost, st));
     }
     VO_CUDA_CHECK(cudaEventRecord(slot->done, st));
-    slot->u0 = first_unit; slot->n = n_units; slot->active = true;
+    slot->u0 = first_unit; slot->n = n_units; slot->active = true; slot->device_in = device_in;
     return VO_OK;
 }
 
@@ -683,13 +705,91 @@ extern "C" int vo_batch_wait_mono(vo_ctx* ctx, int first_unit, int n_units, vo_u
     return batch_wait(ctx, "vo_batch_wait_mono", first_unit, n_units, results, mono);
 }
 
+// whether a unit of [u0, u0 + n) ran the mono_rotation branch in its last run
+static bool range_mono_ran(const vo_ctx* ctx, int u0, int n)
+{
+    for (int u = u0; u < u0 + n && u < (int)ctx->batch_mono_ran.size(); u++)
+        if (ctx->batch_mono_ran[u]) return true;
+    return false;
+}
+
+// vo_batch_wait_device: ONE k_seq_collect launch on ctx->stream, after the caller's work there and after the submission's
+// `done`; the host only moves its bookkeeping on.  The records are those the submission folded on the device (the bytes
+// vo_batch_wait copies out of pinned staging); the lists come straight from the unit buffers, which a resubmission of the
+// range overwrites only after this launch (it forks from ctx->stream).  The switch table d_batch_mono holds the switches
+// the submission ran with: vo_batch_mono_rotation is refused while it is pending and queues its write behind this launch.
+extern "C" int vo_batch_wait_device(vo_ctx* ctx, int first_unit, int n_units, const vo_batch_dresults* r)
+{
+    static const char* who = "vo_batch_wait_device";
+    if (!ctx) return VO_E_INVALID;
+    vo_ctx::Pending* p = nullptr;
+    for (auto& q : ctx->pending)
+        if (q.active && q.u0 == first_unit && q.n == n_units) { p = &q; break; }
+    if (!p) {
+        vo_set_error(ctx, "%s: no pending submission for slots [%d, %d)", who, first_unit, first_unit + n_units);
+        return VO_E_INVALID;
+    }
+    if (!p->device_in) {
+        vo_set_error(ctx, "%s: slots [%d, %d) were submitted from host images, which only vo_batch_wait releases", who,
+                     first_unit, first_unit + n_units);
+        return VO_E_INVALID;
+    }
+    if (!r) { vo_set_error(ctx, "%s: null result table", who); return VO_E_INVALID; }
+    const bool lists = r->pts4 || r->kept_idx || r->points3d || r->inliers || r->ess_mask;
+    if (r->pts_cap < 0 || (lists && r->pts_cap == 0)) {
+        vo_set_error(ctx, "%s: pts_cap = %d with point arrays", who, r->pts_cap);
+        return VO_E_INVALID;
+    }
+    VO_CUDA_CHECK(cudaSetDevice(ctx->device));
+    const struct { const char* name; const void* p; } ptrs[] = {
+        {"records", r->records}, {"pts4", r->pts4}, {"kept_idx", r->kept_idx}, {"points3d", r->points3d},
+        {"inliers", r->inliers}, {"mono", r->mono}, {"ess_mask", r->ess_mask}};
+    int rc;
+    for (const auto& x : ptrs)
+        if ((rc = vo_check_dptr(ctx, who, x.name, x.p))) return rc;
+    static_assert(sizeof(vo_unit_result) == sizeof(vo_unit_result_dev), "k_seq_collect writes vo_unit_result records");
+    const size_t cs = (size_t)ctx->units * ctx->cap, uo = (size_t)first_unit * ctx->cap;
+    CollectArgs a;
+    memset(&a, 0, sizeof(a));
+    a.all_ran = true;
+    a.res = ctx->d_results + first_unit; a.cap = ctx->cap;
+    a.valid4 = ctx->d_valid4 + uo; a.plane_stride = cs;
+    a.X = ctx->d_X + uo; a.inliers = ctx->d_inliers + uo; a.idx5 = ctx->d_idx5 + uo;
+    if (range_mono_ran(ctx, first_unit, n_units)) {
+        EssArgs e;
+        batch_ess_args(ctx, first_unit, n_units, ctx->cap, e);
+        a.ess = e.result; a.ess_mask = e.mask; a.ess_stride = ctx->batch_ess_bytes; a.ess_on = ctx->d_batch_mono + first_unit;
+    }
+    a.records = (vo_unit_result_dev*)r->records; a.pts_cap = r->pts_cap;
+    a.pts4 = (float2*)r->pts4; a.kept_out = r->kept_idx; a.points3d = (float3*)r->points3d; a.inliers_out = r->inliers;
+    a.mono = r->mono; a.mask_out = r->ess_mask;
+    VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, p->done, 0));
+    ctx->launches += vo_launch_seq_collect(a, n_units, ctx->stream);
+    VO_CUDA_CHECK(cudaGetLastError());
+    p->active = false;
+    p->device_retired = true;
+    return VO_OK;
+}
+
+// After vo_batch_wait_device the host reads of a unit (pinned staging, or the unit buffers) first wait for its submission.
+static int sync_device_retired_unit(vo_ctx* ctx, int unit)
+{
+    for (auto& p : ctx->pending)
+        if (p.device_retired && unit >= p.u0 && unit < p.u0 + p.n) {
+            VO_CUDA_CHECK(cudaSetDevice(ctx->device));
+            VO_CUDA_CHECK(cudaEventSynchronize(p.done));
+            p.device_retired = false;
+        }
+    return VO_OK;
+}
+
 // VO_E_INVALID + message unless `unit` is resident and not part of a submission that has not been waited for
 static int check_waited(vo_ctx* ctx, const char* who, int unit)
 {
     if (unit < 0 || unit >= ctx->batch_uploaded) { vo_set_error(ctx, "%s: unit %d outside the resident batch", who, unit); return VO_E_INVALID; }
     for (auto& p : ctx->pending)
         if (p.active && unit >= p.u0 && unit < p.u0 + p.n) { vo_set_error(ctx, "%s: unit %d has not been waited for", who, unit); return VO_E_INVALID; }
-    return VO_OK;
+    return sync_device_retired_unit(ctx, unit);
 }
 
 // The branch's result of the unit's last run and its mask (n_valid bytes, aligned with vo_batch_fetch's lists), read
@@ -728,6 +828,8 @@ extern "C" int vo_batch_outputs(vo_ctx* ctx, int unit, vo_point2f* pts4, int32_t
     if (unit < 0 || unit >= ctx->batch_uploaded || unit >= ctx->out_units) { vo_set_error(ctx, "unit %d outside the resident batch", unit); return VO_E_INVALID; }
     for (auto& p : ctx->pending)
         if (p.active && unit >= p.u0 && unit < p.u0 + p.n) { vo_set_error(ctx, "vo_batch_outputs: unit %d has not been waited for", unit); return VO_E_INVALID; }
+    int rc = sync_device_retired_unit(ctx, unit);
+    if (rc) return rc;
     const vo_unit_result_dev& r = pinned_results(ctx)[unit];
     const int per = ctx->out_per;
     const int nv = r.n_valid < per ? r.n_valid : per, ni = r.n_inliers < per ? r.n_inliers : per;
@@ -762,6 +864,8 @@ extern "C" int vo_batch_fetch(vo_ctx* ctx, int unit, vo_point2f* pts_in, vo_poin
 {
     if (!ctx) return VO_E_INVALID;
     if (unit < 0 || unit >= ctx->batch_uploaded) { vo_set_error(ctx, "unit %d outside the resident batch", unit); return VO_E_INVALID; }
+    int rc = sync_device_retired_unit(ctx, unit);
+    if (rc) return rc;
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
     vo_unit_result_dev r;
     VO_CUDA_CHECK(cudaMemcpyAsync(&r, ctx->d_results + unit, sizeof(r), cudaMemcpyDeviceToHost, ctx->stream));

@@ -170,7 +170,10 @@ extern "C" void vo_destroy(vo_ctx* ctx)
     vo_partition_destroy(ctx);
     vo_free_state(ctx);
     for (cudaEvent_t e : ctx->ev_pool) cudaEventDestroy(e);
-    for (auto& p : ctx->pending) if (p.done) cudaEventDestroy(p.done);
+    for (auto& p : ctx->pending) {
+        if (p.done) cudaEventDestroy(p.done);
+        if (p.staged) cudaEventDestroy(p.staged);
+    }
     for (int k = 0; k < 2; k++) {
         if (ctx->seq_front_ev[k]) cudaEventDestroy(ctx->seq_front_ev[k]);
         if (ctx->seq_back_ev[k]) cudaEventDestroy(ctx->seq_back_ev[k]);
@@ -274,6 +277,16 @@ int vo_refuse_pending_batches(vo_ctx* ctx, const char* who)
         if (p.active) {
             vo_set_error(ctx, "%s: the vo_batch_submit submission of slots [%d, %d) has not been waited for", who, p.u0, p.u0 + p.n);
             return VO_E_INVALID;
+        }
+    return vo_sync_device_retired(ctx);
+}
+
+int vo_sync_device_retired(vo_ctx* ctx)
+{
+    for (auto& p : ctx->pending)
+        if (p.device_retired) {
+            VO_CUDA_CHECK(cudaEventSynchronize(p.done));
+            p.device_retired = false;
         }
     return VO_OK;
 }
@@ -389,6 +402,8 @@ int vo_drain_pending(vo_ctx* ctx)
             VO_CUDA_CHECK(cudaEventSynchronize(p.done));
             p.active = false;
         }
+    int rc = vo_sync_device_retired(ctx);
+    if (rc) return rc;
     // frames of the sequence mode still in flight on the pose-solve stream
     if (ctx->seq_inflight > 0 && ctx->lane[0].side) VO_CUDA_CHECK(cudaStreamSynchronize(ctx->lane[0].side));
     return VO_OK;

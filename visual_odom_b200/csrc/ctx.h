@@ -225,8 +225,16 @@ struct vo_ctx {
     };
     Lane lane[VO_LANES];
     cudaEvent_t fork_ev = nullptr;
-    struct Pending { int u0 = 0, n = 0; bool active = false; cudaEvent_t done = nullptr; };
-    std::vector<Pending> pending;   // vo_batch_submit / vo_batch_wait
+    // A submission in flight (active) until vo_batch_wait retires it, or until vo_batch_wait_device does: that one only
+    // orders ctx->stream after `done`, so the submission may still be running (device_retired) until `done` completes.
+    // `staged` follows the H2D copies of its pinned input staging (t_prev, counts, image descriptors); a later submission
+    // of the same units rewrites that staging only after it.  device_in: made from device images or units == NULL (the
+    // only kind vo_batch_wait_device accepts: a wait that does not block never frees a pinned host image).
+    struct Pending {
+        int u0 = 0, n = 0; bool active = false; cudaEvent_t done = nullptr;
+        bool device_in = false, device_retired = false; cudaEvent_t staged = nullptr;
+    };
+    std::vector<Pending> pending;   // vo_batch_submit / vo_batch_wait[_device]
     // full outputs of a submission (what matchingFeatures / trackingFrame2Frame hand back): packed per unit on the
     // device and copied with ONE D2H per submission into pinned staging (vo_set_option "batch_outputs")
     bool batch_outputs = false;
@@ -293,8 +301,13 @@ void vo_partition_destroy(vo_ctx* ctx);
 int vo_dist_order_after_gathers(vo_ctx* ctx, cudaStream_t st);
 void vo_dist_shutdown(vo_ctx* ctx);
 int vo_claim_buffers(vo_ctx* ctx, const char* who, bool allow_pending_batches = false);
-// VO_E_INVALID + message while a vo_batch_submit submission has not been waited for
+// VO_E_INVALID + message while a vo_batch_submit submission has not been waited for; otherwise waits on the host for the
+// submissions vo_batch_wait_device retired that may still be running (the caller is about to reuse what they use)
 int vo_refuse_pending_batches(vo_ctx* ctx, const char* who);
+// waits on the host for every submission vo_batch_wait_device retired that may still be running
+int vo_sync_device_retired(vo_ctx* ctx);
+// VO_E_INVALID + message unless p is NULL or device (managed) memory of the context's GPU (seq_api.cu)
+int vo_check_dptr(vo_ctx* ctx, const char* who, const char* name, const void* p);
 int vo_ensure_pinned(vo_ctx* ctx, size_t bytes);
 // H2D of a host image (h rows of row_bytes, pitch bytes apart) into a packed device plane on st: one 1-D copy when the
 // rows are contiguous, else a 2-D copy

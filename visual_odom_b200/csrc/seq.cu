@@ -203,13 +203,15 @@ __global__ void k_seq_mono(vo_unit_result_dev* res, const EssResult* __restrict_
 // seq_wait does on the host from the pinned copies, and the point lists, points3D and inliers it leaves in the units.
 // Thread 0 writes the status / record / mono result and integrates frame_pose (main.cpp:196-208: a frame is integrated
 // when its PnP ran (VO_OK or no model) and, with mono_rotation, the essential branch did not abort); the block copies the
-// lists.  Sequences are independent, so the launch is one grid however many of them there are.
+// lists.  Sequences are independent, so the launch is one grid however many of them there are.  The batched mode's
+// vo_batch_wait_device runs the same kernel over the units of a submission (CollectArgs: all_ran, no pose, ess_on).
 __global__ void __launch_bounds__(256) k_seq_collect(const CollectArgs a)
 {
-    const int q = blockIdx.x, mode = a.mode[q];
+    const int q = blockIdx.x, mode = a.all_ran ? 1 : a.mode[q];
     const vo_unit_result_dev* res = a.res + q;
-    const EssResult* ess = a.ess ? (const EssResult*)((const char*)a.ess + (size_t)q * a.ess_stride) : nullptr;
-    double* pose = a.pose + 16 * (size_t)q;
+    const bool on = a.ess && (!a.ess_on || a.ess_on[q]);
+    const EssResult* ess = on ? (const EssResult*)((const char*)a.ess + (size_t)q * a.ess_stride) : nullptr;
+    double* pose = a.pose ? a.pose + 16 * (size_t)q : nullptr;
     const int nv = mode == 1 ? min(res->n_valid, a.pts_cap) : 0;
     const int ni = mode == 1 ? min(res->n_inliers, a.pts_cap) : 0;
     if (threadIdx.x == 0) {
@@ -221,7 +223,7 @@ __global__ void __launch_bounds__(256) k_seq_collect(const CollectArgs a)
         if (mode == 1) {
             r = *res;
             const bool mono_ok = !ess || ess->status == ESS_OK;
-            if ((r.pnp_status == VO_OK || r.pnp_status == VO_PNP_NO_MODEL) && mono_ok) vo_pose_step_dev(pose, r.R, r.tvec);
+            if (pose && (r.pnp_status == VO_OK || r.pnp_status == VO_PNP_NO_MODEL) && mono_ok) vo_pose_step_dev(pose, r.R, r.tvec);
             if (ess) {
                 m.status = mono_ok ? VO_OK : VO_E_TOO_FEW_POINTS;
                 m.n_inliers = ess->n_inliers; m.ransac_iters = ess->iters; m.n_good = ess->n_good;
@@ -229,22 +231,23 @@ __global__ void __launch_bounds__(256) k_seq_collect(const CollectArgs a)
                 for (int k = 0; k < 3; k++) m.t[k] = ess->t[k];
             }
             // bit 8 (a tracked point outside the bucket grid) is not an error, as in seq_wait
-            status = (a.err[q] & ~8) ? VO_E_CAPACITY : VO_OK;
-        } else if (mode == SEQ_STARTED) {              // the new sequence's frame_pose starts here (main.cpp:90)
+            status = a.err && (a.err[q] & ~8) ? VO_E_CAPACITY : VO_OK;
+        } else if (mode == SEQ_STARTED && pose) {      // the new sequence's frame_pose starts here (main.cpp:90)
             for (int i = 0; i < 16; i++) pose[i] = i % 5 == 0 ? 1.0 : 0.0;
         }
         if (a.status) a.status[q] = status;
         if (a.records) a.records[q] = r;
         if (a.mono) a.mono[q] = m;
-        if (a.pose_out)
+        if (a.pose_out && pose)
             for (int i = 0; i < 16; i++) a.pose_out[16 * (size_t)q + i] = pose[i];
     }
     const size_t src = (size_t)q * a.cap, dst = (size_t)q * a.pts_cap;
     for (int i = threadIdx.x; i < nv; i += blockDim.x) {
         if (a.pts4)
             for (int k = 0; k < 4; k++) a.pts4[(4 * (size_t)q + k) * a.pts_cap + i] = a.valid4[k * a.plane_stride + src + i];
+        if (a.kept_out) a.kept_out[dst + i] = a.idx5[src + i];
         if (a.points3d) a.points3d[dst + i] = a.X[src + i];
-        if (a.mask_out) a.mask_out[dst + i] = a.ess_mask[(size_t)q * a.ess_stride + i];
+        if (a.mask_out && ess) a.mask_out[dst + i] = a.ess_mask[(size_t)q * a.ess_stride + i];
     }
     if (a.inliers_out)
         for (int i = threadIdx.x; i < ni; i += blockDim.x) a.inliers_out[dst + i] = a.inliers[src + i];

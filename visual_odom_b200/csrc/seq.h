@@ -43,15 +43,19 @@ int vo_launch_mono_fold(vo_unit_result_dev* res, const EssResult* ess, size_t es
 // vo_mseq_wait_device: the oldest submission's results (buffer units u0 .. u0 + n_seq - 1) into caller device buffers.
 // mode[q]: 1 the sequence ran in that submission, 0 retired or empty, SEQ_STARTED started by it.  Sources are
 // sequence 0's (the unit u0) with the strides of SeqArgs (cap for the point lists, ess_stride bytes for ess / ess_mask);
-// every destination may be NULL.
+// every destination may be NULL.  vo_batch_wait_device retires a batched submission with the same launch: every unit
+// ran (all_ran, mode unused), no pose (NULL: nothing integrated), no error words (err NULL), the tracked-feature indices
+// (idx5 -> kept_out) and a per-unit branch switch (ess_on[q] == 0: no mono result and no mask for that unit).
 struct CollectArgs {
     const vo_unit_result_dev* res; const int* err; int cap;
     const float2* valid4; size_t plane_stride;          // the four lists of unit u0: valid4 + k * plane_stride
-    const float3* X; const int* inliers;
+    const float3* X; const int* inliers; const int* idx5;
     const EssResult* ess; const uint8_t* ess_mask; size_t ess_stride;   // mono runs only (else NULL)
-    double* pose;                                       // [n_seq][16] device frame_pose, integrated here
+    const int* ess_on;                                  // NULL: every unit has its ess entry
+    double* pose;                                       // [n_seq][16] device frame_pose, integrated here (NULL: none)
     int* status; vo_unit_result_dev* records; double* pose_out; int pts_cap;
-    float2* pts4; float3* points3d; int* inliers_out; vo_mono_result* mono; uint8_t* mask_out;
+    float2* pts4; float3* points3d; int* inliers_out; int* kept_out; vo_mono_result* mono; uint8_t* mask_out;
+    bool all_ran;
     unsigned char mode[VO_MSEQ_MAX];
 };
 int vo_launch_seq_collect(const CollectArgs& a, int n_seq, cudaStream_t s);

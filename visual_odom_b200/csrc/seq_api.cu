@@ -832,7 +832,7 @@ static int seq_wait(vo_ctx* ctx, const char* who, bool multi, bool want_mono, vo
 static_assert(sizeof(vo_unit_result) == sizeof(vo_unit_result_dev), "k_seq_collect writes vo_unit_result records");
 
 // VO_E_INVALID + message unless p is NULL or device (managed) memory of the context's GPU
-static int seq_check_dptr(vo_ctx* ctx, const char* who, const char* name, const void* p)
+int vo_check_dptr(vo_ctx* ctx, const char* who, const char* name, const void* p)
 {
     if (!p) return VO_OK;
     cudaPointerAttributes a;
@@ -875,7 +875,7 @@ static int seq_wait_device(vo_ctx* ctx, const char* who, const vo_mseq_dresults*
         {"status", r->status}, {"records", r->records}, {"frame_pose", r->frame_pose}, {"pts4", r->pts4},
         {"points3d", r->points3d}, {"inliers", r->inliers}, {"mono", r->mono}, {"ess_mask", r->ess_mask}};
     for (const auto& x : ptrs)
-        if ((rc = seq_check_dptr(ctx, who, x.name, x.p))) return rc;
+        if ((rc = vo_check_dptr(ctx, who, x.name, x.p))) return rc;
     const int n = ctx->seq_n;
     const int p = (int)((ctx->seq_submitted - ctx->seq_inflight) & 1);      // the parity of the oldest frame in flight
     const int u0 = p * n;
