@@ -248,9 +248,13 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
     const int tn = has_tail ? 3 + (seg & 1) : 0;
     // chain-buffer positions (floats) inside a quantity's slots.
     //   A (setup)     : SIMD element (row, col) at chain*84 + row*4 + cpos ; tail element at 336 + row*5 + (tcol-16)
-    //   b (iteration) : SIMD pair (col, col+4) of a row at chain*84 + row*2 + cpos/2 (written by the even-cpos lane)
+    //   b (iteration) : SIMD pair (col, col+4) of a row at chain*84 + row*2 + cpos/2; the even-cpos lane writes b1's
+    //                   pair, its partner lane ^ 8 (col + 4, same chain and row half) b2's, in the second quantity
     const int a_pos = chain * SLOT_S + r0 * 4 + cpos;
-    const int b_pos = chain * SLOT_S + r0 * 2 + (cpos >> 1);
+    const int b_pos = (cpos & 1) * QSTRIDE + chain * SLOT_S + r0 * 2 + (cpos >> 1);
+    // a strip element's packed gradients: (Ix, Iy) in an even-cpos lane, (Iy, Ix) in an odd one -- low half first, so that
+    // the low product is the one a lane keeps for its own pair sum and the high one the one it hands its partner
+    const unsigned g_sel = (cpos & 1) ? 0x1054 : 0x5410;
     const int t_pos = TAIL_OFF + tr0 * 5 + (tcol - 16);
     // runner lane L sums slot (quantity L/5, chain L%5)
     const int rq = lane / 5, rc = lane - rq * 5;
@@ -367,7 +371,7 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                 if (USE_TMA) { mbar_wait(&sm.bar, phase); phase ^= 1; }
 
                 // ---- patch extraction: I (x32), Ix, Iy of the strip elements; A addends in chain order ----
-                int dxy[15];          // lo16 = Ix, hi16 = Iy
+                int dxy[15];          // lo16 = Ix, hi16 = Iy; swapped in the strip elements of odd-cpos lanes (g_sel)
                 int Ipk[8];           // int16 patch intensities, two per register: strip 0..10, tail 11..14
                 float A11, A12, A22;
                 {
@@ -396,7 +400,7 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                             if (k >= nvalid) { ix = 0; iy = 0; }
                             const int e = part ? 11 + k : k;
                             if (e & 1) Ipk[e >> 1] |= ival << 16; else Ipk[e >> 1] = ival & 0xffff;
-                            dxy[e] = (ix & 0xffff) | (iy << 16);
+                            dxy[e] = __byte_perm(ix, iy, part ? 0x5410 : g_sel);
                             const float fx = (float)ix, fy = (float)iy;
                             const int pos = part ? t_pos + k * 5 : a_pos + k * 4;
                             // a dummy element's position belongs to another lane: no store
@@ -468,14 +472,17 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                     a = npx - (float)inx; b = npy - (float)iny;
                     bilinear_weights(a, b, w00, w01, w10, w11);
                     const unsigned wt = (unsigned)w00 | ((unsigned)w01 << 16), wb = (unsigned)w10 | ((unsigned)(w11 & 0xffff) << 16);
-                    int sxs = 0, sys = 0, sxt = 0, syt = 0;         // signed sums: strip (my SIMD chain) / tail
-                    unsigned axs = 0, ays = 0, axt = 0, ayt = 0;    // sums of |addend|
-                    int dpk[8];                       // int16 residuals, two per register (same element order as the I patch)
+                    // signed sums: strip (my SIMD chain; products with the low / high packed gradient) / tail
+                    int s0s = 0, s1s = 0, sxt = 0, syt = 0;
+                    unsigned a0s = 0, a1s = 0, axt = 0, ayt = 0;    // sums of |addend|
+                    int dpk[8];                       // full pass: int16 residuals, two per register (same element order as the I patch)
+                    int dv[15];                       // light pass: the residuals unpacked, as the replay consumes them
                     // The residual pass.  WITH_SUMS: also the products with the gradients, their exact integer sums and the
                     // sums of |addend| that decide whether the integer sums ARE the float32 chain sums.  Once an iteration of
                     // a level needed the faithful replay the following ones nearly always do (oracle: 94 %), and the replay
                     // recomputes the products from the residuals anyway -- so after a replay the rest of the level runs the
-                    // light pass and goes straight to the replay (always valid, only slower than the exact path).
+                    // light pass and goes straight to the replay (always valid, only slower than the exact path).  The light
+                    // pass has the registers to hand the replay its residuals unpacked; the full pass packs them.
                     auto residual_pass = [&](auto with_sums) {
                         constexpr bool WITH_SUMS = decltype(with_sums)::value;
 #pragma unroll
@@ -491,33 +498,62 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                                 const int e = part ? 11 + k : k;
                                 const int Iv = (e & 1) ? (Ipk[e >> 1] >> 16) : (int)(short)(Ipk[e >> 1] & 0xffff);
                                 const int diff = (dp2a_taps(wb, pbot, dp2a_taps(wt, ptop, 1 << (W_BITS - 6))) >> (W_BITS - 5)) - Iv;
-                                if (e & 1) dpk[e >> 1] |= diff << 16; else dpk[e >> 1] = diff & 0xffff;
                                 if (WITH_SUMS) {
-                                    const int vx = diff * (int)(short)(dxy[e] & 0xffff);      // gradients are 0 for dummy elements
-                                    const int vy = diff * (dxy[e] >> 16);
+                                    if (e & 1) dpk[e >> 1] |= diff << 16; else dpk[e >> 1] = diff & 0xffff;
+                                    const int v0 = diff * (int)(short)(dxy[e] & 0xffff);      // gradients are 0 for dummy elements
+                                    const int v1 = diff * (dxy[e] >> 16);
                                     // |v| + acc in one VABSDIFF (|v| <= 2^28, 15 of them per lane: no overflow)
-                                    if (part) { sxt += vx; syt += vy; axt = __sad(vx, 0, axt); ayt = __sad(vy, 0, ayt); }
-                                    else { sxs += vx; sys += vy; axs = __sad(vx, 0, axs); ays = __sad(vy, 0, ays); }
+                                    if (part) { sxt += v0; syt += v1; axt = __sad(v0, 0, axt); ayt = __sad(v1, 0, ayt); }
+                                    else { s0s += v0; s1s += v1; a0s = __sad(v0, 0, a0s); a1s = __sad(v1, 0, a1s); }
+                                } else {
+                                    dv[e] = diff;
                                 }
                                 ptop = pbot;
+                            }
+                        }
+                    };
+                    // The faithful replay's addends, in chain order.  The pair sum of columns (x, x+4) is split by quantity:
+                    // the x lane (even cpos) keeps its vx and hands vy to its partner lane ^ 8 (x+4: same chain and row half,
+                    // so the same b_pos), which keeps vy and hands over vx -- with g_sel's packing, each lane keeps its low
+                    // product and hands over its high one.  Each lane forms one pair sum, the integer vx(x) + vx(x+4) or
+                    // vy(x) + vy(x+4) (the same in either order), and writes its float to its quantity's copy of the slot.
+                    auto stage_b = [&](auto resid) {
+#pragma unroll
+                        for (int k = 0; k < 11; k++) {
+                            const int d = resid(k);
+                            const int s = d * (int)(short)(dxy[k] & 0xffff) + __shfl_xor_sync(FULL, d * (dxy[k] >> 16), 8);
+                            if (k < nvalid_s) sm.chain[b_pos + k * 2] = (float)s;     // a dummy element's slot is another lane's
+                        }
+#pragma unroll
+                        for (int k = 0; k < 4; k++) {
+                            const int e = 11 + k;
+                            const int d = resid(e);
+                            if (k < tn) {
+                                sm.chain[t_pos + k * 5] = (float)(d * (int)(short)(dxy[e] & 0xffff));
+                                sm.chain[QSTRIDE + t_pos + k * 5] = (float)(d * (dxy[e] >> 16));
                             }
                         }
                     };
                     bool exact = false;
                     if (force_replay) {
                         residual_pass(BoolC<false>{});
+                        stage_b([&](int e) { return dv[e]; });
                     } else {
                         residual_pass(BoolC<true>{});
                         // per-chain totals (exact integers) and per-chain sums of |addend| (REDUX over the chain's lanes)
+                        const bool odd = cpos & 1;
+                        const unsigned axs = odd ? a1s : a0s, ays = odd ? a0s : a1s;
                         const unsigned cax = chain_sum_u(axs), cay = chain_sum_u(ays);
                         const unsigned tax = __reduce_add_sync(FULL, axt), tay = __reduce_add_sync(FULL, ayt);
                         // |pair sum| <= |v0| + |v1|, so the bound is conservative for the SIMD chains
                         exact = __all_sync(FULL, cax <= (1u << 24) && cay <= (1u << 24) && tax <= (1u << 24) && tay <= (1u << 24));
+                        if (!exact) stage_b([&](int e) { return (e & 1) ? (dpk[e >> 1] >> 16) : (int)(short)(dpk[e >> 1] & 0xffff); });
                     }
                     float ib1, ib2;
                     if (exact) {
                         // every partial sum of every chain is an exactly representable integer.
                         // chain c's total sits in lanes 2c (x) / 2c+1 (y): even lanes carry b1, odd lanes b2
+                        const int sxs = (cpos & 1) ? s1s : s0s, sys = (cpos & 1) ? s0s : s1s;
                         const float fx = (float)(int)chain_sum_u((unsigned)sxs), fy = (float)(int)chain_sum_u((unsigned)sys);
                         const float tx = (float)__reduce_add_sync(FULL, sxt), ty = (float)__reduce_add_sync(FULL, syt);
                         const float v = half ? fy : fx;
@@ -526,26 +562,7 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                         const float tot = __fadd_rn(half ? ty : tx, t2);
                         ib1 = __shfl_sync(FULL, tot, 0); ib2 = __shfl_sync(FULL, tot, 1);
                     } else {
-                        // faithful replay: float addends in chain order, runner lanes add them
-#pragma unroll
-                        for (int k = 0; k < 11; k++) {
-                            const int d = (k & 1) ? (dpk[k >> 1] >> 16) : (int)(short)(dpk[k >> 1] & 0xffff);
-                            const int vx = d * (int)(short)(dxy[k] & 0xffff), vy = d * (dxy[k] >> 16);
-                            const int px2 = vx + __shfl_down_sync(FULL, vx, 8), py2 = vy + __shfl_down_sync(FULL, vy, 8);   // + column x+4
-                            if (!(cpos & 1) && k < nvalid_s) {
-                                sm.chain[b_pos + k * 2] = (float)px2;
-                                sm.chain[QSTRIDE + b_pos + k * 2] = (float)py2;
-                            }
-                        }
-#pragma unroll
-                        for (int k = 0; k < 4; k++) {
-                            const int e = 11 + k;
-                            const int d = (e & 1) ? (dpk[e >> 1] >> 16) : (int)(short)(dpk[e >> 1] & 0xffff);
-                            if (k < tn) {
-                                sm.chain[t_pos + k * 5] = (float)(d * (int)(short)(dxy[e] & 0xffff));
-                                sm.chain[QSTRIDE + t_pos + k * 5] = (float)(d * (dxy[e] >> 16));
-                            }
-                        }
+                        // faithful replay: runner lanes add the staged addends
                         __syncwarp();
                         float acc = 0.f;
                         force_replay = true;
