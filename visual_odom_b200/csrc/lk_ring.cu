@@ -33,14 +33,14 @@
 // + a funnel shift), serve as the bottom taps of one pixel and the top taps of the next, and feed
 // the fixed-point bilinear interpolation as packed operands of dp2a.
 //
-// Summation (who adds): all addends are integers, so when the sum of |addend| over every chain is
-// <= 2^24 each partial sum is exact and the chain totals are integer warp reductions (REDUX) --
+// Summation (who adds): all addends are integers, so when sum |product| + |total| of every chain is
+// <= 2^25 each partial sum is exact and the chain totals are integer warp reductions (REDUX) --
 // the fast path.  Otherwise the float addends are written to shared memory in chain order and one
 // RUNNER lane per (quantity, chain) adds them strictly in order with 128-bit loads.  The A sums
 // always take the faithful path (they pass 2^24 on any corner-like texture).
 //
 // Shared memory is re-used over a level's life: the derivative window is dead once the patch is extracted and then
-// holds A22's chain slots; the packed I patch and the packed residuals stay in registers.  WarpSmem keeps the 8960 B
+// holds A22's chain slots; the I patch and the packed residuals stay in registers.  WarpSmem keeps the 8960 B
 // layout that lets 24 warps fit per SM: shrinking it would move every shared-memory address, a change to be measured
 // on its own.
 #include "common.cuh"
@@ -127,7 +127,7 @@ __device__ __forceinline__ void fence_proxy_async()
 #define A22_OFF 8               // words into dwin
 struct __align__(128) WarpSmem {
     uint8_t jtile[TW * J_ROWS];             // next-image tile                                             1536
-    uint8_t iwin[TW * I_ROWS + 96];         // previous-image window; afterwards the packed I patch       1152
+    uint8_t iwin[TW * I_ROWS + 96];         // previous-image window                                       1152
     uint32_t dwin[DW * I_ROWS + 24];        // derivative window; then A22 chain slots; then residuals    2560
     float chain[2 * QSTRIDE];               // chain-ordered float addends of two quantities              3616
     uint64_t bar;                           // mbarrier for TMA completion
@@ -252,9 +252,7 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
     //                   pair, its partner lane ^ 8 (col + 4, same chain and row half) b2's, in the second quantity
     const int a_pos = chain * SLOT_S + r0 * 4 + cpos;
     const int b_pos = (cpos & 1) * QSTRIDE + chain * SLOT_S + r0 * 2 + (cpos >> 1);
-    // a strip element's packed gradients: (Ix, Iy) in an even-cpos lane, (Iy, Ix) in an odd one -- low half first, so that
-    // the low product is the one a lane keeps for its own pair sum and the high one the one it hands its partner
-    const unsigned g_sel = (cpos & 1) ? 0x1054 : 0x5410;
+    const bool odd = cpos & 1;
     const int t_pos = TAIL_OFF + tr0 * 5 + (tcol - 16);
     // runner lane L sums slot (quantity L/5, chain L%5)
     const int rq = lane / 5, rc = lane - rq * 5;
@@ -371,8 +369,12 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                 if (USE_TMA) { mbar_wait(&sm.bar, phase); phase ^= 1; }
 
                 // ---- patch extraction: I (x32), Ix, Iy of the strip elements; A addends in chain order ----
-                int dxy[15];          // lo16 = Ix, hi16 = Iy; swapped in the strip elements of odd-cpos lanes (g_sel)
-                int Ipk[8];           // int16 patch intensities, two per register: strip 0..10, tail 11..14
+                // a strip element's gradients as the Newton loop consumes them: the kept one (Ix in an even-cpos lane, Iy in an odd
+                // one) and the one handed to the partner lane; a tail element's in order (Ix, Iy)
+                int gk[15], gh[15];
+                // the patch intensities I (x32) folded into the rounding constant of J's interpolation: (X + 2^8) >> 9 - I is
+                // (X + 2^8 - I * 2^9) >> 9, as I * 2^9 is a multiple of 2^9; strip elements 0..10, tail 11..14
+                int Ic[15];
                 float A11, A12, A22;
                 {
                     float a22v[15];       // A22 addends: their slots alias the derivative window, stored after the extraction
@@ -386,21 +388,26 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                         const int ish = 8 * (ioff & 3);
                         const uint32_t* dw = sm.dwin + row0 * DW + odx + c0;
                         unsigned ptop = __funnelshift_r(iw[0], iw[1], ish);
-                        unsigned d00 = dw[0], d01 = dw[1];
+                        // the top row's half of the derivative interpolation, rounding constant included; the next element's top
+                        // row is this element's bottom row
+                        int tx = (int)(short)(dw[0] & 0xffff) * w00 + (int)(short)(dw[1] & 0xffff) * w01 + (1 << (W_BITS - 1));
+                        int ty = ((int)dw[0] >> 16) * w00 + ((int)dw[1] >> 16) * w01 + (1 << (W_BITS - 1));
 #pragma unroll
                         for (int k = 0; k < ne; k++) {
                             // a dummy element (k >= nvalid) reads rows that exist (<= row 21 of the windows) and is zeroed
                             const unsigned pbot = __funnelshift_r(iw[(k + 1) * TWW], iw[(k + 1) * TWW + 1], ish);
                             const unsigned d10 = dw[(k + 1) * DW], d11 = dw[(k + 1) * DW + 1];
                             const int ival = (dp2a_taps(wb, pbot, dp2a_taps(wt, ptop, 1 << (W_BITS - 6))) >> (W_BITS - 5));
-                            int ix = ((int)(short)(d00 & 0xffff) * w00 + (int)(short)(d01 & 0xffff) * w01 +
-                                      (int)(short)(d10 & 0xffff) * w10 + (int)(short)(d11 & 0xffff) * w11 + (1 << (W_BITS - 1))) >> W_BITS;
-                            int iy = (((int)d00 >> 16) * w00 + ((int)d01 >> 16) * w01 +
-                                      ((int)d10 >> 16) * w10 + ((int)d11 >> 16) * w11 + (1 << (W_BITS - 1))) >> W_BITS;
+                            const int x0 = (int)(short)(d10 & 0xffff), x1 = (int)(short)(d11 & 0xffff), y0 = (int)d10 >> 16, y1 = (int)d11 >> 16;
+                            int ix = (tx + x0 * w10 + x1 * w11) >> W_BITS;
+                            int iy = (ty + y0 * w10 + y1 * w11) >> W_BITS;
+                            tx = x0 * w00 + x1 * w01 + (1 << (W_BITS - 1));
+                            ty = y0 * w00 + y1 * w01 + (1 << (W_BITS - 1));
                             if (k >= nvalid) { ix = 0; iy = 0; }
                             const int e = part ? 11 + k : k;
-                            if (e & 1) Ipk[e >> 1] |= ival << 16; else Ipk[e >> 1] = ival & 0xffff;
-                            dxy[e] = __byte_perm(ix, iy, part ? 0x5410 : g_sel);
+                            Ic[e] = (1 << (W_BITS - 6)) - (ival << (W_BITS - 5));
+                            gk[e] = part || !odd ? ix : iy;
+                            gh[e] = part || !odd ? iy : ix;
                             const float fx = (float)ix, fy = (float)iy;
                             const int pos = part ? t_pos + k * 5 : a_pos + k * 4;
                             // a dummy element's position belongs to another lane: no store
@@ -409,7 +416,7 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                                 sm.chain[QSTRIDE + pos] = __fmul_rn(fx, fy);
                             }
                             a22v[e] = __fmul_rn(fy, fy);
-                            ptop = pbot; d00 = d10; d01 = d11;
+                            ptop = pbot;
                         }
                     }
                     __syncwarp();                   // every lane has read its I / dI windows
@@ -496,12 +503,11 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                             for (int k = 0; k < ne; k++) {
                                 const unsigned pbot = __funnelshift_r(jw[(k + 1) * TWW], jw[(k + 1) * TWW + 1], jsh);
                                 const int e = part ? 11 + k : k;
-                                const int Iv = (e & 1) ? (Ipk[e >> 1] >> 16) : (int)(short)(Ipk[e >> 1] & 0xffff);
-                                const int diff = (dp2a_taps(wb, pbot, dp2a_taps(wt, ptop, 1 << (W_BITS - 6))) >> (W_BITS - 5)) - Iv;
+                                const int diff = dp2a_taps(wb, pbot, dp2a_taps(wt, ptop, Ic[e])) >> (W_BITS - 5);
                                 if (WITH_SUMS) {
                                     if (e & 1) dpk[e >> 1] |= diff << 16; else dpk[e >> 1] = diff & 0xffff;
-                                    const int v0 = diff * (int)(short)(dxy[e] & 0xffff);      // gradients are 0 for dummy elements
-                                    const int v1 = diff * (dxy[e] >> 16);
+                                    const int v0 = diff * gk[e];      // gradients are 0 for dummy elements
+                                    const int v1 = diff * gh[e];
                                     // |v| + acc in one VABSDIFF (|v| <= 2^28, 15 of them per lane: no overflow)
                                     if (part) { sxt += v0; syt += v1; axt = __sad(v0, 0, axt); ayt = __sad(v1, 0, ayt); }
                                     else { s0s += v0; s1s += v1; a0s = __sad(v0, 0, a0s); a1s = __sad(v1, 0, a1s); }
@@ -514,14 +520,14 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                     };
                     // The faithful replay's addends, in chain order.  The pair sum of columns (x, x+4) is split by quantity:
                     // the x lane (even cpos) keeps its vx and hands vy to its partner lane ^ 8 (x+4: same chain and row half,
-                    // so the same b_pos), which keeps vy and hands over vx -- with g_sel's packing, each lane keeps its low
-                    // product and hands over its high one.  Each lane forms one pair sum, the integer vx(x) + vx(x+4) or
+                    // so the same b_pos), which keeps vy and hands over vx -- each lane keeps its gk product and hands
+                    // over its gh one.  Each lane forms one pair sum, the integer vx(x) + vx(x+4) or
                     // vy(x) + vy(x+4) (the same in either order), and writes its float to its quantity's copy of the slot.
                     auto stage_b = [&](auto resid) {
 #pragma unroll
                         for (int k = 0; k < 11; k++) {
                             const int d = resid(k);
-                            const int s = d * (int)(short)(dxy[k] & 0xffff) + __shfl_xor_sync(FULL, d * (dxy[k] >> 16), 8);
+                            const int s = d * gk[k] + __shfl_xor_sync(FULL, d * gh[k], 8);
                             if (k < nvalid_s) sm.chain[b_pos + k * 2] = (float)s;     // a dummy element's slot is another lane's
                         }
 #pragma unroll
@@ -529,33 +535,36 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                             const int e = 11 + k;
                             const int d = resid(e);
                             if (k < tn) {
-                                sm.chain[t_pos + k * 5] = (float)(d * (int)(short)(dxy[e] & 0xffff));
-                                sm.chain[QSTRIDE + t_pos + k * 5] = (float)(d * (dxy[e] >> 16));
+                                sm.chain[t_pos + k * 5] = (float)(d * gk[e]);
+                                sm.chain[QSTRIDE + t_pos + k * 5] = (float)(d * gh[e]);
                             }
                         }
                     };
                     bool exact = false;
+                    int csx, csy, ctx, cty;           // the chain totals, formed by the full pass
                     if (force_replay) {
                         residual_pass(BoolC<false>{});
                         stage_b([&](int e) { return dv[e]; });
                     } else {
                         residual_pass(BoolC<true>{});
                         // per-chain totals (exact integers) and per-chain sums of |addend| (REDUX over the chain's lanes)
-                        const bool odd = cpos & 1;
                         const unsigned axs = odd ? a1s : a0s, ays = odd ? a0s : a1s;
                         const unsigned cax = chain_sum_u(axs), cay = chain_sum_u(ays);
                         const unsigned tax = __reduce_add_sync(FULL, axt), tay = __reduce_add_sync(FULL, ayt);
-                        // |pair sum| <= |v0| + |v1|, so the bound is conservative for the SIMD chains
-                        exact = __all_sync(FULL, cax <= (1u << 24) && cay <= (1u << 24) && tax <= (1u << 24) && tay <= (1u << 24));
+                        csx = (int)chain_sum_u((unsigned)(odd ? s1s : s0s)); csy = (int)chain_sum_u((unsigned)(odd ? s0s : s1s));
+                        ctx = __reduce_add_sync(FULL, sxt); cty = __reduce_add_sync(FULL, syt);
+                        // A chain's prefix sums lie in [-N, P], P and N the sums of its positive and of its negative products (a
+                        // SIMD chain's addends are pair sums of them), and max(P, N) = (sum |product| + |total|) / 2.  Every prefix
+                        // is exact when that is <= 2^24.  The first comparison keeps the sum from wrapping (|total| <= sum |product|).
+                        auto fits = [](unsigned a, int t) { return a <= (1u << 25) && a + (unsigned)abs(t) <= (1u << 25); };
+                        exact = __all_sync(FULL, fits(cax, csx) && fits(cay, csy) && fits(tax, ctx) && fits(tay, cty));
                         if (!exact) stage_b([&](int e) { return (e & 1) ? (dpk[e >> 1] >> 16) : (int)(short)(dpk[e >> 1] & 0xffff); });
                     }
                     float ib1, ib2;
                     if (exact) {
                         // every partial sum of every chain is an exactly representable integer.
                         // chain c's total sits in lanes 2c (x) / 2c+1 (y): even lanes carry b1, odd lanes b2
-                        const int sxs = (cpos & 1) ? s1s : s0s, sys = (cpos & 1) ? s0s : s1s;
-                        const float fx = (float)(int)chain_sum_u((unsigned)sxs), fy = (float)(int)chain_sum_u((unsigned)sys);
-                        const float tx = (float)__reduce_add_sync(FULL, sxt), ty = (float)__reduce_add_sync(FULL, syt);
+                        const float fx = (float)csx, fy = (float)csy, tx = (float)ctx, ty = (float)cty;
                         const float v = half ? fy : fx;
                         const float t1 = __fadd_rn(v, __shfl_down_sync(FULL, v, 4));      // lanes 0/1: c0 + c2, lanes 2/3: c1 + c3
                         const float t2 = __fadd_rn(t1, __shfl_down_sync(FULL, t1, 2));    // lanes 0/1: (c0 + c2) + (c1 + c3)
@@ -631,8 +640,7 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                             for (int k = 0; k < ne; k++) {
                                 const unsigned pbot = __funnelshift_r(jw[(k + 1) * TWW], jw[(k + 1) * TWW + 1], jsh);
                                 const int e = part ? 11 + k : k;
-                                const int Iv = (e & 1) ? (Ipk[e >> 1] >> 16) : (int)(short)(Ipk[e >> 1] & 0xffff);
-                                const int diff = (dp2a_taps(wb, pbot, dp2a_taps(wt, ptop, 1 << (W_BITS - 6))) >> (W_BITS - 5)) - Iv;
+                                const int diff = dp2a_taps(wb, pbot, dp2a_taps(wt, ptop, Ic[e])) >> (W_BITS - 5);
                                 if (k < nvalid) s += abs(diff);
                                 ptop = pbot;
                             }
