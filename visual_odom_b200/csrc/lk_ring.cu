@@ -19,8 +19,15 @@
 // shared memory: the 48x22 u8 window of the previous image, the 28x22 s16x2 window of its Scharr derivative,
 // and a 48x32 u8 tile of the next image around the current estimate (re-issued only if the 22x22 search
 // window drifts out of the tile).  The planes are physically padded (see common.cuh), so no box ever needs
-// border handling.  The u8 windows are used where TMA writes them (row pitch 48 B): the work mapping below
-// is chosen so that the rows a warp reads in one LDS fall into different banks at that pitch.
+// border handling.  The I window is used where TMA writes it (row pitch 48 B): the work mapping below is chosen
+// so that the rows a warp reads in one LDS fall into different banks at that pitch.  The Newton loop reads the
+// J tile as PAIRS: each time a tile is in place the warp expands it once into halfword (r, x) = p[r][x] |
+// p[r][x+1] << 8, in the I and derivative windows (dead by then), so a residual element's two taps of a row are
+// one LDS.U16.  The pair tile's pitch of 54 halfwords (27 words) is the one pitch in 47..58 at which no LDS.U16
+// of the loop has a bank conflict, for every window origin in the tile (strip halves 10 rows apart land 14
+// banks apart; the tail segments' starts 0,3,7,10,14,17 differ by 3,4,7,10,11,14,17 rows = 17,12,29,14,9,26,11
+// banks, and a tail segment spans <= 3 words).  At 48 halfwords rows 4 apart share their banks, and any six tail
+// segment starts have two of them 4k apart.
 //
 // Summation chains: OpenCV accumulates A11/A12/A22 and b1/b2 in float32 with 4 SIMD lanes over
 // columns 0..15 (lane = x & 3) and a scalar tail over columns 16..20, rows outermost.  The 441
@@ -29,9 +36,10 @@
 //
 // Work mapping (who computes which pixel): COLUMN STRIPS.  Lane L owns window column L>>1, rows
 // 0..9 (L even) or 10..20 (L odd), plus 3 or 4 rows of one tail column (lanes 0..29).  A strip
-// walks down its column, so the two byte taps of a row are fetched once (two aligned 32-bit loads
-// + a funnel shift), serve as the bottom taps of one pixel and the top taps of the next, and feed
-// the fixed-point bilinear interpolation as packed operands of dp2a.
+// walks down its column, so the two byte taps of a row are fetched once (one LDS.U16 of the pair
+// tile in the Newton loop; two aligned 32-bit loads + a funnel shift from the u8 windows elsewhere),
+// serve as the bottom taps of one pixel and the top taps of the next, and feed the fixed-point
+// bilinear interpolation as packed operands of dp2a.
 //
 // Summation (who adds): all addends are integers, so when sum |product| + |total| of every chain is
 // <= 2^25 each partial sum is exact and the chain totals are integer warp reductions (REDUX) --
@@ -40,11 +48,13 @@
 // always take the faithful path (they pass 2^24 on any corner-like texture).
 //
 // Shared memory is re-used over a level's life: the derivative window is dead once the patch is extracted and then
-// holds A22's chain slots; the I patch and the packed residuals stay in registers.  WarpSmem keeps the 8960 B
+// holds A22's chain slots; once A is summed the I and derivative windows hold the J pair tile; the I patch and the
+// packed residuals stay in registers.  WarpSmem keeps the 8960 B
 // layout that lets 24 warps fit per SM: shrinking it would move every shared-memory address, a change to be measured
 // on its own.
 #include "common.cuh"
 #include "lk_ring.h"
+#include <stddef.h>
 
 #define FULL 0xffffffffu
 #define W_BITS 14
@@ -140,6 +150,12 @@ struct __align__(128) WarpSmem {
 };
 static_assert(sizeof(WarpSmem) == 8960, "WarpSmem layout");
 static_assert(A22_OFF + QSTRIDE <= DW * I_ROWS + 24, "A22 slots must fit the derivative window");
+// the J pair tile (see the header): J_ROWS rows of PP halfwords over the I and derivative windows.  A window origin
+// has rx <= TW - 22 and its last column is 20, so positions 0..TW - 2 are read.
+#define PP 54
+static_assert(offsetof(WarpSmem, dwin) == offsetof(WarpSmem, iwin) + sizeof(WarpSmem::iwin), "iwin, dwin contiguous");
+static_assert(J_ROWS * PP * 2 <= sizeof(WarpSmem::iwin) + sizeof(WarpSmem::dwin), "pair tile must fit iwin + dwin");
+static_assert(PP >= TW - 1 && PP % 2 == 0, "pair tile pitch");
 
 #define I_BYTES (TW * I_ROWS)
 #define J_BYTES (TW * J_ROWS)
@@ -159,6 +175,23 @@ __device__ __forceinline__ void ldg_box_u32(uint32_t* dst, const uint32_t* plane
     const uint32_t* src = plane + (size_t)y * pitch + x;
     if (lane < DW)
         for (int r = 0; r < I_ROWS; r++) dst[r * DW + lane] = __ldg(src + (size_t)r * pitch + lane);
+}
+
+// the pair tile of the J tile in place: lane r expands row r (three 128-bit loads, one PRMT and one store per output
+// word).  Halfword TW - 1 pairs the last byte with 0 and is never read.
+__device__ __forceinline__ void expand_pairs(const uint8_t* jtile, uint16_t* pairs, int lane)
+{
+    static_assert(J_ROWS == 32 && TW == 48, "one tile row of 12 words per lane");
+    const uint4* src = reinterpret_cast<const uint4*>(jtile + lane * TW);
+    uint32_t* dst = reinterpret_cast<uint32_t*>(pairs + lane * PP);
+    const uint4 q0 = src[0], q1 = src[1], q2 = src[2];
+    const uint32_t w[13] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w, 0u};
+#pragma unroll
+    for (int i = 0; i < 12; i++) {
+        dst[2 * i] = __byte_perm(w[i], 0u, 0x2110);             // (x, x+1), (x+1, x+2) for x = 4i
+        dst[2 * i + 1] = __byte_perm(w[i], w[i + 1], 0x4332);   // (x+2, x+3), (x+3, x+4)
+    }
+    __syncwarp();                           // the Newton loop reads other lanes' rows
 }
 
 __device__ __forceinline__ void bilinear_weights(float a, float b, int& w00, int& w01, int& w10, int& w11)
@@ -259,6 +292,7 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
     const int run_off = rc < 4 ? rc * SLOT_S : TAIL_OFF;
     const float* const run_slot = (rq < 2 ? sm.chain + rq * QSTRIDE : reinterpret_cast<const float*>(sm.dwin) + A22_OFF) + run_off;
     float* const a22 = reinterpret_cast<float*>(sm.dwin) + A22_OFF;
+    uint16_t* const pairs = reinterpret_cast<uint16_t*>(sm.iwin);
 
     if (USE_TMA) {
         if (lane == 0) {
@@ -346,6 +380,8 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                 const int ibx = (ipx + VO_PAD) & ~15, iby = ipy + VO_PAD;       // u8 window of I
                 const int dbx = (ipx + VO_PAD) & ~3;                            // derivative window (4 elements = 16 B)
                 int jbx = (inx - 5 + VO_PAD) & ~15, jby = iny - 5 + VO_PAD;     // tile of J
+                // every lane is done with the previous level-solve's generic accesses of the windows (A22's chain slots
+                // and the pair tile in iwin / dwin, the J tile), and lane 0's proxy fence orders them before the TMA writes
                 __syncwarp();
                 if (USE_TMA) {
                     if (lane == 0) {
@@ -444,10 +480,12 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                     }
                 }
                 D = __fdiv_rn(1.f, D);
+                // the windows are dead (the runner's reads of A22's slots precede the __syncwarp above)
+                if (j_ok0) expand_pairs(sm.jtile, pairs, lane);
 
                 // ---- Newton iterations ------------------------------------------------------------
                 float pdx = 0.f, pdy = 0.f;
-                bool tile_valid = j_ok0;
+                bool tile_valid = j_ok0;            // the J tile, and so its pair tile, holds this level's window
                 bool force_replay = false;          // set by the first faithful replay of this level-solve
                 // in registers for the Newton loop, whose shared-memory stores would otherwise make every iteration reload them
                 const int max_iters = sm.max_iters;
@@ -474,6 +512,7 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                             ldg_box_u8(sm.jtile, args.img_base[level] + args.plane[level] * img_next, args.pitch[level], jbx, jby, J_ROWS, lane);
                             __syncwarp();
                         }
+                        expand_pairs(sm.jtile, pairs, lane);
                         tile_valid = true;
                     }
                     a = npx - (float)inx; b = npy - (float)iny;
@@ -495,13 +534,11 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
 #pragma unroll
                         for (int part = 0; part < 2; part++) {
                             const int c0 = part ? tcol : col, row0 = part ? tr0 : r0, ne = part ? 4 : 11;
-                            const int joff = (ry + row0) * TW + rx + c0;
-                            const uint32_t* jw = reinterpret_cast<const uint32_t*>(sm.jtile) + (joff >> 2);
-                            const int jsh = 8 * (joff & 3);
-                            unsigned ptop = __funnelshift_r(jw[0], jw[1], jsh);
+                            const uint16_t* jp = pairs + (ry + row0) * PP + rx + c0;
+                            unsigned ptop = jp[0];
 #pragma unroll
                             for (int k = 0; k < ne; k++) {
-                                const unsigned pbot = __funnelshift_r(jw[(k + 1) * TWW], jw[(k + 1) * TWW + 1], jsh);
+                                const unsigned pbot = jp[(k + 1) * PP];
                                 const int e = part ? 11 + k : k;
                                 const int diff = dp2a_taps(wb, pbot, dp2a_taps(wt, ptop, Ic[e])) >> (W_BITS - 5);
                                 if (WITH_SUMS) {
