@@ -80,22 +80,6 @@ static bool range_mono(const vo_ctx* ctx, int u0, int n)
     return false;
 }
 
-// the mono_rotation problems of units [u0, u0 + n) (one each): pointsLeft_t0 / pointsLeft_t1 = the filtered L0 / L1 lists
-// (d_valid4 planes 0, 2), scratch block u for unit u (laid out for max_features points), the count of d_batch_mono, the
-// camera of the unit's own P_l.  bound (the range's feature bound) sizes the per-point grids.
-static void batch_ess_args(const vo_ctx* ctx, int u0, int n, int bound, EssArgs& a)
-{
-    memset(&a, 0, sizeof(a));
-    const size_t uo = (size_t)u0 * ctx->cap, cs = (size_t)ctx->units * ctx->cap;
-    vo_ess_bind(a, (uint8_t*)ctx->d_batch_ess + (size_t)u0 * ctx->batch_ess_bytes, ctx->cap, VO_ESS_ITERS);
-    a.n_max = bound;
-    a.n = ctx->d_batch_mono + ctx->batch_ess_units + u0;
-    a.cal = ctx->d_cal + u0;
-    a.pts0 = ctx->d_valid4 + uo; a.pts1 = ctx->d_valid4 + 2 * cs + uo;
-    a.n_prob = n;
-    a.scratch_stride = a.result_stride = ctx->batch_ess_bytes; a.pts_stride = ctx->cap; a.n_stride = 1; a.cal_stride = 1;
-}
-
 // largest feature bound of the slots [u0, u0 + n): the LK launch of that range has no unit with more live features
 static int range_bound(const vo_ctx* ctx, int u0, int n)
 {
@@ -220,19 +204,13 @@ extern "C" int vo_batch_mono_rotation(vo_ctx* ctx, int first_unit, int n_units, 
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
     int rc = vo_claim_buffers(ctx, "vo_batch_mono_rotation");
     if (rc) return rc;
-    if (!ctx->batch_mono_stream) {
-        VO_CUDA_CHECK(cudaStreamCreateWithFlags(&ctx->batch_mono_stream, cudaStreamNonBlocking));
-        for (int k = 0; k < 2; k++) VO_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->batch_mono_ev[k], cudaEventDisableTiming));
-    }
-    if (!ctx->d_batch_ess || ctx->batch_ess_units < ctx->batch_units) {
-        const size_t bytes = (vo_ess_scratch_bytes(ctx->cap, VO_ESS_ITERS) + 255) / 256 * 256;
-        const size_t table = ((size_t)2 * ctx->batch_units * sizeof(int) + 255) / 256 * 256;
-        void* q = nullptr;
-        VO_CUDA_CHECK(cudaMalloc(&q, table + (size_t)ctx->batch_units * bytes));
-        vo_drop_graphs(ctx);                    // captured graphs hold the old blocks
-        if (ctx->d_batch_mono) { VO_CUDA_CHECK(cudaDeviceSynchronize()); cudaFree(ctx->d_batch_mono); }      // the allocation's base
-        ctx->d_batch_ess = (uint8_t*)q + table; ctx->d_batch_mono = (int*)q;
-        ctx->batch_ess_bytes = bytes; ctx->batch_ess_units = ctx->batch_units;
+    if ((rc = vo_ensure_unit_ess(ctx, ctx->batch_units))) return rc;
+    if (ctx->batch_mono_cap < ctx->batch_units) {
+        int* q = nullptr;
+        VO_CUDA_CHECK(cudaMalloc(&q, 2 * (size_t)ctx->batch_units * sizeof(int)));
+        vo_drop_graphs(ctx);                    // captured graphs hold the old table
+        if (ctx->d_batch_mono) { VO_CUDA_CHECK(cudaDeviceSynchronize()); cudaFree(ctx->d_batch_mono); }
+        ctx->d_batch_mono = q; ctx->batch_mono_cap = ctx->batch_units;
     }
     for (int i = 0; i < n_units; i++) ctx->batch_mono[first_unit + i] = on && on[i] ? 1 : 0;
     if (range_mono(ctx, 0, ctx->batch_units)) ctx->batch_mono_used = true;
@@ -383,8 +361,8 @@ static int run_range_launch(vo_ctx* ctx, const View& v)
     View pre = v, lk = v, post = v;              // FAST + pyramids / the LK ring / the kernels after the ring
     cudaEvent_t* ev = nullptr;
     // the five-point kernels of the mono_rotation branch, forked from post after the filters and joined before the fold
-    cudaStream_t mono_s = ctx->batch_mono_stream;
-    cudaEvent_t mono_ev[2] = {ctx->batch_mono_ev[0], ctx->batch_mono_ev[1]};
+    cudaStream_t mono_s = ctx->mono_stream;
+    cudaEvent_t mono_ev[2] = {ctx->mono_ev[0], ctx->mono_ev[1]};
     for (auto& L : ctx->lane)
         if (L.side && v.s == L.side) {
             if ((rc = ensure_helpers(ctx))) return rc;
@@ -412,10 +390,10 @@ static int run_range_launch(vo_ctx* ctx, const View& v)
     if ((rc = vo_run_filter(ctx, post, false, ctx->d_par))) return rc;
     EssArgs e;
     if (mono) {     // findEssentialMat + recoverPose on (L0, L1) of the units switched on, beside triangulation and PnP
-        batch_ess_args(ctx, v.u0, v.n, v.max_pts, e);
+        int* count = ctx->d_batch_mono + ctx->batch_mono_cap + v.u0;
+        e = vo_unit_ess_args(ctx, v.u0, v.n, v.max_pts, count);
         VO_CUDA_CHECK(cudaEventRecord(mono_ev[0], post.s));
         VO_CUDA_CHECK(cudaStreamWaitEvent(mono_s, mono_ev[0], 0));
-        int* count = ctx->d_batch_mono + ctx->batch_ess_units + v.u0;
         k_batch_mono_n<<<(v.n + 63) / 64, 64, 0, mono_s>>>(count, ctx->d_batch_mono + v.u0, ctx->d_n5 + v.u0, v.n);
         ctx->launches += 1 + vo_launch_essential(e, mono_s);
         VO_CUDA_CHECK(cudaGetLastError());
@@ -634,18 +612,16 @@ static int batch_submit(vo_ctx* ctx, const char* who, const Unit* units, int fir
     vo_unit_result_dev* h_res = pinned_results(ctx);
     VO_CUDA_CHECK(cudaMemcpyAsync(h_res + first_unit, ctx->d_results + first_unit, (size_t)n_units * sizeof(vo_unit_result_dev), cudaMemcpyDeviceToHost, st));
     const bool mono = range_mono(ctx, first_unit, n_units);
-    EssArgs e;
-    if (mono) {                                  // the branch's results for vo_batch_wait_mono: one strided copy
-        batch_ess_args(ctx, first_unit, n_units, max_pts, e);
-        VO_CUDA_CHECK(cudaMemcpy2DAsync(pinned_ess(ctx) + first_unit, sizeof(EssResult), e.result, e.result_stride, sizeof(EssResult),
-                                        n_units, cudaMemcpyDeviceToHost, st));
-    }
+    // the branch's results for vo_batch_wait_mono
+    if (mono && (rc = vo_copy_unit_ess(ctx, pinned_ess(ctx) + first_unit, first_unit, n_units, st))) return rc;
     if (ctx->batch_outputs) {                    // the point lists of the submission: one packed block, one copy
         const size_t cs = (size_t)ctx->units * ctx->cap, ub = (size_t)first_unit * ctx->cap;
+        EssArgs e;
+        if (mono) e = vo_unit_ess_args(ctx, first_unit, n_units, ctx->cap, nullptr);
         k_pack_outputs<<<n_units, 256, 0, st>>>(ctx->d_out + (size_t)first_unit * ctx->out_stride, ctx->out_stride, ctx->out_per,
                                                ctx->d_valid4 + ub, cs, ctx->d_idx5 + ub, ctx->d_X + ub, ctx->d_inliers + ub,
                                                ctx->d_n5 + first_unit, ctx->d_results + first_unit, ctx->cap,
-                                               mono ? e.mask : nullptr, ctx->batch_ess_bytes, ctx->d_batch_mono + first_unit);
+                                               mono ? e.mask : nullptr, ctx->unit_ess_bytes, ctx->d_batch_mono + first_unit);
         ctx->launches += 1;
         VO_CUDA_CHECK(cudaGetLastError());
         VO_CUDA_CHECK(cudaMemcpyAsync(ctx->h_out + (size_t)first_unit * ctx->out_stride, ctx->d_out + (size_t)first_unit * ctx->out_stride,
@@ -667,14 +643,11 @@ extern "C" int vo_batch_submit_device(vo_ctx* ctx, const vo_dunit* units, int fi
 }
 
 // vo_mono_result of a unit whose last run had the branch on (status as vo_seq_wait_mono reports it), zeroed otherwise
-static void mono_result(const vo_ctx* ctx, int unit, const EssResult& ess, vo_mono_result* m)
+static vo_mono_result mono_result(const vo_ctx* ctx, int unit, const EssResult& ess)
 {
-    memset(m, 0, sizeof(*m));
-    if (!ctx->batch_mono_ran[unit]) return;
-    m->status = ess.status == ESS_OK ? VO_OK : VO_E_TOO_FEW_POINTS;
-    m->n_inliers = ess.n_inliers; m->ransac_iters = ess.iters; m->n_good = ess.n_good;
-    for (int k = 0; k < 9; k++) m->R[k] = ess.R[k];
-    for (int k = 0; k < 3; k++) m->t[k] = ess.t[k];
+    vo_mono_result m;
+    memset(&m, 0, sizeof(m));
+    return ctx->batch_mono_ran[unit] ? vo_mono_from_ess(ess) : m;
 }
 
 static int batch_wait(vo_ctx* ctx, const char* who, int first_unit, int n_units, vo_unit_result* results, vo_mono_result* mono)
@@ -687,7 +660,7 @@ static int batch_wait(vo_ctx* ctx, const char* who, int first_unit, int n_units,
             VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, p.done, 0));     // later work on the caller's stream sees the results
             p.active = false;
             if (results) memcpy(results, pinned_results(ctx) + first_unit, (size_t)n_units * sizeof(vo_unit_result));
-            for (int i = 0; mono && i < n_units; i++) mono_result(ctx, first_unit + i, pinned_ess(ctx)[first_unit + i], &mono[i]);
+            for (int i = 0; mono && i < n_units; i++) mono[i] = mono_result(ctx, first_unit + i, pinned_ess(ctx)[first_unit + i]);
             return VO_OK;
         }
     vo_set_error(ctx, "%s: no pending submission for slots [%d, %d)", who, first_unit, first_unit + n_units);
@@ -735,34 +708,18 @@ extern "C" int vo_batch_wait_device(vo_ctx* ctx, int first_unit, int n_units, co
         return VO_E_INVALID;
     }
     if (!r) { vo_set_error(ctx, "%s: null result table", who); return VO_E_INVALID; }
-    const bool lists = r->pts4 || r->kept_idx || r->points3d || r->inliers || r->ess_mask;
-    if (r->pts_cap < 0 || (lists && r->pts_cap == 0)) {
-        vo_set_error(ctx, "%s: pts_cap = %d with point arrays", who, r->pts_cap);
-        return VO_E_INVALID;
-    }
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
-    const struct { const char* name; const void* p; } ptrs[] = {
-        {"records", r->records}, {"pts4", r->pts4}, {"kept_idx", r->kept_idx}, {"points3d", r->points3d},
-        {"inliers", r->inliers}, {"mono", r->mono}, {"ess_mask", r->ess_mask}};
-    int rc;
-    for (const auto& x : ptrs)
-        if ((rc = vo_check_dptr(ctx, who, x.name, x.p))) return rc;
-    static_assert(sizeof(vo_unit_result) == sizeof(vo_unit_result_dev), "k_seq_collect writes vo_unit_result records");
-    const size_t cs = (size_t)ctx->units * ctx->cap, uo = (size_t)first_unit * ctx->cap;
+    const bool mono = range_mono_ran(ctx, first_unit, n_units);
+    EssArgs e;
+    if (mono) e = vo_unit_ess_args(ctx, first_unit, n_units, ctx->cap, nullptr);
     CollectArgs a;
-    memset(&a, 0, sizeof(a));
+    int rc;
+    if ((rc = vo_collect_args(ctx, who, r, r->kept_idx != nullptr, first_unit, mono ? &e : nullptr, a)) ||
+        (rc = vo_check_dptr(ctx, who, "kept_idx", r->kept_idx)))
+        return rc;
     a.all_ran = true;
-    a.res = ctx->d_results + first_unit; a.cap = ctx->cap;
-    a.valid4 = ctx->d_valid4 + uo; a.plane_stride = cs;
-    a.X = ctx->d_X + uo; a.inliers = ctx->d_inliers + uo; a.idx5 = ctx->d_idx5 + uo;
-    if (range_mono_ran(ctx, first_unit, n_units)) {
-        EssArgs e;
-        batch_ess_args(ctx, first_unit, n_units, ctx->cap, e);
-        a.ess = e.result; a.ess_mask = e.mask; a.ess_stride = ctx->batch_ess_bytes; a.ess_on = ctx->d_batch_mono + first_unit;
-    }
-    a.records = (vo_unit_result_dev*)r->records; a.pts_cap = r->pts_cap;
-    a.pts4 = (float2*)r->pts4; a.kept_out = r->kept_idx; a.points3d = (float3*)r->points3d; a.inliers_out = r->inliers;
-    a.mono = r->mono; a.mask_out = r->ess_mask;
+    a.idx5 = ctx->d_idx5 + (size_t)first_unit * ctx->cap; a.kept_out = r->kept_idx;
+    if (mono) a.ess_on = ctx->d_batch_mono + first_unit;
     VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, p->done, 0));
     ctx->launches += vo_launch_seq_collect(a, n_units, ctx->stream);
     VO_CUDA_CHECK(cudaGetLastError());
@@ -802,10 +759,9 @@ extern "C" int vo_batch_fetch_mono(vo_ctx* ctx, int unit, vo_mono_result* mono, 
     if (rc) return rc;
     EssResult ess;
     memset(&ess, 0, sizeof(ess));
-    if (!ctx->batch_mono_ran[unit]) { mono_result(ctx, unit, ess, mono); return VO_OK; }
+    if (!ctx->batch_mono_ran[unit]) { *mono = mono_result(ctx, unit, ess); return VO_OK; }
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
-    EssArgs e;
-    batch_ess_args(ctx, unit, 1, ctx->cap, e);
+    const EssArgs e = vo_unit_ess_args(ctx, unit, 1, ctx->cap, nullptr);
     vo_unit_result_dev r;
     VO_CUDA_CHECK(cudaMemcpyAsync(&r, ctx->d_results + unit, sizeof(r), cudaMemcpyDeviceToHost, ctx->stream));
     VO_CUDA_CHECK(cudaMemcpyAsync(&ess, e.result, sizeof(ess), cudaMemcpyDeviceToHost, ctx->stream));
@@ -814,7 +770,7 @@ extern "C" int vo_batch_fetch_mono(vo_ctx* ctx, int unit, vo_mono_result* mono, 
         VO_CUDA_CHECK(cudaMemcpyAsync(ess_mask, e.mask, (size_t)std::min(r.n_valid, ctx->cap), cudaMemcpyDeviceToHost, ctx->stream));
         VO_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
     }
-    mono_result(ctx, unit, ess, mono);
+    *mono = mono_result(ctx, unit, ess);
     return VO_OK;
 }
 
@@ -851,7 +807,7 @@ extern "C" int vo_batch_outputs_mono(vo_ctx* ctx, int unit, vo_mono_result* mono
     if (unit >= ctx->out_units) { vo_set_error(ctx, "vo_batch_outputs_mono: unit %d outside the resident batch", unit); return VO_E_INVALID; }
     int rc = check_waited(ctx, "vo_batch_outputs_mono", unit);
     if (rc) return rc;
-    mono_result(ctx, unit, pinned_ess(ctx)[unit], mono);
+    *mono = mono_result(ctx, unit, pinned_ess(ctx)[unit]);
     if (ess_mask && ctx->batch_mono_ran[unit] && ctx->out_mask) {
         const int per = ctx->out_per, nv = std::min(pinned_results(ctx)[unit].n_valid, per);
         if (nv > 0) memcpy(ess_mask, packed_unit(ctx->h_out + (size_t)unit * ctx->out_stride, per).om, (size_t)nv);

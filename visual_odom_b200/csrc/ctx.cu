@@ -188,14 +188,12 @@ extern "C" void vo_destroy(vo_ctx* ctx)
     if (ctx->d_bgr) cudaFree(ctx->d_bgr);
     if (ctx->d_lk_queue) cudaFree(ctx->d_lk_queue);
     if (ctx->d_ess) cudaFree(ctx->d_ess);
-    if (ctx->d_seq_ess) cudaFree(ctx->d_seq_ess);
-    if (ctx->d_batch_mono) cudaFree(ctx->d_batch_mono);           // the base of d_batch_ess's allocation
-    for (int k = 0; k < 2; k++) if (ctx->batch_mono_ev[k]) cudaEventDestroy(ctx->batch_mono_ev[k]);
-    if (ctx->batch_mono_stream) cudaStreamDestroy(ctx->batch_mono_stream);
+    if (ctx->d_unit_ess) cudaFree(ctx->d_unit_ess);
+    if (ctx->d_batch_mono) cudaFree(ctx->d_batch_mono);
+    for (cudaEvent_t e : ctx->mono_ev) if (e) cudaEventDestroy(e);
+    if (ctx->mono_stream) cudaStreamDestroy(ctx->mono_stream);
     if (ctx->d_seq_pose) cudaFree(ctx->d_seq_pose);
     for (cudaEvent_t e : ctx->seq_tab_ev) if (e) cudaEventDestroy(e);
-    for (int k = 0; k < 2; k++) if (ctx->seq_mono_ev[k]) cudaEventDestroy(ctx->seq_mono_ev[k]);
-    if (ctx->seq_mono_stream) cudaStreamDestroy(ctx->seq_mono_stream);
     if (ctx->h_out) cudaFreeHost(ctx->h_out);
     if (ctx->own_stream) cudaStreamDestroy(ctx->own_stream);
     delete ctx;
@@ -461,6 +459,54 @@ int vo_ensure_lanes(vo_ctx* ctx)
         for (cudaEvent_t& e : L.ev) VO_CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     }
     return VO_OK;
+}
+
+int vo_ensure_unit_ess(vo_ctx* ctx, int n_units)
+{
+    if (!ctx->mono_stream) {
+        VO_CUDA_CHECK(cudaStreamCreateWithFlags(&ctx->mono_stream, cudaStreamNonBlocking));
+        for (cudaEvent_t& e : ctx->mono_ev) VO_CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    }
+    if (ctx->unit_ess_units >= n_units) return VO_OK;
+    vo_drop_graphs(ctx);                                      // captured graphs hold the old blocks
+    if (ctx->d_unit_ess) { VO_CUDA_CHECK(cudaDeviceSynchronize()); cudaFree(ctx->d_unit_ess); ctx->d_unit_ess = nullptr; ctx->unit_ess_units = 0; }
+    const size_t bytes = (vo_ess_scratch_bytes(ctx->cap, VO_ESS_ITERS) + 255) / 256 * 256;
+    VO_CUDA_CHECK(cudaMalloc(&ctx->d_unit_ess, (size_t)n_units * bytes));
+    ctx->unit_ess_bytes = bytes; ctx->unit_ess_units = n_units;
+    return VO_OK;
+}
+
+EssArgs vo_unit_ess_args(const vo_ctx* ctx, int u0, int n, int n_max, const int* count)
+{
+    EssArgs a;
+    memset(&a, 0, sizeof(a));
+    const size_t uo = (size_t)u0 * ctx->cap, cs = (size_t)ctx->units * ctx->cap;
+    vo_ess_bind(a, (uint8_t*)ctx->d_unit_ess + (size_t)u0 * ctx->unit_ess_bytes, ctx->cap, VO_ESS_ITERS);
+    a.n_max = n_max;
+    a.n = count;
+    a.cal = ctx->d_cal + u0;
+    a.pts0 = ctx->d_valid4 + uo; a.pts1 = ctx->d_valid4 + 2 * cs + uo;
+    a.n_prob = n;
+    a.scratch_stride = a.result_stride = ctx->unit_ess_bytes; a.pts_stride = ctx->cap; a.n_stride = 1; a.cal_stride = 1;
+    return a;
+}
+
+int vo_copy_unit_ess(vo_ctx* ctx, EssResult* dst, int u0, int n, cudaStream_t st)
+{
+    const EssArgs e = vo_unit_ess_args(ctx, u0, n, ctx->cap, nullptr);
+    VO_CUDA_CHECK(cudaMemcpy2DAsync(dst, sizeof(EssResult), e.result, e.result_stride, sizeof(EssResult), n, cudaMemcpyDeviceToHost, st));
+    return VO_OK;
+}
+
+vo_mono_result vo_mono_from_ess(const EssResult& e)
+{
+    vo_mono_result m;
+    memset(&m, 0, sizeof(m));
+    m.status = e.status == ESS_OK ? VO_OK : VO_E_TOO_FEW_POINTS;
+    m.n_inliers = e.n_inliers; m.ransac_iters = e.iters; m.n_good = e.n_good;
+    for (int k = 0; k < 9; k++) m.R[k] = e.R[k];
+    for (int k = 0; k < 3; k++) m.t[k] = e.t[k];
+    return m;
 }
 
 // entries [1 + u0, 1 + u0 + n) of a per-unit table (host copy `host`, device table `dev`)

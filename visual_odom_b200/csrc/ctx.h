@@ -136,7 +136,9 @@ struct vo_ctx {
     bool seq_dres = false;
     double* d_seq_pose = nullptr;
     cudaEvent_t seq_tab_ev[3] = {nullptr, nullptr, nullptr};
-    int seq_lk_bound = 0;               // the LK launch bound: the largest bucket grid of the run's sizes (raised by starts)
+    // the LK launch bound: the largest bucket grid of the run's sizes (raised by starts).  Also the mono branch's bound,
+    // which a mono run keeps from its begin call: seq_starts_fit refuses a start of that run above it.
+    int seq_lk_bound = 0;
     std::vector<CamCalib> seq_cal_next; // [2 * seq_n] calibration and parameter entries of started sequences that the
     std::vector<UnitParams> seq_par_next;   // frame in flight still reads: written by the next submission of that buffer
     std::vector<char> seq_cal_due;      // parity
@@ -170,16 +172,17 @@ struct vo_ctx {
     void* d_ess = nullptr;
     int ess_cap = 0;
     // the same branch inside the sequence mode (vo_set_option "mono_rotation" for vo_seq_begin*, the flag
-    // VO_MSEQ_MONO_ROTATION for vo_mseq_begin_ex): one scratch block per buffer unit (2 * seq_n: two frames in flight),
-    // separate from d_ess, allocated at the begin call; the front graph runs it for every sequence on seq_mono_stream
+    // VO_MSEQ_MONO_ROTATION for vo_mseq_begin_ex) and per batched unit (vo_batch_mono_rotation): one scratch block per
+    // buffer unit, laid out for max_features points and separate from d_ess (vo_ensure_unit_ess).  The two modes never use
+    // the buffer units at the same time, so they share the blocks.  A range on ctx->stream (the sequence mode's front
+    // stage, a batched range there) forks the branch to mono_stream by mono_ev; lane ranges use Lane::mono.
     bool mono_opt = false;              // the option; a vo_seq_* sequence takes it at vo_seq_begin
     bool seq_mono = false;              // the running sequences' value
-    void* d_seq_ess = nullptr;          // [seq_ess_units][seq_ess_bytes], block u = buffer unit u
-    size_t seq_ess_bytes = 0;
-    int seq_ess_cap = 0;                // points each block holds (the bucket grid, at most cap)
-    int seq_ess_units = 0;              // blocks allocated
-    cudaStream_t seq_mono_stream = nullptr;
-    cudaEvent_t seq_mono_ev[2] = {nullptr, nullptr};     // fork, join
+    void* d_unit_ess = nullptr;         // [unit_ess_units][unit_ess_bytes], block u = buffer unit u
+    size_t unit_ess_bytes = 0;
+    int unit_ess_units = 0;             // blocks allocated
+    cudaStream_t mono_stream = nullptr;
+    cudaEvent_t mono_ev[2] = {nullptr, nullptr};         // fork, join
     std::vector<void*> allocs;          // everything cudaMalloc'ed for the batch state
 
     // ---- pinned host staging ------------------------------------------------------------------
@@ -247,17 +250,13 @@ struct vo_ctx {
     // trackingFrame2Frame's mono_rotation branch per batched unit (vo_batch_mono_rotation): batch_mono[u] is unit u's switch,
     // mirrored in the device table d_batch_mono[u] that the kernels read (so a toggle never recaptures a graph);
     // batch_mono_ran[u] what the unit's last run did.  A range with no unit switched on launches what it did without the
-    // branch.  d_batch_ess: one five-point scratch block per configured unit, sized for max_features, allocated by
-    // vo_batch_mono_rotation (outside any capture); d_batch_mono[batch_ess_units + u] is unit u's count for the branch
-    // (its n_valid, 0 when it is off, which ends its problem at k_ess_init).
+    // branch.  The branch's scratch is the unit blocks (d_unit_ess), which vo_batch_mono_rotation grows to the configured
+    // units (outside any capture); d_batch_mono[batch_mono_cap + u] is unit u's count for the branch (its n_valid, 0 when
+    // it is off, which ends its problem at k_ess_init).
     std::vector<int> batch_mono, batch_mono_ran;
     bool batch_mono_used = false;   // a unit was switched on since vo_batch_configure (the packed outputs carry masks)
-    void* d_batch_ess = nullptr;    // [batch_ess_units][batch_ess_bytes]
-    int* d_batch_mono = nullptr;    // [2][batch_ess_units]: switch | count (the allocation's base, d_batch_ess after it)
-    size_t batch_ess_bytes = 0;
-    int batch_ess_units = 0;
-    cudaStream_t batch_mono_stream = nullptr;       // the fork of a range on ctx->stream (lanes use Lane::mono)
-    cudaEvent_t batch_mono_ev[2] = {nullptr, nullptr};
+    int* d_batch_mono = nullptr;    // [2][batch_mono_cap]: switch | count
+    int batch_mono_cap = 0;
 };
 
 void vo_set_error(vo_ctx* ctx, const char* fmt, ...);
@@ -308,6 +307,24 @@ int vo_refuse_pending_batches(vo_ctx* ctx, const char* who);
 int vo_sync_device_retired(vo_ctx* ctx);
 // VO_E_INVALID + message unless p is NULL or device (managed) memory of the context's GPU (seq_api.cu)
 int vo_check_dptr(vo_ctx* ctx, const char* who, const char* name, const void* p);
+// The mono_rotation branch of the sequence and batched modes (ctx.cu).  vo_ensure_unit_ess: at least n_units scratch
+// blocks, and the fork stream and events; the block count only grows, and growing drops every captured graph (they hold
+// the old blocks).  Outside any capture.
+int vo_ensure_unit_ess(vo_ctx* ctx, int n_units);
+// the problems of buffer units [u0, u0 + n), one each: pointsLeft_t0 / pointsLeft_t1 = the filtered L0 / L1 lists
+// (d_valid4 planes 0, 2), the unit's scratch block and camera, count[i] the point count of unit u0 + i; n_max (the launch
+// bound of the counts) sizes the per-point grids.  Args that only locate results and masks need no count.
+EssArgs vo_unit_ess_args(const vo_ctx* ctx, int u0, int n, int n_max, const int* count);
+// the results of units [u0, u0 + n) into dst[0 .. n) (pinned staging) on st: one strided copy
+int vo_copy_unit_ess(vo_ctx* ctx, EssResult* dst, int u0, int n, cudaStream_t st);
+// a result as the wait and fetch calls report it: status VO_E_TOO_FEW_POINTS where the reference throws (R = I)
+vo_mono_result vo_mono_from_ess(const EssResult& e);
+// The CollectArgs fields both device waits fill alike (seq_api.cu), from their result table r (vo_mseq_dresults,
+// vo_batch_dresults): the records and point lists of buffer units from u0 and, with ess (their vo_unit_ess_args), the
+// branch's results and masks, into r's destinations.  VO_E_INVALID + message when r->pts_cap does not fit its lists
+// (`lists`: the caller's own list is set too) or one of those destinations is not device memory of the context's GPU.
+template <typename R>
+int vo_collect_args(vo_ctx* ctx, const char* who, const R* r, bool lists, int u0, const EssArgs* ess, CollectArgs& a);
 int vo_ensure_pinned(vo_ctx* ctx, size_t bytes);
 // H2D of a host image (h rows of row_bytes, pitch bytes apart) into a packed device plane on st: one 1-D copy when the
 // rows are contiguous, else a 2-D copy

@@ -282,10 +282,6 @@ int vo_launch_seq_finish(const SeqArgs& a, int n_seq, cudaStream_t s)
     k_seq_finish<<<dim3(1, n_seq), 32, 0, s>>>(a.res, a.tprev, a.tprev_cur, a.out_n, a.n_det, a.n3, a.n5, a.err, a.err_out, a.live);
     return 1;
 }
-int vo_launch_seq_mono(const SeqArgs& a, const EssResult* ess, size_t ess_stride, int n_seq, cudaStream_t s)
-{
-    return vo_launch_mono_fold(a.res, ess, ess_stride, a.live, n_seq, s);
-}
 int vo_launch_mono_fold(vo_unit_result_dev* res, const EssResult* ess, size_t ess_stride, const int* on, int n, cudaStream_t s)
 {
     k_seq_mono<<<dim3(1, n), 32, 0, s>>>(res, ess, ess_stride, on);

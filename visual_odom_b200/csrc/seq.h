@@ -33,11 +33,9 @@ int vo_launch_seq_append(const SeqArgs& a, int n_seq, cudaStream_t s);
 int vo_launch_seq_bucket(const SeqArgs& a, int n_seq, cudaStream_t s);
 int vo_launch_seq_carry(const SeqArgs& a, int n_seq, cudaStream_t s);
 int vo_launch_seq_finish(const SeqArgs& a, int n_seq, cudaStream_t s);
-// mono_rotation = true: each live sequence's record R becomes recoverPose's rotation (I where the branch aborted);
-// everything else in the record stays the PnP's.  ess: sequence 0's result, sequence q's ess_stride bytes further on.
-int vo_launch_seq_mono(const SeqArgs& a, const EssResult* ess, size_t ess_stride, int n_seq, cudaStream_t s);
-// the same fold for n records res[0 .. n) and their results (ess_stride bytes apart): record q takes ess q's rotation
-// when on[q] != 0 (the batched mode's per-unit switch, vo_batch_mono_rotation)
+// mono_rotation = true: record q of res[0 .. n) takes recoverPose's rotation from ess q (ess_stride bytes apart; I where
+// the branch aborted) when on[q] != 0 (a live sequence, SeqArgs::live; a batched unit's switch, vo_batch_mono_rotation);
+// everything else in the record stays the PnP's
 int vo_launch_mono_fold(vo_unit_result_dev* res, const EssResult* ess, size_t ess_stride, const int* on, int n, cudaStream_t s);
 
 // vo_mseq_wait_device: the oldest submission's results (buffer units u0 .. u0 + n_seq - 1) into caller device buffers.

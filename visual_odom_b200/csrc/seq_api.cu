@@ -28,8 +28,9 @@
 //
 // With the option "mono_rotation" (vo_seq_*) or the flag VO_MSEQ_MONO_ROTATION (vo_mseq_begin_ex) -- trackingFrame2Frame's
 // header default, reference src/visualOdometry.cpp:146-157 -- the front stage also forks the essential-matrix RANSAC +
-// recoverPose (ess.cu) onto seq_mono_stream as soon as the filters have compacted L0 / L1: one launch sequence for the
-// n_seq units of the parity (one problem per sequence), which runs beside the feature carry and the triangulation and is
+// recoverPose (ess.cu) onto the context's mono_stream as soon as the filters have compacted L0 / L1: one launch sequence
+// for the n_seq units of the parity (one problem per sequence, in the units' scratch blocks that the batched mode's
+// branch also uses), which runs beside the feature carry and the triangulation and is
 // joined before the front stage ends; it reads no carried translation, so it stays off the back stage, whose PnP chain
 // serialises consecutive frames.  The back stage then writes each sequence's recoverPose rotation into its record
 // (k_seq_mono); rvec / tvec / inliers stay the PnP's.
@@ -132,39 +133,6 @@ static int seq_grid_check(vo_ctx* ctx, const char* who, const char* who_q, int w
     return VO_OK;
 }
 
-// the mono branch of buffer units unit .. unit + n_prob - 1 (one problem each): pointsLeft_t0 / pointsLeft_t1 = the
-// filtered L0 / L1 lists (d_valid4 planes 0, 2), scratch block u for unit u
-static void seq_ess_args(vo_ctx* ctx, int unit, int n_prob, EssArgs& a)
-{
-    memset(&a, 0, sizeof(a));
-    const size_t uo = (size_t)unit * ctx->cap, cs = (size_t)ctx->units * ctx->cap;
-    vo_ess_bind(a, (uint8_t*)ctx->d_seq_ess + (size_t)unit * ctx->seq_ess_bytes, ctx->seq_ess_cap, VO_ESS_ITERS);
-    a.n = ctx->d_n5 + unit;
-    a.cal = ctx->d_cal + unit;                                // focal / pp / threshold of each unit's P_l
-    a.pts0 = ctx->d_valid4 + uo; a.pts1 = ctx->d_valid4 + 2 * cs + uo;
-    a.n_prob = n_prob;
-    a.scratch_stride = a.result_stride = ctx->seq_ess_bytes; a.pts_stride = ctx->cap; a.n_stride = 1; a.cal_stride = 1;
-}
-
-// per-unit scratch of the mono branch for the 2 * n units of n sequences, sized for the bucket grid (outside any capture:
-// the begin calls)
-static int seq_mono_scratch(vo_ctx* ctx, int n)
-{
-    const long long grid = seq_grid(ctx);
-    const int n_max = (int)std::min<long long>(grid, ctx->cap);
-    if (!ctx->seq_mono_stream) {
-        VO_CUDA_CHECK(cudaStreamCreateWithFlags(&ctx->seq_mono_stream, cudaStreamNonBlocking));
-        for (int k = 0; k < 2; k++) VO_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->seq_mono_ev[k], cudaEventDisableTiming));
-    }
-    if (ctx->d_seq_ess && ctx->seq_ess_cap >= n_max && ctx->seq_ess_units >= 2 * n) return VO_OK;
-    vo_drop_graphs(ctx);                                      // captured graphs hold the old blocks
-    if (ctx->d_seq_ess) { VO_CUDA_CHECK(cudaDeviceSynchronize()); cudaFree(ctx->d_seq_ess); ctx->d_seq_ess = nullptr; ctx->seq_ess_units = 0; }
-    const size_t bytes = (vo_ess_scratch_bytes(n_max, VO_ESS_ITERS) + 255) / 256 * 256;
-    VO_CUDA_CHECK(cudaMalloc(&ctx->d_seq_ess, 2 * (size_t)n * bytes));
-    ctx->seq_ess_bytes = bytes; ctx->seq_ess_cap = n_max; ctx->seq_ess_units = 2 * n;
-    return VO_OK;
-}
-
 // front stage of one frame of every sequence on the caller's stream; s0 / s1 = image slots of the previous / new pairs,
 // p = buffer parity (per-frame buffers: units p * n_seq .. p * n_seq + n_seq - 1)
 static int seq_front(vo_ctx* ctx, int s0, int s1, int p, bool bgr)
@@ -187,19 +155,18 @@ static int seq_front(vo_ctx* ctx, int s0, int s1, int p, bool bgr)
     if ((rc = vo_run_lk_ring(ctx, v, 4, ip, in, false, ctx->d_par))) return rc;
     if ((rc = vo_run_filter(ctx, v, true, ctx->d_par))) return rc;
     if (ctx->seq_mono) {        // findEssentialMat + recoverPose on (L0, L1) of every sequence, beside the carry and the triangulation
-        EssArgs e;
-        seq_ess_args(ctx, unit, n, e);
-        VO_CUDA_CHECK(cudaEventRecord(ctx->seq_mono_ev[0], ctx->stream));
-        VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->seq_mono_stream, ctx->seq_mono_ev[0], 0));
-        ctx->launches += vo_launch_essential(e, ctx->seq_mono_stream);
+        const EssArgs e = vo_unit_ess_args(ctx, unit, n, ctx->seq_lk_bound, ctx->d_n5 + unit);
+        VO_CUDA_CHECK(cudaEventRecord(ctx->mono_ev[0], ctx->stream));
+        VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->mono_stream, ctx->mono_ev[0], 0));
+        ctx->launches += vo_launch_essential(e, ctx->mono_stream);
         VO_CUDA_CHECK(cudaGetLastError());
-        VO_CUDA_CHECK(cudaEventRecord(ctx->seq_mono_ev[1], ctx->seq_mono_stream));
+        VO_CUDA_CHECK(cudaEventRecord(ctx->mono_ev[1], ctx->mono_stream));
     }
     // state carry: features.points = pointsLeft_t1, ages keep their A3 length
     ctx->launches += vo_launch_seq_carry(a, n, ctx->stream);
     const size_t cs = (size_t)ctx->units * ctx->cap;
     if ((rc = vo_run_triangulate(ctx, v, ctx->d_valid4, ctx->d_valid4 + cs, ctx->d_n5, ctx->d_cal))) return rc;
-    if (ctx->seq_mono) VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->seq_mono_ev[1], 0));
+    if (ctx->seq_mono) VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->mono_ev[1], 0));
     VO_CUDA_CHECK(cudaGetLastError());
     return VO_OK;
 }
@@ -216,10 +183,9 @@ static int seq_back(vo_ctx* ctx, int p)
     SeqArgs a;
     seq_args(ctx, p, a);
     ctx->launches += vo_launch_seq_finish(a, n, st);
-    if (ctx->seq_mono) {
-        EssArgs e;
-        seq_ess_args(ctx, unit, n, e);
-        ctx->launches += vo_launch_seq_mono(a, e.result, e.result_stride, n, st);
+    if (ctx->seq_mono) {        // each live sequence's record R becomes recoverPose's rotation
+        const EssArgs e = vo_unit_ess_args(ctx, unit, n, ctx->cap, nullptr);
+        ctx->launches += vo_launch_mono_fold(a.res, e.result, e.result_stride, a.live, n, st);
     }
     VO_CUDA_CHECK(cudaGetLastError());
     return VO_OK;
@@ -436,9 +402,9 @@ static int seq_begin(vo_ctx* ctx, const char* who, bool multi, int n, int flags,
             for (int q = 0; q < n; q++) g[2 * n * s + 2 * q] = g[2 * n * s + 2 * q + 1] = vo_plane_geom(ctx, w[q], h[q]);
         if ((rc = vo_write_geo(ctx, 0, 6 * n, g.data()))) return rc;
     }
-    // the LK launch bound (and the mono scratch): the begun sizes' largest bucket grid, or the envelope's for an open run
+    // the LK launch bound (and the mono branch's): the begun sizes' largest bucket grid, or the envelope's for an open run
     ctx->seq_lk_bound = (int)seq_grid(ctx);
-    if (ctx->seq_mono && (rc = seq_mono_scratch(ctx, n))) return rc;
+    if (ctx->seq_mono && (rc = vo_ensure_unit_ess(ctx, 2 * n))) return rc;
     if ((rc = vo_ensure_pinned(ctx, seq_pinned(ctx, n).bytes))) return rc;
     ctx->seq_dres = multi && (flags & VO_MSEQ_DEVICE_RESULTS);
     if (ctx->seq_dres && !ctx->d_seq_pose) {
@@ -532,8 +498,8 @@ static int seq_starts_check(vo_ctx* ctx, const char* who, int n_start, const vo_
     return VO_OK;
 }
 
-// the sizes a run can start: the run's planes, pyramid depth and mono scratch are those of its begin; the bucketing
-// scratch holds any bucket bound within max_features
+// the sizes a run can start: the run's planes, pyramid depth and, with the mono branch, launch bound are those of its
+// begin; the bucketing scratch holds any bucket bound within max_features
 static int seq_starts_fit(vo_ctx* ctx, const char* who, int n_start, const vo_mseq_start* starts)
 {
     for (int i = 0; i < n_start; i++) {
@@ -556,10 +522,11 @@ static int seq_starts_fit(vo_ctx* ctx, const char* who, int n_start, const vo_ms
             vo_set_error(ctx, "%s: slot %d: %d x %d has %d pyramid levels, the run %d", who, q, w, h, depth, ctx->pg.nlevels);
             return VO_E_UNSUPPORTED;
         }
+        // (seq_grid_check above keeps the grid within max_features)
         const int grid = (int)seq_grid(ctx->slot_par[q], w, h);
-        if (ctx->seq_mono && std::min(grid, ctx->cap) > ctx->seq_ess_cap) {
+        if (ctx->seq_mono && grid > ctx->seq_lk_bound) {
             vo_set_error(ctx, "%s: slot %d: %d x %d needs mono scratch for %d points, the run reserved %d", who, q, w, h,
-                         std::min(grid, ctx->cap), ctx->seq_ess_cap);
+                         grid, ctx->seq_lk_bound);
             return VO_E_CAPACITY;
         }
     }
@@ -723,12 +690,7 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
     if (!ctx->seq_dres) {
         VO_CUDA_CHECK(cudaMemcpyAsync(pin.rec + u0, ctx->d_results + u0, n * sizeof(vo_unit_result_dev), cudaMemcpyDeviceToHost, sb));
         VO_CUDA_CHECK(cudaMemcpyAsync(pin.err + u0, ctx->d_seq_err + 1 + u0, n * sizeof(int), cudaMemcpyDeviceToHost, sb));
-        if (ctx->seq_mono) {            // the n results, one per scratch block, into n consecutive records: one strided copy
-            EssArgs e;
-            seq_ess_args(ctx, u0, n, e);
-            VO_CUDA_CHECK(cudaMemcpy2DAsync(pin.ess + u0, sizeof(EssResult), e.result, e.result_stride, sizeof(EssResult), n,
-                                            cudaMemcpyDeviceToHost, sb));
-        }
+        if (ctx->seq_mono && (rc = vo_copy_unit_ess(ctx, pin.ess + u0, u0, n, sb))) return rc;
     }
     VO_CUDA_CHECK(cudaEventRecord(ctx->seq_back_ev[p], sb));
     ctx->seq_slot = s1;                 // imageLeft_t0 = imageLeft_t1 (main.cpp:157-158)
@@ -791,13 +753,7 @@ static int seq_wait(vo_ctx* ctx, const char* who, bool multi, bool want_mono, vo
         const EssResult& ess = pin.ess[u0 + q];
         const bool mono_ok = !ctx->seq_mono || ess.status == ESS_OK;
         if ((r.pnp_status == VO_OK || r.pnp_status == VO_PNP_NO_MODEL) && mono_ok) vo_pose_step(ctx->seq_pose.data() + 16 * q, r.R, r.tvec);
-        if (mono) {
-            vo_mono_result& m = mono[q];
-            m.status = mono_ok ? VO_OK : VO_E_TOO_FEW_POINTS;
-            m.n_inliers = ess.n_inliers; m.ransac_iters = ess.iters; m.n_good = ess.n_good;
-            for (int k = 0; k < 9; k++) m.R[k] = ess.R[k];
-            for (int k = 0; k < 3; k++) m.t[k] = ess.t[k];
-        }
+        if (mono) mono[q] = vo_mono_from_ess(ess);
         // the frame's point lists (and essential mask) stay in its buffer units until the frame after next is submitted
         const size_t uo = (size_t)(u0 + q) * ctx->cap;
         if (pts4 && pts_cap > 0 && r.n_valid > 0) {
@@ -808,8 +764,7 @@ static int seq_wait(vo_ctx* ctx, const char* who, bool multi, bool want_mono, vo
             copies = true;
         }
         if (ess_mask && mask_cap > 0 && r.n_valid > 0) {
-            EssArgs e;
-            seq_ess_args(ctx, u0 + q, 1, e);
+            const EssArgs e = vo_unit_ess_args(ctx, u0 + q, 1, ctx->cap, nullptr);
             const int m = r.n_valid < mask_cap ? r.n_valid : mask_cap;
             VO_CUDA_CHECK(cudaMemcpyAsync(ess_mask + (size_t)mask_cap * q, e.mask, (size_t)m, cudaMemcpyDeviceToHost, sb));
             copies = true;
@@ -846,6 +801,33 @@ int vo_check_dptr(vo_ctx* ctx, const char* who, const char* name, const void* p)
     return VO_OK;
 }
 
+template <typename R>
+int vo_collect_args(vo_ctx* ctx, const char* who, const R* r, bool lists, int u0, const EssArgs* ess, CollectArgs& a)
+{
+    lists = lists || r->pts4 || r->points3d || r->inliers || r->ess_mask;
+    if (r->pts_cap < 0 || (lists && r->pts_cap == 0)) {
+        vo_set_error(ctx, "%s: pts_cap = %d with point arrays", who, r->pts_cap);
+        return VO_E_INVALID;
+    }
+    const struct { const char* name; const void* p; } ptrs[] = {
+        {"records", r->records}, {"pts4", r->pts4}, {"points3d", r->points3d}, {"inliers", r->inliers}, {"mono", r->mono},
+        {"ess_mask", r->ess_mask}};
+    int rc;
+    for (const auto& x : ptrs)
+        if ((rc = vo_check_dptr(ctx, who, x.name, x.p))) return rc;
+    const size_t uo = (size_t)u0 * ctx->cap;
+    memset(&a, 0, sizeof(a));
+    a.res = ctx->d_results + u0; a.cap = ctx->cap;
+    a.valid4 = ctx->d_valid4 + uo; a.plane_stride = (size_t)ctx->units * ctx->cap;
+    a.X = ctx->d_X + uo; a.inliers = ctx->d_inliers + uo;
+    if (ess) { a.ess = ess->result; a.ess_mask = ess->mask; a.ess_stride = ess->result_stride; }
+    a.records = (vo_unit_result_dev*)r->records; a.pts_cap = r->pts_cap;
+    a.pts4 = (float2*)r->pts4; a.points3d = (float3*)r->points3d; a.inliers_out = r->inliers; a.mono = r->mono;
+    a.mask_out = r->ess_mask;
+    return VO_OK;
+}
+template int vo_collect_args(vo_ctx*, const char*, const vo_batch_dresults*, bool, int, const EssArgs*, CollectArgs&);
+
 // vo_mseq_wait_device: the oldest submission retired by ONE k_seq_collect launch on the context's stream, after the
 // caller's work there and after that submission's back stage (seq_back_ev of its parity; the next submission's back stage
 // on the side stream is not waited for).  The stream order also covers the unit buffers: the next submission of the same
@@ -861,39 +843,23 @@ static int seq_wait_device(vo_ctx* ctx, const char* who, const vo_mseq_dresults*
         return VO_E_INVALID;
     }
     if (!r) { vo_set_error(ctx, "%s: null result table", who); return VO_E_INVALID; }
-    const bool lists = r->pts4 || r->points3d || r->inliers || r->ess_mask;
-    if (r->pts_cap < 0 || (lists && r->pts_cap == 0)) {
-        vo_set_error(ctx, "%s: pts_cap = %d with point arrays", who, r->pts_cap);
-        return VO_E_INVALID;
-    }
     if ((r->mono || r->ess_mask) && !ctx->seq_mono) {
         vo_set_error(ctx, "%s: mono / ess_mask: the sequences were begun without the flag VO_MSEQ_MONO_ROTATION", who);
         return VO_E_INVALID;
     }
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
-    const struct { const char* name; const void* p; } ptrs[] = {
-        {"status", r->status}, {"records", r->records}, {"frame_pose", r->frame_pose}, {"pts4", r->pts4},
-        {"points3d", r->points3d}, {"inliers", r->inliers}, {"mono", r->mono}, {"ess_mask", r->ess_mask}};
-    for (const auto& x : ptrs)
-        if ((rc = vo_check_dptr(ctx, who, x.name, x.p))) return rc;
     const int n = ctx->seq_n;
     const int p = (int)((ctx->seq_submitted - ctx->seq_inflight) & 1);      // the parity of the oldest frame in flight
     const int u0 = p * n;
-    const size_t cs = (size_t)ctx->units * ctx->cap, uo = (size_t)u0 * ctx->cap;
+    EssArgs e;
+    if (ctx->seq_mono) e = vo_unit_ess_args(ctx, u0, n, ctx->cap, nullptr);
     CollectArgs a;
-    memset(&a, 0, sizeof(a));
-    a.res = ctx->d_results + u0; a.err = ctx->d_seq_err + 1 + u0; a.cap = ctx->cap;
-    a.valid4 = ctx->d_valid4 + uo; a.plane_stride = cs;
-    a.X = ctx->d_X + uo; a.inliers = ctx->d_inliers + uo;
-    if (ctx->seq_mono) {
-        EssArgs e;
-        seq_ess_args(ctx, u0, n, e);
-        a.ess = e.result; a.ess_mask = e.mask; a.ess_stride = ctx->seq_ess_bytes;
-    }
+    if ((rc = vo_collect_args(ctx, who, r, false, u0, ctx->seq_mono ? &e : nullptr, a)) ||
+        (rc = vo_check_dptr(ctx, who, "status", r->status)) || (rc = vo_check_dptr(ctx, who, "frame_pose", r->frame_pose)))
+        return rc;
+    a.err = ctx->d_seq_err + 1 + u0;
     a.pose = ctx->d_seq_pose;
-    a.status = r->status; a.records = (vo_unit_result_dev*)r->records; a.pose_out = r->frame_pose; a.pts_cap = r->pts_cap;
-    a.pts4 = (float2*)r->pts4; a.points3d = (float3*)r->points3d; a.inliers_out = r->inliers; a.mono = r->mono;
-    a.mask_out = r->ess_mask;
+    a.status = r->status; a.pose_out = r->frame_pose;
     for (int q = 0; q < n; q++) a.mode[q] = (unsigned char)ctx->seq_live[u0 + q];
     VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->seq_back_ev[p], 0));
     ctx->launches += vo_launch_seq_collect(a, n, ctx->stream);
