@@ -19,8 +19,15 @@ _lib = None
 LK_EVENT = np.dtype([("pt", "<i4"), ("level", "<i4"), ("iter", "<i4"), ("kind", "<i4"),
                      ("min_eig", "<f4"), ("D", "<f4"), ("dx", "<f4"), ("dy", "<f4"), ("sdx", "<f4"), ("sdy", "<f4"),
                      ("ipx", "<i4"), ("ipy", "<i4"), ("inx", "<i4"), ("iny", "<i4"),
-                     ("d2", "<f8"), ("d2f", "<f4"), ("pad_", "<i4"), ("sabs", "<i8", (10,))])
+                     ("d2", "<f8"), ("d2f", "<f4"), ("pad_", "<i4"), ("sabs", "<i8", (10,)),
+                     ("pos", "<i8", (10,)), ("neg", "<i8", (10,)), ("total", "<i8", (10,)),
+                     ("maxpre", "<i8", (10,)), ("maxadd", "<i8", (10,)), ("fchain", "<f4", (10,))])
 EV_ITER, EV_EPS, EV_HALF, EV_CAP, EV_JOUT, EV_SETUP, EV_REJECT, EV_IOUT, EV_FINAL = range(9)
+
+# lk_set_sum_mode (lk_ref.c: LK_SUM_*).  SUM_CV2 is the pinned order; SUM_KERNEL is k_lk_ring's exact-path vote and
+# combination (equal to SUM_CV2 on every input); SUM_M1..SUM_M6 are wrong votes or orders
+SUM_CV2, SUM_SEQ, SUM_PAIRS, SUM_SCALAR = 0, 1, 2, 9
+SUM_KERNEL, SUM_M1, SUM_M2, SUM_M3, SUM_M4, SUM_M5, SUM_M6 = range(10, 17)
 
 
 def lib():

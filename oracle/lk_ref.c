@@ -160,20 +160,121 @@ const int16_t *lk_pyr_level_deriv(const lk_pyr_t *p, int l) { return p->lv[l].de
 
 /* ------------------------------------------------------------------------- */
 /* accumulation-order selector (the pinned one is mode 0; the others exist so
- * tests can show that the order matters and that mode 0 is the cv2 one)      */
+ * tests can show that the order matters and that mode 0 is the cv2 one).  oracle/cref.py names them (SUM_*).
+ * From LK_SUM_KERNEL on, b1 / b2 follow k_lk_ring's two paths: an iteration whose vote passes takes the exact path
+ * (the ten b chain totals as integers, combined in float as tail + ((c0 + c2) + (c1 + c3))), any other takes the float
+ * chains; after the first rejected iteration of a level-solve the rest of it replays, as in the kernel.  LK_SUM_KERNEL
+ * is the kernel's rule and must equal mode 0; LK_SUM_M1..M6 are wrong rules that tests use to show the LK sum-edge
+ * fixture notices one. */
+enum {
+    LK_SUM_CV2 = 0,         /* cv2's order: (q0 + q2) + (q1 + q3) lane reduction                                  */
+    LK_SUM_SEQ = 1,         /* lane reduction ((q0 + q1) + q2) + q3                                               */
+    LK_SUM_PAIRS = 2,       /* lane reduction (q0 + q1) + (q2 + q3)                                               */
+    LK_SUM_SCALAR = 9,      /* no SIMD body: every column in the scalar chain                                     */
+    LK_SUM_KERNEL = 10,     /* vote max(P, N) <= 2^24 on all ten chains (sum |product| + |total| <= 2^25)           */
+    LK_SUM_M1 = 11,         /* vote max(P, N) <= 2^25 (twice too permissive)                                       */
+    LK_SUM_M2 = 12,         /* vote sum |product| <= 2^25, without the sign term                                   */
+    LK_SUM_M3 = 13,         /* the vote ignores the two tail chains                                                */
+    LK_SUM_M4 = 14,         /* the vote ignores b2's five chains                                                   */
+    LK_SUM_M5 = 15,         /* the exact path combines (c0 + c1) + (c2 + c3)                                       */
+    LK_SUM_M6 = 16,         /* the replay adds the tail chain column-major                                         */
+};
 static int g_sum_mode = 0;
 void lk_set_sum_mode(int m) { g_sum_mode = m; }
 
+/* The ten b chains of one Newton iteration (b1 chains 0..3, b1 tail, b2 chains 0..3, b2 tail), split as k_lk_ring
+ * splits them: a SIMD chain q holds the products of columns x = q (mod 4), x < nsimd, and adds them in pairs (x, x+4)
+ * row by row; the tail holds columns nsimd.. row-major. */
+typedef struct {
+    int64_t sabs[10];       /* sum |product|                                                                      */
+    int64_t pos[10];        /* P: sum of the positive products                                                    */
+    int64_t neg[10];        /* N: sum of |negative products|                                                      */
+    int64_t total[10];      /* P - N                                                                              */
+    int64_t maxpre[10];     /* largest |prefix sum| in cv2's chain order                                          */
+    int64_t maxadd[10];     /* largest |addend| (a pair sum in the SIMD chains, a product in the tail)            */
+    float tail_colmajor[2]; /* the tail chains added column-major in float (LK_SUM_M6)                            */
+} lk_chains_t;
+
+static void lk_chain_info(const int *diffs_all, const int16_t *dIbuf, int win, lk_chains_t *c)
+{
+    const int nsimd = (win / 8) * 8;
+    memset(c, 0, sizeof(*c));
+    for (int comp = 0; comp < 2; comp++) {
+        for (int q = 0; q < 5; q++) {
+            const int k = comp * 5 + q;
+            long long pre = 0;
+            for (int y = 0; y < win; y++) {
+                const int *d = diffs_all + y * win;
+                const int16_t *g = dIbuf + y * win * 2 + comp;
+                if (q < 4) {
+                    for (int x0 = q; x0 < nsimd; x0 += 8) {
+                        long long v0 = (long long)d[x0] * g[2 * x0], v1 = (long long)d[x0 + 4] * g[2 * (x0 + 4)];
+                        long long pair = v0 + v1;
+                        c->pos[k] += (v0 > 0 ? v0 : 0) + (v1 > 0 ? v1 : 0);
+                        c->neg[k] += (v0 < 0 ? -v0 : 0) + (v1 < 0 ? -v1 : 0);
+                        pre += pair;
+                        if (llabs(pre) > c->maxpre[k]) c->maxpre[k] = llabs(pre);
+                        if (llabs(pair) > c->maxadd[k]) c->maxadd[k] = llabs(pair);
+                    }
+                } else {
+                    for (int x = nsimd; x < win; x++) {
+                        long long v = (long long)d[x] * g[2 * x];
+                        c->pos[k] += v > 0 ? v : 0;
+                        c->neg[k] += v < 0 ? -v : 0;
+                        pre += v;
+                        if (llabs(pre) > c->maxpre[k]) c->maxpre[k] = llabs(pre);
+                        if (llabs(v) > c->maxadd[k]) c->maxadd[k] = llabs(v);
+                    }
+                }
+            }
+            c->sabs[k] = c->pos[k] + c->neg[k];
+            c->total[k] = pre;
+        }
+        float t = 0.f;
+        for (int x = nsimd; x < win; x++)
+            for (int y = 0; y < win; y++)
+                t += (float)(diffs_all[y * win + x] * dIbuf[(y * win + x) * 2 + comp]);
+        c->tail_colmajor[comp] = t;
+    }
+}
+
+/* k_lk_ring's vote (mode LK_SUM_KERNEL) or a wrong one (LK_SUM_M1..M4): may this iteration take the exact path?
+ * Every prefix of a chain lies in [-N, P], so max(P, N) <= 2^24 makes each one an exact float. */
+static int lk_vote(const lk_chains_t *c, int mode)
+{
+    const long long LIM = 1LL << 24;
+    for (int k = 0; k < 10; k++) {
+        if (mode == LK_SUM_M3 && (k == 4 || k == 9)) continue;
+        if (mode == LK_SUM_M4 && k >= 5) continue;
+        const long long P = c->pos[k], N = c->neg[k];
+        const int ok = mode == LK_SUM_M1 ? (P <= 2 * LIM && N <= 2 * LIM)
+                     : mode == LK_SUM_M2 ? (P + N <= 2 * LIM)
+                     : (P <= LIM && N <= LIM);
+        if (!ok) return 0;
+    }
+    return 1;
+}
+
+/* the exact path's float combination of one quantity's chain totals t[0..3] and tail t[4] */
+static float lk_exact_combine(const int64_t *t, int mode)
+{
+    const float c0 = (float)t[0], c1 = (float)t[1], c2 = (float)t[2], c3 = (float)t[3];
+    const float simd = mode == LK_SUM_M5 ? (c0 + c1) + (c2 + c3) : (c0 + c2) + (c1 + c3);
+    return (float)t[4] + simd;
+}
+
 /* Optional bookkeeping for kernel design (not part of the checker): how often are all partial sums of the b chains
- * exactly representable?  [0] iterations, [1] sum|addend| <= 2^24 on every chain (the kernel's current test),
+ * exactly representable?  [0] iterations, [1] sum|addend| <= 2^24 on every chain (the kernel's former test),
  * [2] strip bound: sum over the kernel's strips of max|running strip sum| <= 2^24 and every addend <= 2^24,
- * [3] truth: every chain prefix and every addend <= 2^24 in magnitude. */
+ * [3] truth: every chain prefix and every addend <= 2^24 in magnitude,
+ * [4] sign split: max(P, N) <= 2^24 on every chain (the vote k_lk_ring runs),
+ * [5] iterations the sign split accepts although a prefix or an addend leaves +-2^24 (0 if the vote is sound). */
 static long long g_stats[8];
 static int g_stats_on = 0;
 void lk_stats_enable(int on) { g_stats_on = on; for (int i = 0; i < 8; i++) g_stats[i] = 0; }
 void lk_stats_get(long long *out) { for (int i = 0; i < 8; i++) out[i] = g_stats[i]; }
 
-static void lk_chain_stats(const int *diffs_all, const int16_t *dIbuf, int win)
+static void lk_chain_stats(const int *diffs_all, const int16_t *dIbuf, int win, const lk_chains_t *ch)
 {
     /* diffs_all: win x win residuals; dIbuf: win x win x 2 gradients */
     const long long LIM = 1LL << 24;
@@ -236,13 +337,16 @@ static void lk_chain_stats(const int *diffs_all, const int16_t *dIbuf, int win)
             if (bound > LIM || maxadd > LIM) ok_strip = 0;
         }
     }
+    const int ok_sign = lk_vote(ch, LK_SUM_KERNEL);
     g_stats[0]++; g_stats[1] += ok_old; g_stats[2] += ok_strip; g_stats[3] += ok_true;
+    g_stats[4] += ok_sign; g_stats[5] += ok_sign && !ok_true;
 }
 
 /* Optional per-point event log (off by default; tests/test_oracle_lk_edges.py and tests/golden/make_lk_edges.py read it
  * to find and check the inputs that sit on the decision edges of a level-solve).  One record per level-solve set-up
  * (minEig, D, the I window origin) and one per Newton iteration (the step, the half-step sums, the J window origin,
- * ||delta||^2 in double and in float, sum |addend| of the ten b chains as the kernel bounds them), plus one for the
+ * ||delta||^2 in double and in float, and per b chain as k_lk_ring splits them: sum |product|, P and N, the signed
+ * total, the largest |prefix| and |addend| in cv2's order and the float32 chain as cv2 adds it), plus one for the
  * level-0 final re-check when it clears the status.  The layout is mirrored by oracle/cref.py:LK_EVENT. */
 enum {
     LK_EV_ITER = 0,     /* an iteration after which the solve goes on                                   */
@@ -262,7 +366,10 @@ typedef struct {
     double d2;                              /* (double)dx*dx + (double)dy*dy                                  */
     float d2f;                              /* dx*dx + dy*dy in float                                         */
     int32_t pad_;
-    int64_t sabs[10];                       /* b1 chains 0..3, b1 tail, b2 chains 0..3, b2 tail               */
+    int64_t sabs[10];                       /* b1 chains 0..3, b1 tail, b2 chains 0..3, b2 tail: sum |product| */
+    int64_t pos[10], neg[10], total[10];    /* P, N, P - N (lk_chains_t)                                      */
+    int64_t maxpre[10], maxadd[10];         /* largest |prefix|, |addend| in cv2's chain order                */
+    float fchain[10];                       /* the chain's float32 sum as cv2 forms it                        */
 } lk_event_t;
 static lk_event_t *g_log = NULL;
 static long long g_log_cap = 0, g_log_n = 0;
@@ -278,25 +385,6 @@ static lk_event_t *lk_log_add(int pt, int level, int iter, int kind)
     memset(e, 0, sizeof(*e));
     e->pt = pt; e->level = level; e->iter = iter; e->kind = kind;
     return e;
-}
-
-/* sum |addend| of each b chain as k_lk_ring bounds it: |v0| + |v1| for the pair addends of the SIMD chains */
-static void lk_chain_sabs(const int *diffs_all, const int16_t *dIbuf, int win, int64_t out[10])
-{
-    for (int comp = 0; comp < 2; comp++) {
-        for (int q = 0; q < 4; q++) {
-            long long s = 0;
-            for (int y = 0; y < win; y++)
-                for (int x = q; x < (win / 8) * 8; x += 4)
-                    s += llabs((long long)diffs_all[y * win + x] * dIbuf[(y * win + x) * 2 + comp]);
-            out[comp * 5 + q] = s;
-        }
-        long long s = 0;
-        for (int y = 0; y < win; y++)
-            for (int x = (win / 8) * 8; x < win; x++)
-                s += llabs((long long)diffs_all[y * win + x] * dIbuf[(y * win + x) * 2 + comp]);
-        out[comp * 5 + 4] = s;
-    }
 }
 
 static inline float reduce4(const float q[4])
@@ -413,6 +501,7 @@ void lk_track(const lk_pyr_t *prev, const lk_pyr_t *next,
 
             float npx = nx - half, npy = ny - half;
             float pdx = 0, pdy = 0;
+            int replayed = 0;
             for (int j = 0; j < max_count; j++) {
                 int inx = cv_floor(npx), iny = cv_floor(npy);
                 if (inx < -win || inx >= J->w || iny < -win || iny >= J->h) {
@@ -459,7 +548,18 @@ void lk_track(const lk_pyr_t *prev, const lk_pyr_t *next,
                         ib2 += (float)(diffs[x] * dIp[2 * x + 1]);
                     }
                 }
-                if (g_stats_on && win == 21) lk_chain_stats(diffs_all, dIbuf, win);
+                const int want_chains = g_log || (g_stats_on && win == 21) || g_sum_mode >= LK_SUM_KERNEL;
+                lk_chains_t ch;
+                if (want_chains) lk_chain_info(diffs_all, dIbuf, win, &ch);
+                if (g_stats_on && win == 21) lk_chain_stats(diffs_all, dIbuf, win, &ch);
+                /* the float chains as cv2 forms them: SIMD chain q is lane q's bx / by, the tails are ib1 / ib2 so far */
+                float fchain[10];
+                for (int q = 0; q < 4; q++) {
+                    const float *qq = (q < 2) ? qb0 : qb1;
+                    fchain[q] = qq[(q & 1) * 2]; fchain[5 + q] = qq[(q & 1) * 2 + 1];
+                }
+                fchain[4] = ib1; fchain[9] = ib2;
+                if (g_sum_mode == LK_SUM_M6) { ib1 = ch.tail_colmajor[0]; ib2 = ch.tail_colmajor[1]; }
                 if (g_sum_mode != 9) {
                     /* qf0 = interleave_pairs(qb0+qb1) low half = [s0, s2, 0, 0], qf1 = [s1, s3, 0, 0] */
                     float s[4];
@@ -467,6 +567,14 @@ void lk_track(const lk_pyr_t *prev, const lk_pyr_t *next,
                     float qf0[4] = {s[0], s[2], 0.f, 0.f}, qf1[4] = {s[1], s[3], 0.f, 0.f};
                     ib1 += reduce4(qf0);
                     ib2 += reduce4(qf1);
+                }
+                if (g_sum_mode >= LK_SUM_KERNEL) {
+                    if (!replayed && lk_vote(&ch, g_sum_mode)) {
+                        ib1 = lk_exact_combine(ch.total, g_sum_mode);
+                        ib2 = lk_exact_combine(ch.total + 5, g_sum_mode);
+                    } else {
+                        replayed = 1;       /* k_lk_ring replays the rest of the level-solve without a vote */
+                    }
                 }
                 float b1 = ib1 * FLT_SCALE, b2 = ib2 * FLT_SCALE;
                 float dx = (float)((A12 * b2 - A22 * b1) * D);
@@ -479,7 +587,13 @@ void lk_track(const lk_pyr_t *prev, const lk_pyr_t *next,
                     ev->min_eig = minEig; ev->D = D; ev->dx = dx; ev->dy = dy; ev->sdx = dx + pdx; ev->sdy = dy + pdy;
                     ev->ipx = ipx; ev->ipy = ipy; ev->inx = inx; ev->iny = iny;
                     ev->d2 = (double)dx * dx + (double)dy * dy; ev->d2f = dx * dx + dy * dy;
-                    lk_chain_sabs(diffs_all, dIbuf, win, ev->sabs);
+                    memcpy(ev->sabs, ch.sabs, sizeof ch.sabs);
+                    memcpy(ev->pos, ch.pos, sizeof ch.pos);
+                    memcpy(ev->neg, ch.neg, sizeof ch.neg);
+                    memcpy(ev->total, ch.total, sizeof ch.total);
+                    memcpy(ev->maxpre, ch.maxpre, sizeof ch.maxpre);
+                    memcpy(ev->maxadd, ch.maxadd, sizeof ch.maxadd);
+                    memcpy(ev->fchain, fchain, sizeof fchain);
                 }
                 if ((double)dx * dx + (double)dy * dy <= eps2) { if (ev) ev->kind = LK_EV_EPS; break; }
                 if (j > 0 && fabs(dx + pdx) < 0.01 && fabs(dy + pdy) < 0.01) {

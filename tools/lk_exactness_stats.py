@@ -1,9 +1,12 @@
 #!/usr/bin/env python
 """Kernel-design bookkeeping on the CPU (no GPU): how often could an LK iteration of the benchmark scene take the exact
 integer path of k_lk_ring?  Uses the instrumentation hook of the oracle's C restatement (oracle/lk_ref.c, lk_chain_stats):
-  current   sum |addend| <= 2^24 on every chain             (the test the kernel runs)
+  former    sum |addend| <= 2^24 on every chain             (the kernel's test before the sign split)
   strips    sum over the kernel's strips of max |running strip sum| <= 2^24
+  sign      max(P, N) <= 2^24 on every chain, P and N the sums of the positive products and of |negative products|
+            (sum |product| + |total| <= 2^25: the vote the kernel runs)
   truth     every chain prefix and every addend <= 2^24      (the best any test could do)
+and how many iterations the sign split accepts although a prefix or an addend leaves +-2^24 (0 if the vote is sound).
 This script only reads the oracle; it is not part of any timed or shipped path (DESIGN.md K2 quotes its output)."""
 import ctypes as C
 import os
@@ -37,8 +40,10 @@ def main():
         tot += out
     it = max(int(tot[0]), 1)
     print(f"{len(seeds)} unit(s) x {n_feat} features: {it} Newton iterations over the four calls of the ring")
-    for name, k in (("current test (sum |addend|)", 1), ("strip bound", 2), ("truth (prefix sums)", 3)):
-        print(f"  exact by {name:28s}: {100.0 * tot[k] / it:5.1f} %")
+    for name, k in (("former test (sum |addend|)", 1), ("strip bound", 2), ("sign split (the kernel's vote)", 4),
+                    ("truth (prefix sums)", 3)):
+        print(f"  exact by {name:30s}: {100.0 * tot[k] / it:5.1f} %")
+    print(f"  sign split accepts, a prefix rounds: {int(tot[5])}")
 
 
 if __name__ == "__main__":
