@@ -51,15 +51,20 @@ typedef struct vo_point3f { float x, y, z; } vo_point3f;
 /* All literals the reference hard-codes, as run-time parameters (SURVEY.md section 5, "Config").  Away from the
  * reference's values each one does what OpenCV does with it: clamped where OpenCV clamps, refused where it asserts.
  * vo_create sets the context's values.  Every field but lk_win, lk_max_level, fast_nonmax, max_features and max_units
- * can also differ per multi-sequence slot (vo_mseq_params) and per batched unit (vo_batch_params). */
+ * can also differ per multi-sequence slot (vo_mseq_params) and per batched unit (vo_batch_params): those five are
+ * context-wide (the window and the depth fix the pyramids every slot and unit shares). */
 typedef struct vo_params {
     int fast_threshold;      /* 20      reference src/feature.cpp:43; vo_create refuses values
                                         outside [0, 255] (VO_E_INVALID)                           */
     int fast_nonmax;         /* 1       reference src/feature.cpp:44; 0: every FAST corner is kept
                                         with response 0 (as cv::FAST).  Fixed at vo_create: the
                                         corner capacity of a frame depends on it                  */
-    int lk_win;              /* 21      reference src/feature.cpp:127 (only 21 is built; vo_create
-                                        refuses others with VO_E_UNSUPPORTED)                     */
+    int lk_win;              /* 21      reference src/feature.cpp:127: the square window winSize;
+                                        3..32.  vo_create refuses values below 3 as cv2 asserts
+                                        (VO_E_INVALID) and above 32 (VO_E_UNSUPPORTED).  21 runs
+                                        the tuned ring kernel, every other window a second one
+                                        (run-time width, plain loads), bit for bit with cv2 both.
+                                        The pyramid depth depends on it (lk_max_level)            */
     int lk_max_level;        /* 3       reference src/feature.cpp:136 (0-based: 4 images); 0..7,
                                         vo_create refuses others (VO_E_UNSUPPORTED).  A pyramid
                                         stops early where a level would not exceed the window     */

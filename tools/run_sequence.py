@@ -8,7 +8,7 @@ are pushed through vo_seq_submit / vo_seq_wait (two in flight), frame_pose is in
 scale gates, the trajectory is written in the KITTI text format and, with --gt, scored with the KITTI segment metric.
 `--mono-rotation` runs trackingFrame2Frame as its header default does (mono_rotation = true: the rotation from
 findEssentialMat + recoverPose, the translation from the PnP; frames where that branch would abort are reported and not
-integrated).  `--check` only validates the inputs (no GPU needed)."""
+integrated).  `--lk-win W` tracks with a W x W window (3 to 32; the reference's 21 by default).  `--check` only validates the inputs (no GPU needed)."""
 import argparse
 import os
 import re
@@ -56,6 +56,18 @@ def add_bucket_args(ap):
                     help="FAST corners are appended while fewer than THRESHOLD features are tracked (default 2000)")
 
 
+def add_lk_win_arg(ap):
+    """calcOpticalFlowPyrLK's winSize (vo_params.lk_win): one value for the whole context"""
+    ap.add_argument("--lk-win", type=int, default=21, metavar="W",
+                    help="track with a W x W LK window, 3 <= W <= 32 (default 21, the reference's Size(21,21))")
+
+
+def lk_win_param(a):
+    if not 3 <= a.lk_win <= 32:
+        raise SystemExit(f"--lk-win {a.lk_win}: the LK window runs from 3 to 32")
+    return a.lk_win
+
+
 def bucket_params(a, sizes):
     """the Context keywords of the flags; max_features is raised from 4096 to the largest read-back bound of the sizes"""
     if a.features_per_bucket < 1 or a.bucket_divisor < 1:
@@ -78,6 +90,7 @@ def main():
     ap.add_argument("--mono-rotation", action="store_true",
                     help="rotation from findEssentialMat + recoverPose (trackingFrame2Frame's header default)")
     add_bucket_args(ap)
+    add_lk_win_arg(ap)
     ap.add_argument("--check", action="store_true")
     a = ap.parse_args()
     from visual_odom_b200 import capi, synth
@@ -93,6 +106,8 @@ def main():
     print("rotation: " + ("findEssentialMat + recoverPose (mono_rotation = true)" if a.mono_rotation else
                           "Rodrigues of the PnP rvec (mono_rotation = false)"))
     prm = bucket_params(a, [(w, h)])
+    prm["lk_win"] = lk_win_param(a)
+    print(f"LK window: {a.lk_win}x{a.lk_win}")
     print(f"bucketing: {a.features_per_bucket} feature(s) per bucket of rows/{a.bucket_divisor}, ages < {a.age_threshold}, "
           f"refill below {a.refill_threshold} features; max_features {prm['max_features']}")
     if a.check:

@@ -24,7 +24,8 @@ is the same for every N.  `--params-for NAME=FIELD=V[,FIELD=V...]` gives the dat
 context-wide lk_win, lk_max_level, fast_nonmax, max_features and max_units are refused); each sequence runs in its own
 slot as a context created with its parameters would run it alone (vo_mseq_params).  `--sweep FIELD=V1,V2,...` runs the
 first dataset once per value, each in its own slot of one context, with pose files OUTDIR/<name>_<FIELD>=<V>.txt.
-`--check` only validates the inputs and prints each sequence's parameters and the schedule of --slots (no GPU needed)."""
+`--lk-win W` tracks every sequence with a W x W LK window (3 to 32; the reference's 21 by default; one window per
+context, so a dataset's --params-for cannot set it).  `--check` only validates the inputs and prints each sequence's parameters and the schedule of --slots (no GPU needed)."""
 import argparse
 import os
 import sys
@@ -34,13 +35,14 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import numpy as np
 
-from run_sequence import add_bucket_args, bucket_grid, bucket_params, count_frames, read_calibration
+from run_sequence import (add_bucket_args, add_lk_win_arg, bucket_grid, bucket_params, count_frames, lk_win_param,
+                          read_calibration)
 
 
-def pyramid_depth(w, h):
+def pyramid_depth(w, h, win):
     """pyramid images of a w x h image as the library builds them (vo_pyr_depth, csrc/common.cuh): levels up to the
-    default vo_params.lk_max_level, a level dropped once it is not larger than the lk_win window.  Both values are read
-    from the library's vo_default_params, which the run's context is created with."""
+    default vo_params.lk_max_level (read from the library's vo_default_params, which the run's context is created with),
+    a level dropped once it is not larger than the win x win window (--lk-win)."""
     import ctypes as C
     from visual_odom_b200 import capi
     p = capi.VoParams()
@@ -48,7 +50,7 @@ def pyramid_depth(w, h):
     n = 1
     for _ in range(p.lk_max_level):
         w, h = (w + 1) // 2, (h + 1) // 2
-        if w <= p.lk_win or h <= p.lk_win:
+        if w <= win or h <= win:
             break
         n += 1
     return n
@@ -111,6 +113,7 @@ def main():
     ap.add_argument("--slots", type=int, metavar="N",
                     help="run the datasets as a queue through N slots, each starting in the first slot that frees")
     add_bucket_args(ap)
+    add_lk_win_arg(ap)
     ap.add_argument("--params-for", action="append", default=[], metavar="NAME=FIELD=V[,FIELD=V...]",
                     help="tracking parameters of the dataset named NAME (repeatable; the others use the flags' values)")
     ap.add_argument("--sweep", metavar="FIELD=V1,V2,...",
@@ -119,6 +122,7 @@ def main():
     a = ap.parse_args()
     from visual_odom_b200 import capi, synth
     default_cal = read_calibration(a.calibration)
+    lk_win_param(a)
     if a.slots is not None and not 1 <= a.slots <= capi.VO_MSEQ_MAX:
         raise SystemExit(f"--slots {a.slots}: one context holds 1 to {capi.VO_MSEQ_MAX} slots")
     sized = a.mixed_sizes or a.slots is not None
@@ -169,9 +173,9 @@ def main():
                              "--mixed-sizes)")
         if sized and h // max(a.bucket_divisor, 1) == 0:
             raise SystemExit(f"{d}: {w}x{h} images are too small for the rows/{a.bucket_divisor} bucket size")
-        if sized and seqs and pyramid_depth(w, h) != pyramid_depth(seqs[0]["w"], seqs[0]["h"]):
-            raise SystemExit(f"{d}: {w}x{h} images have {pyramid_depth(w, h)} pyramid levels, {a.datasets[0]} "
-                             f"({seqs[0]['w']}x{seqs[0]['h']}) has {pyramid_depth(seqs[0]['w'], seqs[0]['h'])}: "
+        if sized and seqs and pyramid_depth(w, h, a.lk_win) != pyramid_depth(seqs[0]["w"], seqs[0]["h"], a.lk_win):
+            raise SystemExit(f"{d}: {w}x{h} images have {pyramid_depth(w, h, a.lk_win)} pyramid levels, {a.datasets[0]} "
+                             f"({seqs[0]['w']}x{seqs[0]['h']}) has {pyramid_depth(seqs[0]['w'], seqs[0]['h'], a.lk_win)}: "
                              "one context runs one pyramid depth")
         gt = os.path.join(a.gt, name + ".txt") if a.gt else None
         if gt and not os.path.exists(gt):
@@ -210,9 +214,9 @@ def main():
         print("image sizes: " + ", ".join(f"{s['name']} {s['w']}x{s['h']}" for s in seqs))
     if a.slots is not None:
         W, H = max(s["w"] for s in seqs), max(s["h"] for s in seqs)
-        if pyramid_depth(W, H) != pyramid_depth(seqs[0]["w"], seqs[0]["h"]):
-            raise SystemExit(f"the envelope {W}x{H} of the sizes has {pyramid_depth(W, H)} pyramid levels, the sizes "
-                             f"{pyramid_depth(seqs[0]['w'], seqs[0]['h'])}: one context runs one pyramid depth")
+        if pyramid_depth(W, H, a.lk_win) != pyramid_depth(seqs[0]["w"], seqs[0]["h"], a.lk_win):
+            raise SystemExit(f"the envelope {W}x{H} of the sizes has {pyramid_depth(W, H, a.lk_win)} pyramid levels, the sizes "
+                             f"{pyramid_depth(seqs[0]['w'], seqs[0]['h'], a.lk_win)}: one context runs one pyramid depth")
         # every slot opens at the densest sequence's parameters, which size the mono scratch for the envelope
         densest = max(seqs, key=lambda s: bucket_grid(W, H, s["params"]["bucket_rows_divisor"], s["params"]["features_per_bucket"]))
         a.open_params = densest["params"]
@@ -235,6 +239,8 @@ def main():
     prm["max_features"] = max([prm["max_features"]] + [s["grid"] for s in seqs] +
                               ([env] if a.slots is not None else []))
     prm["pnp_iterations"] = max(max(s["params"]["pnp_iterations"] for s in seqs), base.pnp_iterations)
+    prm["lk_win"] = a.lk_win
+    print(f"LK window: {a.lk_win}x{a.lk_win} (every sequence)")
     print(f"bucketing: {a.features_per_bucket} feature(s) per bucket of rows/{a.bucket_divisor}, ages < {a.age_threshold}, "
           f"refill below {a.refill_threshold} features; max_features {prm['max_features']}")
     if a.check:

@@ -19,7 +19,10 @@
 
 #define VO_PAD 32            // border (pixels) on every side of every level
 #define VO_MAX_LEVELS 8      // pyramid images (maxLevel + 1)
-#define VO_WIN 21            // LK window (the reference hard-codes Size(21,21), feature.cpp:127)
+#define VO_WIN 21            // LK window (the reference hard-codes Size(21,21), feature.cpp:127): k_lk_ring's
+#define VO_WIN_MIN 3         // vo_params.lk_win range: cv2 asserts winSize > 2; other windows run k_lk_win (lk_win.cu)
+#define VO_WIN_MAX 32        // a window of up to VO_PAD pixels reads inside the padded planes
+static_assert(VO_WIN_MAX <= VO_PAD, "every window read must stay inside the padding");
 
 struct LevelGeom {
     int w, h;            // image size at this level
@@ -46,13 +49,14 @@ struct PlaneGeom {
     int pad_;
 };
 
-// effective pyramid depth (maxLevel + 1) of a w x h image: OpenCV stops adding levels once one is not larger than the window
-static inline int vo_pyr_depth(int w, int h, int max_level)
+// effective pyramid depth (maxLevel + 1) of a w x h image: OpenCV stops adding levels once one is not larger than the
+// win x win window
+static inline int vo_pyr_depth(int w, int h, int max_level, int win)
 {
     int n = 1;
     for (int l = 1; l <= max_level; l++) {
         const int nw = (w + 1) / 2, nh = (h + 1) / 2;
-        if (nw <= VO_WIN || nh <= VO_WIN) break;
+        if (nw <= win || nh <= win) break;
         w = nw; h = nh; n++;
     }
     return n;

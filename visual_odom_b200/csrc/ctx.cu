@@ -54,8 +54,14 @@ int vo_check_params(vo_ctx* ctx, const vo_params& p)
         vo_set_error(ctx, "features_per_bucket=%d: a bucket holds at least one feature", p.features_per_bucket);
         return VO_E_INVALID;
     }
-    if (p.lk_win != VO_WIN) {
-        vo_set_error(ctx, "lk_win=%d unsupported: the LK kernel is built for the reference's 21x21 window", p.lk_win);
+    if (p.lk_win < VO_WIN_MIN) {
+        // cv::calcOpticalFlowPyrLK asserts winSize.width > 2 && winSize.height > 2
+        vo_set_error(ctx, "lk_win=%d: the LK window must be at least %dx%d", p.lk_win, VO_WIN_MIN, VO_WIN_MIN);
+        return VO_E_INVALID;
+    }
+    if (p.lk_win > VO_WIN_MAX) {
+        vo_set_error(ctx, "lk_win=%d unsupported: the LK kernels are built for windows from %d to %d", p.lk_win, VO_WIN_MIN,
+                     VO_WIN_MAX);
         return VO_E_UNSUPPORTED;
     }
     if (p.lk_max_level < 0 || p.lk_max_level >= VO_MAX_LEVELS) {
@@ -606,7 +612,7 @@ static int encode_maps(vo_ctx* ctx)
 int vo_ensure_state(vo_ctx* ctx, int w, int h, int units, int levels)
 {
     if (w <= 0 || h <= 0 || units <= 0) { vo_set_error(ctx, "bad geometry %dx%d units=%d", w, h, units); return VO_E_INVALID; }
-    const int depth = vo_pyr_depth(w, h, ctx->p.lk_max_level);
+    const int depth = vo_pyr_depth(w, h, ctx->p.lk_max_level, ctx->p.lk_win);
     if (levels <= 0 || levels > depth) levels = depth;
     if (ctx->w == w && ctx->h == h && ctx->units >= units && ctx->pg.nlevels == levels) return VO_OK;
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
@@ -809,10 +815,14 @@ int vo_run_lk_ring(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, 
         a.progress = ctx->d_lk_progress + uo;
         int lk_sms = ctx->sm_count;
         for (const auto& L : ctx->lane) if (ctx->part_on && v.s == L.lk) lk_sms = ctx->part_lk_sms;
-        // a launch with fewer features than resident warps gains nothing from splitting its rings
-        const bool big = (long)a.n_units * a.per_unit > (long)lk_sms * LK_CTAS_PER_SM * LK_WARPS_PER_CTA;
-        a.span = ctx->lk_span > 0 ? ctx->lk_span : (big ? 2 : 0);
-        VO_CUDA_CHECK(vo_launch_lk_ring(ctx->maps, a, lk_sms, v.s));
+        if (ctx->p.lk_win != VO_WIN) {          // every other window: k_lk_win, one work item per feature-ring
+            VO_CUDA_CHECK(vo_launch_lk_win(a, ctx->p.lk_win, lk_sms, v.s));
+        } else {
+            // a launch with fewer features than resident warps gains nothing from splitting its rings
+            const bool big = (long)a.n_units * a.per_unit > (long)lk_sms * LK_CTAS_PER_SM * LK_WARPS_PER_CTA;
+            a.span = ctx->lk_span > 0 ? ctx->lk_span : (big ? 2 : 0);
+            VO_CUDA_CHECK(vo_launch_lk_ring(ctx->maps, a, lk_sms, v.s));
+        }
     }
     ctx->launches += 1;
     if (e1) VO_CUDA_CHECK(cudaEventRecord(e1, v.s));

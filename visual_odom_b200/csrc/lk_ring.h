@@ -48,4 +48,8 @@ size_t vo_lk_smem_bytes();
 cudaError_t vo_lk_prepare();
 // sm_count sizes the persistent grid (CTAs = min(needed, sm_count * LK_CTAS_PER_SM))
 cudaError_t vo_launch_lk_ring(const LkMaps& maps, const LkArgs& args, int sm_count, cudaStream_t stream);
+// k_lk_win (lk_win.cu): the same ring at a win x win window, VO_WIN_MIN <= win <= VO_WIN_MAX.  It reads the planes with
+// plain loads (img_base / der_base / pitch / plane) and runs one work item per feature-ring: use_tma, span and progress
+// are not read
+cudaError_t vo_launch_lk_win(const LkArgs& args, int win, int sm_count, cudaStream_t stream);
 int vo_launch_pyramid(const PyrGeom& pg, const uint8_t* const* src_tab_dev, int src_pitch, const PlaneGeom* geo, cudaStream_t stream);

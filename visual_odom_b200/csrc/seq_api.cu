@@ -351,14 +351,14 @@ static int seq_begin(vo_ctx* ctx, const char* who, bool multi, int n, int flags,
                                              : std::vector<vo_params>(1, ctx->p);
     // the envelope of the sizes (the planes' allocation) and the one pyramid depth they must share
     int W = 0, H = 0;
-    const int depth = vo_pyr_depth(w[0], h[0], ctx->p.lk_max_level);
+    const int depth = vo_pyr_depth(w[0], h[0], ctx->p.lk_max_level, ctx->p.lk_win);
     for (int q = 0; q < n; q++) {
         char who_q[32];
         snprintf(who_q, sizeof(who_q), open ? "the envelope at slot %d's parameters" : "sequence %d", q);
         if ((rc = seq_grid_check(ctx, who, who_q, w[q], h[q], par[q]))) return rc;
-        if (vo_pyr_depth(w[q], h[q], ctx->p.lk_max_level) != depth) {
+        if (vo_pyr_depth(w[q], h[q], ctx->p.lk_max_level, ctx->p.lk_win) != depth) {
             vo_set_error(ctx, "%s: sequence 0 (%d x %d) has %d pyramid levels, sequence %d (%d x %d) %d: one run needs one pyramid depth",
-                         who, w[0], h[0], depth, q, w[q], h[q], vo_pyr_depth(w[q], h[q], ctx->p.lk_max_level));
+                         who, w[0], h[0], depth, q, w[q], h[q], vo_pyr_depth(w[q], h[q], ctx->p.lk_max_level, ctx->p.lk_win));
             return VO_E_UNSUPPORTED;
         }
         W = std::max(W, w[q]); H = std::max(H, h[q]);
@@ -517,7 +517,7 @@ static int seq_starts_fit(vo_ctx* ctx, const char* who, int n_start, const vo_ms
         snprintf(who_q, sizeof(who_q), "slot %d", q);
         int rc;
         if ((rc = seq_grid_check(ctx, who, who_q, w, h, ctx->slot_par[q]))) return rc;
-        const int depth = vo_pyr_depth(w, h, ctx->p.lk_max_level);
+        const int depth = vo_pyr_depth(w, h, ctx->p.lk_max_level, ctx->p.lk_win);
         if (depth != ctx->pg.nlevels) {
             vo_set_error(ctx, "%s: slot %d: %d x %d has %d pyramid levels, the run %d", who, q, w, h, depth, ctx->pg.nlevels);
             return VO_E_UNSUPPORTED;
