@@ -122,8 +122,8 @@ VO_API long long vo_kernel_launches(const vo_ctx* ctx);
  * measured with CUDA events on the launching stream; n = launches counted. */
 VO_API int vo_lk_kernel_time(vo_ctx* ctx, double* ms_total, long long* n, int reset);
 /* Run-time knobs (measurement / debugging): "batch_streams" = 1|2 (unit ranges the batched path runs
- * concurrently, default 2), "lk_staging" = 0 (TMA, default) | 1 (plain loads), "lk_span" = phases (level-solves)
- * per LK work item (0 = automatic, default), "graphs" = 1 (default: kernel sequences on the context's stream, and
+ * concurrently, default 2), "lk_span" = phases (level-solves) per LK work item (0 = automatic, default),
+ * "graphs" = 1 (default: kernel sequences on the context's stream, and
  * the two stages of a sequence frame, are replayed as CUDA graphs; unit ranges on the side streams of
  * vo_frame_batch, vo_batch_run and vo_batch_submit are always launched plainly, because their kernels fork to the
  * SM partition or to high-priority helper streams) | 0 (plain launches; needed for vo_lk_kernel_time),

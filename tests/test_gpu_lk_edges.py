@@ -18,7 +18,7 @@ sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_lk_edges as mk          # noqa: E402
 
 SPANS = (0, 1, 2, 3, 5, 7, 16)      # tests/test_gpu_lk_variants.py
-CONFIGS = [dict()] + [dict(lk_span=s) for s in SPANS] + [dict(lk_staging=1, lk_span=s) for s in SPANS]
+CONFIGS = [dict()] + [dict(lk_span=s) for s in SPANS]
 
 
 def _cv2():

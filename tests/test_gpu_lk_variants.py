@@ -1,10 +1,9 @@
-"""The LK ring kernel under every instantiation and work schedule the library can launch, bit for bit against the oracle
-(oracle/lk_ref.c, pinned to cv2 in test_oracle_lk.py).
+"""The LK ring kernel under every work schedule the library can launch, bit for bit against the oracle (oracle/lk_ref.c,
+pinned to cv2 in test_oracle_lk.py).
 
 The default launch is what test_gpu_lk.py sees.  Here every configuration gets a fresh context and runs the same inputs:
-- k_lk_ring<true> (TMA boxes) and k_lk_ring<false> (lk_staging = 1: plain loads);
-- work items of 1, 2, 3, 5, 7 phases (lk_span): the running estimate and the progress counter are handed from item to
-  item, items straddle call boundaries, and an item may end mid-call.
+work items of 1, 2, 3, 5, 7 phases (lk_span): the running estimate and the progress counter are handed from item to
+item, items straddle call boundaries, and an item may end mid-call.
 The automatic span only applies to a launch with more features than resident warps; the tests check that their inputs
 are that large on the GPU they run on.  Consecutive configurations alternate between two input sets, so a
 launch that skipped work cannot pass on what the previous context left in recycled device memory.
@@ -110,7 +109,7 @@ def _run(case, opts, need_big):
         c.close()
 
 
-CONFIGS = [dict(lk_span=s) for s in SPANS] + [dict(lk_staging=1, lk_span=s) for s in SPANS]
+CONFIGS = [dict(lk_span=s) for s in SPANS]
 
 
 @pytest.mark.parametrize("i", range(len(CONFIGS)),

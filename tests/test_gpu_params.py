@@ -4,8 +4,8 @@ every result bit for bit as cv2 (and the oracle, pinned to cv2 at the same value
 - vo_lk_track and vo_circular_match at every pyramid depth the library accepts (up to 8 images: 32 phases per feature in
   the ring), at iteration counts inside and outside calcOpticalFlowPyrLK's clamp, at minEig thresholds including ones a
   quarter ulp from a window's minEig, and on flat and saturated windows at threshold 0 (the D < FLT_EPSILON rejection);
-  the 8-image pyramid and the logged thresholds under every LK launch configuration (TMA and plain-load staging, work
-  items of 1 to 16 phases and the whole ring).
+  the 8-image pyramid and the logged thresholds under every LK launch configuration (work items of 1 to 16 phases and
+  the whole ring).
 - vo_pnp_ransac at iteration counts on and around the wave boundaries of the PnP launch (32, 128) and at or below 0.
 - circ_threshold through vo_frame_batch and the sequence mode.
 - one context with every one of these parameters off its default through vo_frame_batch, vo_seq_push, vo_seq_submit and
@@ -23,7 +23,7 @@ import test_oracle_params as OP  # noqa: E402
 
 POSE_TOL = 1e-8
 SPANS = (0, 1, 2, 3, 5, 7, 16, 32)           # 0 = automatic; 32 = the whole ring of an 8-image pyramid in one item
-CONFIGS = [dict(lk_span=s) for s in SPANS] + [dict(lk_staging=1, lk_span=s) for s in SPANS]
+CONFIGS = [dict(lk_span=s) for s in SPANS]
 CONFIG_IDS = ["-".join(f"{k}={v}" for k, v in c.items()) for c in CONFIGS]
 
 

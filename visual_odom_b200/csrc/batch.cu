@@ -427,7 +427,7 @@ static int run_range(vo_ctx* ctx, int u0, int n, cudaStream_t s)
     for (const auto& L : ctx->lane) on_side = on_side || (L.side && s == L.side);
     if (on_side) return run_range_launch(ctx, v);
     GraphKey key{};
-    key.kind = GraphKey::BATCH_RANGE; key.s = s; key.tma = ctx->lk_use_tma;
+    key.kind = GraphKey::BATCH_RANGE; key.s = s;
     key.u0 = u0; key.n = n; key.max_pts = v.max_pts; key.detect = ctx->batch_detect; key.mono = range_mono(ctx, u0, n);
     return vo_run_graph(ctx, key, [&] { return run_range_launch(ctx, v); });
 }

@@ -157,12 +157,8 @@ extern "C" int vo_create(int device, const vo_params* params, vo_ctx** out)
     ctx->bucket_cap = 2 * (size_t)ctx->cap;
     VO_CUDA_CHECK(cudaMalloc(&ctx->d_lk_queue, LK_QUEUES * 2 * sizeof(int)));
     VO_CUDA_CHECK(cudaMemset(ctx->d_lk_queue, 0, LK_QUEUES * 2 * sizeof(int)));
-    {   // VO_LK_STAGING=ldg switches the LK window staging from TMA to plain loads (debug / A-B runs)
-        const char* st = getenv("VO_LK_STAGING");
-        ctx->lk_use_tma = !(st && strcmp(st, "ldg") == 0);
-        const char* sp = getenv("VO_LK_SPAN");      // force the LK work-item size (tests/test_gpu_lk_variants.py sets it per context with "lk_span")
-        if (sp) ctx->lk_span = atoi(sp);
-    }
+    const char* sp = getenv("VO_LK_SPAN");          // force the LK work-item size (tests/test_gpu_lk_variants.py sets it per context with "lk_span")
+    if (sp) ctx->lk_span = atoi(sp);
     return VO_OK;
 }
 
@@ -226,7 +222,6 @@ extern "C" int vo_set_option(vo_ctx* ctx, const char* key, double value)
 {
     if (!ctx || !key) return VO_E_INVALID;
     if (strcmp(key, "batch_streams") == 0) { ctx->batch_streams = value >= 2 ? 2 : 1; return VO_OK; }
-    if (strcmp(key, "lk_staging") == 0) { ctx->lk_use_tma = !(value >= 1); return VO_OK; }
     if (strcmp(key, "batch_outputs") == 0) { ctx->batch_outputs = value >= 1; vo_drop_graphs(ctx); return VO_OK; }
     if (strcmp(key, "sm_partition") == 0) {          // k > 0: the kernels after the LK ring on k SMs of their own; 0: no partition
         if (value < 0) { vo_set_error(ctx, "sm_partition=%g: the number of SMs must not be negative", value); return VO_E_INVALID; }
@@ -422,7 +417,7 @@ void vo_drop_graphs(vo_ctx* ctx)
 
 static bool same_key(const GraphKey& a, const GraphKey& b)
 {
-    return a.kind == b.kind && a.s == b.s && a.tma == b.tma && a.u0 == b.u0 && a.n == b.n && a.max_pts == b.max_pts &&
+    return a.kind == b.kind && a.s == b.s && a.u0 == b.u0 && a.n == b.n && a.max_pts == b.max_pts &&
            a.detect == b.detect && a.mono == b.mono && a.slot == b.slot && a.parity == b.parity && a.bgr == b.bgr;
 }
 
@@ -784,7 +779,6 @@ int vo_run_lk_ring(vo_ctx* ctx, const View& v, int ncalls, const int* img_prev, 
     a.status_out = ctx->d_status + uo;
     a.err_out = want_err ? ctx->d_err + uo : nullptr;
     a.call_stride = (size_t)ctx->units * ctx->cap;
-    a.use_tma = ctx->lk_use_tma ? 1 : 0;
     for (int l = 0; l < pg.nlevels; l++) {      // absolute plane bases (indexed with the absolute plane number)
         a.img_base[l] = ctx->pg.lv[l].img; a.der_base[l] = ctx->pg.lv[l].der;
         a.pitch[l] = pg.lv[l].pitch; a.plane[l] = pg.lv[l].plane;

@@ -21,7 +21,6 @@
 struct GraphKey {
     enum Kind { BATCH_RANGE, SEQ_FRONT, SEQ_BACK } kind;
     cudaStream_t s;
-    bool tma;
     int u0, n, max_pts; bool detect;        // BATCH_RANGE: the unit range, its feature bound, on-GPU detection
                                             // (SEQ_FRONT: max_pts = the LK launch bound, the sequences' largest bucket grid)
     bool mono;                              // BATCH_RANGE: a unit of the range runs the mono_rotation branch
@@ -195,7 +194,6 @@ struct vo_ctx {
     double lk_ms = 0.0;
     long long lk_n = 0;
     bool lk_timing = true;
-    bool lk_use_tma = true;
     int lk_span = 0;                    // phases per LK work item: 0 = automatic (one level-solve per item when a launch has
                                         // more features than resident warps, else one item per feature-ring)
     int* d_lk_progress = nullptr;       // [units][cap] hand-over counters of the LK work items (zero between launches)

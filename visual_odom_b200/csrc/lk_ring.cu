@@ -161,22 +161,6 @@ static_assert(PP >= TW - 1 && PP % 2 == 0, "pair tile pitch");
 #define J_BYTES (TW * J_ROWS)
 #define D_BYTES (DW * I_ROWS * 4)
 
-// plain-load staging of one box (debug / A-B path): rows x 48 bytes from a padded plane
-__device__ __forceinline__ void ldg_box_u8(uint8_t* dst, const uint8_t* plane, int pitch, int x, int y, int rows, int lane)
-{
-    const uint8_t* src = plane + (size_t)y * pitch + x;
-    for (int r = 0; r < rows; r++) {
-        dst[r * TW + lane] = __ldg(src + (size_t)r * pitch + lane);
-        if (lane < TW - 32) dst[r * TW + 32 + lane] = __ldg(src + (size_t)r * pitch + 32 + lane);
-    }
-}
-__device__ __forceinline__ void ldg_box_u32(uint32_t* dst, const uint32_t* plane, int pitch, int x, int y, int lane)
-{
-    const uint32_t* src = plane + (size_t)y * pitch + x;
-    if (lane < DW)
-        for (int r = 0; r < I_ROWS; r++) dst[r * DW + lane] = __ldg(src + (size_t)r * pitch + lane);
-}
-
 // the pair tile of the J tile in place: lane r expands row r (three 128-bit loads, one PRMT and one store per output
 // word).  Halfword TW - 1 pairs the last byte with 0 and is never read.
 __device__ __forceinline__ void expand_pairs(const uint8_t* jtile, uint16_t* pairs, int lane)
@@ -192,6 +176,20 @@ __device__ __forceinline__ void expand_pairs(const uint8_t* jtile, uint16_t* pai
         dst[2 * i + 1] = __byte_perm(w[i], w[i + 1], 0x4332);   // (x+2, x+3), (x+3, x+4)
     }
     __syncwarp();                           // the Newton loop reads other lanes' rows
+}
+
+// re-stage the J tile at box origin (jbx, jby) of `map` and wait for it: every lane is done with the old tile and its
+// pair tile, and lane 0's proxy fence orders those accesses before the TMA write
+__device__ __forceinline__ void reload_jtile(WarpSmem& sm, const CUtensorMap* map, int jbx, int jby, int img, int lane,
+                                             uint32_t& phase)
+{
+    __syncwarp();
+    if (lane == 0) {
+        fence_proxy_async();
+        mbar_expect_tx(&sm.bar, J_BYTES);
+        tma_load_3d(sm.jtile, map, &sm.bar, jbx, jby, img);
+    }
+    mbar_wait(&sm.bar, phase); phase ^= 1;
 }
 
 __device__ __forceinline__ void bilinear_weights(float a, float b, int& w00, int& w01, int& w10, int& w11)
@@ -260,7 +258,7 @@ __device__ __forceinline__ float combine_chains(float acc)
 // ---------------------------------------------------------------------------------------------
 // SIZED: the units' images have sizes of their own (args.geo); the other instantiation is the launch-wide-size kernel
 // exactly, so runs of one image size pay nothing for the table
-template <bool USE_TMA, bool SIZED>
+template <bool SIZED>
 __global__ void __launch_bounds__(LK_WARPS_PER_CTA * 32, LK_CTAS_PER_SM)
 k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
 {
@@ -294,13 +292,11 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
     float* const a22 = reinterpret_cast<float*>(sm.dwin) + A22_OFF;
     uint16_t* const pairs = reinterpret_cast<uint16_t*>(sm.iwin);
 
-    if (USE_TMA) {
-        if (lane == 0) {
-            mbar_init(&sm.bar, 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncwarp();
+    if (lane == 0) {
+        mbar_init(&sm.bar, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
+    __syncwarp();
     uint32_t phase = 0;
 
     const float half_win = (VO_WIN - 1) * 0.5f;
@@ -383,26 +379,18 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                 // every lane is done with the previous level-solve's generic accesses of the windows (A22's chain slots
                 // and the pair tile in iwin / dwin, the J tile), and lane 0's proxy fence orders them before the TMA writes
                 __syncwarp();
-                if (USE_TMA) {
-                    if (lane == 0) {
-                        fence_proxy_async();
-                        mbar_expect_tx(&sm.bar, I_BYTES + D_BYTES + (j_ok0 ? J_BYTES : 0));
-                        tma_load_3d(sm.iwin, &maps.img_i[level], &sm.bar, ibx, iby, img_prev);
-                        tma_load_3d(sm.dwin, &maps.der[level], &sm.bar, dbx, iby, img_prev);
-                        if (j_ok0)
-                            tma_load_3d(sm.jtile, &maps.img_j[level], &sm.bar, jbx, jby, img_next);
-                    }
-                } else {
-                    ldg_box_u8(sm.iwin, args.img_base[level] + args.plane[level] * img_prev, args.pitch[level], ibx, iby, I_ROWS, lane);
-                    ldg_box_u32(sm.dwin, args.der_base[level] + args.plane[level] * img_prev, args.pitch[level], dbx, iby, lane);
+                if (lane == 0) {
+                    fence_proxy_async();
+                    mbar_expect_tx(&sm.bar, I_BYTES + D_BYTES + (j_ok0 ? J_BYTES : 0));
+                    tma_load_3d(sm.iwin, &maps.img_i[level], &sm.bar, ibx, iby, img_prev);
+                    tma_load_3d(sm.dwin, &maps.der[level], &sm.bar, dbx, iby, img_prev);
                     if (j_ok0)
-                        ldg_box_u8(sm.jtile, args.img_base[level] + args.plane[level] * img_next, args.pitch[level], jbx, jby, J_ROWS, lane);
-                    __syncwarp();
+                        tma_load_3d(sm.jtile, &maps.img_j[level], &sm.bar, jbx, jby, img_next);
                 }
                 float a = px - (float)ipx, b = py - (float)ipy;
                 int w00, w01, w10, w11;
                 bilinear_weights(a, b, w00, w01, w10, w11);
-                if (USE_TMA) { mbar_wait(&sm.bar, phase); phase ^= 1; }
+                mbar_wait(&sm.bar, phase); phase ^= 1;
 
                 // ---- patch extraction: I (x32), Ix, Iy of the strip elements; A addends in chain order ----
                 // a strip element's gradients as the Newton loop consumes them: the kept one (Ix in an even-cpos lane, Iy in an odd
@@ -500,18 +488,7 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                     if (!tile_valid || rx < 0 || ry < 0 || rx > TW - 22 || ry > J_ROWS - 22) {
                         jbx = (inx - 5 + VO_PAD) & ~15; jby = iny - 5 + VO_PAD;
                         rx = inx + VO_PAD - jbx; ry = 5;
-                        __syncwarp();
-                        if (USE_TMA) {
-                            if (lane == 0) {
-                                fence_proxy_async();
-                                mbar_expect_tx(&sm.bar, J_BYTES);
-                                tma_load_3d(sm.jtile, &maps.img_j[level], &sm.bar, jbx, jby, img_next);
-                            }
-                            mbar_wait(&sm.bar, phase); phase ^= 1;
-                        } else {
-                            ldg_box_u8(sm.jtile, args.img_base[level] + args.plane[level] * img_next, args.pitch[level], jbx, jby, J_ROWS, lane);
-                            __syncwarp();
-                        }
+                        reload_jtile(sm, &maps.img_j[level], jbx, jby, img_next, lane, phase);
                         expand_pairs(sm.jtile, pairs, lane);
                         tile_valid = true;
                     }
@@ -647,18 +624,7 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
                         if (!tile_valid || rx < 0 || ry < 0 || rx > TW - 22 || ry > J_ROWS - 22) {
                             jbx = (inx - 5 + VO_PAD) & ~15; jby = iny - 5 + VO_PAD;
                             rx = inx + VO_PAD - jbx; ry = 5;
-                            __syncwarp();
-                            if (USE_TMA) {
-                                if (lane == 0) {
-                                    fence_proxy_async();
-                                    mbar_expect_tx(&sm.bar, J_BYTES);
-                                    tma_load_3d(sm.jtile, &maps.img_j[0], &sm.bar, jbx, jby, img_next);
-                                }
-                                mbar_wait(&sm.bar, phase); phase ^= 1;
-                            } else {
-                                ldg_box_u8(sm.jtile, args.img_base[0] + args.plane[0] * img_next, args.pitch[0], jbx, jby, J_ROWS, lane);
-                                __syncwarp();
-                            }
+                            reload_jtile(sm, &maps.img_j[0], jbx, jby, img_next, lane, phase);
                         }
                         a = fxp - (float)inx; b = fyp - (float)iny;
                         bilinear_weights(a, b, w00, w01, w10, w11);
@@ -721,18 +687,16 @@ k_lk_ring(const __grid_constant__ LkMaps maps, const LkArgs args)
 // ---------------------------------------------------------------------------------------------
 size_t vo_lk_smem_bytes() { return sizeof(WarpSmem) * LK_WARPS_PER_CTA; }
 
-template <bool T, bool S>
+template <bool S>
 static cudaError_t prep()
 {
-    return cudaFuncSetAttribute(k_lk_ring<T, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)vo_lk_smem_bytes());
+    return cudaFuncSetAttribute(k_lk_ring<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)vo_lk_smem_bytes());
 }
 
 cudaError_t vo_lk_prepare()
 {
-    cudaError_t e = prep<false, false>();
-    if (e == cudaSuccess) e = prep<true, false>();
-    if (e == cudaSuccess) e = prep<false, true>();
-    return e != cudaSuccess ? e : prep<true, true>();
+    const cudaError_t e = prep<false>();
+    return e != cudaSuccess ? e : prep<true>();
 }
 
 cudaError_t vo_launch_lk_ring(const LkMaps& maps, const LkArgs& args, int sm_count, cudaStream_t stream)
@@ -744,10 +708,7 @@ cudaError_t vo_launch_lk_ring(const LkMaps& maps, const LkArgs& args, int sm_cou
     if (ctas > resident) ctas = resident;
     const int thr = LK_WARPS_PER_CTA * 32;
     const size_t sh = vo_lk_smem_bytes();
-    if (args.geo) {
-        if (args.use_tma) k_lk_ring<true, true><<<(int)ctas, thr, sh, stream>>>(maps, args);
-        else k_lk_ring<false, true><<<(int)ctas, thr, sh, stream>>>(maps, args);
-    } else if (args.use_tma) k_lk_ring<true, false><<<(int)ctas, thr, sh, stream>>>(maps, args);
-    else k_lk_ring<false, false><<<(int)ctas, thr, sh, stream>>>(maps, args);
+    if (args.geo) k_lk_ring<true><<<(int)ctas, thr, sh, stream>>>(maps, args);
+    else k_lk_ring<false><<<(int)ctas, thr, sh, stream>>>(maps, args);
     return cudaGetLastError();
 }

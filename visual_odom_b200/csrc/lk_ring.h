@@ -36,8 +36,7 @@ struct LkArgs {
     int per_unit;           // feature slots per unit that can be live (<= cap)
     int span;               // phases (level-solves) per work item; 0 or >= ncalls*nlevels = one item per feature-ring
     int* progress;          // [n_units][cap] phases completed per feature (hand-over between items; all zero between launches)
-    // plain-load staging (debug / A-B measurement; VO_LK_STAGING=ldg): plane geometry per level
-    int use_tma;
+    // plane geometry per level, for k_lk_win's plain loads (k_lk_ring reads the planes through LkMaps)
     const uint8_t* img_base[VO_MAX_LEVELS];
     const uint32_t* der_base[VO_MAX_LEVELS];
     int pitch[VO_MAX_LEVELS];
@@ -49,7 +48,7 @@ cudaError_t vo_lk_prepare();
 // sm_count sizes the persistent grid (CTAs = min(needed, sm_count * LK_CTAS_PER_SM))
 cudaError_t vo_launch_lk_ring(const LkMaps& maps, const LkArgs& args, int sm_count, cudaStream_t stream);
 // k_lk_win (lk_win.cu): the same ring at a win x win window, VO_WIN_MIN <= win <= VO_WIN_MAX.  It reads the planes with
-// plain loads (img_base / der_base / pitch / plane) and runs one work item per feature-ring: use_tma, span and progress
-// are not read
+// plain loads (img_base / der_base / pitch / plane) and runs one work item per feature-ring: span and progress are not
+// read
 cudaError_t vo_launch_lk_win(const LkArgs& args, int win, int sm_count, cudaStream_t stream);
 int vo_launch_pyramid(const PyrGeom& pg, const uint8_t* const* src_tab_dev, int src_pitch, const PlaneGeom* geo, cudaStream_t stream);

@@ -16,7 +16,7 @@
 // Parallelisation: one warp per feature-ring, taken from the launch's work queue (queue[0] = next feature, queue[1] = warps
 // that ran dry; the last warp to retire resets both, the contract k_lk_ring keeps).  One work item is a whole ring:
 // LkArgs::span and progress are not used (progress stays all zero), and the windows are read with plain loads from the
-// padded planes (img_base / der_base / pitch / plane), never with TMA, so the lk_span and lk_staging options do not apply.
+// padded planes (img_base / der_base / pitch / plane), never with TMA, so the lk_span option does not apply.
 // The padding of VO_PAD = 32 pixels covers every read: a window starts at -W <= ipx <= w - 1 and reads columns
 // ipx .. ipx + W, so reads stay in [-32, w + 31] (rows likewise).
 //

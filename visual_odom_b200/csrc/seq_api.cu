@@ -668,7 +668,7 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
         VO_CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->lane[1].join, 0));
     }
     GraphKey key{};
-    key.kind = GraphKey::SEQ_FRONT; key.s = ctx->stream; key.tma = ctx->lk_use_tma;
+    key.kind = GraphKey::SEQ_FRONT; key.s = ctx->stream;
     key.slot = s0; key.parity = p; key.bgr = bgr;
     // the LK launch bound: the largest bucket grid of the sequences' sizes, which a new set of sizes inside the same
     // envelope, or a start, can raise (the sizes themselves are in the geometry table, not in the graph)
@@ -679,7 +679,7 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
     cudaStream_t sb = ctx->lane[0].side;
     VO_CUDA_CHECK(cudaStreamWaitEvent(sb, ctx->seq_front_ev[p], 0));
     key = GraphKey{};
-    key.kind = GraphKey::SEQ_BACK; key.s = sb; key.tma = ctx->lk_use_tma; key.parity = p;
+    key.kind = GraphKey::SEQ_BACK; key.s = sb; key.parity = p;
     if ((rc = vo_run_graph(ctx, key, [&] { return seq_back(ctx, p); }))) return rc;
     // a started sequence's next frame solves from zeros: after k_seq_finish of this frame copied the slot's translation
     for (int i = 0; i < n_start; i++)
