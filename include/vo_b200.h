@@ -650,6 +650,59 @@ VO_API int vo_mseq_wait_device(vo_ctx* ctx, const vo_mseq_dresults* r);
 VO_API int vo_mseq_pose(vo_ctx* ctx, int q, double frame_pose[16]);
 VO_API int vo_mseq_state(vo_ctx* ctx, int q, vo_point2f* points, int32_t* ages, int cap, int* n_points, int* n_ages, double t_out[3]);
 
+/* ---- rectification of raw stereo frames (the sequence modes) ---------------------------------------------------------
+ * For rigs that deliver raw frames (EuRoC-style datasets, raw ZED / RealSense streams) ORB-SLAM2's stereo settings file
+ * carries LEFT.K / LEFT.D / LEFT.R / LEFT.P and the same four for RIGHT, and its driver runs
+ *     cv::initUndistortRectifyMap(K, D, R, P, size, CV_32F, M1, M2);  cv::remap(raw, rect, M1, M2, cv::INTER_LINEAR);
+ * on both images of every frame.  The sequence modes do this on the GPU, bit for bit.
+ *   vo_rectify_cam     one camera in the settings file's terms; P is the left 3 x 3 of LEFT.P (its fourth column, the
+ *                      baseline, belongs in the P_l / P_r the sequence is begun with)
+ *   vo_rectify_maps    cv2.initUndistortRectifyMap(K, D, R, P, (w, h), CV_32FC1) bit for bit as cv2 computes it on an
+ *                      x86-64 CPU with AVX2 (host code in the operation order of that build: steps of 8 pixels with fused
+ *                      multiply-adds, each row's last w % 8 pixels by its scalar loop); map_x / map_y: w * h floats each.
+ *                      Refused with VO_E_INVALID: n_d not 4, 5 or 8, a non-finite entry, a singular P * R, w or h <= 0,
+ *                      NULL pointers.
+ *   vo_remap           cv2.remap(src, map_x, map_y, INTER_LINEAR, borderMode = BORDER_CONSTANT, 0) of a w x h gray host
+ *                      image through w x h float maps into dst, by the GPU kernel the sequence modes use (stage-level
+ *                      entry point, for parity tests; synchronous)
+ *   vo_seq_rectify     the rectification of the sequences vo_seq_begin* begin from then on (NULL: none).  Host state only.
+ *   vo_mseq_rectify    slots [first_slot, first_slot + n) get r[i] (r == NULL or r[i].left.n_d == 0: the slot is plain), with
+ *                      vo_mseq_params' rules: host state only (it may be called while frames are in flight), read by every
+ *                      begin (vo_mseq_begin*, vo_mseq_begin_device), vo_mseq_open and every start of the slot; a running
+ *                      sequence keeps what it began with.
+ * A rectified sequence's frames -- its first pair included -- are remapped at its own w x h (the raw size, as ORB-SLAM2
+ * passes it) through maps built once by its begin or start: the result is cv2.remap(cvtColor(raw)) of each image (colour is
+ * converted per tap, as the reference converts at load), and every record, point list, carried state and frame_pose is
+ * that of the same sequence fed the cv2-rectified frames, bit for bit.  Every input works: host gray and BGR, device gray,
+ * HWC and CHW, sized runs, starts, VO_MSEQ_MONO_ROTATION, VO_MSEQ_DEVICE_RESULTS.
+ * Launches: a submission with no rectified sequence launches exactly what it launched before (a retired sequence is
+ * not rectified any more).  With any: device input adds
+ * none (the conversion launch remaps); host gray input adds one (one remap launch for every rectified image of the
+ * submission, on the copy stream under the frame in flight); host BGR input adds none (its in-graph conversion becomes
+ * that one launch, which converts the plain sequences' images too).  A start costs no kernel launch: its maps are an H2D
+ * copy ordered on the copy stream before the remap that first reads them.  Unlike a plain start, a rectified start
+ * allocates when its slot's map block is too small for its size (the outgrown block is freed by the next begin) and
+ * when it is the run's first rectified sequence (the gray staging of the envelope).
+ * Device memory per rectified sequence: 6 bytes per pixel and camera of maps (cv::convertMaps(CV_16SC2)'s form), 5.6 MB
+ * at 1241 x 376, plus 2 bytes per pixel of staging for host gray frames.  Host time of a rectified begin or start: the
+ * maps of both cameras in double and one pageable H2D copy, 89 ms more than a plain begin at 1241 x 376 (one host core of
+ * an H100 80GB HBM3 machine; tools/rectify_timing.py).
+ * Refused, changing nothing: vo_seq_rectify / vo_mseq_rectify entries that vo_rectify_maps refuses, and a range outside
+ * 0 .. VO_MSEQ_MAX (VO_E_INVALID). */
+typedef struct vo_rectify_cam {
+    double K[9];   /* camera matrix, row-major (LEFT.K)                   */
+    double D[8];   /* k1 k2 p1 p2 [k3 [k4 k5 k6]] (LEFT.D)                 */
+    int    n_d;    /* 4, 5 or 8                                           */
+    double R[9];   /* rectifying rotation, row-major (LEFT.R)             */
+    double P[9];   /* new camera matrix: the left 3 x 3 of LEFT.P         */
+} vo_rectify_cam;
+typedef struct vo_rectify { vo_rectify_cam left, right; } vo_rectify;
+VO_API int vo_rectify_maps(const vo_rectify_cam* c, int w, int h, float* map_x, float* map_y);
+VO_API int vo_remap(vo_ctx* ctx, const uint8_t* src, size_t pitch, int w, int h, const float* map_x, const float* map_y,
+                    uint8_t* dst, size_t dst_pitch);
+VO_API int vo_seq_rectify(vo_ctx* ctx, const vo_rectify* r);
+VO_API int vo_mseq_rectify(vo_ctx* ctx, int first_slot, int n, const vo_rectify* r);
+
 /* ---- image ingest (SURVEY.md 8f, row N3) ---------------------------------------------------------------
  * What loadImageLeft / loadImageRight do (reference src/utils.cpp:172-190): read <dir>/image_0/%06d.png and
  * <dir>/image_1/%06d.png with cv::imread(IMREAD_COLOR) and cvtColor(BGR2GRAY).  The decoder is host code

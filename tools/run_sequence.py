@@ -8,7 +8,9 @@ are pushed through vo_seq_submit / vo_seq_wait (two in flight), frame_pose is in
 scale gates, the trajectory is written in the KITTI text format and, with --gt, scored with the KITTI segment metric.
 `--mono-rotation` runs trackingFrame2Frame as its header default does (mono_rotation = true: the rotation from
 findEssentialMat + recoverPose, the translation from the PnP; frames where that branch would abort are reported and not
-integrated).  `--lk-win W` tracks with a W x W window (3 to 32; the reference's 21 by default).  `--check` only validates the inputs (no GPU needed)."""
+integrated).  `--lk-win W` tracks with a W x W window (3 to 32; the reference's 21 by default).  `--rectify SETTINGS.yaml`
+rectifies raw frames on the GPU as ORB-SLAM2's stereo driver does (initUndistortRectifyMap + remap(INTER_LINEAR) with the
+settings file's LEFT / RIGHT K, D, R, P).  `--check` only validates the inputs (no GPU needed)."""
 import argparse
 import os
 import re
@@ -30,6 +32,41 @@ def read_calibration(path):
     if missing:
         raise SystemExit(f"{path}: missing Camera.{missing[0]}")
     return vals
+
+
+def _opencv_matrices(text):
+    """name -> float64 array of every `name: !!opencv-matrix` node of an OpenCV-YAML text (rows, cols, data)."""
+    out = {}
+    for m in re.finditer(r"^\s*([\w.]+)\s*:\s*!!opencv-matrix\s*\n((?:[ \t]+.*\n?)+)", text, re.M):
+        body = m.group(2)
+        rows = int(re.search(r"rows\s*:\s*(\d+)", body).group(1))
+        cols = int(re.search(r"cols\s*:\s*(\d+)", body).group(1))
+        data = re.search(r"data\s*:\s*\[([^\]]*)\]", body, re.S).group(1)
+        vals = np.array([float(v) for v in data.replace("\n", " ").split(",") if v.strip()], np.float64)
+        if vals.size != rows * cols:
+            raise SystemExit(f"{m.group(1)}: {vals.size} values for a {rows} x {cols} matrix")
+        out[m.group(1)] = vals.reshape(rows, cols)
+    return out
+
+
+def read_rectify(path):
+    """The rectification of an ORB-SLAM2 stereo settings file: {"left": (K, D, R, P), "right": (K, D, R, P),
+    "size": (LEFT.width, LEFT.height)} from its LEFT.K / D / R / P and RIGHT.* opencv-matrix nodes (P is 3 x 4; the
+    library takes its left 3 x 3).  What cv2.FileStorage reads from the same file, without cv2."""
+    text = open(path).read()
+    mats = _opencv_matrices(text)
+    out = {}
+    for side in ("LEFT", "RIGHT"):
+        try:
+            K, D, R, P = (mats[f"{side}.{k}"] for k in "KDRP")
+        except KeyError as e:
+            raise SystemExit(f"{path}: missing {e.args[0]}")
+        if K.shape != (3, 3) or R.shape != (3, 3) or P.shape[0] != 3 or P.shape[1] not in (3, 4) or D.size not in (4, 5, 8):
+            raise SystemExit(f"{path}: {side}: K, R must be 3 x 3, P 3 x 3 or 3 x 4, D 4, 5 or 8 coefficients")
+        out[side.lower()] = (K, D.ravel(), R, P)
+    size = [re.search(r"^\s*LEFT\.%s\s*:\s*(\d+)" % k, text, re.M) for k in ("width", "height")]
+    out["size"] = tuple(int(m.group(1)) for m in size) if all(size) else None
+    return out
 
 
 def count_frames(dataset, first):
@@ -91,6 +128,8 @@ def main():
                     help="rotation from findEssentialMat + recoverPose (trackingFrame2Frame's header default)")
     add_bucket_args(ap)
     add_lk_win_arg(ap)
+    ap.add_argument("--rectify", metavar="SETTINGS.yaml",
+                    help="rectify the raw frames with the LEFT / RIGHT K, D, R, P of an ORB-SLAM2 stereo settings file")
     ap.add_argument("--check", action="store_true")
     a = ap.parse_args()
     from visual_odom_b200 import capi, synth
@@ -105,6 +144,11 @@ def main():
     print(f"{n} stereo pairs of {w}x{h} (PNG colour type {ctype}, {depth} bit); P_left =\n{P_l}\nP_right =\n{P_r}")
     print("rotation: " + ("findEssentialMat + recoverPose (mono_rotation = true)" if a.mono_rotation else
                           "Rodrigues of the PnP rvec (mono_rotation = false)"))
+    rect = read_rectify(a.rectify) if a.rectify else None
+    if rect:
+        if rect["size"] and rect["size"] != (w, h):
+            raise SystemExit(f"{a.rectify}: LEFT.width / height {rect['size']} differ from the {w}x{h} frames")
+        print(f"rectification: {a.rectify} (initUndistortRectifyMap + remap(INTER_LINEAR) on the GPU)")
     prm = bucket_params(a, [(w, h)])
     prm["lk_win"] = lk_win_param(a)
     print(f"LK window: {a.lk_win}x{a.lk_win}")
@@ -114,6 +158,7 @@ def main():
         return
     ctx = capi.Context(a.device, max_units=2, **prm)
     ctx.set_option("mono_rotation", 1 if a.mono_rotation else 0)
+    ctx.seq_rectify(rect)
     aborted = 0
     rd = capi.SequenceReader(a.dataset, a.first, n, threads=a.threads, depth=a.threads + 3)
     lp, rp, rw, rh, pitch, ch, fid = rd.next_ptr()

@@ -36,7 +36,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import numpy as np
 
 from run_sequence import (add_bucket_args, add_lk_win_arg, bucket_grid, bucket_params, count_frames, lk_win_param,
-                          read_calibration)
+                          read_calibration, read_rectify)
 
 
 def pyramid_depth(w, h, win):
@@ -108,6 +108,9 @@ def main():
                     help="rotation from findEssentialMat + recoverPose (trackingFrame2Frame's header default)")
     ap.add_argument("--calibration-for", action="append", default=[], metavar="NAME=YAML",
                     help="calibration of the dataset named NAME (repeatable; the others use the positional one)")
+    ap.add_argument("--rectify-for", action="append", default=[], metavar="NAME=SETTINGS.yaml",
+                    help="rectify the raw frames of the dataset named NAME with the LEFT / RIGHT K, D, R, P of an "
+                         "ORB-SLAM2 stereo settings file (repeatable; the others run as they are)")
     ap.add_argument("--mixed-sizes", action="store_true",
                     help="run sequences of different image sizes together, each at its own size")
     ap.add_argument("--slots", type=int, metavar="N",
@@ -161,6 +164,18 @@ def main():
         if not os.path.isfile(path):
             raise SystemExit(f"--calibration-for {spec}: {path} does not exist")
         cal_for[name] = (path, read_calibration(path))
+    rect_for = {}
+    for spec in a.rectify_for:
+        name, sep, path = spec.partition("=")
+        if not sep or not name or not path:
+            raise SystemExit(f"--rectify-for {spec}: expected NAME=SETTINGS.yaml")
+        if name not in names:
+            raise SystemExit(f"--rectify-for {spec}: no dataset is named {name} (names: {', '.join(names)})")
+        if name in rect_for:
+            raise SystemExit(f"--rectify-for: {name} is given twice")
+        if not os.path.isfile(path):
+            raise SystemExit(f"--rectify-for {spec}: {path} does not exist")
+        rect_for[name] = (path, read_rectify(path))
     seqs = []
     for d, name in zip(a.datasets, names):
         n = count_frames(d, 0)
@@ -182,8 +197,13 @@ def main():
             raise SystemExit(f"{gt}: no ground truth for sequence {name}")
         cal_path, cal = cal_for.get(name, (a.calibration, default_cal))
         P_l, P_r = synth.proj_matrices(cal)
-        seqs.append(dict(dir=d, name=name, n=n, w=w, h=h, gray=ctype == 0, gt=gt, P_l=P_l, P_r=P_r, own=params_for.get(name, {})))
-        print(f"{name}: {n} stereo pairs of {w}x{h} (PNG colour type {ctype}, {depth} bit), calibration {cal_path}")
+        rect_path, rect = rect_for.get(name, (None, None))
+        if rect and rect["size"] and rect["size"] != (w, h):
+            raise SystemExit(f"{rect_path}: LEFT.width / height {rect['size']} differ from {name}'s {w}x{h} frames")
+        seqs.append(dict(dir=d, name=name, n=n, w=w, h=h, gray=ctype == 0, gt=gt, P_l=P_l, P_r=P_r, own=params_for.get(name, {}),
+                         rect=rect))
+        print(f"{name}: {n} stereo pairs of {w}x{h} (PNG colour type {ctype}, {depth} bit), calibration {cal_path}"
+              + (f", rectified with {rect_path}" if rect else ""))
         print(f"  P_left =\n{P_l}\n  P_right =\n{P_r}")
         if sweep:
             break                            # the sweep runs the first dataset only
@@ -253,6 +273,7 @@ def main():
     force = 0 if len({s["gray"] for s in seqs}) == 1 else 1
     ctx = capi.Context(a.device, **a.context_params)
     ctx.mseq_params(0, [s["params"] for s in seqs])
+    ctx.mseq_rectify(0, [s["rect"] for s in seqs])
     rds = [capi.SequenceReader(s["dir"], 0, s["n"], threads=a.threads, depth=a.threads + 3, force_channels=force) for s in seqs]
 
     def pairs(k):
@@ -340,6 +361,7 @@ def run_queue(a, capi, seqs, sched, W, H):
                 rds[i] = capi.SequenceReader(s["dir"], 0, s["n"], threads=a.threads, depth=a.threads + 3, force_channels=force)
                 start[s["slot"]] = (s["w"], s["h"], s["P_l"], s["P_r"])
                 ctx.mseq_params(s["slot"], [s["params"]])         # read by the start (host state: the slot may be in flight)
+                ctx.mseq_rectify(s["slot"], [s["rect"]])
             l, r, _, _, pitch, ch, _ = rds[i].next_ptr()
             lp[s["slot"]], rp[s["slot"]], pitches[s["slot"]] = l, r, pitch
             chs.add(ch)

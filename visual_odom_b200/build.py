@@ -135,9 +135,9 @@ def build_facade(force=False):
 
 
 def build_hostcheck(force=False):
-    """pnp_math.cuh compiled for the host (g++), used by the CPU tests to check the kernels' math."""
+    """pnp_math.cuh (and the other *_math.cuh) compiled for the host (g++), used by the CPU tests to check the kernels' math."""
     src = os.path.join(CSRC, "host_check.cpp")
-    dep = [src] + [os.path.join(CSRC, f) for f in ("pnp_math.cuh", "ess_math.cuh", "p3p_math.cuh")]
+    dep = [src] + [os.path.join(CSRC, f) for f in ("pnp_math.cuh", "ess_math.cuh", "p3p_math.cuh", "remap_math.cuh")]
     cmd = ["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-x", "c++", src, "-o", HOSTCHECK_LIB]
     _build(dep, HOSTCHECK_LIB, cmd, "hostcheck build failed", force)
     return HOSTCHECK_LIB

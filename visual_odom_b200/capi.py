@@ -103,6 +103,52 @@ class VoMseqStart(C.Structure):
     _fields_ = [("slot", C.c_int), ("w", C.c_int), ("h", C.c_int), ("P_l", C.c_float * 12), ("P_r", C.c_float * 12)]
 
 
+class VoRectifyCam(C.Structure):
+    """vo_rectify_cam: one camera of an ORB-SLAM2 stereo settings file (LEFT.K / D / R and the left 3 x 3 of LEFT.P)."""
+    _fields_ = [("K", C.c_double * 9), ("D", C.c_double * 8), ("n_d", C.c_int), ("R", C.c_double * 9), ("P", C.c_double * 9)]
+
+
+class VoRectify(C.Structure):
+    _fields_ = [("left", VoRectifyCam), ("right", VoRectifyCam)]
+
+
+def rectify_cam(K, D, R, P):
+    """A VoRectifyCam from K (3 x 3), D (4, 5 or 8 coefficients), R (3 x 3) and P (3 x 3 or the settings file's 3 x 4)."""
+    c = VoRectifyCam()
+    D = np.asarray(D, np.float64).ravel()
+    if len(D) > 8:
+        raise ValueError(f"rectify_cam: {len(D)} distortion coefficients (4, 5 or 8)")
+    c.K[:] = [float(v) for v in np.asarray(K, np.float64).reshape(9)]
+    c.D[:len(D)] = [float(v) for v in D]
+    c.n_d = len(D)
+    c.R[:] = [float(v) for v in np.asarray(R, np.float64).reshape(9)]
+    c.P[:] = [float(v) for v in np.asarray(P, np.float64).reshape(3, -1)[:, :3].reshape(9)]
+    return c
+
+
+def rectify_struct(rect):
+    """A VoRectify from {"left": (K, D, R, P), "right": (K, D, R, P)} (what tools/run_sequence.py's read_rectify returns,
+    or synth.rectify_rig) or a VoRectify."""
+    if isinstance(rect, VoRectify):
+        return rect
+    r = VoRectify()
+    r.left = rectify_cam(*rect["left"])
+    r.right = rectify_cam(*rect["right"])
+    return r
+
+
+def rectify_maps(cam, w, h):
+    """cv2.initUndistortRectifyMap(K, D, R, P, (w, h), CV_32FC1) of a camera (K, D, R, P) or VoRectifyCam, by
+    vo_rectify_maps (host code; no GPU needed)."""
+    c = cam if isinstance(cam, VoRectifyCam) else rectify_cam(*cam)
+    mx = np.empty((h, w), np.float32)
+    my = np.empty((h, w), np.float32)
+    rc = load_library().vo_rectify_maps(C.byref(c), int(w), int(h), _p(mx), _p(my))
+    if rc != VO_OK:
+        raise VoError(rc, "vo_rectify_maps refused the camera or the size")
+    return mx, my
+
+
 class VoMonoResult(C.Structure):
     _fields_ = [
         ("status", C.c_int), ("n_inliers", C.c_int), ("ransac_iters", C.c_int), ("n_good", C.c_int),
@@ -227,6 +273,10 @@ SIGNATURES = {
     "vo_mseq_wait_device": (C.c_int, [C.c_void_p, C.POINTER(VoMseqDResults)]),
     "vo_pose_step_device": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vo_mseq_pose": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
+    "vo_rectify_maps": (C.c_int, [C.POINTER(VoRectifyCam), C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vo_remap": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "vo_seq_rectify": (C.c_int, [C.c_void_p, C.POINTER(VoRectify)]),
+    "vo_mseq_rectify": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(VoRectify)]),
     "vo_mseq_state": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
                                 C.c_void_p]),
 }
@@ -679,6 +729,36 @@ class Context:
         out = np.empty(a.shape[:2], np.uint8)
         self._check(self.lib.vo_bgr_to_gray(self.h, _p(a), a.strides[0], a.shape[1], a.shape[0], _p(out), out.strides[0]))
         return out
+
+    def remap(self, src, map_x, map_y):
+        """cv2.remap(src, map_x, map_y, INTER_LINEAR, BORDER_CONSTANT 0) of an H x W gray image through H x W float maps,
+        by the sequence modes' kernel (vo_remap, stage-level entry point)."""
+        a = np.ascontiguousarray(src, np.uint8)
+        mx = np.ascontiguousarray(map_x, np.float32); my = np.ascontiguousarray(map_y, np.float32)
+        assert a.ndim == 2 and mx.shape == a.shape and my.shape == a.shape
+        out = np.empty(a.shape, np.uint8)
+        self._check(self.lib.vo_remap(self.h, _p(a), a.strides[0], a.shape[1], a.shape[0], _p(mx), _p(my), _p(out), out.strides[0]))
+        return out
+
+    @staticmethod
+    def rectify_maps(cam, w, h):
+        return rectify_maps(cam, w, h)
+
+    def seq_rectify(self, rect):
+        """The rectification of the sequences seq_begin* begins from then on (vo_seq_rectify): {"left": (K, D, R, P),
+        "right": (...)}, a VoRectify, or None for none."""
+        self._check(self.lib.vo_seq_rectify(self.h, None if rect is None else C.byref(rectify_struct(rect))))
+
+    def mseq_rectify(self, first_slot, rects):
+        """Slots [first_slot, first_slot + len(rects)) get rects[i] (vo_mseq_rectify; None: the slot is plain), read by
+        the next begin, open or start of each slot.  Host state only: allowed while frames are in flight."""
+        if not rects:
+            raise ValueError("mseq_rectify: no slots")
+        arr = (VoRectify * len(rects))()
+        for i, r in enumerate(rects):
+            if r is not None:
+                arr[i] = rectify_struct(r)
+        self._check(self.lib.vo_mseq_rectify(self.h, first_slot, len(rects), arr))
 
     def seq_submit(self, left1, right1):
         """Asynchronous push (gray H x W or BGR H x W x 3); at most two frames in flight. Keep the arrays alive."""

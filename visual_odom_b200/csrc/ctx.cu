@@ -136,6 +136,10 @@ extern "C" int vo_create(int device, const vo_params* params, vo_ctx** out)
     int rc = vo_check_params(ctx, ctx->p);
     if (rc) return rc;
     ctx->slot_par.assign(VO_MSEQ_MAX, ctx->p);
+    ctx->slot_rect_on.assign(VO_MSEQ_MAX, 0);
+    ctx->slot_rect.assign(VO_MSEQ_MAX, vo_rectify{});
+    ctx->d_rect.assign(VO_MSEQ_MAX, nullptr);
+    ctx->rect_bytes.assign(VO_MSEQ_MAX, 0);
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
     if (e != cudaSuccess || ndev <= 0) {
@@ -188,6 +192,9 @@ extern "C" void vo_destroy(vo_ctx* ctx)
     }
     if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
     if (ctx->d_bgr) cudaFree(ctx->d_bgr);
+    for (void* p : ctx->d_rect) if (p) cudaFree(p);
+    for (void* p : ctx->rect_dead) cudaFree(p);
+    if (ctx->d_rect_stage) cudaFree(ctx->d_rect_stage);
     if (ctx->d_lk_queue) cudaFree(ctx->d_lk_queue);
     if (ctx->d_ess) cudaFree(ctx->d_ess);
     if (ctx->d_unit_ess) cudaFree(ctx->d_unit_ess);
@@ -637,6 +644,7 @@ int vo_ensure_state(vo_ctx* ctx, int w, int h, int units, int levels)
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_raw, (size_t)n_img * w * h));
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_raw_tab, (size_t)n_img));
     VO_CUDA_CHECK(dalloc(ctx, &ctx->d_ingest_tab, (size_t)n_img));
+    VO_CUDA_CHECK(dalloc(ctx, &ctx->d_ingest_map, (size_t)n_img));
     {
         std::vector<const uint8_t*> tab(n_img);
         for (int i = 0; i < n_img; i++) tab[i] = ctx->d_raw + (size_t)i * w * h;

@@ -7,6 +7,7 @@
 #include "pnp.h"
 #include "seq.h"
 #include "ess.h"
+#include "remap_math.cuh"
 #include "../../include/vo_b200.h"
 #include <vector>
 #include <functional>
@@ -26,6 +27,9 @@ struct GraphKey {
     bool mono;                              // BATCH_RANGE: a unit of the range runs the mono_rotation branch
     int slot, parity; bool bgr;             // SEQ_FRONT / SEQ_BACK: image slot of the previous pairs, buffer parity, colour input
 };
+
+// One image's rectification maps in fixed point (remap_math.cuh), rows at the image's own width (rectify.cu)
+struct RectMap { const vorect::MapEntry* xy; const uint16_t* a; };
 
 struct vo_ctx {
     int device = 0;
@@ -65,6 +69,7 @@ struct vo_ctx {
     uint8_t* d_raw = nullptr;           // [units*4][h*w] raw images (a smaller image: its own rows packed from the plane start)
     const uint8_t** d_raw_tab = nullptr;// [units*4] pointers into d_raw
     vo_dimage* d_ingest_tab = nullptr;  // [units*4] descriptors of caller device images, per raw plane (staged per submission)
+    RectMap* d_ingest_map = nullptr;    // [units*4] rectification maps of those images (staged with them, sequence mode only)
     float2* d_pts_in = nullptr;         // [units][cap]
     int* d_npts = nullptr;              // [units]
     float2* d_pts_out = nullptr;        // [4][units][cap]
@@ -144,6 +149,23 @@ struct vo_ctx {
     std::vector<char> seq_geo_due;      // [seq_n] image slots whose geometry entries still hold the slot's previous size
     uint8_t* d_bgr = nullptr;           // staging of colour (BGR) inputs, converted by k_bgr_to_gray (ingest.cu)
     size_t bgr_bytes = 0;
+    // rectification of raw frames (vo_seq_rectify, vo_mseq_rectify; rectify.cu).  The settings are host state that the
+    // begin and start calls read: rect_single for vo_seq_begin*, slot_rect[q] for slot q (rect_on: set).  A rectified
+    // sequence q has its maps (both cameras, fixed point) in d_rect[q]; the host frames of rectified sequences are
+    // uploaded to d_rect_stage (gray) or d_bgr (colour) and remapped into the raw planes by one k_bgr_to_gray launch on
+    // the copy stream.  Map blocks that a start outgrew wait in rect_dead until the next begin (a frame in flight may
+    // still read them).
+    bool rect_single_on = false;
+    vo_rectify rect_single{};
+    std::vector<char> slot_rect_on;     // [VO_MSEQ_MAX]
+    std::vector<vo_rectify> slot_rect;  // [VO_MSEQ_MAX]
+    std::vector<char> seq_rect;         // [seq_n] the running sequence q is rectified
+    std::vector<void*> d_rect;          // [VO_MSEQ_MAX]
+    std::vector<size_t> rect_bytes;     // [VO_MSEQ_MAX]
+    std::vector<void*> rect_dead;
+    uint8_t* d_rect_stage = nullptr;
+    size_t rect_stage_bytes = 0;
+    bool seq_bgr_graph = false;         // the last submission converted host BGR inside its front graph (reading d_bgr there)
     // SM partition (green contexts, ctx.cu vo_partition_enable): the LK ring kernel -- persistent, 100 % of the registers of
     // every SM it runs on -- shares its SMs only with the throughput kernels before it (FAST, pyramids); the latency-bound
     // kernels after the ring (filters, triangulation, PnP) run on the rest, so those of one unit range execute WHILE the
@@ -328,18 +350,29 @@ int vo_ensure_pinned(vo_ctx* ctx, size_t bytes);
 // rows are contiguous, else a 2-D copy
 int vo_upload_plane(vo_ctx* ctx, uint8_t* dst, const uint8_t* src, size_t row_bytes, int h, size_t pitch, cudaStream_t st);
 int vo_ensure_bgr(vo_ctx* ctx, size_t bytes);
+// rectify.cu: the refusals of vo_rectify_maps for one camera (who / name: the calling entry point, "left" / "right")
+int vo_rect_check(vo_ctx* ctx, const char* who, const char* name, const vo_rectify_cam* c);
+// the maps of sequence q (rectification r at w x h) into d_rect[q] on st, growing the block when it is too small
+// (grow_ok: the old block may be freed at once; otherwise it waits in rect_dead).  Host time: the maps in double
+int vo_rect_upload(vo_ctx* ctx, int q, const vo_rectify& r, int w, int h, cudaStream_t st, bool grow_ok);
+// sequence q's maps of camera k (0 left, 1 right) at w x h pixels
+RectMap vo_rect_map(const vo_ctx* ctx, int q, int k, int w, int h);
 // k_bgr_to_gray: images tab[0 .. n_img) (device table), or with d_tab == nullptr `packed` advanced by packed_stride per image,
 // into gray planes img_stride_out apart; geo: the images' geometry table entries (nullptr: all w x h).  A table entry
 // with data == NULL is skipped.
+// maps: per image of the table, the fixed-point maps it is remapped through (RectMap, nullptr: none; an entry with xy ==
+// NULL: that image is only converted)
 int vo_launch_bgr_to_gray(const vo_dimage* d_tab, const vo_dimage& packed, size_t packed_stride, uint8_t* d_gray, size_t img_stride_out,
-                          int w, int h, int n_img, cudaStream_t s, const PlaneGeom* geo = nullptr);
+                          int w, int h, int n_img, cudaStream_t s, const PlaneGeom* geo = nullptr, const RectMap* maps = nullptr);
 vo_dimage vo_packed_bgr(const uint8_t* d_bgr, int w);      // the descriptor of w-pixel packed BGR rows
 // VO_E_INVALID + message unless `im` can be read as an image `w` pixels wide in device memory of the context's GPU
 int vo_check_dimage(vo_ctx* ctx, const char* who, const char* name, const vo_dimage* im, int w);
 // caller device images h_tab[0 .. n) (pinned staging, untouched until the copy has run on st) -> raw planes
 // [plane0, plane0 + n): one descriptor copy into d_ingest_tab + plane0 and one k_bgr_to_gray launch on st.  geo: the
-// planes' geometry table entries (images of several sizes, each written packed from its plane's start; nullptr: all w x h)
-int vo_ingest_device(vo_ctx* ctx, const vo_dimage* h_tab, int n, int plane0, cudaStream_t st, const PlaneGeom* geo = nullptr);
+// planes' geometry table entries (images of several sizes, each written packed from its plane's start; nullptr: all w x h).
+// h_maps (pinned, like h_tab): each image's rectification maps, copied into d_ingest_map + plane0 (nullptr: none)
+int vo_ingest_device(vo_ctx* ctx, const vo_dimage* h_tab, int n, int plane0, cudaStream_t st, const PlaneGeom* geo = nullptr,
+                     const RectMap* h_maps = nullptr);
 // a contiguous range of resident work units processed on one stream
 // plane0 >= 0 overrides the image-plane base (default u0 * imgs): the sequence mode ping-pongs its per-frame buffers
 // between two buffer parities while both address the same image ring.  imgs: image planes per unit (4: a stereo pair at

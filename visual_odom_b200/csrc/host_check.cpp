@@ -113,3 +113,13 @@ __attribute__((visibility("default"))) int vo_hostcheck_mono_rotation(const floa
     return max_good;
 }
 }
+// the ingest kernel's remap arithmetic (remap_math.cuh) on a w x h gray image through fixed maps (xy: 2 shorts per pixel,
+// a: the fractions) of w x h pixels
+#include "remap_math.cuh"
+extern "C" __attribute__((visibility("default"))) void vo_hostcheck_remap(const unsigned char* src, int w, int h, const short* xy,
+                                                                          const unsigned short* a, unsigned char* dst)
+{
+    auto tap = [&](int x, int y) { return (int)src[(size_t)y * w + x]; };
+    for (size_t i = 0; i < (size_t)w * h; i++)
+        dst[i] = vorect::remap_pixel(vorect::MapEntry{xy[2 * i], xy[2 * i + 1]}, a[i], w, h, tap);
+}

@@ -14,6 +14,7 @@
 //   * images already in device memory (vo_dimage: gray, interleaved or planar BGR / RGB, any pitch and alignment) are
 //     read by the same kernel straight into the raw gray planes (vo_seq_*_device, vo_batch_submit_device).
 #include "ctx.h"
+#include "remap_math.cuh"
 #include <zlib.h>
 #include <atomic>
 #include <condition_variable>
@@ -352,7 +353,7 @@ extern "C" void vo_reader_close(vo_reader* rd)
 // source rows 3 * w[0] bytes apart (a table source keeps its own pitch) and its gray rows w[0].  A table entry with
 // data == NULL (a retired or empty slot of the multi-sequence mode) is skipped: its plane keeps what it held.
 __global__ void k_bgr_to_gray(const vo_dimage* __restrict__ tab, vo_dimage packed, size_t packed_stride, uint8_t* __restrict__ gray,
-                              size_t img_stride_out, int w, int h, const PlaneGeom* __restrict__ geo)
+                              size_t img_stride_out, int w, int h, const PlaneGeom* __restrict__ geo, const RectMap* __restrict__ maps)
 {
     const int img = blockIdx.z, y = blockIdx.y;
     const int x0 = 4 * (blockIdx.x * blockDim.x + threadIdx.x);
@@ -363,21 +364,24 @@ __global__ void k_bgr_to_gray(const vo_dimage* __restrict__ tab, vo_dimage packe
         src = tab[img];
         if (!src.data) return;
     } else src.data += (size_t)img * packed_stride;
-    const uint8_t* s = src.data + (size_t)y * src.row_pitch + (size_t)x0 * src.pixel_stride;
     const size_t cs = src.channel_stride;
+    // the gray value of source pixel (x, y)
+    auto px = [&](int x, int yy) -> int {
+        const uint8_t* p = src.data + (size_t)yy * src.row_pitch + (size_t)x * src.pixel_stride;
+        if (src.format == VO_FMT_GRAY) return p[0];
+        const int c0 = p[0], g = p[cs], c2 = p[2 * cs];
+        return src.format == VO_FMT_RGB ? vorect::gray_of(c2, g, c0) : vorect::gray_of(c0, g, c2);
+    };
+    const RectMap m = maps ? maps[img] : RectMap{nullptr, nullptr};
     uint8_t* d = gray + (size_t)img * img_stride_out + (size_t)y * w + x0;
     uint8_t o[4];
 #pragma unroll
     for (int i = 0; i < 4; i++) {
-        if (x0 + i < w) {
-            const uint8_t* p = s + (size_t)i * src.pixel_stride;
-            if (src.format == VO_FMT_GRAY) o[i] = p[0];
-            else {
-                const int c0 = p[0], g = p[cs], c2 = p[2 * cs];
-                const int b = src.format == VO_FMT_RGB ? c2 : c0, r = src.format == VO_FMT_RGB ? c0 : c2;
-                o[i] = (uint8_t)((b * 3735 + g * 19235 + r * 9798 + (1 << 14)) >> 15);
-            }
-        } else o[i] = 0;
+        if (x0 + i >= w) o[i] = 0;
+        else if (m.xy) {            // cv::remap(INTER_LINEAR, BORDER_CONSTANT 0) of the converted image
+            const size_t k = (size_t)y * w + x0 + i;
+            o[i] = vorect::remap_pixel(m.xy[k], m.a[k], w, h, px);
+        } else o[i] = (uint8_t)px(x0 + i, y);
     }
     if (x0 + 3 < w && ((size_t)(d - gray) & 3) == 0 && (((size_t)gray) & 3) == 0)
         *reinterpret_cast<uint32_t*>(d) = o[0] | (o[1] << 8) | (o[2] << 16) | ((uint32_t)o[3] << 24);
@@ -386,10 +390,10 @@ __global__ void k_bgr_to_gray(const vo_dimage* __restrict__ tab, vo_dimage packe
 }
 
 int vo_launch_bgr_to_gray(const vo_dimage* d_tab, const vo_dimage& packed, size_t packed_stride, uint8_t* d_gray, size_t img_stride_out,
-                          int w, int h, int n_img, cudaStream_t s, const PlaneGeom* geo)
+                          int w, int h, int n_img, cudaStream_t s, const PlaneGeom* geo, const RectMap* maps)
 {
     dim3 grid(((w + 3) / 4 + 127) / 128, h, n_img);
-    k_bgr_to_gray<<<grid, 128, 0, s>>>(d_tab, packed, packed_stride, d_gray, img_stride_out, w, h, geo);
+    k_bgr_to_gray<<<grid, 128, 0, s>>>(d_tab, packed, packed_stride, d_gray, img_stride_out, w, h, geo, maps);
     return 1;
 }
 
@@ -427,12 +431,15 @@ int vo_check_dimage(vo_ctx* ctx, const char* who, const char* name, const vo_dim
     return VO_OK;
 }
 
-int vo_ingest_device(vo_ctx* ctx, const vo_dimage* h_tab, int n, int plane0, cudaStream_t st, const PlaneGeom* geo)
+int vo_ingest_device(vo_ctx* ctx, const vo_dimage* h_tab, int n, int plane0, cudaStream_t st, const PlaneGeom* geo,
+                     const RectMap* h_maps)
 {
     const size_t plane = (size_t)ctx->w * ctx->h;
     VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_ingest_tab + plane0, h_tab, (size_t)n * sizeof(vo_dimage), cudaMemcpyHostToDevice, st));
+    if (h_maps)
+        VO_CUDA_CHECK(cudaMemcpyAsync(ctx->d_ingest_map + plane0, h_maps, (size_t)n * sizeof(RectMap), cudaMemcpyHostToDevice, st));
     ctx->launches += vo_launch_bgr_to_gray(ctx->d_ingest_tab + plane0, vo_dimage{}, 0, ctx->d_raw + (size_t)plane0 * plane, plane,
-                                           ctx->w, ctx->h, n, st, geo);
+                                           ctx->w, ctx->h, n, st, geo, h_maps ? ctx->d_ingest_map + plane0 : nullptr);
     VO_CUDA_CHECK(cudaGetLastError());
     return VO_OK;
 }

@@ -41,7 +41,7 @@
 // the new host pairs of image slot `slot` (sequence q: lefts[q], rights[q]; a NULL pair is skipped): gray into the raw
 // planes, colour (BGR) bytes into the staging area, converted inside the frame's graph
 // planes (a staging image holds an envelope plane's pixels); every image goes with its own rows of its own width, pitch[q]
-// bytes apart in host memory
+// bytes apart in host memory.  A rectified sequence's gray images go to the rectification staging instead (same layout).
 static int upload_pairs(vo_ctx* ctx, int slot, const uint8_t* const* lefts, const uint8_t* const* rights, const size_t* pitch,
                         int channels, cudaStream_t st)
 {
@@ -56,10 +56,30 @@ static int upload_pairs(vo_ctx* ctx, int slot, const uint8_t* const* lefts, cons
     for (int q = 0; q < n; q++) {
         if (!lefts[q]) continue;
         const uint8_t* imgs[2] = {lefts[q], rights[q]};
+        uint8_t* d = channels == 1 && ctx->seq_rect[q] ? ctx->d_rect_stage : dst;
         for (int k = 0; k < 2; k++)
-            if ((rc = vo_upload_plane(ctx, dst + (2 * q + k) * img, imgs[k], (size_t)channels * ctx->seq_w[q], ctx->seq_h[q], pitch[q], st)))
+            if ((rc = vo_upload_plane(ctx, d + (2 * q + k) * img, imgs[k], (size_t)channels * ctx->seq_w[q], ctx->seq_h[q], pitch[q], st)))
                 return rc;
     }
+    return VO_OK;
+}
+
+static bool seq_rect_any(const vo_ctx* ctx)
+{
+    for (char r : ctx->seq_rect) if (r) return true;
+    return false;
+}
+
+// the host-gray staging of rectified sequences: 2 * n_seq envelope planes, allocated once per run size (when a run
+// starts its first rectified sequence, nothing reads it yet)
+static int seq_rect_stage(vo_ctx* ctx)
+{
+    const size_t bytes = 2 * (size_t)ctx->seq_n * ctx->w * ctx->h;
+    if (!seq_rect_any(ctx) || ctx->rect_stage_bytes >= bytes) return VO_OK;
+    if (ctx->d_rect_stage) cudaFree(ctx->d_rect_stage);
+    ctx->d_rect_stage = nullptr; ctx->rect_stage_bytes = 0;
+    VO_CUDA_CHECK(cudaMalloc(&ctx->d_rect_stage, bytes));
+    ctx->rect_stage_bytes = bytes;
     return VO_OK;
 }
 
@@ -197,14 +217,17 @@ static int seq_back(vo_ctx* ctx, int p)
 // rewritten by the submission that stages into s, three submissions after the one that last copied them to the device;
 // with at most two submissions in flight that one has been waited for, so its copy has run -- when the wait blocks.
 // vo_mseq_wait_device does not, so runs begun with VO_MSEQ_DEVICE_RESULTS wait for seq_tab_ev[s], recorded after the copy.
-struct SeqPinned { vo_unit_result_dev* rec; int* err; EssResult* ess; vo_dimage* tab; size_t bytes; };
+// RectMap[6 * n_seq] follows, indexed as the descriptors: the maps of rectified sequences' images (host or device pairs).
+struct SeqPinned { vo_unit_result_dev* rec; int* err; EssResult* ess; vo_dimage* tab; RectMap* map; size_t bytes; };
 static SeqPinned seq_pinned(vo_ctx* ctx, int n)
 {
     auto up = [](size_t b) { return (b + 255) / 256 * 256; };
     const size_t o_err = up(2 * (size_t)n * sizeof(vo_unit_result_dev)), o_ess = up(o_err + 2 * (size_t)n * sizeof(int));
-    const size_t o_tab = up(o_ess + 2 * (size_t)n * sizeof(EssResult)), end = up(o_tab + 6 * (size_t)n * sizeof(vo_dimage));
+    const size_t o_tab = up(o_ess + 2 * (size_t)n * sizeof(EssResult)), o_map = up(o_tab + 6 * (size_t)n * sizeof(vo_dimage));
+    const size_t end = up(o_map + 6 * (size_t)n * sizeof(RectMap));
     uint8_t* b = (uint8_t*)ctx->h_pinned;
-    return SeqPinned{(vo_unit_result_dev*)b, (int*)(b + o_err), (EssResult*)(b + o_ess), (vo_dimage*)(b + o_tab), end};
+    return SeqPinned{(vo_unit_result_dev*)b, (int*)(b + o_err), (EssResult*)(b + o_ess), (vo_dimage*)(b + o_tab),
+                     (RectMap*)(b + o_map), end};
 }
 
 // the per-sequence device state (FeatureSet, bucket scratch, error and live words) for n sequences, in one allocation that
@@ -308,14 +331,36 @@ static int seq_pairs_check(vo_ctx* ctx, const char* who, bool multi, int n, cons
 // slot's 2 * n_seq raw planes by ONE k_bgr_to_gray launch through the slot's entries of the pinned descriptor table (a
 // retiring or empty slot's entries have data == NULL: its planes keep their stale contents, as a skipped host upload
 // leaves them), each image at its plane's own size from the geometry table in a run of several sizes
+// With rectified sequences (seq_rect) the same launch remaps their images through their maps.  Host pairs are then
+// uploaded first (upload_pairs) and converted / remapped by that one launch as well: colour images of every sequence from
+// the BGR staging, gray images of rectified sequences from the rectification staging (plain gray ones went straight into
+// their planes, and the launch skips them).
 static int stage_pairs(vo_ctx* ctx, int slot, const SeqPairs& in, cudaStream_t st)
 {
-    if (!in.device) return upload_pairs(ctx, slot, in.lefts, in.rights, in.pitch, in.channels, st);
+    const bool rect = seq_rect_any(ctx);
+    int rc;
+    if (!in.device && ((rc = upload_pairs(ctx, slot, in.lefts, in.rights, in.pitch, in.channels, st)) || !rect)) return rc;
     const int n = ctx->seq_n;
-    vo_dimage* tab = seq_pinned(ctx, n).tab + 2 * n * slot;
+    const SeqPinned pin = seq_pinned(ctx, n);
+    vo_dimage* tab = pin.tab + 2 * n * slot;
+    RectMap* map = pin.map + 2 * n * slot;
     if (ctx->seq_dres) VO_CUDA_CHECK(cudaEventSynchronize(ctx->seq_tab_ev[slot]));
-    for (int q = 0; q < n; q++) { tab[2 * q] = in.dl[q]; tab[2 * q + 1] = in.dr[q]; }
-    const int rc = vo_ingest_device(ctx, tab, 2 * n, 2 * n * slot, st, ctx->seq_sized ? ctx->d_geo + 2 * n * slot : nullptr);
+    const size_t plane = (size_t)ctx->w * ctx->h;
+    for (int q = 0; q < n; q++)
+        for (int k = 0; k < 2; k++) {
+            vo_dimage& d = tab[2 * q + k];
+            if (in.device) d = k ? in.dr[q] : in.dl[q];
+            else if (!in.lefts[q] || (in.channels == 1 && !ctx->seq_rect[q])) d = vo_dimage{};
+            else if (in.channels == 3) d = vo_packed_bgr(ctx->d_bgr + (2 * q + k) * 3 * plane, ctx->seq_w[q]);
+            else {
+                d = vo_dimage{};
+                d.data = ctx->d_rect_stage + (2 * q + k) * plane; d.row_pitch = (size_t)ctx->seq_w[q];
+                d.pixel_stride = 1; d.format = VO_FMT_GRAY;
+            }
+            map[2 * q + k] = ctx->seq_rect[q] ? vo_rect_map(ctx, q, k, ctx->seq_w[q], ctx->seq_h[q]) : RectMap{nullptr, nullptr};
+        }
+    rc = vo_ingest_device(ctx, tab, 2 * n, 2 * n * slot, st, ctx->seq_sized ? ctx->d_geo + 2 * n * slot : nullptr,
+                          rect ? map : nullptr);
     if (!rc && ctx->seq_dres) VO_CUDA_CHECK(cudaEventRecord(ctx->seq_tab_ev[slot], st));
     return rc;
 }
@@ -406,6 +451,18 @@ static int seq_begin(vo_ctx* ctx, const char* who, bool multi, int n, int flags,
     ctx->seq_lk_bound = (int)seq_grid(ctx);
     if (ctx->seq_mono && (rc = vo_ensure_unit_ess(ctx, 2 * n))) return rc;
     if ((rc = vo_ensure_pinned(ctx, seq_pinned(ctx, n).bytes))) return rc;
+    // rectification: each sequence's slot setting (vo_mseq_rectify) or the vo_seq_rectify one; an open run has none yet.
+    // Nothing runs, so map blocks outgrown by starts of the previous run can go.
+    for (void* b : ctx->rect_dead) cudaFree(b);
+    ctx->rect_dead.clear();
+    ctx->seq_rect.assign(n, 0);
+    for (int q = 0; q < n && !open; q++) {
+        ctx->seq_rect[q] = multi ? ctx->slot_rect_on[q] : ctx->rect_single_on;
+        if (ctx->seq_rect[q] && (rc = vo_rect_upload(ctx, q, multi ? ctx->slot_rect[q] : ctx->rect_single, w[q], h[q], ctx->stream, true)))
+            return rc;
+    }
+    if ((rc = seq_rect_stage(ctx))) return rc;
+    ctx->seq_bgr_graph = false;
     ctx->seq_dres = multi && (flags & VO_MSEQ_DEVICE_RESULTS);
     if (ctx->seq_dres && !ctx->d_seq_pose) {
         VO_CUDA_CHECK(cudaMalloc(&ctx->d_seq_pose, 16 * (size_t)VO_MSEQ_MAX * sizeof(double)));
@@ -440,7 +497,8 @@ static int seq_begin(vo_ctx* ctx, const char* who, bool multi, int n, int flags,
     // the first pairs into image slot 0 on the caller's stream, after the work already enqueued there (the synchronise
     // below is the release of device images)
     if (!open) {
-        if ((rc = stage_pairs(ctx, 0, *in, ctx->stream)) || (in->bgr() && (rc = convert_pairs(ctx, 0)))) return rc;
+        if ((rc = stage_pairs(ctx, 0, *in, ctx->stream)) || (in->bgr() && !seq_rect_any(ctx) && (rc = convert_pairs(ctx, 0))))
+            return rc;
         if ((rc = vo_run_pyramid(ctx, 0, 2 * n, ctx->stream, sized))) return rc;
     }
     // both event pairs start out signalled, so the first two frames do not wait for a predecessor
@@ -580,9 +638,13 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
         (rc = seq_starts_fit(ctx, who, n_start, starts)))
         return rc;
     for (int q = 0; multi && q < n; q++)
-        if (!in.left(q)) ctx->seq_retired[q] = 1;
+        if (!in.left(q)) {                  // (a retired sequence's images are never staged again: it stops counting as rectified)
+            ctx->seq_retired[q] = 1;
+            ctx->seq_rect[q] = 0;
+        }
     for (int i = 0; i < n_start; i++) {
         const vo_mseq_start& s = starts[i];
+        ctx->seq_rect[s.slot] = ctx->slot_rect_on[s.slot];
         ctx->seq_retired[s.slot] = 0;
         ctx->seq_w[s.slot] = s.w; ctx->seq_h[s.slot] = s.h;
         ctx->seq_par[s.slot] = ctx->slot_par[s.slot];
@@ -591,9 +653,11 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
         ctx->seq_lk_bound = std::max(ctx->seq_lk_bound, (int)seq_grid(ctx->seq_par[s.slot], s.w, s.h));
     }
     VO_CUDA_CHECK(cudaSetDevice(ctx->device));
+    if ((rc = seq_rect_stage(ctx))) return rc;
     const int p = (int)(ctx->seq_submitted & 1);
     const int s0 = ctx->seq_slot, s1 = (s0 + 1) % 3;
-    const bool bgr = in.bgr();
+    // host colour is converted inside the front graph unless a sequence is rectified: then the staging launch converts it
+    const bool rect = seq_rect_any(ctx), bgr = in.bgr() && !rect;
     // Producer ordering of device images: the conversion reads them after the caller's work enqueued so far.  The event is
     // recorded BEFORE the front stream waits for frame k-2's back stage below, so that the conversion does not queue
     // behind that pose solve.
@@ -628,11 +692,13 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
             VO_CUDA_CHECK(cudaMemsetAsync(ctx->d_seq_live + p * n + q, want == 1 ? 1 : 0, sizeof(int), ctx->stream));
         ctx->seq_live[p * n + q] = want;
     }
-    // geometry entries of the image slot s1 for the pairs of started sequences staged into it, on stream gs.  Host pairs:
-    // on the front stream here (their upload reads no entry; the front stage's kernels do).  Device pairs: the conversion
-    // on the copy stream reads them, and it is not ordered after this point of the front stream (it follows fork_ev,
-    // recorded before the wait for seq_back_ev[p] above, so that it does not queue behind frame k-2's pose solve); they are
-    // written on the copy stream after its waits below instead.  Either way every earlier reader of slot s1's entries (the
+    // geometry entries of the image slot s1 for the pairs of started sequences staged into it, on stream gs.  Host pairs
+    // of a submission without rectified sequences: on the front stream here (their upload reads no entry; the front
+    // stage's kernels do).  Device pairs, and host pairs when a rectified sequence sends them through the staging launch:
+    // that launch on the copy stream reads them, and it is not ordered after this point of the front stream (it follows
+    // fork_ev, recorded before the wait for seq_back_ev[p] above, or only the copy stream's own waits for host pairs, so
+    // that it does not queue behind frame k-2's pose solve); they are written on the copy stream after its waits below
+    // instead.  Either way every earlier reader of slot s1's entries (the
     // front stage of frame k-2, which seq_front_ev[p] covers) is done, and every later one (the conversion, the front
     // stage of this frame) follows the write.
     auto write_geo = [&](cudaStream_t gs) {
@@ -645,7 +711,8 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
             }
         return VO_OK;
     };
-    if (!in.device && (rc = write_geo(ctx->stream))) return rc;
+    const bool geo_on_copy = in.device || rect;        // the staging launch on the copy stream reads the entries
+    if (!geo_on_copy && (rc = write_geo(ctx->stream))) return rc;
     if (bgr) {
         // colour frames share one staging buffer: upload + convert stay on the front stream
         if ((rc = stage_pairs(ctx, s1, in, ctx->stream))) return rc;
@@ -660,7 +727,15 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
         cudaStream_t sc = ctx->lane[1].side;
         VO_CUDA_CHECK(cudaStreamWaitEvent(sc, ctx->seq_front_ev[p], 0));
         if (in.device) VO_CUDA_CHECK(cudaStreamWaitEvent(sc, ctx->fork_ev, 0));
-        if (in.device && (rc = write_geo(sc))) return rc;
+        // colour staged here while the previous frame's graph converts the BGR staging: after that graph
+        if (in.bgr() && ctx->seq_bgr_graph) VO_CUDA_CHECK(cudaStreamWaitEvent(sc, ctx->seq_front_ev[1 - p], 0));
+        if (geo_on_copy && (rc = write_geo(sc))) return rc;
+        // the maps of rectified starts, before the remap that first reads them (every earlier reader of the slot's
+        // block is an earlier launch on this stream)
+        for (int i = 0; i < n_start; i++) {
+            const int q = starts[i].slot;
+            if (ctx->seq_rect[q] && (rc = vo_rect_upload(ctx, q, ctx->slot_rect[q], starts[i].w, starts[i].h, sc, false))) return rc;
+        }
         if ((rc = stage_pairs(ctx, s1, in, sc))) return rc;
         // The join is also the release of device images: the caller's later work on ctx->stream is ordered after the
         // conversion, the last read of the images.
@@ -693,6 +768,7 @@ static int seq_submit(vo_ctx* ctx, const char* who, bool multi, const SeqPairs& 
         if (ctx->seq_mono && (rc = vo_copy_unit_ess(ctx, pin.ess + u0, u0, n, sb))) return rc;
     }
     VO_CUDA_CHECK(cudaEventRecord(ctx->seq_back_ev[p], sb));
+    ctx->seq_bgr_graph = bgr;
     ctx->seq_slot = s1;                 // imageLeft_t0 = imageLeft_t1 (main.cpp:157-158)
     ctx->seq_submitted++;
     ctx->seq_inflight++;

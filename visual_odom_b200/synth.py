@@ -15,6 +15,45 @@ import cv2
 KITTI00 = dict(fx=718.856, fy=718.856, cx=607.1928, cy=185.2157, bf=-386.1448)      # calibration/kitti00.yaml:8-14
 ZED = dict(fx=684.367919921875 * 1.5, fy=684.367919921875 * 1.5, cx=960.0, cy=540.0,
            bf=-82.12415128946304 * 1.5)                                               # calibration/zed.yaml scaled to 1920x1080
+# Stereo rigs in the terms of an ORB-SLAM2 settings file (LEFT / RIGHT .K, .D, .R, .P; P is 3 x 4), for rectification
+# (vo_seq_rectify, vo_mseq_rectify): EuRoC's cam0 / cam1 as ORB-SLAM2's EuRoC.yaml gives them, and a KITTI-raw-like colour
+# pair (5 coefficients, small rectifying rotations).
+_EUROC_CAM0 = dict(
+    K=[458.654, 0.0, 367.215, 0.0, 457.296, 248.375, 0.0, 0.0, 1.0],
+    D=[-0.28340811, 0.07395907, 0.00019359, 1.76187114e-05, 0.0],
+    R=[0.999966347530033, -0.001422739138722922, 0.008079580483432283, 0.001365741834644127, 0.9999741760894847,
+       0.007055629199258132, -0.008089410156878961, -0.007044357138835809, 0.9999424675829176],
+    P=[435.2046959714599, 0, 367.4517211914062, 0, 0, 435.2046959714599, 252.2008514404297, 0, 0, 0, 1, 0])
+_EUROC_CAM1 = dict(
+    K=[457.587, 0.0, 379.999, 0.0, 456.134, 255.238, 0.0, 0.0, 1],
+    D=[-0.28368365, 0.07451284, -0.00010473, -3.55590700e-05, 0.0],
+    R=[0.9999633526194376, -0.003625811871560086, 0.007755443660172947, 0.003680398547259526, 0.9999684752771629,
+       -0.007035845251224894, -0.007729688520722713, 0.007064130529506649, 0.999945173484644],
+    P=[435.2046959714599, 0, 367.4517211914062, -47.90639384423901, 0, 435.2046959714599, 252.2008514404297, 0, 0, 0, 1, 0])
+_KITTI_RAW_LEFT = dict(
+    K=[959.791, 0.0, 696.0217, 0.0, 956.9251, 224.1806, 0.0, 0.0, 1.0],
+    D=[-0.3691481, 0.1968681, 0.001353473, 0.0005677587, -0.06770705],
+    R=[0.9999239, 0.00983776, -0.007445048, -0.009869795, 0.9999421, -0.004278459, 0.007402527, 0.004351614, 0.9999631],
+    P=[721.5377, 0.0, 609.5593, 44.85728, 0.0, 721.5377, 172.854, 0.2163791, 0.0, 0.0, 1.0, 0.002745884])
+_KITTI_RAW_RIGHT = dict(
+    _KITTI_RAW_LEFT,
+    R=[0.9999805, -0.006070, 0.001402, 0.006073, 0.9999793, -0.002209, -0.001389, 0.002218, 0.9999966],
+    P=[721.5377, 0.0, 609.5593, -339.5242, 0.0, 721.5377, 172.854, 2.199936, 0.0, 0.0, 1.0, 0.002729905])
+RECTIFY_CAMS = {"euroc_cam0": _EUROC_CAM0, "euroc_cam1": _EUROC_CAM1, "kitti_raw_left": _KITTI_RAW_LEFT,
+                "kitti_raw_right": _KITTI_RAW_RIGHT}
+
+
+def rectify_cam_matrices(c):
+    """(K 3x3, D, R 3x3, P 3x4) float64 of one RECTIFY_CAMS entry."""
+    return (np.asarray(c["K"], np.float64).reshape(3, 3), np.asarray(c["D"], np.float64),
+            np.asarray(c["R"], np.float64).reshape(3, 3), np.asarray(c["P"], np.float64).reshape(3, -1))
+
+
+def rectify_rig(left, right):
+    """{"left": (K, D, R, P), "right": (...)} of two RECTIFY_CAMS names: what Context.seq_rectify / mseq_rectify take."""
+    return {"left": rectify_cam_matrices(RECTIFY_CAMS[left]), "right": rectify_cam_matrices(RECTIFY_CAMS[right])}
+
+
 EGO_RVEC = np.array([0.004, -0.02, 0.001])
 EGO_T = np.array([0.03, -0.01, -0.9])
 
