@@ -25,9 +25,11 @@ LK_EVENT = np.dtype([("pt", "<i4"), ("level", "<i4"), ("iter", "<i4"), ("kind", 
 EV_ITER, EV_EPS, EV_HALF, EV_CAP, EV_JOUT, EV_SETUP, EV_REJECT, EV_IOUT, EV_FINAL = range(9)
 
 # lk_set_sum_mode (lk_ref.c: LK_SUM_*).  SUM_CV2 is the pinned order; SUM_KERNEL is k_lk_ring's exact-path vote and
-# combination (equal to SUM_CV2 on every input); SUM_M1..SUM_M6 are wrong votes or orders
+# combination (equal to SUM_CV2 on every input); SUM_M1..SUM_M6 are wrong votes or orders.  SUM_WIN is k_lk_win's b
+# chains (equal to SUM_CV2); SUM_TAILCOL, SUM_SIMD4, SUM_ADJ and SUM_COMBINE are wrong orders of them (vote-free)
 SUM_CV2, SUM_SEQ, SUM_PAIRS, SUM_SCALAR = 0, 1, 2, 9
 SUM_KERNEL, SUM_M1, SUM_M2, SUM_M3, SUM_M4, SUM_M5, SUM_M6 = range(10, 17)
+SUM_WIN, SUM_TAILCOL, SUM_SIMD4, SUM_ADJ, SUM_COMBINE = range(17, 22)
 
 
 def lib():

@@ -178,6 +178,15 @@ enum {
     LK_SUM_M4 = 14,         /* the vote ignores b2's five chains                                                   */
     LK_SUM_M5 = 15,         /* the exact path combines (c0 + c1) + (c2 + c3)                                       */
     LK_SUM_M6 = 16,         /* the replay adds the tail chain column-major                                         */
+    /* From LK_SUM_WIN on, b1 / b2 are formed by lk_win_b, k_lk_win's chains (no vote, no exact path).  LK_SUM_WIN is that
+     * kernel's rule and must equal mode 0; the others change one piece of it, so that tests can show the LK window-edge
+     * fixture notices each change. */
+    LK_SUM_WIN = 17,        /* k_lk_win's rule                                                                     */
+    LK_SUM_TAILCOL = 18,    /* the b tail chains add column-major                                                  */
+    LK_SUM_SIMD4 = 19,      /* a 4-wide SIMD split nsimd = W & ~3 (A and b; a b column without a partner x + 4 < nsimd
+                             * is added alone)                                                                      */
+    LK_SUM_ADJ = 20,        /* b chain q adds the pair sums of columns (x, x + 1), x = 2q + 8m, not (x, x + 4)       */
+    LK_SUM_COMBINE = 21,    /* the chain totals of A and b combine as (c0 + c1) + (c2 + c3)                        */
 };
 static int g_sum_mode = 0;
 void lk_set_sum_mode(int m) { g_sum_mode = m; }
@@ -393,8 +402,37 @@ static inline float reduce4(const float q[4])
     default:
     case 0: return (q[0] + q[2]) + (q[1] + q[3]);   /* SSE v_reduce_sum: movehl + shuffle */
     case 1: return ((q[0] + q[1]) + q[2]) + q[3];
-    case 2: return (q[0] + q[1]) + (q[2] + q[3]);
+    case 2: case LK_SUM_COMBINE: return (q[0] + q[1]) + (q[2] + q[3]);
     }
+}
+
+/* b1 (comp 0) or b2 (comp 1) as k_lk_win forms them in mode LK_SUM_WIN: SIMD chain q adds, row by row, the float of the
+ * integer pair sum of columns (x, x + 4), x = q + 8m < nsimd; the tail adds the products of columns nsimd.. row-major;
+ * the total is tail + ((c0 + c2) + (c1 + c3)).  The modes after it change one piece (see LK_SUM_*). */
+static float lk_win_b(const int *d, const int16_t *g, int win, int comp, int mode)
+{
+    const int nsimd = mode == LK_SUM_SIMD4 ? (win & ~3) : (win / 8) * 8;
+    float c[4] = {0.f, 0.f, 0.f, 0.f}, t = 0.f;
+    for (int y = 0; y < win; y++) {
+        const int *dr = d + y * win;
+        const int16_t *gr = g + y * win * 2 + comp;
+        for (int q = 0; q < 4; q++) {
+            if (mode == LK_SUM_ADJ) {
+                for (int x = 2 * q; x < nsimd; x += 8)
+                    c[q] += (float)(dr[x] * gr[2 * x] + dr[x + 1] * gr[2 * (x + 1)]);
+            } else {
+                for (int x = q; x < nsimd; x += 8)
+                    c[q] += (float)(dr[x] * gr[2 * x] + (x + 4 < nsimd ? dr[x + 4] * gr[2 * (x + 4)] : 0));
+            }
+        }
+        if (mode != LK_SUM_TAILCOL)
+            for (int x = nsimd; x < win; x++) t += (float)(dr[x] * gr[2 * x]);
+    }
+    if (mode == LK_SUM_TAILCOL)
+        for (int x = nsimd; x < win; x++)
+            for (int y = 0; y < win; y++) t += (float)(d[y * win + x] * g[(y * win + x) * 2 + comp]);
+    const float simd = mode == LK_SUM_COMBINE ? (c[0] + c[1]) + (c[2] + c[3]) : (c[0] + c[2]) + (c[1] + c[3]);
+    return t + simd;
 }
 
 #define W_BITS 14
@@ -425,7 +463,8 @@ void lk_track(const lk_pyr_t *prev, const lk_pyr_t *next,
     const float min_eig_f = (float)min_eig_thr;
     int16_t *Ibuf = (int16_t *)malloc(sizeof(int16_t) * win * win * 3);
     int16_t *dIbuf = Ibuf + win * win;
-    const int nsimd = (win / 8) * 8;   /* columns handled by the 8-wide SIMD body */
+    /* columns handled by the 8-wide SIMD body (LK_SUM_SIMD4: a wrong 4-wide split) */
+    const int nsimd = g_sum_mode == LK_SUM_SIMD4 ? (win & ~3) : (win / 8) * 8;
 
     for (int i = 0; i < npts; i++) { status[i] = 1; if (err) err[i] = 0.f; if (iters_out) iters_out[i] = 0; }
 
@@ -548,7 +587,8 @@ void lk_track(const lk_pyr_t *prev, const lk_pyr_t *next,
                         ib2 += (float)(diffs[x] * dIp[2 * x + 1]);
                     }
                 }
-                const int want_chains = g_log || (g_stats_on && win == 21) || g_sum_mode >= LK_SUM_KERNEL;
+                const int kernel_mode = g_sum_mode >= LK_SUM_KERNEL && g_sum_mode <= LK_SUM_M6;
+                const int want_chains = g_log || (g_stats_on && win == 21) || kernel_mode;
                 lk_chains_t ch;
                 if (want_chains) lk_chain_info(diffs_all, dIbuf, win, &ch);
                 if (g_stats_on && win == 21) lk_chain_stats(diffs_all, dIbuf, win, &ch);
@@ -568,7 +608,11 @@ void lk_track(const lk_pyr_t *prev, const lk_pyr_t *next,
                     ib1 += reduce4(qf0);
                     ib2 += reduce4(qf1);
                 }
-                if (g_sum_mode >= LK_SUM_KERNEL) {
+                if (g_sum_mode >= LK_SUM_WIN) {
+                    ib1 = lk_win_b(diffs_all, dIbuf, win, 0, g_sum_mode);
+                    ib2 = lk_win_b(diffs_all, dIbuf, win, 1, g_sum_mode);
+                }
+                if (kernel_mode) {
                     if (!replayed && lk_vote(&ch, g_sum_mode)) {
                         ib1 = lk_exact_combine(ch.total, g_sum_mode);
                         ib2 = lk_exact_combine(ch.total + 5, g_sum_mode);

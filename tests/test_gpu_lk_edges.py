@@ -1,7 +1,8 @@
 """k_lk_ring at the edges of calcOpticalFlowPyrLK, bit for bit against the oracle (oracle/lk_ref.c) and against cv2 where
 it is importable: the mined edge fixture (tests/golden/lk_edges/lk_edges.npz) under every LK launch configuration, window-bound
 starts in closed form, every pyramid-depth transition and images smaller than the window, saturated images, and host
-images whose row pitch is not their width."""
+images whose row pitch is not their width.  The helpers take the window; the pyramid-depth test also runs k_lk_win at one
+or more windows of each of its classes (tests/test_gpu_lk_win_edges.py has the rest of k_lk_win's edges)."""
 import json
 import os
 import sys
@@ -29,16 +30,16 @@ def _cv2():
         return None
 
 
-def _single_refs(a, b, pts):
+def _single_refs(a, b, pts, win=21):
     """(oracle, cv2 or None) results of one call"""
     from oracle import cref
-    ref = cref.lk_track(a, b, pts)
+    ref = cref.lk_track(a, b, pts, win=win)
     cv2 = _cv2()
     if cv2 is None:
         return ref, None
     crit = (cv2.TERM_CRITERIA_COUNT + cv2.TERM_CRITERIA_EPS, 30, 0.01)
     o, s, e = cv2.calcOpticalFlowPyrLK(a, b, np.ascontiguousarray(pts, np.float32).reshape(-1, 1, 2), None,
-                                       winSize=(21, 21), maxLevel=3, criteria=crit, flags=0, minEigThreshold=0.001)
+                                       winSize=(win, win), maxLevel=3, criteria=crit, flags=0, minEigThreshold=0.001)
     return ref, (o.reshape(-1, 2), s.ravel(), e.ravel())
 
 
@@ -51,8 +52,8 @@ def _assert_single(got, ref, what):
     assert np.array_equal(ge[rs == 1], re[rs == 1]), what
 
 
-def _check_single(ctx, a, b, pts, what):
-    ref, cvr = _single_refs(a, b, pts)
+def _check_single(ctx, a, b, pts, what, win=21):
+    ref, cvr = _single_refs(a, b, pts, win)
     got = ctx.lk_track(a, b, pts)
     _assert_single(got, ref, f"{what} vs oracle")
     if cvr is not None:
@@ -60,12 +61,21 @@ def _check_single(ctx, a, b, pts, what):
     return ref
 
 
-def _check_ring(ctx, imgs, pts, what):
+def _circular(imgs, pts, fs, win, backend):
+    """the reference's circularMatching on the oracle ("c") or on cv2, at a win x win window"""
+    from oracle import ref_path
+    if win == 21:
+        return ref_path.circular_matching(*imgs, pts, fs, backend=backend)
+    import lk_window_scenes as S
+    return S.circular_matching(*imgs, pts, fs, win, backend)
+
+
+def _check_ring(ctx, imgs, pts, what, win=21):
     from oracle import ref_path
     fs = ref_path.FeatureSet()
     fs.points = pts.copy(); fs.ages = np.arange(len(pts), dtype=np.int32) % 5
     ages0 = fs.ages.copy()
-    ref = ref_path.circular_matching(*imgs, pts, fs, backend="c")
+    ref = _circular(imgs, pts, fs, win, "c")
     got = ctx.circular_match(*imgs, pts, ages=ages0)
     assert np.array_equal(got["status4"], ref["raw"]["status"]), f"{what}: ring status differs"
     for k, name in enumerate(("r0", "r1", "l1", "l0_ret")):
@@ -74,7 +84,7 @@ def _check_ring(ctx, imgs, pts, what):
     assert np.array_equal(got["kept_idx"], ref["kept_idx"]), what
     assert np.array_equal(got["ages"], fs.ages), what
     if _cv2() is not None:
-        cvr = ref_path.circular_matching(*imgs, pts, ref_path.FeatureSet(), backend="cv2")["raw"]
+        cvr = _circular(imgs, pts, ref_path.FeatureSet(), win, "cv2")["raw"]
         assert np.array_equal(cvr["status"], ref["raw"]["status"]), f"{what}: oracle ring status differs from cv2"
         for name in ("r0", "r1", "l1", "l0_ret"):
             assert np.array_equal(cvr[name], ref["raw"][name]), f"{what}: oracle ring differs from cv2 ({name})"
@@ -121,12 +131,12 @@ def test_edge_fixture_bit_exact(edges, i):
 ITER_KINDS = (0, 1, 2, 3)           # oracle/cref.py EV_ITER, EV_EPS, EV_HALF, EV_CAP
 
 
-def _eps_flip_cases(a, b, pts, want):
+def _eps_flip_cases(a, b, pts, want, win=21):
     """(start, epsilon) pairs whose track, at that epsilon, has an iteration where delta.ddot(delta) <= eps^2 (double, as
     OpenCV decides) and the float-only test (float)(dx^2 + dy^2) <= (float)eps^2 disagree.  At eps = 0.01 such an
     iteration is rarer than one in 10^8; choosing eps from a logged step makes one per start.  One case per start."""
     from oracle import cref
-    _, _, _, log = cref.lk_track(a, b, pts, return_log=True)
+    _, _, _, log = cref.lk_track(a, b, pts, win=win, return_log=True)
     it = log[np.isin(log["kind"], ITER_KINDS) & (log["d2"] > 1e-6) & (log["d2"] < 1e-2)]
     out, used = [], set()
     for ev in it:
@@ -141,7 +151,7 @@ def _eps_flip_cases(a, b, pts, want):
         else:
             continue
         p = pts[ev["pt"]][None]
-        lg = cref.lk_track(a, b, p, epsilon=float(eps), return_log=True)[3]
+        lg = cref.lk_track(a, b, p, win=win, epsilon=float(eps), return_log=True)[3]
         li = lg[np.isin(lg["kind"], ITER_KINDS)]
         if ((li["d2"] <= e2) != (li["d2f"] <= np.float32(e2))).any():
             out.append((p, float(eps)))
@@ -175,22 +185,66 @@ def test_eps_decided_in_double(built):
 
 
 # ---- window-bound starts in closed form ----------------------------------------------------------------------------
-def _bound_starts(w, h, nlev):
-    """At level l the I window's origin floor(x / 2^l - 10) is in range iff -11 * 2^l <= x < (lw + 10) * 2^l: both bounds
-    and the float just below each, for every level, in x (y mid-image) and in y (x mid-image)."""
-    lw, lh = w, h
+def _level_sizes(w, h, nlev):
     sizes = []
     for l in range(nlev):
-        sizes.append((lw, lh))
-        lw, lh = (lw + 1) // 2, (lh + 1) // 2
+        sizes.append((w, h))
+        w, h = (w + 1) // 2, (h + 1) // 2
+    return sizes
+
+
+def _outside(x, l, win, lw):
+    """is the level-l origin floor(x * 2^-l - (W - 1) / 2), in float32 as the level-solve forms it, out of [-W, lw)?"""
+    o = np.floor(np.float32(x) * np.float32(1.0 / (1 << l)) - np.float32((win - 1) * 0.5))
+    return o < -win or o >= lw
+
+
+def _bound_starts(w, h, nlev, win=21, shift=0.0):
+    """At level l the I window's origin floor(x / 2^l - (W - 1) / 2) is in range (-W <= origin < lw) iff
+    -(W + 1) / 2 * 2^l <= x < (lw + (W - 1) / 2) * 2^l: per level, axis (x with y mid-image, y with x mid-image) and
+    bound v, the three starts v, the float just below v, and the first float below v (at most 64 ulps down) whose origin,
+    rounded as the level-solve rounds it, lies on the other side of the edge from v's.  The float just below a lower
+    bound can round back onto the edge once (W - 1) / 2 is subtracted; the third start then does cross it.  12 starts a
+    level, in that order (_straddle_failures reads them so).  `shift` moves every bound by shift * 2^l (a wrong closed
+    form, whose v and third start then do not straddle the edge)."""
     pts = []
-    for l, (lw, lh) in enumerate(sizes):
+    for l, (lw, lh) in enumerate(_level_sizes(w, h, nlev)):
         s = float(1 << l)
-        for lo, hi, mid, axis in ((-11 * s, (lw + 10) * s, h / 2 + 0.3, 0), (-11 * s, (lh + 10) * s, w / 2 + 0.3, 1)):
+        lo = (-(win + 1) / 2 + shift) * s
+        for hi, mid, axis, n in (((lw + (win - 1) / 2 + shift) * s, h / 2 + 0.3, 0, lw),
+                                 ((lh + (win - 1) / 2 + shift) * s, w / 2 + 0.3, 1, lh)):
             for v in (lo, hi):
-                for x in (np.float32(v), np.nextafter(np.float32(v), np.float32(-np.inf))):
+                v = np.float32(v)
+                below = np.nextafter(v, np.float32(-np.inf))
+                cross = below
+                for _ in range(64):
+                    if _outside(cross, l, win, n) != _outside(v, l, win, n):
+                        break
+                    cross = np.nextafter(cross, np.float32(-np.inf))
+                else:
+                    cross = below
+                for x in (v, below, cross):
                     pts.append((x, mid) if axis == 0 else (mid, x))
     return np.array(pts, np.float32)
+
+
+def _straddle_failures(a, b, pts, win, nlev):
+    """The bounds of _bound_starts(..., nlev, win) whose first and third start do not straddle the edge in the oracle's
+    log: at a lower bound v itself must reach the level-solve and the third start must get EV_IOUT at that level; at an
+    upper bound the other way round.  Returns [(level, axis, "lo" / "hi")] of the bounds that fail."""
+    from oracle import cref
+    log = cref.lk_track(a, b, pts, win=win, return_log=True)[3]
+    sel = log["kind"] == cref.EV_IOUT
+    iout = set(zip(log["pt"][sel].tolist(), log["level"][sel].tolist()))
+    bad = []
+    for l in range(nlev):
+        for axis in (0, 1):
+            for k, side in enumerate(("lo", "hi")):
+                p = 3 * ((l * 2 + axis) * 2 + k)
+                at, cross = (p, l) in iout, (p + 2, l) in iout
+                if (at, cross) != ((False, True) if side == "lo" else (True, False)):
+                    bad.append((l, axis, side))
+    return bad
 
 
 def test_window_bound_starts(ctx):
@@ -198,6 +252,7 @@ def test_window_bound_starts(ctx):
     u = synth.stereo_unit(w, h, 31)
     imgs = [u[k] for k in ("l0", "r0", "l1", "r1")]
     pts = _bound_starts(w, h, 4)
+    assert _straddle_failures(imgs[0], imgs[1], pts, 21, 4) == []
     # a start outside level 0 still carries the estimate of the coarser levels into its (status 0) output position
     _check_single(ctx, imgs[0], imgs[1], pts, "window bounds")
     _check_ring(ctx, imgs, pts, "window bounds ring")
@@ -209,20 +264,57 @@ def test_window_bound_starts(ctx):
 SIZES = [(42, 300, 1), (43, 300, 2), (84, 300, 2), (85, 300, 3), (168, 300, 3), (169, 300, 4),
          (500, 42, 1), (500, 43, 2), (500, 84, 2), (500, 85, 3), (500, 168, 3), (500, 169, 4),
          (40, 30, 1), (20, 200, 1), (200, 20, 1), (7, 60, 1), (60, 5, 1), (3, 3, 1)]
+# k_lk_win: windows of each of its classes (all-tail 3, 4, 7; no tail 8, 16, 24, 32; SIMD + tail 9, 13, 17, 31)
+WIN_WINDOWS = (3, 4, 7, 8, 9, 13, 16, 17, 24, 31, 32)
 
 
-@pytest.mark.parametrize("w,h,nlev", SIZES)
-def test_pyramid_depth_and_tiny_images(ctx, w, h, nlev):
+def _win_sizes(win):
+    """(w, h, levels) at a window W: the pyramid stops once a level is not larger than W, so the depth changes between
+    2^k W and 2^k W + 1 (k = 1..3), in width and in height separately (the other side never limits it); images narrower
+    and shorter than the window, down to 3 x 3."""
+    out = []
+    for k in (1, 2, 3):
+        out += [((1 << k) * win, 300, k), ((1 << k) * win + 1, 300, k + 1)]
+        out += [(500, (1 << k) * win, k), (500, (1 << k) * win + 1, k + 1)]
+    small = max(3, win - 1)
+    out += [(small, 200, 1), (200, small, 1), (max(3, win // 2), max(3, win // 3), 1), (3, 3, 1)]
+    return list(dict.fromkeys(out))
+
+
+DEPTH_CASES = [pytest.param(21, w, h, n, id=f"{w}-{h}-{n}") for w, h, n in SIZES] + \
+              [pytest.param(win, w, h, n, id=f"W{win}-{w}-{h}-{n}") for win in WIN_WINDOWS for w, h, n in _win_sizes(win)]
+
+
+@pytest.fixture(scope="module")
+def win_ctxs(built):
+    """a context per window, made when first asked for"""
+    from visual_odom_b200.capi import Context
+    made = {}
+
+    def get(win):
+        if win not in made:
+            made[win] = Context(0, max_features=8192, lk_win=win)
+        return made[win]
+    yield get
+    for c in made.values():
+        c.close()
+
+
+@pytest.mark.parametrize("win,w,h,nlev", DEPTH_CASES)
+def test_pyramid_depth_and_tiny_images(ctx, win_ctxs, win, w, h, nlev):
     from oracle import cref
+    c = ctx if win == 21 else win_ctxs(win)
     u = synth.stereo_unit(1241, 376, 41)
-    imgs = [np.ascontiguousarray(u[k][100:100 + h, 300:300 + w]) for k in ("l0", "r0", "l1", "r1")]
-    assert cref.Pyramid(imgs[0]).nlevels() == nlev
+    y0 = min(100, 376 - h)
+    imgs = [np.ascontiguousarray(u[k][y0:y0 + h, 300:300 + w]) for k in ("l0", "r0", "l1", "r1")]
+    assert imgs[0].shape == (h, w)
+    assert cref.Pyramid(imgs[0], win).nlevels() == nlev
     rng = np.random.default_rng(w * 1000 + h)
     pts = np.concatenate([np.stack([rng.uniform(-25, w + 25, 300), rng.uniform(-25, h + 25, 300)], 1),
                           np.stack([rng.uniform(0, w, 200), rng.uniform(0, h, 200)], 1),
-                          _bound_starts(w, h, nlev)]).astype(np.float32)
-    _check_single(ctx, imgs[0], imgs[1], pts, f"{w}x{h}")
-    _check_ring(ctx, imgs, pts, f"{w}x{h} ring")
+                          _bound_starts(w, h, nlev, win)]).astype(np.float32)
+    _check_single(c, imgs[0], imgs[1], pts, f"W={win} {w}x{h}", win)
+    _check_ring(c, imgs, pts, f"W={win} {w}x{h} ring", win)
 
 
 # ---- saturated images ----------------------------------------------------------------------------------------------
